@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- STEP inference throughput (clips/s) on B200, BASELINE.json config 4.
+"""bench.py -- STEP inference throughput (clips/s) on H100, BASELINE.json config 4.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic clips: I3D trunk -> (ROIAlign ->
 two-branch head -> tube update) x max_iter=3, B=8 clips per GPU, T=32, 224x224, 11 proposals/clip,
@@ -12,9 +12,13 @@ over NCCL.  Prints ONE JSON line (contract in the task brief).
 value : clips/s with the batch already resident in HBM (device-timed, max over ranks).
 e2e   : same call through the public API with pinned-host clips: H2D of the batch and D2H of the
         last step's scores/boxes inside the timed region.
-roofline : the dominant kernel class (conv_umma_kernel, tcgen05 implicit GEMM): algorithmic conv
+roofline : the dominant kernel class (conv_umma_kernel, wgmma implicit GEMM): algorithmic conv
         FLOPs of one step (SURVEY.md section 8d: 362.06 GFLOP/clip) / the device time of exactly those
-        launches replayed back-to-back, against MEASURED_PEAKS.json's sustained bf16 figure.
+        launches replayed back-to-back, against MEASURED_PEAKS.json's sustained bf16 figure (else the H100 SXM
+        data sheet's dense fp16 figure).
+--dump-outputs DIR : after the timed steps, the outputs of the last timed step (per refinement step the scores and
+        tube boxes, and the detections of the last one) as DIR/<name>.npy, float32; the inputs are seeded, so two
+        builds can be compared output for output.
 cpu_baseline : the oracle port (oracle/model.py, torch-CPU fp32 == the reference's arithmetic) on
         this box's host cores on a bounded sample (1 clip per timed pass).
 --impl reference : the same oracle timed as the reference arm (its own CPU implementation of the path).
@@ -37,30 +41,16 @@ WORKLOAD = dict(B=8, T_in=32, HW=224, N=11, max_iter=3)
 DETECT = dict(conf_thresh=0.01, nms_thresh=0.4, topk=300)
 
 
-CONV_CLASS_SOURCES = ("bottleneck_exit.cu", "common.cuh", "conv_halo.cu", "conv_umma.cu", "umma_ptx.cuh")
-
-
-def csrc_sha():
-    """Hash of the sources of the tcgen05 conv class (the kernels whose DRAM traffic profiles/r2_conv_traffic.json holds), to tie
-    that capture to the build it was taken from; edits to the other kernels do not invalidate it."""
-    import hashlib
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, "step_b200", "csrc")
-    for f in CONV_CLASS_SOURCES:
-        h.update(open(os.path.join(d, f), "rb").read())
-    return h.hexdigest()[:16]
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(tflops=d.get("bf16_tflops_sustained", 1451.1), hbm=d.get("hbm_gbs", 6586.1), src="measured")
-    return dict(tflops=1400.0, hbm=6650.0, src="fallback")
+        return dict(tflops=d.get("bf16_tflops_sustained", 989.0), hbm=d.get("hbm_gbs", 3350.0), src="measured bf16 sustained")
+    return dict(tflops=989.0, hbm=3350.0, src="H100 SXM data sheet, dense fp16 (700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason samples during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clock / throttle-reason samples during the timed region."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -198,7 +188,7 @@ def run_ours(args):
         cur = torch.cuda.current_stream(dev)
         streams[i].wait_stream(cur)
         with torch.cuda.stream(streams[i]):
-            runners[i](x)
+            step.last_hist = runners[i](x)
             last = runners[i].detections[cfg.max_iter - 1]     # per-class NMS + top-k ran inside the captured step
         step.last_stream = streams[i]
         if n_run == 1:
@@ -257,10 +247,12 @@ def run_ours(args):
     mark("warm-up enqueued")
     ms = timed(lambda: step(clips_dev), args.steps)
     mark("device-resident region timed")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step.last_hist, runners[(turn[0] - 1) % n_run].detections[cfg.max_iter - 1])
     launches = launches_per_step * args.steps
 
     # Insurance for the measured number: should the end-to-end region ever fail to drain (seen with programmatic dependent
-    # launch on, DESIGN.md section 3.1), say so on the JSON line with the device-resident value already measured instead of
+    # launch on and the earlier Blackwell kernels, DESIGN.md section 3.1), say so on the JSON line with the device-resident value already measured instead of
     # hanging the caller.  A stalled CUDA context cannot be torn down, hence os._exit.
     def stalled():
         if rank == 0:
@@ -346,24 +338,12 @@ def run_ours(args):
             taps = q.KT * q.KH * q.KW
             alg_bytes += 2 * (q.N * q.T * q.H * q.W * q.Cin + q.Cout * taps * q.Cin +
                               q.N * q.OT * q.OH * q.OW * q.Cout * (2 if q.residual else 1))
-        # DRAM bytes the same launches moved in one ncu capture (tools/gpu_profiles.sh -> profiles/r2_conv_traffic.json).
-        # Only reported when that capture was taken from THIS build (the file is stamped with a hash of the kernel
-        # sources); otherwise null -- a stale number is worse than none.
-        traffic, traffic_src = None, None
-        tp = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r2_conv_traffic.json")
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                if tj.get("csrc_sha") == csrc_sha():
-                    traffic, traffic_src = tj.get("dram_bytes_per_step"), "profiles/r2_conv_traffic.json (ncu, same kernel sources %s)" % tj.get("csrc_sha")
-            except Exception:
-                traffic = None
         flops = ALG_GFLOP_PER_CLIP * 1e9 * B
         achieved = flops / (ms_conv / max(3, args.steps) * 1e-3) / 1e12
-        roof = {"bound": "tensor", "kernel": "tcgen05 conv class: conv_umma_kernel + conv_umma_persist_kernel + conv_halo_kernel + bottleneck_exit_kernel",
+        roof = {"bound": "tensor", "kernel": "wgmma conv class: conv_umma_kernel + conv_halo_kernel + bottleneck_exit_kernel",
                 "achieved": round(achieved, 2),
-                "peak": pk["tflops"], "peak_source": pk["src"] + " bf16 sustained", "unit": "TFLOP/s",
-                "frac": round(achieved / pk["tflops"], 4), "traffic": traffic, "traffic_unit": "DRAM bytes per step, all conv launches (ncu)", "traffic_source": traffic_src,
+                "peak": pk["tflops"], "peak_source": pk["src"], "unit": "TFLOP/s",
+                "frac": round(achieved / pk["tflops"], 4),
                 "algorithmic_bytes_per_step": int(alg_bytes),
                 "launches_per_step": len(rec), "replay": "cuda graph" if replay_fn is not replay else "eager", "ms_per_step_in_kernel": round(ms_conv / max(3, args.steps), 4),
                 "algorithmic_gflop_per_step": round(flops / 1e9, 1)}
@@ -398,6 +378,23 @@ def run_ours(args):
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, hist, last):
+    """The arrays the caller of the timed step receives, from its last execution: per refinement step i the tube scores
+    (pred_prob_i) and boxes (pred_loc_i), and the detections of the last step (det: {x1,y1,x2,y2,score,class,tube,0} rows,
+    det_count: kept rows per clip).  float32, well under 64 MB at the C4 shape."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for i, h in enumerate(hist):
+        arrays["pred_prob_%d" % i] = h["pred_prob"]
+        arrays["pred_loc_%d" % i] = h["pred_loc"]
+    arrays["det"], arrays["det_count"] = last["det"], last["count"]
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def timed_local(torch, fn, steps):
@@ -591,6 +588,8 @@ if __name__ == "__main__":
     ap.add_argument("--no-graph", action="store_true", help="launch the step eagerly instead of replaying the CUDA graph")
     ap.add_argument("--inflight", type=int, default=3, help="independent batches kept in flight on separate streams")
     ap.add_argument("--verbose", action="store_true", help="phase markers on stderr (to locate a stall)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3) if a.impl == "ours" else a.warmup
     if a.impl == "reference":

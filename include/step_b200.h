@@ -1,5 +1,5 @@
 /*
- * step_b200.h -- C ABI of libstep_b200.so: the sm_100a implementation of the STEP hot path.
+ * step_b200.h -- C ABI of libstep_b200.so: the sm_90a implementation of the STEP hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  Every entry point takes raw device
  * pointers, plain sizes and an explicit cudaStream_t; none allocates, synchronises or touches
@@ -152,7 +152,7 @@ int step_nchw_to_nhwc(const float* in, int N, int S, int C, void* out, int dtype
 
 /* ------------------------------------------------------------------ conv / pool / linear - */
 typedef struct {
-  int dtype;                 /* STEP_F32: SIMT fp32 path.  STEP_F16: tcgen05 implicit GEMM, fp32 accumulate */
+  int dtype;                 /* STEP_F32: SIMT fp32 path.  STEP_F16: wgmma implicit GEMM, fp32 accumulate */
   int N, T, H, W;            /* input extent (pixels) */
   int Cin, in_ld;            /* input channels read, channel stride of x */
   int Cout, out_ld, out_coff;/* output channels, channel stride of y, first channel written in y */
@@ -182,8 +182,8 @@ typedef struct {
   int ld_extra[2];
   int coff_extra[2];
   /* Structured zeros of the weights (a_mode 4 only): for the filter taps of the LAST t plane (kt == KT-1) the input
-   * channels [zero_cin_last_kt, Cin) carry zero weights, so their 16-channel MMA steps are skipped.  0 = no such
-   * structure.  The space-to-depth stem has it: tap plane qt = 2 only holds the rt = 0 sub-position (k = 2(q+1)+r <= 6),
+   * channels [zero_cin_last_kt, Cin) carry zero weights.  0 = no such structure.  Advisory: the kernels multiply the
+   * zeros (exactly) rather than skip them.  The space-to-depth stem has it: tap plane qt = 2 only holds the rt = 0 sub-position (k = 2(q+1)+r <= 6),
    * engine.pack_stem_s2d. */
   int zero_cin_last_kt;
 } step_conv_params;

@@ -1,4 +1,4 @@
-"""step_b200 -- the STEP (NVlabs/STEP) inference hot path on B200 (sm_100a).
+"""step_b200 -- the STEP (NVlabs/STEP) inference hot path on H100 (sm_90a).
 
 Public surface mirrors the reference (SURVEY.md section 8b):
     from step_b200 import BaseNet, ROINet, TwoBranchNet, ContextNet      # models/__init__.py:6-7

@@ -58,13 +58,12 @@ extern "C" int step_conv3d_fwd(const step_conv_params* p, step_stream_t stream) 
   }
   if (p->a_mode == 5) {
     // "best": thin inputs on large maps go to the patch kernel, which needs far fewer bytes through TMA than one
-    // im2col tile per tap (measured, tools/conv_bench.py with CB_AMODE=4 vs 3); on 7x7 maps its 16 x 8 pixel tile
-    // is mostly padding.  Everything else: TMA im2col (k > 1) / linear (1x1x1).
+    // im2col tile per tap; on 7x7 maps its 16 x 8 pixel tile is mostly padding.  Everything else: TMA im2col (k > 1) / linear (1x1x1).
     static const bool halo_on = !(getenv("STEP_B200_HALO") && getenv("STEP_B200_HALO")[0] == '0');
     const int taps = p->KT * p->KH * p->KW;
     const int small = p->OH < p->OW ? p->OH : p->OW;
     if (halo_on && taps > 1 && p->ST == 1 && p->SH == 1 && p->SW == 1 && conv3d_halo_supported(p) &&
-        p->Cin <= 32 && small >= 14)   // (Cin = 64, Cout = 192 on 56 x 56 measured equal to im2col: 255 vs 250 us)
+        p->Cin <= 32 && small >= 14)
       return conv3d_halo_launch(p, stream);
     step_conv_params q = *p;
     q.a_mode = taps == 1 ? 0 : 3;

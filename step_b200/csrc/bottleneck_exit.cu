@@ -5,376 +5,177 @@
 //     Y[M, 1024] = relu(H[M, 256] * W3[1024, 256]^T + X[M, 1024])          conv3 + residual + ReLU     (stored unless y == NULL)
 //     Z[M,  256] = act(Y[M, 1024] * W1[256, 1024]^T + shift2)               next conv1 (ReLU) / downsample2 (bias, no ReLU)
 //
-// As two launches of the implicit-GEMM kernel these cost 53 + 20 us at the C4 batch (M = 34496 rows): the first is bound by
-// reading its 1024-wide fp32 accumulator out of TMEM (K is only 256) and the second re-reads the 70 MB activation.  Here a CTA
-// PAIR (cta_group::2, 256 rows) walks the 1024 columns of Y in 16 chunks of 64: GEMM1 chunk -> TMEM (64 columns, 4 buffers) ->
-// epilogue warps add the residual, ReLU, round to fp16 and write the chunk as a K-major 128B-swizzled A operand into shared
-// memory (the same bytes are bulk-stored to Y) -> GEMM2 accumulates Z += Y_chunk * W1[:, chunk]^T in a second TMEM region
-// (256 columns).  Y is rounded to fp16 before GEMM2 exactly as the two-launch path rounds it, and both GEMMs accumulate K in
-// the same order as the library kernel (64-wide k-blocks), so the results are bit-identical to the unfused path.
+// As two launches of the implicit-GEMM kernel the 1024-wide Y makes a round trip through HBM between them.  Here a CTA owns
+// 64 rows and walks the 1024 columns of Y in 16 chunks of 64: consumer warpgroup (chunk & 1) computes the GEMM1 chunk with
+// wgmma (registers), adds the residual, applies the ReLU, rounds to fp16 and writes the chunk as a K-major 128B-swizzled A
+// operand into shared memory (and to Y when it is stored); then both warpgroups accumulate Z += Y_chunk * W1[:, chunk]^T, each
+// for 128 of Z's 256 columns.  Y is rounded to fp16 before GEMM2 exactly as the two-launch path rounds it, and both GEMMs issue
+// the same m64n64k16 wgmma sequence in the same K order as conv_umma.cu, so the results are bit-identical to the unfused path.
 //
-// Per CTA (384 threads): warp 0 loads H and the W3 chunks (TMA), warp 1 issues GEMM1 (leader CTA), warps 2-5 / 6-9 are the
-// epilogue groups of the even / odd chunks, warp 10 loads the W1 slices and prefetches the residual into L2, warp 11 issues
-// GEMM2.  Lessons measured while building it (tools/probe/fused_exit_probe.cu, tools/experiments/README.md): a shared W3 / W1
-// producer thread serialises the two rings; `mbarrier.arrive.release.cluster` compiles to MEMBAR.ALL.GPU and waits for every
-// outstanding global load of the thread (2-4k cycles); MMAs issued from inside a divergent `lane == 0` branch cost ~90 cycles
-// each (R2UR / ELECT loops), which paces N = 64 MMAs -- the issuing warps stay convergent and elect per instruction.
+// Per CTA (384 threads): warp 0 loads H and the W3 chunks (TMA, 3-slot ring), warp 1 loads the W1 slices (2-slot ring),
+// warpgroups 1 and 2 compute.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "common.cuh"
+#include "umma_ptx.cuh"
 
 namespace step {
 namespace bexit {
 
-constexpr int kThreads = 384;                   // warp 0: H + W3 loads, 1: GEMM1 issue, 2-9: epilogue, 10: W1 loads + X prefetch, 11: GEMM2 issue
+constexpr int kThreads = 384;
+constexpr int BM = 64;                          // rows per CTA
 constexpr int K1 = 256, N1 = 1024, N2 = 256, CH = 64, NCH = N1 / CH;   // 16 chunks of 64 columns of Y
-constexpr int kHBytes = 4 * 128 * 128;          // H tile: 4 k-blocks x [128 rows x 128 B]
-constexpr int kB1Bytes = 4 * 32 * 128;          // W3 chunk half: 4 k-blocks x [32 rows x 128 B]
-constexpr int kB2Bytes = 128 * 128;             // W1 half x K slice: [128 rows x 128 B]
-constexpr int kA2Bytes = 128 * 128;             // Y chunk of this CTA: [128 rows x 128 B]
-constexpr int kRing = 3;                        // W3 / W1 chunk rings
-constexpr int kAcc = 4;                         // GEMM1 accumulator buffers (64 TMEM columns each) == A2 (Y chunk) buffers
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t c) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(c)); }
-__device__ __forceinline__ void mbar_expect(uint64_t* b, uint32_t n) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(b)), "r"(n) : "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t ph) {
-  asm volatile("{\n\t.reg .pred p;\n\tWP:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra.uni DP;\n\tbra.uni WP;\n\tDP:\n\t}" ::"r"(smem_u32(b)), "r"(ph) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* b, uint32_t ph) {
-  asm volatile("{\n\t.reg .pred p;\n\tWC:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra.uni DC;\n\tbra.uni WC;\n\tDC:\n\t}" ::"r"(smem_u32(b)), "r"(ph) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* b, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(b)), "r"(cta));
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// pair loads: data into my shared memory, bytes signalled on the LEADER's barrier
-__device__ __forceinline__ void tma2_2d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
-  const uint32_t mbar = smem_u32(bar) & 0xFEFFFFFFu;
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(m), "r"(mbar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_2d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void umma2(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(d), "l"(ad), "l"(bd), "r"(idesc), "r"(acc) : "memory");
-}
-// warp-convergent issue: every lane of the MMA warp runs the loop, one elected lane issues. Inside a divergent `lane == 0`
-// branch the compiler wraps each tcgen05 instruction in an R2UR / ELECT loop (~90 cycles per MMA), which paces N = 64 MMAs.
-__device__ __forceinline__ void umma2_elect(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n\t.reg .pred p, e;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|e, 0xffffffff;\n\t"
-               "@e tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(d), "l"(ad), "l"(bd), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void commit_pair_elect(uint64_t* bar) {
-  asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-               "@e tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void ldg256(const void* p, uint32_t* v) {
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "l"(p));
-}
-__device__ __forceinline__ void stg256(void* p, const uint32_t* v) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-               "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
-}
+constexpr int kHBytes = 4 * BM * 128;           // H tile: 4 k-blocks x [64 rows x 128 B]
+constexpr int kW3Bytes = 4 * CH * 128;          // W3 chunk: 4 k-blocks x [64 rows x 128 B]
+constexpr int kW1Bytes = N2 * 128;              // W1 slice: [256 rows x 128 B]
+constexpr int kYBytes = BM * 128;               // Y chunk: [64 rows x 128 B]
+constexpr int kW3Ring = 3, kW1Ring = 2;
 
 struct Geom {
-  int M, tiles, store_y, relu2, z_ld, x_ld;
+  int M, store_y, relu2, x_ld, y_ld, z_ld;
 };
 
-// barrier block (8-byte slots)
 struct Bars {
-  uint64_t h_full, h_empty;
-  uint64_t b1_full[kRing], b1_empty[kRing];
-  uint64_t b2_full[kRing], b2_empty[kRing];
-  uint64_t acc1_full[kAcc], acc1_empty[kAcc];
-  uint64_t a2_full[kAcc], a2_empty[kAcc];
-  uint64_t acc2_full, acc2_empty;
-  uint32_t tmem_ptr, pad;
+  uint64_t h_full;
+  uint64_t w3_full[kW3Ring], w3_empty[kW3Ring];
+  uint64_t w1_full[kW1Ring], w1_empty[kW1Ring];
 };
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 bottleneck_exit_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_w3,
-                  const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1,
-                  const __grid_constant__ CUtensorMap map_y, Geom g, const float* __restrict__ shift2, const __half* __restrict__ xres,
-                  __half* __restrict__ z) {
+                       const __grid_constant__ CUtensorMap map_w1, Geom g, const float* __restrict__ shift2,
+                       const __half* __restrict__ x, __half* __restrict__ y, __half* __restrict__ z) {
   extern __shared__ __align__(1024) uint8_t raw[];
   Bars* bars = (Bars*)raw;
-  uint8_t* smem = (uint8_t*)(((uintptr_t)raw + sizeof(Bars) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sH = smem;
-  uint8_t* sB1 = sH + kHBytes;
-  uint8_t* sB2 = sB1 + kRing * kB1Bytes;
-  uint8_t* sA2 = sB2 + kRing * kB2Bytes;
-
+  uint8_t* base = (uint8_t*)(((uintptr_t)raw + sizeof(Bars) + 1023) & ~(uintptr_t)1023);
+  uint8_t* sH = base;
+  uint8_t* sW3 = sH + kHBytes;
+  uint8_t* sW1 = sW3 + kW3Ring * kW3Bytes;
+  uint8_t* sY = sW1 + kW1Ring * kW1Bytes;        // [2][kYBytes]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
+  const int m0 = blockIdx.x * BM;
 
   if (threadIdx.x == 0) {
-    mbar_init(&bars->h_full, 1); mbar_init(&bars->h_empty, 1);
-    for (int s = 0; s < kRing; ++s) {
-      mbar_init(&bars->b1_full[s], 1); mbar_init(&bars->b1_empty[s], 1);
-      mbar_init(&bars->b2_full[s], 1); mbar_init(&bars->b2_empty[s], 1);
-    }
-    for (int b = 0; b < kAcc; ++b) {
-      mbar_init(&bars->acc1_full[b], 1); mbar_init(&bars->acc1_empty[b], 8);     // 4 warps x 2 CTAs
-      mbar_init(&bars->a2_full[b], 8);   mbar_init(&bars->a2_empty[b], 1);
-    }
-    mbar_init(&bars->acc2_full, 1); mbar_init(&bars->acc2_empty, 16);            // 8 warps x 2 CTAs
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_h) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w3) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w1) : "memory");
+    mbar_init(&bars->h_full, 1);
+    for (int i = 0; i < kW3Ring; ++i) { mbar_init(&bars->w3_full[i], 1); mbar_init(&bars->w3_empty[i], 1); }
+    for (int i = 0; i < kW1Ring; ++i) { mbar_init(&bars->w1_full[i], 1); mbar_init(&bars->w1_empty[i], 2); }
+    fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars->tmem_ptr)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  cluster_sync();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, bars->tmem_ptr, 0);
-  // programmatic dependent launch: everything above overlapped the previous kernel's tail; nothing below may touch global
-  // memory before that kernel has completed
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  const uint32_t t_acc1 = tmem_base;                    // kAcc x 64 columns
-  const uint32_t t_acc2 = tmem_base + kAcc * CH;        // 256 columns
+  pdl_wait();
+  pdl_launch_dependents();
 
   if (warp == 0) {
-    // ============================== producer ==============================
-    if (lane == 0) {
-      int it = 0;                                 // tiles done by this pair
-      uint32_t cc = 0;                            // chunk counter over the whole kernel (ring / buffer phases)
-      for (int tile = pair; tile < g.tiles; tile += npairs, ++it) {
-        const int row0 = tile * 256 + (int)rank * 128;
-        // H tile (A of GEMM1): reusable once the last GEMM1 of the previous tile retired
-        mbar_wait(&bars->h_empty, ((uint32_t)it & 1u) ^ 1u);
-        if (rank == 0) mbar_expect(&bars->h_full, 2u * kHBytes);
-        for (int kb = 0; kb < 4; ++kb) tma2_2d(&map_h, &bars->h_full, sH + kb * (128 * 128), kb * 64, row0);
-        for (int c = 0; c < NCH; ++c, ++cc) {
-          const int s = (int)(cc % kRing);
-          const uint32_t ring_ph = (cc / kRing) & 1u;
-          // W3 rows [c*64 + rank*32, +32) x K 256 (B of GEMM1)
-          mbar_wait(&bars->b1_empty[s], ring_ph ^ 1u);
-          if (rank == 0) mbar_expect(&bars->b1_full[s], 2u * kB1Bytes);
-          for (int kb = 0; kb < 4; ++kb)
-            tma2_2d(&map_w3, &bars->b1_full[s], sB1 + s * kB1Bytes + kb * (32 * 128), kb * 64, c * CH + (int)rank * 32);
-        }
-      }
-    }
-  } else if (warp == 10) {
-    // ============================== W1 producer (own thread: its ring must not stall the W3 ring) ==============================
-    if (lane == 0) {
-      uint32_t cc = 0;
-      for (int tile = pair; tile < g.tiles; tile += npairs) {
-        // residual rows of this tile -> L2 a few chunks ahead of the epilogue's register loads (all at once would queue in
-        // front of the H / W3 loads the first GEMM waits for)
-        constexpr int kXAhead = 4;
-        const int xr0 = tile * 256 + (int)rank * 128;
-        auto prefetch_x = [&](int c) {
-          asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(&map_x), "r"(c * CH), "r"(xr0) : "memory");
-        };
-        for (int c = 0; c < kXAhead; ++c) prefetch_x(c);
-        for (int c = 0; c < NCH; ++c, ++cc) {
-          if (c + kXAhead < NCH) prefetch_x(c + kXAhead);
-          const int s = (int)(cc % kRing);
-          // W1 rows [rank*128, +128) x K [c*64, +64) (B of GEMM2)
-          mbar_wait(&bars->b2_empty[s], ((cc / kRing) & 1u) ^ 1u);
-          if (rank == 0) mbar_expect(&bars->b2_full[s], 2u * kB2Bytes);
-          tma2_2d(&map_w1, &bars->b2_full[s], sB2 + s * kB2Bytes, c * CH, (int)rank * 128);
-        }
+    if (elect_one()) {
+      mbar_expect_tx(&bars->h_full, kHBytes);
+      for (int kb = 0; kb < 4; ++kb) tma_load_2d(&map_h, &bars->h_full, sH + kb * BM * 128, kb * 64, m0);
+      for (int c = 0; c < NCH; ++c) {
+        const int s = c % kW3Ring;
+        mbar_wait(&bars->w3_empty[s], ((uint32_t)(c / kW3Ring) & 1u) ^ 1u);
+        mbar_expect_tx(&bars->w3_full[s], kW3Bytes);
+        for (int kb = 0; kb < 4; ++kb)
+          tma_load_2d(&map_w3, &bars->w3_full[s], sW3 + s * kW3Bytes + kb * CH * 128, kb * 64, c * CH);
       }
     }
   } else if (warp == 1) {
-    // ============================== GEMM1 issuer (leader CTA; whole warp runs the loop, one elected lane issues) ==============================
-    if (rank == 0) {
-      constexpr uint64_t kDescHi = ((uint64_t)(1024 >> 4) << 32) | (1ULL << 46) | (2ULL << 61);   // K-major, 128B swizzle, SBO 1024
-      const uint32_t idesc1 = (1u << 4) | ((uint32_t)(CH >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);    // M 256, N 64
-      auto lo = [&](const void* p) { return (uint64_t)((smem_u32(p) & 0x3FFFF) >> 4); };
-      int it = 0;
-      uint32_t cc = 0;
-      for (int tile = pair; tile < g.tiles; tile += npairs, ++it) {
-        mbar_wait(&bars->h_full, (uint32_t)it & 1u);
-        for (int c = 0; c < NCH; ++c, ++cc) {
-          const int s = (int)(cc % kRing), b = (int)(cc % kAcc);
-          mbar_wait(&bars->b1_full[s], (cc / kRing) & 1u);
-          mbar_wait_cluster(&bars->acc1_empty[b], ((cc / kAcc) & 1u) ^ 1u);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t d = t_acc1 + (uint32_t)b * CH;
-#pragma unroll
-          for (int kb = 0; kb < 4; ++kb) {
-            const uint64_t a0 = lo(sH + kb * (128 * 128)), b0 = lo(sB1 + s * kB1Bytes + kb * (32 * 128));
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma2_elect(d, kDescHi | (a0 + 2 * k), kDescHi | (b0 + 2 * k), idesc1, (kb | k) ? 1u : 0u);
-          }
-          commit_pair_elect(&bars->b1_empty[s]);
-          commit_pair_elect(&bars->acc1_full[b]);
-        }
-        commit_pair_elect(&bars->h_empty);          // every GEMM1 of this tile is issued: H is free when they retire
+    if (elect_one()) {
+      for (int c = 0; c < NCH; ++c) {
+        const int s = c % kW1Ring;
+        mbar_wait(&bars->w1_empty[s], ((uint32_t)(c / kW1Ring) & 1u) ^ 1u);
+        mbar_expect_tx(&bars->w1_full[s], kW1Bytes);
+        tma_load_2d(&map_w1, &bars->w1_full[s], sW1 + s * kW1Bytes, c * CH, 0);
       }
     }
-  } else if (warp == 11) {
-    // ============================== GEMM2 issuer (leader CTA) ==============================
-    if (rank == 0) {
-      constexpr uint64_t kDescHi = ((uint64_t)(1024 >> 4) << 32) | (1ULL << 46) | (2ULL << 61);
-      const uint32_t idesc2 = (1u << 4) | ((uint32_t)(N2 >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);    // M 256, N 256
-      auto lo = [&](const void* p) { return (uint64_t)((smem_u32(p) & 0x3FFFF) >> 4); };
-      int it = 0;
-      uint32_t cc = 0;
-      for (int tile = pair; tile < g.tiles; tile += npairs, ++it) {
-        for (int c = 0; c < NCH; ++c, ++cc) {
-          const int s = (int)(cc % kRing), b = (int)(cc % kAcc);
-          mbar_wait(&bars->b2_full[s], (cc / kRing) & 1u);
-          mbar_wait_cluster(&bars->a2_full[b], (cc / kAcc) & 1u);
-          if (c == 0) mbar_wait_cluster(&bars->acc2_empty, ((uint32_t)it & 1u) ^ 1u);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t a0 = lo(sA2 + b * kA2Bytes), b0 = lo(sB2 + s * kB2Bytes);
+  } else if (warp >= 4) {
+    const int wg = (warp >> 2) - 1;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const uint64_t hi = desc_hi_kmajor<64>();
+    const uint64_t h_lo = desc_lo(sH), w3_lo = desc_lo(sW3), w1_lo = desc_lo(sW1), y_lo = desc_lo(sY);
+    const int r0 = (warp & 3) * 16 + (lane >> 2);          // rows r0, r0 + 8 of the tile
+    float accz[64];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma2_elect(t_acc2, kDescHi | (a0 + 2 * k), kDescHi | (b0 + 2 * k), idesc2, (c | k) ? 1u : 0u);
-          commit_pair_elect(&bars->b2_empty[s]);
-          commit_pair_elect(&bars->a2_empty[b]);
-        }
-        commit_pair_elect(&bars->acc2_full);
-      }
-    }
-  } else if (warp < 10) {
-    // ============================== epilogue ==============================
-    const int q = warp & 3;                         // TMEM lane quarter = rows [32 q, +32) of my 128
-    const int grp = (warp - 2) >> 2;                // chunk parity this warp serves
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    int it = 0;
-    uint32_t cc0 = 0;                               // global chunk counter at the start of the current tile
-    for (int tile = pair; tile < g.tiles; tile += npairs, ++it, cc0 += NCH) {
-      const int row0 = tile * 256 + (int)rank * 128 + q * 32;
-      const int grow = row0 + lane;
-      const bool row_ok = grow < g.M;
-      const __half* xrow = xres + (size_t)(row_ok ? grow : 0) * g.x_ld;
-      // the residual row segment of a chunk (64 columns = 128 B) goes straight into registers, one chunk of this group ahead
-      uint32_t rcur[32], rnext[32];
-      if (row_ok) {
+    for (int i = 0; i < 64; ++i) accz[i] = 0.0f;
+    mbar_wait(&bars->h_full, 0);
+    for (int p = 0; p < NCH / 2; ++p) {
+      // ---- GEMM1: this warpgroup's chunk c1 of Y ----
+      const int c1 = 2 * p + wg, s3 = c1 % kW3Ring;
+      float acc[32];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) ldg256(xrow + grp * CH + j * 16, rcur + 8 * j);
-      } else {
+      for (int i = 0; i < 32; ++i) acc[i] = 0.0f;
+      mbar_wait(&bars->w3_full[s3], (uint32_t)(c1 / kW3Ring) & 1u);
+      wg_fence();
 #pragma unroll
-        for (int j = 0; j < 32; ++j) rcur[j] = 0;
-      }
-      for (int c = grp; c < NCH; c += 2) {
-        const uint32_t cc = cc0 + (uint32_t)c;
-        const int b = (int)(cc % kAcc);
-        const uint32_t ph = (cc / kAcc) & 1u;
-        if (c + 2 < NCH && row_ok) {
+      for (int kb = 0; kb < 4; ++kb)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) ldg256(xrow + (c + 2) * CH + j * 16, rnext + 8 * j);
-        }
-        mbar_wait(&bars->acc1_full[b], ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t v[64];
-        tmem_ld32(t_acc1 + lane_base + (uint32_t)b * CH, v);
-        tmem_ld32(t_acc1 + lane_base + (uint32_t)b * CH + 32, v + 32);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(&bars->acc1_empty[b], 0);           // accumulator buffer back to the MMA warp
-        // A2 buffer b: GEMM2 of chunk cc - kAcc must have retired, and my own bulk store of that chunk must have read it
-        // (my store of chunk cc - 2 may still be in flight)
-        mbar_wait(&bars->a2_empty[b], ph ^ 1u);
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        __syncwarp();
-        const int row = q * 32 + lane;
-        uint8_t* arow = sA2 + b * kA2Bytes + row * 128;
+        for (int k = 0; k < 4; ++k)
+          wgmma_64x64(acc, hi | (h_lo + (uint64_t)((kb * BM * 128) >> 4) + 2 * k),
+                      hi | (w3_lo + (uint64_t)((s3 * kW3Bytes + kb * CH * 128) >> 4) + 2 * k), 1u);
+      wg_commit();
+      wg_wait<0>();
+      if (leader) mbar_arrive(&bars->w3_empty[s3]);
+      // ---- residual + ReLU -> fp16 Y chunk (swizzled A operand; Y in global memory when stored) ----
+      uint8_t* ybuf = sY + wg * kYBytes;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {                                          // 8 chunks of 16 B = 8 columns each
-          const int sw = (j ^ (row & 7)) << 4;
-          const __half2* rh = reinterpret_cast<const __half2*>(&rcur[4 * j]);
-          uint32_t o[4];
+      for (int i = 0; i < 2; ++i) {
+        const int r = r0 + 8 * i;
+        const bool valid = m0 + r < g.M;
+        const __half* xrow = x + (size_t)(m0 + r) * g.x_ld + c1 * CH;
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float2 rf = __half22float2(rh[k]);
-            const float f0 = fmaxf(__uint_as_float(v[j * 8 + 2 * k]) + rf.x, 0.0f);
-            const float f1 = fmaxf(__uint_as_float(v[j * 8 + 2 * k + 1]) + rf.y, 0.0f);
-            const __half2 h = __floats2half2_rn(f0, f1);
-            o[k] = *reinterpret_cast<const uint32_t*>(&h);
+        for (int j = 0; j < 8; ++j) {
+          const int col = 8 * j + 2 * (lane & 3);
+          float f0 = fmaf(acc[4 * j + 2 * i], 1.0f, 0.0f), f1 = fmaf(acc[4 * j + 2 * i + 1], 1.0f, 0.0f);
+          if (valid) {
+            const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(xrow + col));
+            f0 += rf.x; f1 += rf.y;
           }
-          *reinterpret_cast<uint4*>(arow + sw) = make_uint4(o[0], o[1], o[2], o[3]);
+          f0 = fmaxf(f0, 0.0f); f1 = fmaxf(f1, 0.0f);
+          const __half2 hv = __floats2half2_rn(f0, f1);
+          *reinterpret_cast<__half2*>(ybuf + r * 128 + ((j ^ (r & 7)) << 4) + 4 * (lane & 3)) = hv;
+          if (valid && g.store_y) *reinterpret_cast<__half2*>(y + (size_t)(m0 + r) * g.y_ld + c1 * CH + col) = hv;
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // generic writes -> visible to UMMA / TMA
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive_remote(&bars->a2_full[b], 0);
-          if (g.store_y) tma_store_2d(&map_y, sA2 + b * kA2Bytes + q * 32 * 128, c * CH, row0);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-#pragma unroll
-        for (int j = 0; j < 32; ++j) rcur[j] = rnext[j];
       }
-      // ---- final epilogue: Z tile, 256 columns; warp (q, grp) takes columns [grp*128, +128)
-      mbar_wait(&bars->acc2_full, (uint32_t)it & 1u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int row = tile * 256 + (int)rank * 128 + q * 32 + lane;
-      for (int cb = 0; cb < 128; cb += 32) {
-        uint32_t v[32];
-        const int col = grp * 128 + cb;
-        tmem_ld32(t_acc2 + lane_base + (uint32_t)col, v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (cb + 32 >= 128) {
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive_remote(&bars->acc2_empty, 0);
-        }
-        uint32_t o[16];
+      fence_proxy_async();                                  // generic-proxy writes of Y -> visible to wgmma
+      named_sync(1, 256);
+      // ---- GEMM2: Z[:, 128 wg + (0..127)] += Y_chunk(c) * W1[:, chunk c]^T for c = 2p, 2p + 1, in K order ----
 #pragma unroll
-        for (int k = 0; k < 16; ++k) {
-          float f0 = __uint_as_float(v[2 * k]), f1 = __uint_as_float(v[2 * k + 1]);
-          if (shift2) { f0 += shift2[col + 2 * k]; f1 += shift2[col + 2 * k + 1]; }
+      for (int h = 0; h < 2; ++h) {
+        const int c = 2 * p + h, s1 = c % kW1Ring;
+        mbar_wait(&bars->w1_full[s1], (uint32_t)(c / kW1Ring) & 1u);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+          for (int n = 0; n < 2; ++n)
+            wgmma_64x64(accz + n * 32, hi | (y_lo + (uint64_t)((h * kYBytes) >> 4) + 2 * k),
+                        hi | (w1_lo + (uint64_t)((s1 * kW1Bytes + (128 * wg + 64 * n) * 128) >> 4) + 2 * k), 1u);
+        wg_commit();
+      }
+      wg_wait<0>();
+      if (leader) { mbar_arrive(&bars->w1_empty[0]); mbar_arrive(&bars->w1_empty[1]); }
+      named_sync(1, 256);                                   // both Y buffers are free for the next pair
+    }
+    // ---- Z epilogue: + shift2, optional ReLU, fp16 ----
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = r0 + 8 * i;
+      if (m0 + r >= g.M) continue;
+      __half* zrow = z + (size_t)(m0 + r) * g.z_ld + 128 * wg;
+#pragma unroll
+      for (int n = 0; n < 2; ++n)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int col = 64 * n + 8 * j + 2 * (lane & 3);
+          const float b0 = shift2 ? shift2[128 * wg + col] : 0.0f, b1 = shift2 ? shift2[128 * wg + col + 1] : 0.0f;
+          float f0 = fmaf(accz[n * 32 + 4 * j + 2 * i], 1.0f, b0), f1 = fmaf(accz[n * 32 + 4 * j + 2 * i + 1], 1.0f, b1);
           if (g.relu2) { f0 = fmaxf(f0, 0.0f); f1 = fmaxf(f1, 0.0f); }
-          const __half2 h = __floats2half2_rn(f0, f1);
-          o[k] = *reinterpret_cast<const uint32_t*>(&h);
+          *reinterpret_cast<__half2*>(zrow + col) = __floats2half2_rn(f0, f1);
         }
-        if (row < g.M) {
-          __half* dst = z + (size_t)row * g.z_ld + col;
-          stg256(dst, o); stg256(dst + 16, o + 8);
-        }
-      }
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  cluster_sync();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
@@ -405,9 +206,9 @@ extern "C" int step_bottleneck_exit_f16(const void* h, long long h_ld, const voi
                  planes, inplanes, outplanes);
   STEP_CHECK_ARG(M >= 1 && M <= 0x7fffff00LL, "bottleneck_exit: M = %lld", M);
   STEP_CHECK_ARG(h_ld >= K1 && x_ld >= N1 && z_ld >= N2 && (!y || y_ld >= N1), "bottleneck_exit: row pitch below the channel count");
-  STEP_CHECK_ARG(h_ld % 8 == 0 && x_ld % 8 == 0 && z_ld % 16 == 0 && (!y || y_ld % 8 == 0), "bottleneck_exit: row pitches must keep 16-byte (z: 32-byte) alignment");
-  STEP_CHECK_ARG(((uintptr_t)h | (uintptr_t)w3 | (uintptr_t)w1 | (uintptr_t)y) % 16 == 0 && ((uintptr_t)x | (uintptr_t)z) % 32 == 0,
-                 "bottleneck_exit: pointers must be 16-byte (x, z: 32-byte) aligned");
+  STEP_CHECK_ARG(h_ld % 8 == 0 && x_ld % 8 == 0 && z_ld % 8 == 0 && (!y || y_ld % 8 == 0), "bottleneck_exit: row pitches must keep 16-byte alignment");
+  STEP_CHECK_ARG(((uintptr_t)h | (uintptr_t)w3 | (uintptr_t)w1 | (uintptr_t)y | (uintptr_t)x | (uintptr_t)z) % 16 == 0,
+                 "bottleneck_exit: pointers must be 16-byte aligned");
   if (!g_enc) {
     cudaDriverEntryPointQueryResult q;
     void* f = nullptr;
@@ -415,22 +216,19 @@ extern "C" int step_bottleneck_exit_f16(const void* h, long long h_ld, const voi
       return fail(STEP_E_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
     g_enc = (EncFn)f;
   }
-  CUtensorMap mh, mw3, mx, mw1, my;
+  CUtensorMap mh, mw3, mw1;
   int r;
-  if ((r = enc2d(&mh, h, K1, M, h_ld, 128, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map h (%d)", r);
-  if ((r = enc2d(&mw3, w3, K1, N1, K1, 32, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map w3 (%d)", r);
-  if ((r = enc2d(&mx, x, N1, M, x_ld, 128, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map x (%d)", r);
-  if ((r = enc2d(&mw1, w1, N1, N2, N1, 128, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map w1 (%d)", r);
-  if ((r = enc2d(&my, y ? y : x, N1, M, y ? y_ld : x_ld, 32, CU_TENSOR_MAP_L2_PROMOTION_NONE))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map y (%d)", r);
+  if ((r = enc2d(&mh, h, K1, M, h_ld, BM, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map h (%d)", r);
+  if ((r = enc2d(&mw3, w3, K1, N1, K1, CH, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map w3 (%d)", r);
+  if ((r = enc2d(&mw1, w1, N1, N2, N1, N2, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map w1 (%d)", r);
   Geom g;
-  g.M = (int)M; g.tiles = (int)((M + 255) / 256); g.store_y = y ? 1 : 0; g.relu2 = relu2 ? 1 : 0; g.z_ld = (int)z_ld; g.x_ld = (int)x_ld;
-  const size_t smem = sizeof(Bars) + 1024 + kHBytes + kRing * (kB1Bytes + kB2Bytes) + kAcc * kA2Bytes;
+  g.M = (int)M; g.store_y = y ? 1 : 0; g.relu2 = relu2 ? 1 : 0; g.x_ld = (int)x_ld; g.y_ld = (int)y_ld; g.z_ld = (int)z_ld;
+  const size_t smem = sizeof(Bars) + 1024 + kHBytes + kW3Ring * kW3Bytes + kW1Ring * kW1Bytes + 2 * kYBytes;
   static std::atomic<unsigned long long> attr_seen{0};
   if (first_use_on_device(attr_seen)) {
     cudaError_t e = cudaFuncSetAttribute(bottleneck_exit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return fail((int)e, "bottleneck_exit: smem attribute: %s", cudaGetErrorString(e));
   }
-  const int pairs = g.tiles < kNumSMs / 2 ? g.tiles : kNumSMs / 2;
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   int na = 0;
@@ -440,11 +238,11 @@ extern "C" int step_bottleneck_exit_f16(const void* h, long long h_ld, const voi
     ++na;
   }
   cfg.attrs = attr; cfg.numAttrs = na;
-  cfg.gridDim = dim3(2 * pairs);                 // cluster size 2 is a compile-time attribute of the kernel
+  cfg.gridDim = dim3((unsigned)((M + BM - 1) / BM));
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = cu(stream);
-  cudaError_t le = cudaLaunchKernelEx(&cfg, bottleneck_exit_kernel, mh, mw3, mx, mw1, my, g, shift2, (const __half*)x, (__half*)z);
+  cudaError_t le = cudaLaunchKernelEx(&cfg, bottleneck_exit_kernel, mh, mw3, mw1, g, shift2, (const __half*)x, (__half*)y, (__half*)z);
   if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "bottleneck_exit_kernel launch: %s", cudaGetErrorString(le)); }
   STEP_LAUNCH_CHECK("bottleneck_exit_kernel");
   return 0;

@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libstep_b200 (sm_100a only).
+// common.cuh -- shared host/device helpers for libstep_b200 (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -35,11 +35,9 @@ inline cudaStream_t cu(step_stream_t s) { return reinterpret_cast<cudaStream_t>(
     }                                                                               \
   } while (0)
 
-// Programmatic dependent launch of the conv kernels is OPT-IN (STEP_B200_PDL=1).  It is worth ~3 % (conv class 3.63 -> 3.55 ms
-// per step), but with three batches in flight (graphs on three streams + the pinned-host H2D copies of the end-to-end region) one
-// bench.py run in eight stalled in a stream that never drained (4 of 33 runs with it, 0 of 12 without; tools/experiments/
-// r2_fused_stress.sh).  The cause was not found -- every kernel allocates its TMEM before it triggers its dependents -- so the
-// default is the configuration that never stalled.
+// Programmatic dependent launch of the conv kernels is OPT-IN (STEP_B200_PDL=1).  History: with the earlier Blackwell (tcgen05)
+// kernels one bench.py run with three batches in flight stalled under it, cause not found.  It has not been measured or
+// stress-tested with the current wgmma kernels, so it stays off by default.
 inline bool pdl_enabled() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("STEP_B200_PDL"); v = (e && e[0] == '1') ? 1 : 0; }
@@ -48,7 +46,7 @@ inline bool pdl_enabled() {
 
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // Function attributes (dynamic shared memory limit) are per device: a process driving several GPUs (nn.DataParallel,
 // test.py:79-95 of the reference) must set them once on each.  `seen` is a per-kernel bitmask owned by the caller.

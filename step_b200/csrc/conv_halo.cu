@@ -1,71 +1,55 @@
 // conv_halo.cu -- stride-1 k>1 convolution on thin inputs (Cin <= 64 channels: the space-to-depth I3D stem,
 // models/i3dpt.py:184-190 after engine.pack_stem_s2d) with the input neighbourhood staged ONCE in shared memory.
 //
-// The im2col kernels of conv_umma.cu fetch a fresh 128-row A tile from L2 for every filter tap; with 32 input
-// channels a tap is a K=32 sliver, the tensor pipe finishes it in 64 cycles and the kernel is bound by the 12 KB
-// it pulls through TMA for each of them (~46 % of the tensor peak, profiles/r1_conv_layers.txt).  Here a CTA owns an
-// output tile of TT x 16 x 8 pixels; ONE 5-D TMA box load brings the (TT+KT-1) x (16+KH-1) x (8+KW-1) input patch
-// (zero-filled outside the tensor == the TF-"SAME" halo, i3dpt.py:14-31) into swizzled shared memory, and every tap
-// is TT tcgen05.mma whose A descriptor simply starts at the tap's pixel offset inside the patch: the 8 rows of a
-// core-matrix group are 8 consecutive w pixels, consecutive groups are consecutive h rows (SBO = patch row pitch).
-// The swizzle XOR is a function of the shared-memory address, so a shifted start stays consistent with what TMA
-// wrote (tools/probe/umma_shift_probe.cu).  Only the weights (Cout x Cin per tap) stream through a TMA ring.
+// The im2col path of conv_umma.cu fetches a fresh 128-row A tile from L2 for every filter tap; with 32 input channels a tap
+// is a K=32 sliver and the kernel is bound by the bytes it pulls through TMA for each of them.  Here a CTA owns an output
+// tile of TT x 16 x 8 pixels; BK/8 TMA box loads bring the (TT+KT-1) x (16+KH-1) x (8+KW-1) input patch (zero-filled outside
+// the tensor == the TF-"SAME" halo, i3dpt.py:14-31) into shared memory, and every tap is TT wgmma sequences whose A
+// descriptor simply starts at the tap's pixel offset inside the patch.
 //
-// Warp roles (192 threads; up to 8 output planes = all 512 TMEM columns per CTA, so one CTA per SM):
-//   warp 0 producer (patch + weight ring), warp 1 TMEM allocator + MMA issuer, warps 2..5 epilogue
-//   (tcgen05.ld -> BN scale/shift + ReLU -> fp16 -> swizzled slab in the retired patch -> 5-D bulk tensor store).
+// Patch layout: the wgmma no-swizzle K-major layout, [BK/8 channel groups][pixel (t, h, w)][8 channels = 16 bytes].  A core
+// matrix (8 rows x 16 bytes) is 8 consecutive w pixels of one channel group, so the operand of a tap starts at any pixel:
+// LBO (next 8 channels) = one channel group's bytes, SBO (next 8-row group = next h row of the tile) = the patch row pitch.
+// Only the weights (Cout x Cin per tap) stream through a TMA ring (128B / 64B / 32B swizzled like conv_umma.cu).
+//
+// Warp roles (384 threads): warp 0 producer (patch + weight ring), warpgroups 1 and 2 consume output rows h 0-7 / 8-15 of the
+// tile for all TT planes (registers: TT x BN / 2 accumulators) and store the BN scale/shift + ReLU epilogue directly.
 #include <cuda.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "umma_ptx.cuh"
 
 namespace step {
 
-constexpr int kHaloThreads = 192;
-constexpr int kHaloTH = 16, kHaloTW = 8;   // 128 output pixels = one UMMA M tile
+constexpr int kHaloThreads = 384;
+constexpr int kHaloTH = 16, kHaloTW = 8;   // 128 output pixels = two m64 warpgroups
 constexpr int kHaloMaxStages = 16;
 constexpr int kHaloSmemMax = 227 * 1024;
+constexpr int kHaloBook = 4096;            // barriers (first 512 B), scale, shift
 
 struct HaloGeom {
   int KT, KH, KW, PT, PH, PW, taps;
-  int TT;                        // output planes per CTA (accumulator sets)
   int hp_t, hp_h, hp_w;          // patch extent in pixels
+  int chunk_bytes;               // one 8-channel group of the patch, padded to 128 bytes
   int patch_bytes, b_bytes, n_stages;
-  int BN, ncols, Cout, relu;
-  int tiles_w, tiles_h, tiles_t, OT;
-  int k_steps_last_t;            // 16-channel MMA steps issued for the taps of the last t plane (structured zero weights)
-  uint32_t idesc;
+  int Cout, relu, out_ld, out_coff;
+  int tiles_w, tiles_h, tiles_t, OT, OH, OW;
 };
 
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-
-// K-major swizzled operand descriptor with an explicit 8-row group pitch (see make_smem_desc in umma_ptx.cuh)
-template <int BK>
-__device__ __forceinline__ uint64_t make_smem_desc_sbo(uint32_t saddr, uint32_t sbo_bytes) {
-  constexpr uint32_t row_bytes = BK * 2;
-  constexpr uint64_t layout = row_bytes == 128 ? 2 : (row_bytes == 64 ? 4 : 6);
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ULL << 46) | (layout << 61);
-}
-
-template <int BK, int TT>
-__global__ void __launch_bounds__(kHaloThreads, 2)
-conv_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                 const __grid_constant__ CUtensorMap map_y, HaloGeom g, const float* __restrict__ scale,
-                 const float* __restrict__ shift) {
-  constexpr int kRow = BK * 2;   // bytes of one pixel's channels
+template <int BK, int NCH, int TT>
+__global__ void __launch_bounds__(kHaloThreads, 1)
+conv_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, HaloGeom g,
+                 const float* __restrict__ scale, const float* __restrict__ shift, __half* __restrict__ y) {
+  constexpr int BN = NCH * 64;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint64_t* full_bar = (uint64_t*)smem_raw;            // [kHaloMaxStages] weight stage landed
   uint64_t* empty_bar = full_bar + kHaloMaxStages;     // [kHaloMaxStages] weight stage consumed
   uint64_t* pfull_bar = empty_bar + kHaloMaxStages;    // patch landed
-  uint64_t* tfull_bar = pfull_bar + 1;                 // all MMAs retired: accumulators ready, patch reusable
-  uint32_t* tmem_ptr_s = (uint32_t*)(tfull_bar + 1);
-  float* s_scale = (float*)(smem_raw + 512);           // [BN <= 256]
-  float* s_shift = s_scale + 256;
-  uint8_t* ring = (uint8_t*)(((uintptr_t)smem_raw + 512 + 2048 + 1023) & ~(uintptr_t)1023);
+  float* s_scale = (float*)(smem_raw + 512);           // [BN <= 128]
+  float* s_shift = s_scale + 128;
+  uint8_t* ring = (uint8_t*)(((uintptr_t)smem_raw + kHaloBook + 1023) & ~(uintptr_t)1023);
   uint8_t* patch = ring + (size_t)g.n_stages * g.b_bytes;   // 1024-aligned: b_bytes is a multiple of 1024
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -75,38 +59,30 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   const int tt = b % g.tiles_t;
   const int n = b / g.tiles_t;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_y) : "memory");
-    for (int s = 0; s < g.n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
+    for (int s = 0; s < g.n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     mbar_init(pfull_bar, 1);
-    mbar_init(tfull_bar, 1);
     fence_barrier_init();
   }
-  const uint32_t alloc_cols = (uint32_t)(TT * g.ncols);     // power of two >= 32 (host)
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_s)), "r"(alloc_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp >= 2) {
-    for (int i = threadIdx.x - 64; i < g.BN; i += kHaloThreads - 64) {
+  if (threadIdx.x < 128) {
+    for (int i = threadIdx.x; i < BN; i += 128) {
       s_scale[i] = (scale && i < g.Cout) ? scale[i] : 1.0f;
       s_shift[i] = (shift && i < g.Cout) ? shift[i] : 0.0f;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_s;
   pdl_wait();                 // the producer of x (the previous kernel in the stream) has finished
   pdl_launch_dependents();
 
   if (warp == 0) {
     // ===================== producer =====================
     if (elect_one()) {
-      mbar_expect_tx(pfull_bar, (uint32_t)g.patch_bytes);
-      tma_load_5d(&map_a, pfull_bar, patch, 0, tw * kHaloTW - g.PW, th * kHaloTH - g.PH, tt * TT - g.PT, n);
+      mbar_expect_tx(pfull_bar, (uint32_t)((BK / 8) * g.hp_t * g.hp_h * g.hp_w * 16));   // bytes TMA writes (without padding)
+      for (int c = 0; c < BK / 8; ++c)
+        tma_load_5d(&map_a, pfull_bar, patch + (size_t)c * g.chunk_bytes, c * 8, tw * kHaloTW - g.PW, th * kHaloTH - g.PH,
+                    tt * TT - g.PT, n);
       for (int tap = 0; tap < g.taps; ++tap) {
         const int s = tap % g.n_stages, use = tap / g.n_stages;
         if (use > 0) mbar_wait(&empty_bar[s], (uint32_t)(use - 1) & 1u);
@@ -114,95 +90,61 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         tma_load_3d(&map_b, &full_bar[s], ring + (size_t)s * g.b_bytes, 0, tap, 0);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // One thread issues everything.  An M128 x N64 x K16 MMA occupies the tensor pipe for only 32 cycles, so the
-    // issue loop must stay under that per instruction: descriptor high words are loop constants, the low words
-    // (shared-memory address >> 4) advance by adds, and the plane / k-step loops are fully unrolled.
-    if (elect_one()) {
-      mbar_wait(pfull_bar, 0);
-      tc_fence_after();
-      constexpr uint64_t kLayout = kRow == 128 ? 2 : (kRow == 64 ? 4 : 6);
-      const uint64_t a_hi = ((uint64_t)((uint32_t)(g.hp_w * kRow) >> 4) << 32) | (1ULL << 46) | (kLayout << 61);
-      const uint64_t b_hi = ((uint64_t)((8 * kRow) >> 4) << 32) | (1ULL << 46) | (kLayout << 61);
-      const uint32_t patch_lo = (smem_u32(patch) & 0x3FFFF) >> 4, ring_lo = (smem_u32(ring) & 0x3FFFF) >> 4;
-      const uint32_t row16 = kRow >> 4, plane16 = (uint32_t)(g.hp_h * g.hp_w) * row16, b16 = (uint32_t)g.b_bytes >> 4;
-      const uint32_t ncols = (uint32_t)g.ncols, idesc = g.idesc;
-      int kw = 0, kh = 0, kt = 0, s = 0;
-      uint32_t par = 0;
-      for (int tap = 0; tap < g.taps; ++tap) {
-        mbar_wait(&full_bar[s], par);
-        tc_fence_after();
-        uint32_t a_lo = patch_lo + (uint32_t)((kt * g.hp_h + kh) * g.hp_w + kw) * row16;
-        const uint32_t b_lo = ring_lo + (uint32_t)s * b16;
-        const uint32_t acc0 = tap ? 1u : 0u;
-        uint32_t d = tmem_base;
-        const int nk = (kt == g.KT - 1) ? g.k_steps_last_t : BK / 16;   // zero-weight channel tail of the last t plane: no MMA
+  } else if (warp >= 4) {
+    // ===================== consumers =====================
+    const int wg = (warp >> 2) - 1;                      // output rows h = 8 wg .. 8 wg + 7 of the tile
+    const int ct = threadIdx.x - 128;
+    const uint64_t a_hi = ((uint64_t)((uint32_t)g.chunk_bytes >> 4) << 16) | ((uint64_t)((uint32_t)(g.hp_w * 16) >> 4) << 32);
+    const uint64_t b_hi = desc_hi_kmajor<BK>();
+    const uint64_t patch_lo = desc_lo(patch), ring_lo = desc_lo(ring);
+    const uint32_t chunk16 = (uint32_t)g.chunk_bytes >> 4, plane16 = (uint32_t)(g.hp_h * g.hp_w), b16 = (uint32_t)g.b_bytes >> 4;
+    float acc[TT * NCH * 32];                            // plane j: acc[j * NCH * 32 ...]; zeroed by the first tap
+    mbar_wait(pfull_bar, 0);
+    int kw = 0, kh = 0, kt = 0, s = 0, prev = -1;
+    uint32_t par = 0;
+    for (int tap = 0; tap < g.taps; ++tap) {
+      mbar_wait(&full_bar[s], par);
+      // one 16-byte pixel row of the patch == 1 in descriptor units
+      const uint64_t a_lo = patch_lo + (uint64_t)((kt * g.hp_h + kh + 8 * wg) * g.hp_w + kw);
+      const uint64_t b_lo = ring_lo + (uint64_t)s * b16;
+      wg_fence();
 #pragma unroll
-        for (int j = 0; j < TT; ++j) {
+      for (int j = 0; j < TT; ++j)
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            if (k < nk)
-              umma_f16(d, a_hi | (uint64_t)(a_lo + 2 * k), b_hi | (uint64_t)(b_lo + 2 * k), idesc, k ? 1u : acc0);
-          a_lo += plane16;
-          d += ncols;
-        }
-        umma_commit(&empty_bar[s]);
-        if (++kw == g.KW) { kw = 0; if (++kh == g.KH) { kh = 0; ++kt; } }
-        if (++s == g.n_stages) { s = 0; par ^= 1u; }
-      }
-      umma_commit(tfull_bar);
+        for (int k = 0; k < BK / 16; ++k)
+#pragma unroll
+          for (int c = 0; c < NCH; ++c)
+            wgmma_64x64(acc + (j * NCH + c) * 32, a_hi | (a_lo + (uint64_t)(j * plane16 + 2 * k * chunk16)),
+                        b_hi | (b_lo + (uint64_t)(c * ((64 * BK * 2) >> 4)) + 2 * k), (tap | k) ? 1u : 0u);
+      wg_commit();
+      wg_wait<1>();
+      if (prev >= 0 && ct % 128 == 0) mbar_arrive(&empty_bar[prev]);
+      prev = s;
+      if (++kw == g.KW) { kw = 0; if (++kh == g.KH) { kh = 0; ++kt; } }
+      if (++s == g.n_stages) { s = 0; par ^= 1u; }
     }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int lane_grp = warp & 3;                       // TMEM lane quarter == output rows 4*lane_grp .. +3 of the tile
-    mbar_wait(tfull_bar, 0);
-    tc_fence_after();
-    // every MMA has retired: the patch is dead, its first bytes become this warp's staging slabs
-    const int passes = g.BN >> 5;                        // 32-column passes per plane (host: BN % 32 == 0)
-    uint8_t* slab0 = patch + (size_t)lane_grp * TT * passes * 2048;
+    wg_wait<0>();
+    // epilogue: thread rows h = 8 wg + 2 (warp % 4) + i, w = lane / 4; columns 8 j + 2 (lane % 4) + {0, 1}
+    const int ow = tw * kHaloTW + (lane >> 2);
+#pragma unroll
     for (int j = 0; j < TT; ++j) {
       const int ot = tt * TT + j;
-      for (int pz = 0; pz < passes; ++pz) {
-        uint8_t* sl = slab0 + (size_t)(j * passes + pz) * 2048;
-        const int cb = pz * 32;
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(j * g.ncols + cb), v);
-        tmem_ld_wait();
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 a0 = *reinterpret_cast<const float4*>(s_scale + cb + q * 8);
-          const float4 a1 = *reinterpret_cast<const float4*>(s_scale + cb + q * 8 + 4);
-          const float4 b0 = *reinterpret_cast<const float4*>(s_shift + cb + q * 8);
-          const float4 b1 = *reinterpret_cast<const float4*>(s_shift + cb + q * 8 + 4);
-          float f[8];
-          f[0] = fmaf(__uint_as_float(v[q * 8 + 0]), a0.x, b0.x); f[1] = fmaf(__uint_as_float(v[q * 8 + 1]), a0.y, b0.y);
-          f[2] = fmaf(__uint_as_float(v[q * 8 + 2]), a0.z, b0.z); f[3] = fmaf(__uint_as_float(v[q * 8 + 3]), a0.w, b0.w);
-          f[4] = fmaf(__uint_as_float(v[q * 8 + 4]), a1.x, b1.x); f[5] = fmaf(__uint_as_float(v[q * 8 + 5]), a1.y, b1.y);
-          f[6] = fmaf(__uint_as_float(v[q * 8 + 6]), a1.z, b1.z); f[7] = fmaf(__uint_as_float(v[q * 8 + 7]), a1.w, b1.w);
-          if (g.relu) {
+      for (int i = 0; i < 2; ++i) {
+        const int oh = th * kHaloTH + 8 * wg + 2 * (warp & 3) + i;
+        if (ot >= g.OT || oh >= g.OH || ow >= g.OW) continue;
+        __half* dst = y + ((((size_t)n * g.OT + ot) * g.OH + oh) * g.OW + ow) * g.out_ld + g.out_coff;
 #pragma unroll
-            for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], 0.0f);
-          }
-          // slab row = lane (pixel (h = lane >> 3, w = lane & 7) of this quarter), 64-byte rows, 64B swizzle
-          store16(reinterpret_cast<__half*>(sl + lane * 64 + ((q ^ ((lane >> 1) & 3)) << 4)), f);
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0 && cb < g.Cout && ot < g.OT) {
-          tma_store_5d(&map_y, sl, cb, tw * kHaloTW, th * kHaloTH + lane_grp * 4, ot, n);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        for (int q = 0; q < NCH * 8; ++q) {
+          const int col = 8 * q + 2 * (lane & 3);
+          if (col >= g.Cout) continue;
+          float f0 = fmaf(acc[j * NCH * 32 + 4 * q + 2 * i], s_scale[col], s_shift[col]);
+          float f1 = fmaf(acc[j * NCH * 32 + 4 * q + 2 * i + 1], s_scale[col + 1], s_shift[col + 1]);
+          if (g.relu) { f0 = fmaxf(f0, 0.0f); f1 = fmaxf(f1, 0.0f); }
+          *reinterpret_cast<__half2*>(dst + col) = __floats2half2_rn(f0, f1);
         }
       }
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(alloc_cols) : "memory");
   }
 }
 
@@ -220,12 +162,12 @@ bool conv3d_halo_supported(const step_conv_params* p) {
          p->OT == p->T && p->OH == p->H && p->OW == p->W;
 }
 
-template <int BK, int TT>
-static int launch_halo_tt(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& my, const HaloGeom& g, size_t smem,
-                       unsigned grid, const step_conv_params* p, cudaStream_t s) {
+template <int BK, int NCH, int TT>
+static int launch_halo_tt(const CUtensorMap& ma, const CUtensorMap& mb, const HaloGeom& g, size_t smem, unsigned grid,
+                          const step_conv_params* p, const float* scale, const float* shift, __half* y, cudaStream_t s) {
   static std::atomic<unsigned long long> attr_seen{0};
   if (first_use_on_device(attr_seen)) {
-    cudaError_t e = cudaFuncSetAttribute(conv_halo_kernel<BK, TT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHaloSmemMax);
+    cudaError_t e = cudaFuncSetAttribute(conv_halo_kernel<BK, NCH, TT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHaloSmemMax);
     if (e != cudaSuccess) return fail((int)e, "conv_halo_kernel attribute: %s", cudaGetErrorString(e));
   }
   cudaLaunchConfig_t cfg = {};
@@ -236,21 +178,93 @@ static int launch_halo_tt(const CUtensorMap& ma, const CUtensorMap& mb, const CU
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
   }
-  cudaError_t le = cudaLaunchKernelEx(&cfg, conv_halo_kernel<BK, TT>, ma, mb, my, g, p->scale, p->shift);
+  cudaError_t le = cudaLaunchKernelEx(&cfg, conv_halo_kernel<BK, NCH, TT>, ma, mb, g, scale, shift, y);
   if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "conv_halo_kernel launch: %s", cudaGetErrorString(le)); }
   STEP_LAUNCH_CHECK("conv_halo_kernel");
   return 0;
 }
 
 template <int BK>
-static int launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& my, const HaloGeom& g, size_t smem,
+static int launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const HaloGeom& g, int nch, int TT, size_t smem,
                        unsigned grid, const step_conv_params* p, cudaStream_t s) {
-  switch (g.TT) {
-    case 8: return launch_halo_tt<BK, 8>(ma, mb, my, g, smem, grid, p, s);
-    case 4: return launch_halo_tt<BK, 4>(ma, mb, my, g, smem, grid, p, s);
-    case 2: return launch_halo_tt<BK, 2>(ma, mb, my, g, smem, grid, p, s);
-    default: return launch_halo_tt<BK, 1>(ma, mb, my, g, smem, grid, p, s);
+  const float* sc = p->scale;
+  const float* sh = p->shift;
+  __half* y = (__half*)p->y;
+  if (nch == 1) {
+    if (TT == 4) return launch_halo_tt<BK, 1, 4>(ma, mb, g, smem, grid, p, sc, sh, y, s);
+    if (TT == 2) return launch_halo_tt<BK, 1, 2>(ma, mb, g, smem, grid, p, sc, sh, y, s);
+    return launch_halo_tt<BK, 1, 1>(ma, mb, g, smem, grid, p, sc, sh, y, s);
   }
+  if (TT == 2) return launch_halo_tt<BK, 2, 2>(ma, mb, g, smem, grid, p, sc, sh, y, s);
+  return launch_halo_tt<BK, 2, 1>(ma, mb, g, smem, grid, p, sc, sh, y, s);
+}
+
+// one column tile of <= 128 output channels (weights and scale / shift offset by the tile's first channel)
+static int halo_launch_cols(const step_conv_params* p, int c0, int cout, step_stream_t stream) {
+  const int BK = p->Cin, row = BK * 2;
+  HaloGeom g;
+  memset(&g, 0, sizeof(g));
+  g.KT = p->KT; g.KH = p->KH; g.KW = p->KW; g.PT = p->PT; g.PH = p->PH; g.PW = p->PW; g.taps = p->KT * p->KH * p->KW;
+  g.Cout = cout; g.relu = p->relu; g.OT = p->OT; g.OH = p->OH; g.OW = p->OW;
+  g.out_ld = p->out_ld; g.out_coff = p->out_coff + c0;
+  const int nch = cout <= 64 ? 1 : 2;
+  const int BN = nch * 64;
+  // Output planes per CTA (accumulator sets in registers, TT * BN <= 256).  Every tap's weight tile is fetched once per CTA,
+  // so more planes mean less weight traffic per pixel; the patch for TT planes plus >= 2 weight stages must fit 227 KB.
+  int best_tt = 1;
+  for (int tt = 256 / BN > 4 ? 4 : 256 / BN; tt > 1; tt >>= 1) {
+    const long patch = (long)(tt + g.KT - 1) * (kHaloTH + g.KH - 1) * (kHaloTW + g.KW - 1) * row;
+    if (kHaloBook + 1024 + patch + 2L * BN * row > kHaloSmemMax) continue;
+    // prefer the larger tile unless more than a quarter of the computed planes would fall past the end
+    const int groups = (p->OT + tt - 1) / tt;
+    if ((groups * tt - p->OT) * 4 > groups * tt) continue;
+    best_tt = tt;
+    break;
+  }
+  const int TT = best_tt;
+  g.hp_t = TT + g.KT - 1; g.hp_h = kHaloTH + g.KH - 1; g.hp_w = kHaloTW + g.KW - 1;
+  g.chunk_bytes = (g.hp_t * g.hp_h * g.hp_w * 16 + 127) / 128 * 128;   // TMA destinations are 128-byte aligned
+  g.patch_bytes = (BK / 8) * g.chunk_bytes;
+  g.b_bytes = BN * row;
+  long n_st = ((long)kHaloSmemMax - kHaloBook - 1024 - g.patch_bytes) / g.b_bytes;
+  STEP_CHECK_ARG(n_st >= 2, "conv3d(halo): patch of %d bytes leaves no room for the weight ring", g.patch_bytes);
+  if (n_st > kHaloMaxStages) n_st = kHaloMaxStages;
+  if (n_st > g.taps) n_st = g.taps;
+  g.n_stages = (int)n_st;
+  g.tiles_w = (p->OW + kHaloTW - 1) / kHaloTW; g.tiles_h = (p->OH + kHaloTH - 1) / kHaloTH; g.tiles_t = (p->OT + TT - 1) / TT;
+  const long long ctas = (long long)p->N * g.tiles_t * g.tiles_h * g.tiles_w;
+  STEP_CHECK_ARG(ctas < (1LL << 31), "conv3d(halo): grid too large");
+  const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
+  CUtensorMap ma, mb;
+  {
+    cuuint64_t dims[5] = {(cuuint64_t)p->Cin, (cuuint64_t)p->W, (cuuint64_t)p->H, (cuuint64_t)p->T, (cuuint64_t)p->N};
+    cuuint64_t strides[4] = {(cuuint64_t)p->in_ld * 2, (cuuint64_t)p->W * p->in_ld * 2, (cuuint64_t)p->H * p->W * p->in_ld * 2,
+                             (cuuint64_t)p->T * p->H * p->W * p->in_ld * 2};
+    cuuint32_t box[5] = {8, (cuuint32_t)g.hp_w, (cuuint32_t)g.hp_h, (cuuint32_t)g.hp_t, 1};
+    CUresult cr = g_halo_encode(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, (void*)p->x, dims, strides, box, ones,
+                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(halo): tensor map (patch) encode failed: CUresult %d", (int)cr);
+  }
+  {
+    cuuint64_t dims[3] = {(cuuint64_t)p->Cin, (cuuint64_t)g.taps, (cuuint64_t)cout};
+    cuuint64_t strides[2] = {(cuuint64_t)p->w_ld * 2, (cuuint64_t)g.taps * p->w_ld * 2};
+    cuuint32_t box[3] = {(cuuint32_t)BK, 1, (cuuint32_t)BN};
+    const __half* w = (const __half*)p->w + (size_t)c0 * g.taps * p->w_ld;
+    CUresult cr = g_halo_encode(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)w, dims, strides, box, ones,
+                                CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B),
+                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(halo): tensor map (weights) encode failed: CUresult %d", (int)cr);
+  }
+  const size_t smem = kHaloBook + 1024 + (size_t)g.n_stages * g.b_bytes + (size_t)g.patch_bytes;
+  STEP_CHECK_ARG(smem <= (size_t)kHaloSmemMax, "conv3d(halo): %zu bytes of shared memory", smem);
+  step_conv_params q = *p;
+  q.scale = p->scale ? p->scale + c0 : nullptr;
+  q.shift = p->shift ? p->shift + c0 : nullptr;
+  if (BK == 64) return launch_halo<64>(ma, mb, g, nch, TT, smem, (unsigned)ctas, &q, cu(stream));
+  if (BK == 32) return launch_halo<32>(ma, mb, g, nch, TT, smem, (unsigned)ctas, &q, cu(stream));
+  return launch_halo<16>(ma, mb, g, nch, TT, smem, (unsigned)ctas, &q, cu(stream));
 }
 
 int conv3d_halo_launch(const step_conv_params* p, step_stream_t stream) {
@@ -264,98 +278,12 @@ int conv3d_halo_launch(const step_conv_params* p, step_stream_t stream) {
       return fail(STEP_E_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
     g_halo_encode = (HaloEncodeTiledFn)f;
   }
-  const int BK = p->Cin, row = BK * 2;
-  HaloGeom g;
-  memset(&g, 0, sizeof(g));
-  g.KT = p->KT; g.KH = p->KH; g.KW = p->KW; g.PT = p->PT; g.PH = p->PH; g.PW = p->PW; g.taps = p->KT * p->KH * p->KW;
-  g.Cout = p->Cout; g.relu = p->relu; g.OT = p->OT;
-  g.BN = (p->Cout + 31) / 32 * 32;
-  g.ncols = 32;
-  while (g.ncols < g.BN) g.ncols <<= 1;
-  // Output planes per CTA (= accumulator sets in TMEM).  Every tap's weight tile is fetched once per CTA, so more
-  // planes mean less weight traffic per pixel and a weight ring that covers the L2 latency with fewer bytes in
-  // flight; the patch for TT planes plus >= 4 weight stages must fit the 227 KB of one SM.
-  bool two_ctas = false;
-  int tt_env = 0;
-  if (const char* e = getenv("STEP_B200_HALO_TT")) tt_env = atoi(e);
-  int best_tt = 0;
-  // Measured on the stem (tools/conv_bench.py stem_s2d, CB_AMODE=4): two co-resident CTAs of 4 planes (376 us) beat
-  // one CTA of 8 planes (505 us) -- one CTA's patch load and epilogue hide behind the other's MMAs.  So first look
-  // for the deepest tile of which TWO fit an SM (half the shared memory, half the TMEM columns, >= 4 weight stages).
-  for (int pass = 0; pass < 2 && !best_tt; ++pass) {
-    const long smem_cap = pass == 0 ? (long)kHaloSmemMax / 2 - 1024 : (long)kHaloSmemMax;
-    const int col_cap = pass == 0 ? 256 : 512;
-    for (int tt = 8; tt >= 1; tt >>= 1) {
-      if (tt * g.ncols > col_cap) continue;
-      if (tt_env > 0 && tt != tt_env && !(tt == 1)) continue;
-      const long patch = (long)(tt + g.KT - 1) * (kHaloTH + g.KH - 1) * (kHaloTW + g.KW - 1) * row;
-      const long stage = 4L * tt * (g.BN / 32) * 2048;
-      const long room = smem_cap - 512 - 3072 - ((patch > stage ? patch : stage) + 1023) / 1024 * 1024;
-      if (room < (g.taps < 4 ? g.taps : 4) * (long)g.BN * row) continue;
-      // prefer the larger tile unless more than a quarter of the computed planes would fall past the end
-      const int groups = (p->OT + tt - 1) / tt;
-      if (tt > 1 && (groups * tt - p->OT) * 4 > groups * tt) continue;
-      best_tt = tt;
-      two_ctas = pass == 0;
-      break;
-    }
+  // more than 128 output channels: launches of 128-column tiles (registers hold at most 64 accumulators per thread)
+  for (int c0 = 0; c0 < p->Cout; c0 += 128) {
+    const int cout = p->Cout - c0 < 128 ? p->Cout - c0 : 128;
+    if (int rc = halo_launch_cols(p, c0, cout, stream)) return rc;
   }
-  g.TT = best_tt > 0 ? best_tt : 1;
-  g.hp_t = g.TT + g.KT - 1; g.hp_h = kHaloTH + g.KH - 1; g.hp_w = kHaloTW + g.KW - 1;
-  g.patch_bytes = g.hp_t * g.hp_h * g.hp_w * row;
-  g.b_bytes = g.BN * row;
-  const long staging = 4L * g.TT * (g.BN / 32) * 2048;
-  const long patch_area = ((g.patch_bytes > staging ? g.patch_bytes : staging) + 1023) / 1024 * 1024;
-  g.n_stages = (int)(((two_ctas ? (long)kHaloSmemMax / 2 - 1024 : (long)kHaloSmemMax) - 512 - 3072 - patch_area) / g.b_bytes);
-  STEP_CHECK_ARG(g.n_stages >= 2, "conv3d(halo): patch of %d bytes leaves no room for the weight ring", g.patch_bytes);
-  if (g.n_stages > kHaloMaxStages) g.n_stages = kHaloMaxStages;
-  if (const char* e = getenv("STEP_B200_HALO_STAGES")) { int v = atoi(e); if (v >= 2 && v < g.n_stages) g.n_stages = v; }
-  if (g.n_stages > g.taps) g.n_stages = g.taps;
-  STEP_CHECK_ARG(g.hp_t <= 256 && g.hp_h <= 256 && g.hp_w <= 256, "conv3d(halo): patch too large");
-  g.tiles_w = (p->OW + kHaloTW - 1) / kHaloTW; g.tiles_h = (p->OH + kHaloTH - 1) / kHaloTH; g.tiles_t = (p->OT + g.TT - 1) / g.TT;
-  const long long ctas = (long long)p->N * g.tiles_t * g.tiles_h * g.tiles_w;
-  STEP_CHECK_ARG(ctas < (1LL << 31), "conv3d(halo): grid too large");
-  g.idesc = (1u << 4) | ((uint32_t)(g.BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  g.k_steps_last_t = BK / 16;
-  if (p->zero_cin_last_kt > 0 && p->zero_cin_last_kt < p->Cin && !(getenv("STEP_B200_HALO_ZSKIP") && getenv("STEP_B200_HALO_ZSKIP")[0] == '0')) {
-    const int steps = (p->zero_cin_last_kt + 15) / 16;       // steps that still touch a non-zero weight
-    if (steps >= 1 && steps < BK / 16) g.k_steps_last_t = steps;
-  }
-  const CUtensorMapSwizzle sw = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
-  CUtensorMap ma, mb, my;
-  {
-    cuuint64_t dims[5] = {(cuuint64_t)p->Cin, (cuuint64_t)p->W, (cuuint64_t)p->H, (cuuint64_t)p->T, (cuuint64_t)p->N};
-    cuuint64_t strides[4] = {(cuuint64_t)p->in_ld * 2, (cuuint64_t)p->W * p->in_ld * 2, (cuuint64_t)p->H * p->W * p->in_ld * 2,
-                             (cuuint64_t)p->T * p->H * p->W * p->in_ld * 2};
-    cuuint32_t box[5] = {(cuuint32_t)BK, (cuuint32_t)g.hp_w, (cuuint32_t)g.hp_h, (cuuint32_t)g.hp_t, 1};
-    CUresult cr = g_halo_encode(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, (void*)p->x, dims, strides, box, ones,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(halo): tensor map (patch) encode failed: CUresult %d", (int)cr);
-  }
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)p->Cin, (cuuint64_t)g.taps, (cuuint64_t)p->Cout};
-    cuuint64_t strides[2] = {(cuuint64_t)p->w_ld * 2, (cuuint64_t)g.taps * p->w_ld * 2};
-    cuuint32_t box[3] = {(cuuint32_t)BK, 1, (cuuint32_t)g.BN};
-    CUresult cr = g_halo_encode(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)p->w, dims, strides, box, ones,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(halo): tensor map (weights) encode failed: CUresult %d", (int)cr);
-  }
-  {
-    cuuint64_t dims[5] = {(cuuint64_t)p->Cout, (cuuint64_t)p->OW, (cuuint64_t)p->OH, (cuuint64_t)p->OT, (cuuint64_t)p->N};
-    cuuint64_t strides[4] = {(cuuint64_t)p->out_ld * 2, (cuuint64_t)p->OW * p->out_ld * 2, (cuuint64_t)p->OH * p->OW * p->out_ld * 2,
-                             (cuuint64_t)p->OT * p->OH * p->OW * p->out_ld * 2};
-    cuuint32_t box[5] = {32, (cuuint32_t)kHaloTW, 4, 1, 1};
-    CUresult cr = g_halo_encode(&my, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, (void*)((__half*)p->y + p->out_coff), dims, strides, box, ones,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(halo): tensor map (output) encode failed: CUresult %d", (int)cr);
-  }
-  const size_t smem = 512 + 2048 + 1024 + (size_t)g.n_stages * g.b_bytes + (size_t)patch_area;
-  STEP_CHECK_ARG(smem <= (size_t)kHaloSmemMax, "conv3d(halo): %zu bytes of shared memory", smem);
-  if (BK == 64) return launch_halo<64>(ma, mb, my, g, smem, (unsigned)ctas, p, cu(stream));
-  if (BK == 32) return launch_halo<32>(ma, mb, my, g, smem, (unsigned)ctas, p, cu(stream));
-  return launch_halo<16>(ma, mb, my, g, smem, (unsigned)ctas, p, cu(stream));
+  return 0;
 }
 
 }  // namespace step

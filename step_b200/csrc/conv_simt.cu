@@ -1,7 +1,7 @@
 // conv_simt.cu -- channels-last 3-D convolution on CUDA cores (fp32 accumulate), the precision
 // reference path: cfg.fp16 == False runs it in fp32 storage (parity with the reference's fp32
 // Conv3d/Conv2d/BatchNorm3d, models/i3dpt.py:103-111, two_branch.py:60-111); the same kernel with
-// __half storage cross-checks the tcgen05 kernel (conv_umma.cu) on identical inputs.
+// __half storage cross-checks the tensor-core kernel (conv_umma.cu) on identical inputs.
 //
 // Implicit GEMM, CTA tile 64 pixels x 64 output channels, K step 16 input channels per filter tap,
 // 4x4 register micro-tile per thread, zero-fill for the TF-"SAME" halo (i3dpt.py:14-31).

@@ -1,7 +1,7 @@
-// conv_umma.cu -- channels-last 3-D / 2-D convolution as an implicit GEMM on the 5th-generation
-// tensor cores of sm_100a: TMA-staged operand tiles, tcgen05.mma with the accumulator in TMEM,
-// fused BatchNorm-scale/shift (+bias) + residual + ReLU epilogue that writes a channel slice of a
-// wider buffer (the Inception concat, models/i3dpt.py:157-163, never materialises).
+// conv_umma.cu -- channels-last 3-D / 2-D convolution as an implicit GEMM on the Hopper tensor cores (sm_90a):
+// TMA-staged operand tiles, wgmma with the fp32 accumulator in registers, fused BatchNorm-scale/shift (+bias) + residual
+// + ReLU epilogue that writes a channel slice of a wider buffer (the Inception concat, models/i3dpt.py:157-163, never
+// materialises) or scatters column ranges to up to three destinations (horizontally fused 1x1x1 layers).
 //
 // Replaces, for the fp16 path, every Conv3d/BatchNorm3d/ReLU triple of models/i3dpt.py:103-111 and
 // the Conv2d/ReLU/residual chains of models/two_branch.py:60-111,236,258.
@@ -15,13 +15,13 @@
 //       IM2COL  k>1: TMA im2col mode walks 128 consecutive output pixels (w->h->t->n) inside the
 //               padded bounding box; dense M tiles on any map size.
 //   B (weights, [Cout, taps, Cin] fp16, K-major rows = output channels): 3-D map, box (BK,1,BN).
-//   D: fp32 in TMEM, 128 lanes x BN columns.
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2..5 = epilogue (tcgen05.ld -> scale/shift/residual/relu -> fp16 -> global).
-// Pipeline: kStages smem stages, full/empty mbarriers; 2 CTAs per SM overlap one CTA's epilogue with
-// the other's main loop.
+//   D: fp32 in registers; consumer warpgroup w owns rows [64 w, 64 w + 64) x BN columns (BN = 64 | 128: 32 | 64 registers).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread of warp 0) and the epilogue constants,
+// warpgroups 1, 2 = wgmma consumers + epilogue.  Pipeline: n_stages smem stages with full / empty mbarriers; the
+// stage area is reused as the fp16 output staging tile once both consumers are done with it.
 #include <cuda.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "umma_ptx.cuh"
@@ -30,25 +30,19 @@ namespace step {
 
 enum { A_LINEAR = 1, A_BOX = 2, A_IM2COL = 3 };
 
-constexpr int kBM = 128;       // UMMA M (cta_group::1)
-constexpr int kMaxBN = 256;    // <= 256 TMEM columns per CTA so two CTAs (2 x 256 = all 512 columns) share an SM
-constexpr int kMaxBNRes = 128; // residual rows are prefetched into registers: keep that to 16 x uint4
-constexpr int kStages = 6;     // barrier slots; the plan uses 2-3 stages when two CTAs share an SM, up to 6 when a CTA is alone
-constexpr int kThreads = 192;
-constexpr int kBookBytes = (2 * kStages + 1) * 8 + 8 + 2 * kMaxBN * 4;  // barriers, tmem ptr, scale, shift
+constexpr int kBM = 128;       // two m64 warpgroups
+constexpr int kMaxBN = 128;    // 64 fp32 accumulator registers per consumer thread
+constexpr int kStages = 8;     // barrier slots
+constexpr int kThreads = 384;
+constexpr int kConsumers = 256;
+constexpr int kBookBytes = 2 * kStages * 8 + 2 * kMaxBN * 4;  // barriers, scale, shift
 
 struct ConvGeom {
   int mode;
   int taps, KT, KH, KW, PT, PH, PW;
-  int kblocks_per_tap;          // ceil(Cin / BK)
-  int k_tail_steps;             // 16-channel MMA steps of a tap's last channel block that hold real channels
-  int BN, n_tiles;              // N tile (multiple of 16) and count
-  int n_stages;                 // smem pipeline depth used by the one-tile-per-CTA kernel
-  int n_stages_p, mh, tmem_bufs;  // persistent kernel: pipeline depth, 128-row halves per tile, accumulator sets
-  int res_tma, res_bufs;          // residual tile fetched by TMA into shared memory (LINEAR mode, BN % 64 == 0); 1 | 2 buffers
-  int cluster;                    // 1, or 2: CTA pairs sharing the weight tile by TMA multicast
-  int tma_store, st_w;            // epilogue writes 32-row slabs with bulk tensor stores (linear M); box width 16 | 32 columns
-  int col_split;                  // mh == 1: columns [0, col_split) -> epilogue warps 2..5, the rest -> warps 6..9
+  int kblocks_per_tap;          // ceil(Cin / BK); the channel tail of a tap's last block is TMA zero fill in A and B
+  int BN, n_tiles;              // N tile (64 | 128) and count
+  int n_stages;                 // smem pipeline depth
   int n_splits, split[2], ld_extra[2], coff_extra[2];  // fused 1x1x1 layers: extra destinations by column range
   __half* y_extra[2];
   int Cout, out_ld, out_coff, res_ld, res_coff, relu;
@@ -56,76 +50,78 @@ struct ConvGeom {
   long long M;                  // Nimg*OT*OH*OW
   int bw, bh, bt, tiles_w, tiles_h, tiles_t;  // BOX mode
   int a_bytes;                  // bytes TMA writes for A per stage
-  uint32_t idesc;
 };
 
+// output pixel of row `row` of M tile `m_tile`, or -1 (past the end / box overhang)
+__device__ __forceinline__ long long tile_row_pixel(const ConvGeom& g, int m_tile, int row) {
+  if (g.mode == A_BOX) {
+    int r = m_tile;
+    const int bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
+    const int bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
+    const int bt0 = (r % g.tiles_t) * g.bt; const int bn = r / g.tiles_t;
+    const int dw = row % g.bw, rr = row / g.bw;
+    const int dh = rr % g.bh, dt = rr / g.bh;
+    const int ow = bw0 + dw, oh = bh0 + dh, ot = bt0 + dt;
+    if (dt < g.bt && ow < g.OW && oh < g.OH && ot < g.OT) return (((long long)bn * g.OT + ot) * g.OH + oh) * g.OW + ow;
+    return -1;
+  }
+  const long long m = (long long)m_tile * kBM + row;
+  return m < g.M ? m : -1;
+}
+
 // ---- the kernel -----------------------------------------------------------------------------
-template <int BK, bool kHasRes>
-__global__ void __launch_bounds__(kThreads, 2)
+template <int BK, int NCH>
+__global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, ConvGeom g,
                  const float* __restrict__ scale, const float* __restrict__ shift, const __half* __restrict__ residual,
                  __half* __restrict__ y) {
+  constexpr int BN = NCH * 64;
   constexpr int kABytes = kBM * BK * 2;
+  constexpr int kBBytes = BN * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [barriers | tmem ptr | scale | shift] (kBookBytes) then the 1024-aligned stage area
-  // [A stages][B stages], re-used by the epilogue as the fp16 output staging tile.
+  // carve: [barriers | scale | shift] (kBookBytes) then the 1024-aligned stage area [A stages][B stages], re-used by the
+  // epilogue as the fp16 output staging tile.
   uint64_t* full_bar = (uint64_t*)smem_raw;
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full_bar = empty_bar + kStages;
-  uint32_t* tmem_ptr_s = (uint32_t*)(tmem_full_bar + 1);
-  float* s_scale = (float*)(tmem_ptr_s + 2);
+  float* s_scale = (float*)(empty_bar + kStages);
   float* s_shift = s_scale + kMaxBN;
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + kBookBytes + 1023) & ~(uintptr_t)1023);
-  const int b_bytes = g.BN * BK * 2;
   uint8_t* sA = smem;
   uint8_t* sB = smem + g.n_stages * kABytes;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tile = blockIdx.x / g.n_tiles, n_tile = blockIdx.x - m_tile * g.n_tiles;
-  const int n0 = n_tile * g.BN;
+  const int n0 = n_tile * BN;
   const int num_kb = g.taps * g.kblocks_per_tap;
 
-  // tile origin
-  long long m0 = (long long)m_tile * kBM;
-  int bn = 0, bt0 = 0, bh0 = 0, bw0 = 0;  // BOX origin
-  if (g.mode == A_BOX) {
-    int r = m_tile;
-    bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
-    bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
-    bt0 = (r % g.tiles_t) * g.bt; bn = r / g.tiles_t;
-  }
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(tmem_full_bar, 1);
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
-  // TMEM columns: power of two >= 32 covering BN
-  uint32_t ncols = 32;
-  while (ncols < (uint32_t)g.BN) ncols <<= 1;
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_s)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp >= 2) {  // stage the per-channel epilogue constants
-    for (int i = threadIdx.x - 64; i < g.BN; i += 128) {
-      int c = n0 + i;
+  if (threadIdx.x < 128) {  // stage the per-channel epilogue constants
+    for (int i = threadIdx.x; i < BN; i += 128) {
+      const int c = n0 + i;
       s_scale[i] = (scale && c < g.Cout) ? scale[c] : 1.0f;
       s_shift[i] = (shift && c < g.Cout) ? shift[c] : 0.0f;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_s;
   pdl_wait();                 // the producer of x (the previous kernel in the stream) has finished
   pdl_launch_dependents();
 
   if (warp == 0) {
     // ===================== TMA producer =====================
     if (elect_one()) {
+      long long m0 = (long long)m_tile * kBM;
+      int bn = 0, bt0 = 0, bh0 = 0, bw0 = 0;  // BOX origin
+      if (g.mode == A_BOX) {
+        int r = m_tile;
+        bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
+        bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
+        bt0 = (r % g.tiles_t) * g.bt; bn = r / g.tiles_t;
+      }
       // IM2COL start coordinates: output pixel m0 -> (w,h,t,n) + lower corner (= -pad)
       int iw = 0, ih = 0, it = 0, in_ = 0;
       if (g.mode == A_IM2COL) {
@@ -135,16 +131,15 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         it = (int)(r % g.OT); in_ = (int)(r / g.OT);
         iw -= g.PW; ih -= g.PH; it -= g.PT;
       }
-      const uint32_t tx_bytes = (uint32_t)(g.a_bytes + b_bytes);
+      const uint32_t tx_bytes = (uint32_t)(g.a_bytes + kBBytes);
       int stage = 0; uint32_t phase = 0;
       int kw = 0, kh = 0, kt = 0;                  // filter tap, advanced incrementally (no divisions in the loop)
-      uint8_t* a_dst = sA;
-      uint8_t* b_dst = sB;
       for (int tap = 0; tap < g.taps; ++tap) {
         for (int kc = 0; kc < g.kblocks_per_tap; ++kc) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_expect_tx(&full_bar[stage], tx_bytes);
           const int c0 = kc * BK;
+          uint8_t* a_dst = sA + stage * kABytes;
           if (g.mode == A_LINEAR) {
             tma_load_2d(&map_a, &full_bar[stage], a_dst, c0, (int)m0);
           } else if (g.mode == A_BOX) {
@@ -152,664 +147,81 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           } else {
             tma_load_im2col_5d(&map_a, &full_bar[stage], a_dst, c0, iw, ih, it, in_, (uint16_t)kw, (uint16_t)kh, (uint16_t)kt);
           }
-          tma_load_3d(&map_b, &full_bar[stage], b_dst, c0, tap, n0);
-          a_dst += kABytes; b_dst += b_bytes;
-          if (++stage == g.n_stages) { stage = 0; phase ^= 1; a_dst = sA; b_dst = sB; }
+          tma_load_3d(&map_b, &full_bar[stage], sB + stage * kBBytes, c0, tap, n0);
+          if (++stage == g.n_stages) { stage = 0; phase ^= 1; }
         }
         if (++kw == g.KW) { kw = 0; if (++kh == g.KH) { kh = 0; ++kt; } }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // One thread runs the whole loop.  With a narrow N tile an MMA occupies the tensor pipe for as little as 32-64
-    // cycles, so the per-k-block issue path must be a handful of instructions: descriptor high words are constants,
-    // the low words (shared-memory address >> 4) advance by adds (measured on the stem: csrc/conv_halo.cu).
-    if (elect_one()) {
-      constexpr uint64_t kLayout = BK == 64 ? 2 : (BK == 32 ? 4 : 6);
-      constexpr uint64_t kDescHi = ((uint64_t)((8 * BK * 2) >> 4) << 32) | (1ULL << 46) | (kLayout << 61);
-      const uint32_t a_lo0 = (smem_u32(sA) & 0x3FFFF) >> 4, b_lo0 = (smem_u32(sB) & 0x3FFFF) >> 4;
-      const uint32_t a_step = (uint32_t)kABytes >> 4, b_step = (uint32_t)b_bytes >> 4, idesc = g.idesc;
-      uint32_t a_lo = a_lo0, b_lo = b_lo0;
-      int stage = 0; uint32_t phase = 0;
-      int kc = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t acc0 = kb ? 1u : 0u;
-        const int nk = (kc == g.kblocks_per_tap - 1) ? g.k_tail_steps : BK / 16;   // zero-filled channel tail: no MMA
-        if (++kc == g.kblocks_per_tap) kc = 0;
+  } else if (warp >= 4) {
+    // ===================== consumers (warpgroups 1, 2) =====================
+    const int wg = (warp >> 2) - 1;              // 64-row half of the tile
+    const int ct = threadIdx.x - 128;            // 0..255
+    const uint64_t hi = desc_hi_kmajor<BK>();
+    const uint64_t a_lo0 = desc_lo(sA + wg * 64 * BK * 2), b_lo0 = desc_lo(sB);
+    float acc[NCH * 32];
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)          // 16 elements (32 bytes) along K inside the swizzle atom per step
-          if (k < nk)
-            umma_f16(tmem_base, kDescHi | (uint64_t)(a_lo + 2 * k), kDescHi | (uint64_t)(b_lo + 2 * k), idesc, k ? 1u : acc0);
-        umma_commit(&empty_bar[stage]);            // frees the smem stage when the MMAs retire
-        a_lo += a_step; b_lo += b_step;
-        if (++stage == g.n_stages) { stage = 0; phase ^= 1; a_lo = a_lo0; b_lo = b_lo0; }
+    for (int i = 0; i < NCH * 32; ++i) acc[i] = 0.0f;
+    int stage = 0, prev = -1; uint32_t phase = 0;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint64_t a_lo = a_lo0 + (uint64_t)(stage * (kABytes >> 4)), b_lo = b_lo0 + (uint64_t)(stage * (kBBytes >> 4));
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {        // 16 elements (32 bytes) along K inside the swizzle atom per step
+#pragma unroll
+        for (int c = 0; c < NCH; ++c)
+          wgmma_64x64(acc + c * 32, hi | (a_lo + 2 * k), hi | (b_lo + (uint64_t)(c * ((64 * BK * 2) >> 4)) + 2 * k), 1u);
       }
-      umma_commit(tmem_full_bar);                  // accumulator complete
+      wg_commit();
+      wg_wait<1>();                              // the previous k-block's MMAs have retired: free its stage
+      if (prev >= 0 && ct % 128 == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == g.n_stages) { stage = 0; phase ^= 1; }
     }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int lane_grp = warp & 3;  // TMEM lane quarter this warp may access
-    const int row = lane_grp * 32 + lane;
-    // output pixel of this row
-    long long pix = -1;
-    if (g.mode == A_BOX) {
-      int dw = row % g.bw, r = row / g.bw;
-      int dh = r % g.bh, dt = r / g.bh;
-      int ow = bw0 + dw, oh = bh0 + dh, ot = bt0 + dt;
-      if (dt < g.bt && ow < g.OW && oh < g.OH && ot < g.OT) pix = (((long long)bn * g.OT + ot) * g.OH + oh) * g.OW + ow;
-    } else {
-      long long m = m0 + row;
-      if (m < g.M) pix = m;
-    }
-    // Residual (two_branch.py:79-81): this row's BN halves are fetched into registers *before* waiting for
-    // the accumulator, so the row-strided loads overlap the main loop instead of stalling the epilogue.
-    const __half* rrow = residual ? residual + (pix < 0 ? 0 : (size_t)pix * g.res_ld + g.res_coff + n0) : nullptr;
-    uint4 rreg[kMaxBNRes / 8];
-    if (kHasRes) {
+    wg_wait<0>();
+    // both consumers are done reading the stage area: it becomes the output staging tile
+    named_sync(1, kConsumers);
+    // Phase 1: registers -> scale/shift (+residual) (+relu) -> fp16 -> staging row.  Row pitch 2*BN+16 bytes is an odd
+    // multiple of 16, so the rows of one store instruction spread over the banks.
+    const int pitch = BN * 2 + 16;
+    const int wrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-      for (int j = 0; j < kMaxBNRes / 8; ++j) {
-        rreg[j] = make_uint4(0, 0, 0, 0);
-        if (pix >= 0 && j * 8 < g.BN && n0 + j * 8 < g.Cout) rreg[j] = *reinterpret_cast<const uint4*>(rrow + j * 8);
-      }
-    }
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + ((uint32_t)(lane_grp * 32) << 16);
-    // Phase 1: TMEM -> registers -> scale/shift (+residual) (+relu) -> fp16 -> this warp's 32-row slab of the
-    // staging tile (the pipeline stages are idle once tmem_full fired).  Row pitch 2*BN+16 bytes is an odd
-    // multiple of 16, so the 16-byte stores of 8 consecutive rows land in distinct bank groups.
-    const int pitch = g.BN * 2 + 16;
-    uint8_t* slab = smem + (size_t)(lane_grp * 32) * pitch;
-    uint8_t* srow = slab + (size_t)lane * pitch;
+    for (int i = 0; i < 2; ++i) {
+      const int row = wrow + 8 * i;
+      const long long pix = residual ? tile_row_pixel(g, m_tile, row) : -1;
+      const __half* rrow = pix >= 0 ? residual + (size_t)pix * g.res_ld + g.res_coff + n0 : nullptr;
+      uint8_t* srow = smem + (size_t)row * pitch;
 #pragma unroll
-    for (int ci = 0; ci < kMaxBN / 16; ++ci) {
-      const int c = ci * 16;
-      if (c >= g.BN) break;
-      uint32_t v[16];
-      tmem_ld16(taddr + c, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {  // two 8-channel (16-byte) halves
-        const int cc = c + h * 8;
-        float f[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) f[k] = fmaf(__uint_as_float(v[h * 8 + k]), s_scale[cc + k], s_shift[cc + k]);
-        if (kHasRes && ci < kMaxBNRes / 16) {
-          const __half2* hp = reinterpret_cast<const __half2*>(&rreg[ci * 2 + h]);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float2 rf = __half22float2(hp[k]);
-            f[2 * k] += rf.x; f[2 * k + 1] += rf.y;
-          }
+      for (int j = 0; j < NCH * 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+        float f0 = fmaf(acc[4 * j + 2 * i], s_scale[col], s_shift[col]);
+        float f1 = fmaf(acc[4 * j + 2 * i + 1], s_scale[col + 1], s_shift[col + 1]);
+        if (rrow && n0 + col < g.Cout) {
+          const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(rrow + col));
+          f0 += rf.x; f1 += rf.y;
         }
-        if (g.relu) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], 0.0f);
-        }
-        store16(reinterpret_cast<__half*>(srow + cc * 2), f);
+        if (g.relu) { f0 = fmaxf(f0, 0.0f); f1 = fmaxf(f1, 0.0f); }
+        *reinterpret_cast<__half2*>(srow + col * 2) = __floats2half2_rn(f0, f1);
       }
     }
-    __syncwarp();
-    // Phase 2: coalesced copy-out: consecutive lanes write consecutive 16-byte chunks of an output row.
-    const int cpr = g.BN >> 3;  // 16-byte chunks per row
-    for (int i = lane; i < 32 * cpr; i += 32) {
+    named_sync(1, kConsumers);
+    // Phase 2: coalesced copy-out: consecutive threads write consecutive 16-byte chunks of an output row.
+    constexpr int cpr = BN / 8;  // 16-byte chunks per row
+    for (int i = ct; i < kBM * cpr; i += kConsumers) {
       const int rr = i / cpr, ch = i - rr * cpr;
-      const long long rp = __shfl_sync(0xffffffffu, pix, rr);
-      if (rp >= 0 && n0 + ch * 8 < g.Cout) {
-        uint4 val = *reinterpret_cast<const uint4*>(slab + (size_t)rr * pitch + ch * 16);
-        *reinterpret_cast<uint4*>(y + (size_t)rp * g.out_ld + g.out_coff + n0 + ch * 8) = val;
+      const int col = n0 + ch * 8;
+      if (col >= g.Cout) continue;
+      const long long rp = tile_row_pixel(g, m_tile, rr);
+      if (rp < 0) continue;
+      const uint4 val = *reinterpret_cast<const uint4*>(smem + (size_t)rr * pitch + ch * 16);
+      __half* dst = y + (size_t)rp * g.out_ld + g.out_coff + col;
+      if (g.n_splits > 0 && col >= g.split[0]) {
+        const int d = (g.n_splits > 1 && col >= g.split[1]) ? 1 : 0;
+        dst = g.y_extra[d] + (size_t)rp * g.ld_extra[d] + g.coff_extra[d] + (col - g.split[d]);
       }
+      *reinterpret_cast<uint4*>(dst) = val;
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
-  }
-}
-
-// ---- persistent variant ----------------------------------------------------------------------
-// One CTA per SM loops over output tiles of (mh x 128) rows x BN columns, mh in {1, 2}.
-//
-// Why this shape (ncu, profiles/): with 128 x BN tiles the tensor pipe sat at 50-60 % while L2 ran at
-// ~40 % -- the kernel was bound by the latency x bandwidth product: at full MMA rate a 128 x 160 tile needs
-// 112 B/clk of operands per SM, i.e. > 200 KB in flight to cover ~1 us of L2/TMA latency, more than an SM has
-// shared memory for.  Two 128-row halves that share the B (weight) tile cut the operand bytes per MMA
-// cycle by ~1/3 (the weights of a conv are re-read by every M tile and are as much traffic as the
-// activations), and one CTA per SM lets the pipeline use all ~200 KB of shared memory for stages.
-//
-// Pipelines: smem stages (TMA <-> MMA), TMEM accumulators (MMA <-> epilogue; double-buffered when
-// mh * BN <= 256 columns so the MMAs of tile i+1 overlap the epilogue of tile i), per-warp epilogue
-// staging slabs (32 rows x 32 columns) for coalesced stores.  TMEM allocation, barrier setup and
-// descriptor prefetch are paid once per CTA.
-constexpr int kMaxStagesP = 8;
-constexpr int kEpiWarps = 8;
-constexpr int kThreadsP = 64 + kEpiWarps * 32;     // warp 0 producer, warp 1 MMA, warps 2..9 epilogue
-constexpr int kMaxBNP = 256;
-constexpr int kSlabChunk = 32;                     // columns staged per pass by an epilogue warp
-constexpr int kSlabPitch = kSlabChunk * 2 + 16;    // 80 B: odd multiple of 16 -> conflict-free 16-byte stores
-constexpr int kSlabBytes = 4096;                   // per epilogue warp: 2 buffers x 2 halves x (32 rows x 32 B, 32B-swizzled)
-constexpr int kBookBytesP = 4096 + 4 * 2 * kMaxBNP * 4;           // barriers (first 4 KB) + [tile & 3][scale|shift][BN]
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tma_load_3d_mcast(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2,
-                                                  uint16_t mask) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5, %6}], [%2], %3;"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-
-// ---- CTA-pair (cta_group::2) protocol helpers; validated by tools/probe/umma_2cta_probe.cu and conv_pair_probe*.cu ----
-// wait with cluster-scope acquire: the arrivals come from both CTAs of the pair.  (The CTA-scope forms -- a bare SYNCS.ARRIVE
-// instead of MEMBAR.ALL.GPU + arrive -- were measured here as well: no difference for this kernel, whose epilogue arrives once per
-// tile with nothing in flight; the fused bottleneck exit, which arrives per 64-column chunk with loads in flight, needs them.)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAITC_LOOP:\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra.uni WAITC_DONE;\n\t"
-      "bra.uni WAITC_LOOP;\n\t"
-      "WAITC_DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-// TMA loads of a CTA pair: the data lands in the issuing CTA's shared memory, the bytes are signalled on the LEADER's
-// barrier (same offset, CTA-rank bit of the shared::cluster address cleared)
-__device__ __forceinline__ uint32_t leader_bar(uint64_t* bar) { return smem_u32(bar) & 0xFEFFFFFFu; }
-__device__ __forceinline__ void tma2_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(leader_bar(bar)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma2_load_3d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(leader_bar(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma2_load_im2col_5d(const CUtensorMap* map, uint64_t* bar, void* dst, int c, int w, int h, int d,
-                                                    int n, uint16_t ow, uint16_t oh, uint16_t od) {
-  asm volatile("cp.async.bulk.tensor.5d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2], {%8, %9, %10};"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(leader_bar(bar)), "r"(c), "r"(w), "r"(h), "r"(d), "r"(n), "h"(ow), "h"(oh), "h"(od) : "memory");
-}
-__device__ __forceinline__ void umma2_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-// the MMAs issued so far have retired -> one arrival on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma2_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-
-struct HalfOrigin {
-  long long m0;            // first output pixel (linear) of this 128-row half (LINEAR / IM2COL)
-  int bn, bt0, bh0, bw0;   // BOX origin
-};
-
-__device__ __forceinline__ HalfOrigin half_origin(const ConvGeom& g, int m_tile) {
-  HalfOrigin o;
-  o.m0 = (long long)m_tile * kBM;
-  o.bn = o.bt0 = o.bh0 = o.bw0 = 0;
-  if (g.mode == A_BOX) {
-    int r = m_tile;
-    o.bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
-    o.bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
-    o.bt0 = (r % g.tiles_t) * g.bt; o.bn = r / g.tiles_t;   // bn >= Nimg: the whole box is out of bounds -> zeros
-  }
-  return o;
-}
-
-// kPair: a cluster of two CTAs (the two SMs of a TPC) owns a 256-row x BN tile and runs ONE tcgen05.mma.cta_group::2 per
-// k step: CTA r stages rows [128 r, +128) of A and rows [r BN/2, +BN/2) of B, so an SM pulls in 16 KB + BN/2 * 128 B
-// per k-block (64 B/clk at BN = 256) instead of 16 KB + BN * 128 B (96 B/clk) -- the per-SM operand inbound rate is
-// what bounded the 128-row tiles (DESIGN.md section 7.1; 1088 -> 1024: 83 -> 62 us).  Barriers:
-//   full[s]   (leader's) both CTAs' TMA loads complete_tx here;   empty[s] (each CTA's) multicast commit frees stage s
-//   tfull[b]  (each CTA's) multicast commit: accumulator set b done;   tempty[b] (leader's) 2 x 8 epilogue warps arrive
-template <int BK, bool kHasRes, bool kPair>
-__global__ void __launch_bounds__(kThreadsP, 1)
-conv_umma_persist_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                         const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_bh,
-                         const __grid_constant__ CUtensorMap map_y0, const __grid_constant__ CUtensorMap map_y1,
-                         const __grid_constant__ CUtensorMap map_y2, ConvGeom g, int total_tiles,
-                         const float* __restrict__ scale, const float* __restrict__ shift,
-                         const __half* __restrict__ residual, __half* __restrict__ y) {
-  constexpr int kABytes = kBM * BK * 2;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint64_t* full_bar = (uint64_t*)smem_raw;
-  uint64_t* empty_bar = full_bar + kMaxStagesP;
-  uint64_t* tfull_bar = empty_bar + kMaxStagesP;   // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;            // [2]
-  uint64_t* rfull_bar = tempty_bar + 2;            // [2] residual tile landed (TMA)
-  uint64_t* rempty_bar = rfull_bar + 2;            // [2] residual tile consumed by all epilogue warps
-  uint32_t* tmem_ptr_s = (uint32_t*)(rempty_bar + 2);
-  float* ss_all = (float*)(smem_raw + 4096);       // [tile & 3][scale | shift][kMaxBNP]
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + kBookBytesP + 1023) & ~(uintptr_t)1023);
-  const int mh = g.mh;
-  const int b_bytes = (kPair ? (g.BN >> 1) : g.BN) * BK * 2;   // a pair member stages half of the weight rows
-  const int stage_bytes = mh * kABytes + b_bytes;  // multiple of 1024 (BN % 16 == 0)
-  uint8_t* slabs = smem + (size_t)g.n_stages_p * stage_bytes;   // [kEpiWarps][32 rows][kSlabPitch]
-  // residual tiles (kHasRes && g.res_tma): [2 buffers][BN/64 boxes][128 rows x 128 B, 128B-swizzled], 1024-aligned
-  uint8_t* rbuf = (uint8_t*)(((uintptr_t)(slabs + (size_t)kEpiWarps * kSlabBytes) + 1023) & ~(uintptr_t)1023);
-  const bool res_tma = kHasRes && g.res_tma;
-  const int res_boxes = g.BN >> 6;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_kb = g.taps * g.kblocks_per_tap;
-  const int nbuf = g.tmem_bufs;                    // 1 or 2 accumulator sets
-  // Cluster of 2 CTAs (two neighbouring SMs) on adjacent M tiles of the same N tile: each CTA fetches half of the
-  // weight tile and TMA-multicasts it into both CTAs' shared memory, so the weight traffic out of L2 -- the larger
-  // share for wide-N 1x1x1 layers -- is halved.  A stage may only be refilled when BOTH consumers released it.
-  const bool cl2 = !kPair && g.cluster == 2;
-  const bool two = kPair || cl2;                   // the grid is made of CTA pairs
-  const uint32_t crank = two ? cluster_ctarank() : 0;
-  const int tile_step = two ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int tile_first = two ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-    for (int s = 0; s < g.n_stages_p; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], cl2 ? 2 : 1); }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], kPair ? 2 * kEpiWarps : kEpiWarps);
-      mbar_init(&rfull_bar[b], 1); mbar_init(&rempty_bar[b], kEpiWarps);
-    }
-    if (kHasRes) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_r) : "memory");
-    fence_barrier_init();
-  }
-  uint32_t ncols = 32;
-  while (ncols < (uint32_t)g.BN) ncols <<= 1;
-  const uint32_t alloc_cols = ncols * (uint32_t)(mh * nbuf);   // <= 512 by construction (host)
-  if (warp == 1) {
-    if (kPair) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_s)), "r"(alloc_cols) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_s)), "r"(alloc_cols) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (two) cluster_sync_all();   // the peer's barriers must be initialised before anything is multicast into them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_s;
-  pdl_wait();                    // the producer of x / residual (the previous kernel in the stream) has finished
-  pdl_launch_dependents();
-
-  // tile -> (m tile, n offset).  In a cluster the two CTAs take M tiles 2*pm and 2*pm+1 of the same N tile (the odd
-  // one may lie past the end: its loads are zero-filled and nothing is stored, but it still runs the k loop).
-  auto tile_mt = [&](int tile) { const int pm = tile / g.n_tiles; return two ? pm * 2 + (int)crank : pm; };
-  auto tile_n0 = [&](int tile) { return (tile % g.n_tiles) * g.BN; };
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      const uint32_t tx_bytes = (uint32_t)(mh * g.a_bytes + b_bytes);
-      int stage = 0; uint32_t phase = 0;
-      int pit = 0;
-      for (int tile = tile_first; tile < total_tiles; tile += tile_step, ++pit) {
-        const int mt = tile_mt(tile);
-        const int n0 = tile_n0(tile);
-        if (res_tma) {
-          // residual tile of this output tile (two_branch.py:79-81): coalesced, asynchronous, swizzled like an operand
-          const int rb = g.res_bufs == 2 ? (pit & 1) : 0;
-          const uint32_t ruse = (uint32_t)(g.res_bufs == 2 ? (pit >> 1) : pit);
-          mbar_wait(&rempty_bar[rb], (ruse & 1u) ^ 1u);
-          mbar_expect_tx(&rfull_bar[rb], (uint32_t)(res_boxes * kBM * 128));
-          for (int j = 0; j < res_boxes; ++j)
-            tma_load_2d(&map_r, &rfull_bar[rb], rbuf + ((size_t)rb * res_boxes + j) * (kBM * 128), n0 + j * 64, mt * kBM);
-        }
-        HalfOrigin ho[2];
-        int iw[2], ih[2], it[2], in_[2];
-        for (int h = 0; h < mh; ++h) {
-          ho[h] = half_origin(g, mt * mh + h);
-          long long r = ho[h].m0;
-          iw[h] = (int)(r % g.OW); r /= g.OW;
-          ih[h] = (int)(r % g.OH); r /= g.OH;
-          it[h] = (int)(r % g.OT); in_[h] = (int)(r / g.OT);   // in_ >= Nimg: out of bounds -> zeros
-          iw[h] -= g.PW; ih[h] -= g.PH; it[h] -= g.PT;
-        }
-        for (int tap = 0; tap < g.taps; ++tap) {
-          const int kw = tap % g.KW, kh = (tap / g.KW) % g.KH, kt = tap / (g.KW * g.KH);
-          for (int kc = 0; kc < g.kblocks_per_tap; ++kc) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* st = smem + (size_t)stage * stage_bytes;
-            const int c0 = kc * BK;
-            if constexpr (kPair) {
-              // both CTAs' bytes are counted on the leader's barrier; my A rows and my half of the weight rows
-              if (crank == 0) mbar_expect_tx(&full_bar[stage], 2u * tx_bytes);
-              if (g.mode == A_LINEAR) tma2_load_2d(&map_a, &full_bar[stage], st, c0, (int)ho[0].m0);
-              else tma2_load_im2col_5d(&map_a, &full_bar[stage], st, c0, iw[0], ih[0], it[0], in_[0], (uint16_t)kw, (uint16_t)kh, (uint16_t)kt);
-              tma2_load_3d(&map_bh, &full_bar[stage], st + kABytes, c0, tap, n0 + (int)crank * (g.BN >> 1));
-            } else {
-            mbar_expect_tx(&full_bar[stage], tx_bytes);
-            for (int h = 0; h < mh; ++h) {
-              void* a_dst = st + h * kABytes;
-              if (g.mode == A_LINEAR) {
-                tma_load_2d(&map_a, &full_bar[stage], a_dst, c0, (int)ho[h].m0);
-              } else if (g.mode == A_BOX) {
-                tma_load_5d(&map_a, &full_bar[stage], a_dst, c0, ho[h].bw0 + kw - g.PW, ho[h].bh0 + kh - g.PH,
-                            ho[h].bt0 + kt - g.PT, ho[h].bn);
-              } else {
-                tma_load_im2col_5d(&map_a, &full_bar[stage], a_dst, c0, iw[h], ih[h], it[h], in_[h], (uint16_t)kw,
-                                   (uint16_t)kh, (uint16_t)kt);
-              }
-            }
-            if (cl2) {
-              const int hb = b_bytes >> 1;   // my half of the weight rows, delivered to both CTAs
-              tma_load_3d_mcast(&map_bh, &full_bar[stage], st + mh * kABytes + crank * hb, c0, tap, n0 + (int)crank * (g.BN >> 1),
-                                (uint16_t)3);
-            } else {
-              tma_load_3d(&map_b, &full_bar[stage], st + mh * kABytes, c0, tap, n0);
-            }
-            }
-            if (++stage == g.n_stages_p) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // one thread runs the whole loop; descriptor high words are constants, low words advance by adds (see above)
-    if ((!kPair || crank == 0) && elect_one()) {   // in a pair the leader issues for both CTAs
-      constexpr uint64_t kLayout = BK == 64 ? 2 : (BK == 32 ? 4 : 6);
-      constexpr uint64_t kDescHi = ((uint64_t)((8 * BK * 2) >> 4) << 32) | (1ULL << 46) | (kLayout << 61);
-      const uint32_t st_lo0 = (smem_u32(smem) & 0x3FFFF) >> 4, st_step = (uint32_t)stage_bytes >> 4;
-      const uint32_t a_half = (uint32_t)kABytes >> 4, b_off = (uint32_t)(mh * kABytes) >> 4, idesc = g.idesc;
-      uint32_t st_lo = st_lo0;
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int tile = tile_first; tile < total_tiles; tile += tile_step, ++it) {
-        const int buf = nbuf == 2 ? (it & 1) : 0;
-        const uint32_t use = (uint32_t)(nbuf == 2 ? (it >> 1) : it);
-        // the epilogue (of both CTAs in a pair) has drained this accumulator set
-        if (kPair) mbar_wait_cluster(&tempty_bar[buf], (use & 1u) ^ 1u); else mbar_wait(&tempty_bar[buf], (use & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf * mh) * ncols;
-        int kc = 0;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t acc0 = kb ? 1u : 0u;
-          const uint32_t b_lo = st_lo + b_off;
-          const int nk = (kc == g.kblocks_per_tap - 1) ? g.k_tail_steps : BK / 16;   // zero-filled channel tail: no MMA
-          if (++kc == g.kblocks_per_tap) kc = 0;
-          if constexpr (kPair) {
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              if (k < nk)
-                umma2_f16(tmem_d, kDescHi | (uint64_t)(st_lo + 2 * k), kDescHi | (uint64_t)(b_lo + 2 * k), idesc, k ? 1u : acc0);
-            umma2_commit(&empty_bar[stage]);
-          } else {
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            if (k < nk)
-              umma_f16(tmem_d, kDescHi | (uint64_t)(st_lo + 2 * k), kDescHi | (uint64_t)(b_lo + 2 * k), idesc, k ? 1u : acc0);
-          if (mh == 2) {
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              if (k < nk)
-                umma_f16(tmem_d + ncols, kDescHi | (uint64_t)(st_lo + a_half + 2 * k), kDescHi | (uint64_t)(b_lo + 2 * k), idesc,
-                         k ? 1u : acc0);
-          }
-          if (cl2) umma_commit_mcast(&empty_bar[stage], (uint16_t)3); else umma_commit(&empty_bar[stage]);
-          }
-          st_lo += st_step;
-          if (++stage == g.n_stages_p) { stage = 0; phase ^= 1; st_lo = st_lo0; }
-        }
-        if (kPair) umma2_commit(&tfull_bar[buf]); else umma_commit(&tfull_bar[buf]);
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
-    // mh == 2: warp = (lane quarter, row half), all BN columns.  mh == 1: warp = (lane quarter, column half).
-    const int ew = warp - 2;
-    const int lane_grp = warp & 3;                 // TMEM lane quarter this warp may access
-    const int sel = ew >> 2;                       // 0 / 1
-    const int hsel = mh == 2 ? sel : 0;            // which 128-row half
-    const int col0 = (mh == 2 || sel == 0) ? 0 : g.col_split;
-    const int col1 = (mh == 2 || sel == 1) ? g.BN : g.col_split;
-    const int ncol = col1 - col0;                  // multiple of 16, may be 0
-    uint8_t* slab = slabs + (size_t)ew * kSlabBytes;
-    uint8_t* srow = slab + (size_t)lane * kSlabPitch;
-    const int row = lane_grp * 32 + lane;
-    auto row_pixel = [&](int m_tile) -> long long {
-      const HalfOrigin o = half_origin(g, m_tile);
-      if (g.mode == A_BOX) {
-        int dw = row % g.bw, r = row / g.bw;
-        int dh = r % g.bh, dt = r / g.bh;
-        int ow = o.bw0 + dw, oh = o.bh0 + dh, ot = o.bt0 + dt;
-        if (o.bn < g.Nimg && dt < g.bt && ow < g.OW && oh < g.OH && ot < g.OT)
-          return (((long long)o.bn * g.OT + ot) * g.OH + oh) * g.OW + ow;
-        return -1;
-      }
-      long long m = o.m0 + row;
-      return m < g.M ? m : -1;
-    };
-    const bool tma_st = g.tma_store != 0, w32 = g.st_w == 32;
-    int pass = 0;                                  // bulk-store passes issued by this warp (slab double buffer)
-    int it = 0;
-    for (int tile = tile_first; tile < total_tiles; tile += tile_step, ++it) {
-      const int buf = nbuf == 2 ? (it & 1) : 0;
-      const uint32_t use = (uint32_t)(nbuf == 2 ? (it >> 1) : it);
-      const int mt = tile_mt(tile);
-      const int n0 = tile_n0(tile);
-      const long long pix = row_pixel(mt * mh + hsel);
-      const int nbase = n0 + col0;                 // first output channel this warp handles
-      // per-channel epilogue constants of this tile; warps of the same tile write identical values into
-      // slot (tile & 3): a warp reaches this point at most two tiles ahead of the slowest warp (it cannot
-      // pass the tfull wait of tile i+2 before every warp released the accumulator of tile i)
-      float* s_scale = ss_all + (size_t)(it & 3) * 2 * kMaxBNP + col0;
-      float* s_shift = s_scale + kMaxBNP;
-      for (int i = lane; i < ncol; i += 32) {
-        const int c = nbase + i;
-        s_scale[i] = (scale && c < g.Cout) ? scale[c] : 1.0f;
-        s_shift[i] = (shift && c < g.Cout) ? shift[c] : 0.0f;
-      }
-      __syncwarp();
-      mbar_wait(&tfull_bar[buf], use & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(buf * mh + hsel) * ncols + (uint32_t)col0;
-      const __half* rrow = (kHasRes && pix >= 0) ? residual + (size_t)pix * g.res_ld + g.res_coff + nbase : nullptr;
-      const int rb = g.res_bufs == 2 ? (it & 1) : 0;
-      const uint8_t* rtile = rbuf + (size_t)rb * res_boxes * (kBM * 128);
-      if (res_tma) mbar_wait(&rfull_bar[rb], (uint32_t)(g.res_bufs == 2 ? (it >> 1) : it) & 1u);
-      if (tma_st) {
-        // 32-column passes: TMEM -> registers -> scale/shift/residual/ReLU -> fp16 slab -> bulk tensor stores.  The slab
-        // is two 16-column halves ([32 rows][32 B], 32B-swizzled); a half never straddles a destination boundary (splits
-        // are multiples of 16), and the store engine clips rows >= M and columns past the destination's width.
-        const int row0 = (mt * mh + hsel) * kBM + lane_grp * 32;
-        for (int cb = 0; cb < ncol; cb += 32, ++pass) {
-          const int cw = min(32, ncol - cb);       // 32, or 16 in the tail of an odd tile
-          const bool last = cb + 32 >= ncol;
-          uint8_t* sl = slab + (size_t)(pass & 1) * 2048;
-          uint4 rreg[4];
-          if (kHasRes) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              rreg[j] = make_uint4(0, 0, 0, 0);
-              if (j * 8 < cw) {
-                if (res_tma) {
-                  const int tc = col0 + cb + j * 8;
-                  rreg[j] = *reinterpret_cast<const uint4*>(rtile + (size_t)(tc >> 6) * (kBM * 128) + row * 128 +
-                                                            ((((tc & 63) >> 3) ^ (row & 7)) << 4));
-                } else if (rrow && nbase + cb + j * 8 < g.Cout) {
-                  rreg[j] = *reinterpret_cast<const uint4*>(rrow + cb + j * 8);
-                }
-              }
-            }
-          }
-          uint32_t v[32];
-          if (cw == 32) tmem_ld32(taddr + cb, v); else tmem_ld16(taddr + cb, v);
-          // the bulk stores that read this slab buffer two passes ago must have drained it
-          if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-          __syncwarp();
-          tmem_ld_wait();
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            if (q * 8 < cw) {
-              const float4 a0 = *reinterpret_cast<const float4*>(s_scale + cb + q * 8);
-              const float4 a1 = *reinterpret_cast<const float4*>(s_scale + cb + q * 8 + 4);
-              const float4 b0 = *reinterpret_cast<const float4*>(s_shift + cb + q * 8);
-              const float4 b1 = *reinterpret_cast<const float4*>(s_shift + cb + q * 8 + 4);
-              float f[8];
-              f[0] = fmaf(__uint_as_float(v[q * 8 + 0]), a0.x, b0.x); f[1] = fmaf(__uint_as_float(v[q * 8 + 1]), a0.y, b0.y);
-              f[2] = fmaf(__uint_as_float(v[q * 8 + 2]), a0.z, b0.z); f[3] = fmaf(__uint_as_float(v[q * 8 + 3]), a0.w, b0.w);
-              f[4] = fmaf(__uint_as_float(v[q * 8 + 4]), a1.x, b1.x); f[5] = fmaf(__uint_as_float(v[q * 8 + 5]), a1.y, b1.y);
-              f[6] = fmaf(__uint_as_float(v[q * 8 + 6]), a1.z, b1.z); f[7] = fmaf(__uint_as_float(v[q * 8 + 7]), a1.w, b1.w);
-              if (kHasRes) {
-                const __half2* hp = reinterpret_cast<const __half2*>(&rreg[q]);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  float2 rf = __half22float2(hp[k]);
-                  f[2 * k] += rf.x; f[2 * k + 1] += rf.y;
-                }
-              }
-              if (g.relu) {
-#pragma unroll
-                for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], 0.0f);
-              }
-              // 16-column boxes: two halves of [32 rows][32 B], 32B swizzle.  32-column boxes: [32 rows][64 B], 64B swizzle
-              const int soff = w32 ? lane * 64 + ((q ^ ((lane >> 1) & 3)) << 4)
-                                   : (q >> 1) * 1024 + lane * 32 + (((q & 1) ^ ((lane >> 2) & 1)) << 4);
-              store16(reinterpret_cast<__half*>(sl + soff), f);
-            }
-          }
-          if (last) tc_fence_before();
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            if (last) { if (kPair) mbar_arrive_remote(&tempty_bar[buf], 0); else mbar_arrive(&tempty_bar[buf]); }   // accumulator fully read by this warp
-            for (int h = 0; h * 16 < (w32 ? 16 : cw); ++h) {   // one 32-column box, or one 16-column box per half
-              const int gc = nbase + cb + h * 16;
-              if (gc >= g.Cout) break;
-              int d = 0, ds = 0;
-              if (g.n_splits > 0 && gc >= g.split[0]) { d = 1; ds = g.split[0]; }
-              if (g.n_splits > 1 && gc >= g.split[1]) { d = 2; ds = g.split[1]; }
-              tma_store_2d(d == 0 ? &map_y0 : (d == 1 ? &map_y1 : &map_y2), sl + h * 1024, gc - ds, row0);
-            }
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          }
-        }
-      } else
-      for (int cb = 0; cb < ncol; cb += kSlabChunk) {
-        const int cw = min(kSlabChunk, ncol - cb);   // 16 or 32 columns in this pass
-        uint4 rreg[kSlabChunk / 8];
-        if (kHasRes) {
-#pragma unroll
-          for (int j = 0; j < kSlabChunk / 8; ++j) {
-            rreg[j] = make_uint4(0, 0, 0, 0);
-            if (res_tma) {
-              // tile-relative column -> 64-column box, 16-byte chunk inside the 128-byte row, XOR-swizzled by row
-              const int tc = col0 + cb + j * 8;
-              if (j * 8 < cw)
-                rreg[j] = *reinterpret_cast<const uint4*>(rtile + (size_t)(tc >> 6) * (kBM * 128) + row * 128 +
-                                                          ((((tc & 63) >> 3) ^ (row & 7)) << 4));
-            } else if (rrow && j * 8 < cw && nbase + cb + j * 8 < g.Cout) {
-              rreg[j] = *reinterpret_cast<const uint4*>(rrow + cb + j * 8);
-            }
-          }
-        }
-#pragma unroll
-        for (int ci = 0; ci < kSlabChunk / 16; ++ci) {
-          const int c = cb + ci * 16;
-          if (ci * 16 >= cw) break;
-          uint32_t v[16];
-          tmem_ld16(taddr + c, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int cc = c + h * 8;
-            float f[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) f[k] = fmaf(__uint_as_float(v[h * 8 + k]), s_scale[cc + k], s_shift[cc + k]);
-            if (kHasRes) {
-              const __half2* hp = reinterpret_cast<const __half2*>(&rreg[ci * 2 + h]);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                float2 rf = __half22float2(hp[k]);
-                f[2 * k] += rf.x; f[2 * k + 1] += rf.y;
-              }
-            }
-            if (g.relu) {
-#pragma unroll
-              for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], 0.0f);
-            }
-            store16(reinterpret_cast<__half*>(srow + (ci * 16 + h * 8) * 2), f);
-          }
-        }
-        if (cb + kSlabChunk >= ncol) {
-          // last pass: the accumulator is fully read by this warp -> hand the TMEM set back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) { if (kPair) mbar_arrive_remote(&tempty_bar[buf], 0); else mbar_arrive(&tempty_bar[buf]); }
-        } else {
-          __syncwarp();
-        }
-        // coalesced copy-out of the 32 x cw slab: consecutive lanes write consecutive 16-byte chunks of a row
-        const int cpr = cw >> 3;
-        for (int i = lane; i < 32 * cpr; i += 32) {
-          const int rr = i / cpr, ch = i - rr * cpr;
-          const long long rp = __shfl_sync(0xffffffffu, pix, rr);
-          const int col = nbase + cb + ch * 8;
-          if (rp >= 0 && col < g.Cout) {
-            uint4 val = *reinterpret_cast<const uint4*>(slab + (size_t)rr * kSlabPitch + ch * 16);
-            __half* dst = y + (size_t)rp * g.out_ld + g.out_coff + col;
-            if (g.n_splits > 0 && col >= g.split[0]) {
-              const int d = (g.n_splits > 1 && col >= g.split[1]) ? 1 : 0;
-              dst = g.y_extra[d] + (size_t)rp * g.ld_extra[d] + g.coff_extra[d] + (col - g.split[d]);
-            }
-            *reinterpret_cast<uint4*>(dst) = val;
-          }
-        }
-        __syncwarp();
-      }
-      if (ncol == 0) {  // this warp owns no columns (tiny BN): still release the accumulator
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) { if (kPair) mbar_arrive_remote(&tempty_bar[buf], 0); else mbar_arrive(&tempty_bar[buf]); }
-      }
-      if (res_tma) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&rempty_bar[rb]);
-      }
-    }
-    if (tma_st && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // slabs are read, writes are done
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (two) cluster_sync_all();   // do not exit while the peer may still multicast into / signal this CTA
-  if (warp == 1) {
-    tc_fence_after();
-    if (kPair) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(alloc_cols) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(alloc_cols) : "memory");
   }
 }
 
@@ -878,18 +290,16 @@ static CUtensorMapSwizzle swizzle_for(int BK) {
   return BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
+// Channel block width.  A tap's last block is zero-filled past Cin and its zero 16-channel steps are multiplied, not skipped
+// (a data-dependent guard around the wgmma issue makes ptxas serialise the whole sequence), so the width is chosen by the
+// padded K it costs: e.g. Cin = 96 -> 3 blocks of 32 (no padding) rather than 2 blocks of 64 (25 % zero steps).  The zero
+// steps add exact zeros, so the choice does not change the result.
 static int pick_bk(int Cin) {
-  // STEP_B200_BKPOL=1: widest block that the channel count reaches -- the MMA loop skips the zero-filled 16-channel
-  // steps of a tap's last block and TMA does not fetch them, so padding inside a block is (nearly) free
-  if (const char* e = getenv("STEP_B200_BKPOL")) { if (e[0] == '1') return Cin > 32 ? 64 : (Cin > 16 ? 32 : 16); }
-  // more than 64 channels: 64-wide blocks; the zero-filled 16-channel steps of the last block are skipped and the layer becomes
-  // eligible for CTA pairs (measured round 2: Cin = 96, Mixed_3b 3x3x3 103 -> 90 us, Mixed_4b 27 -> 23 us vs three 32-wide blocks)
-  if (Cin > 64) return 64;
   int best = 64; long best_cost = -1;
   const int cands[3] = {64, 32, 16};
   for (int i = 0; i < 3; ++i) {
     int bk = cands[i];
-    long cost = (long)((Cin + bk - 1) / bk) * (bk + 16);  // padded K plus a per-k-block overhead term (measured: 160 -> 3x64 beats 5x32)
+    long cost = (long)((Cin + bk - 1) / bk) * (bk + 16);  // padded K plus a per-k-block overhead term
     if (best_cost < 0 || cost < best_cost) { best = bk; best_cost = cost; }
   }
   return best;
@@ -908,35 +318,36 @@ static void pick_box(int OW, int OH, int OT, int* bw, int* bh, int* bt) {
     }
 }
 
-static int conv_variant() {
-  static int v = -1;
+// Do two CTAs of conv_umma_kernel<BK, NCH> with `smem` bytes of dynamic shared memory fit one SM?  The answer depends only on
+// the instantiation (the caller derives `smem` from BK and NCH), so it is asked once per instantiation.
+template <int BK, int NCH>
+static int two_ctas_fit_t(size_t smem, bool* two) {
+  static std::atomic<int> cached{-1};
+  int v = cached.load(std::memory_order_relaxed);
   if (v < 0) {
-    const char* e = getenv("STEP_B200_CONV");
-    v = (e && e[0] == '1') ? 1 : ((e && e[0] == '3') ? 3 : 2);   // 2 (default) = hybrid, see conv3d_umma_launch
+    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BK, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    int n = 0;
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, conv_umma_kernel<BK, NCH>, kThreads, smem);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail((int)e, "conv3d(f16): occupancy query: %s", cudaGetErrorString(e)); }
+    v = n >= 2 ? 1 : 0;
+    cached.store(v, std::memory_order_relaxed);
   }
-  return v;
+  *two = v == 1;
+  return 0;
+}
+
+static int two_ctas_fit(int BK, int NCH, size_t smem, bool* two) {
+  if (NCH == 1) return BK == 64 ? two_ctas_fit_t<64, 1>(smem, two) : (BK == 32 ? two_ctas_fit_t<32, 1>(smem, two) : two_ctas_fit_t<16, 1>(smem, two));
+  return BK == 64 ? two_ctas_fit_t<64, 2>(smem, two) : (BK == 32 ? two_ctas_fit_t<32, 2>(smem, two) : two_ctas_fit_t<16, 2>(smem, two));
 }
 
 struct ConvPlan {
-  CUtensorMap map_a, map_b, map_r, map_bh, map_y[3];
+  CUtensorMap map_a, map_b;
   ConvGeom g;
   int BK;
   size_t smem_bytes;
   dim3 grid;
-  int persist_tiles;
-  size_t persist_smem;
-  bool persist, pair;   // which kernel the plan was made for
 };
-
-// STEP_B200_PAIR: 0 = never use CTA pairs, 1 = wherever legal, unset = where the pair tiles fill the 74 SM pairs
-static int pair_policy() {
-  static int v = -2;
-  if (v == -2) {
-    const char* e = getenv("STEP_B200_PAIR");
-    v = !e ? -1 : (e[0] == '0' ? 0 : 1);
-  }
-  return v;
-}
 
 static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   if (int rc = load_driver_entry_points()) return rc;
@@ -960,63 +371,14 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   pl->BK = pick_bk(p->Cin);
   const int BK = pl->BK;
   g.kblocks_per_tap = (p->Cin + BK - 1) / BK;
-  g.k_tail_steps = (p->Cin - (g.kblocks_per_tap - 1) * BK + 15) / 16;   // the rest of the block is TMA zero fill: skip it
-  long long m128 = 0;   // number of 128-row M tiles (filled in below once the A mode is known)
-  // CTA pairs (cta_group::2, 256-row tiles): LINEAR / IM2COL addressing, and enough 256-row tiles to fill the 74 SM pairs
-  bool pair = false;
-  if (pair_policy() != 0 && (mode == A_LINEAR || mode == A_IM2COL) && conv_variant() != 1) {
-    const long long mt = ((long long)p->N * p->OT * p->OH * p->OW + kBM - 1) / kBM;
-    const long long nt = (p->Cout + (p->residual ? kMaxBNRes : kMaxBNP) - 1) / (p->residual ? kMaxBNRes : kMaxBNP);
-    const long long pt = ((mt + 1) / 2) * nt;
-    const int num_kb = taps * g.kblocks_per_tap;
-    // Measured layer by layer (tools/experiments/r2_pair.sh, profiles/r2_conv_layers.txt): pairs win where the K loop is
-    // long enough for the operand stream to be the bound (>= 13 k-blocks of 64: 1088 -> 1024 83 -> 65 us, Mixed_5b 3x3x3
-    // 104 -> 80 us, Mixed_4 3x3x3 56 -> 45 us); short-K 1x1 layers are bound by the TMEM read-out / store side and lose
-    // (256 -> 1024: 38 -> 43 us), as do thin-input k > 1 layers, which the co-resident one-tile CTAs serve better.
-    pair = pair_policy() == 1 || (BK == 64 && num_kb >= 13 && !(taps > 1 && p->Cin <= 64) && pt >= 40);
-  }
-  const bool persist = pair || conv_variant() == 3 || (conv_variant() == 2 && taps == 1);
-  pl->pair = pair; pl->persist = persist;
-  {
-    // N tile: as wide as the accumulator allows -- every N tile re-reads the whole A operand through L2.
-    int cap = (persist && !p->residual) ? kMaxBNP : (p->residual ? kMaxBNRes : kMaxBN);
-    // STEP_B200_RESBN=256: 256-wide tiles with a single-buffered 64 KB residual tile.  Halves the re-reads of A but
-    // measured slower (76.6 vs 57.9 us on the 256 -> 1024 bottleneck exit), so the narrow tile stays the default.
-    if (persist && p->residual && p->Cout % 256 == 0 && mode == A_LINEAR && getenv("STEP_B200_RESBN") && atoi(getenv("STEP_B200_RESBN")) == 256)
-      cap = 256;
-    g.n_tiles = (p->Cout + cap - 1) / cap;
-    // STEP_B200_NSPLIT=1 (one tile per CTA kernel, k > 1): when there are fewer M tiles than SMs, split N further so
-    // that ~2 CTAs land on every SM.  Measured worse on the mixed_4 layers (4e 56 -> 78 us, 4f 55 -> 73 us: every extra
-    // N tile re-pulls A through TMA and the layers are bound by exactly that), so it stays an experiment switch.
-    if (!persist && taps > 1 && getenv("STEP_B200_NSPLIT") && getenv("STEP_B200_NSPLIT")[0] == '1') {
-      const long long mt = ((long long)p->N * p->OT * p->OH * p->OW + kBM - 1) / kBM;
-      if (mt < kNumSMs) {
-        int want = (int)((2 * kNumSMs + mt - 1) / mt);
-        while (want > g.n_tiles && (p->Cout + want - 1) / want < 64) --want;   // keep N tiles >= 64 columns
-        if (want > g.n_tiles) g.n_tiles = want;
-      }
-    }
-    g.BN = (((p->Cout + g.n_tiles - 1) / g.n_tiles) + 15) / 16 * 16;
-    // three stages whenever two CTAs of them still fit one SM (<= 112 KB each incl. bookkeeping), else two
-    g.n_stages = (kBookBytes + 1024 + 3L * (kBM * BK * 2 + g.BN * BK * 2) <= 112 * 1024) ? 3 : 2;
-    {
-      // Small maps (mixed_4: 98 M tiles): fewer CTAs than SMs, so each CTA is alone on its SM and its own pipeline depth
-      // is all the latency hiding there is -- give it the whole shared memory (up to kStages stages).
-      const long long mt = ((long long)p->N * p->OT * p->OH * p->OW + kBM - 1) / kBM;
-      if (!persist && mode == A_IM2COL && mt * g.n_tiles <= kNumSMs && !(getenv("STEP_B200_DEEP") && getenv("STEP_B200_DEEP")[0] == '0')) {
-        const long per_stage = kBM * BK * 2 + (long)g.BN * BK * 2;
-        int st = (int)((220L * 1024 - kBookBytes - 1024) / per_stage);
-        if (st > kStages) st = kStages;
-        if (st > g.n_stages) g.n_stages = st;
-      }
-    }
-  }
+  // N tile: as wide as the register accumulator allows -- every N tile re-reads the whole A operand through L2
+  g.BN = p->Cout <= 64 ? 64 : kMaxBN;
+  g.n_tiles = (p->Cout + g.BN - 1) / g.BN;
   g.Cout = p->Cout; g.out_ld = p->out_ld; g.out_coff = p->out_coff; g.res_ld = p->res_ld; g.res_coff = p->res_coff;
   g.relu = p->relu;
   g.n_splits = p->n_splits;
   if (p->n_splits) {
-    STEP_CHECK_ARG(p->n_splits >= 1 && p->n_splits <= 2 && persist && !p->residual,
-                   "conv3d(f16): fused outputs need the persistent kernel, no residual, 1-2 splits");
+    STEP_CHECK_ARG(p->n_splits >= 1 && p->n_splits <= 2 && !p->residual, "conv3d(f16): fused outputs need no residual, 1-2 splits");
     int prev = 0;
     for (int i = 0; i < p->n_splits; ++i) {
       STEP_CHECK_ARG(p->split[i] % 16 == 0 && p->split[i] > prev && p->split[i] < p->Cout && p->y_extra[i] &&
@@ -1029,7 +391,6 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   }
   g.OT = p->OT; g.OH = p->OH; g.OW = p->OW; g.Nimg = p->N;
   g.M = (long long)p->N * p->OT * p->OH * p->OW;
-  g.idesc = (1u << 4) | ((uint32_t)(g.BN >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);  // f16 x f16 -> f32, K-major A/B
   long long m_tiles;
   const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
   CUresult cr;
@@ -1091,106 +452,32 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   }
   STEP_CHECK_ARG(m_tiles * g.n_tiles < (1LL << 31), "conv3d(f16): grid too large");
   pl->grid = dim3((unsigned)(m_tiles * g.n_tiles));
-  {
-    size_t stage_area = (size_t)g.n_stages * (kBM * BK * 2 + g.BN * BK * 2);
-    size_t out_tile = (size_t)kBM * (g.BN * 2 + 16);
-    pl->smem_bytes = kBookBytes + 1024 + (stage_area > out_tile ? stage_area : out_tile);
+  // Pipeline depth: at least four stages within half of an SM's shared memory (<= 113 KB) when the occupancy calculator says
+  // two such CTAs really fit an SM (registers included), so that one CTA's epilogue overlaps the other's main loop; otherwise
+  // as deep as the 227 KB of one SM allow.
+  const long per_stage = (long)kBM * BK * 2 + (long)g.BN * BK * 2;
+  const long fixed = kBookBytes + 1024;
+  const long out_tile = (long)kBM * (g.BN * 2 + 16);
+  int st = (int)((113L * 1024 - fixed) / per_stage);
+  if (st > kStages) st = kStages;
+  bool two = false;
+  if (st >= 4) {
+    const long area = st * per_stage;
+    if (int rc = two_ctas_fit(BK, g.BN / 64, (size_t)(fixed + (area > out_tile ? area : out_tile)), &two)) return rc;
   }
-  // persistent kernel: two 128-row halves per tile when that still leaves at least one full wave of tiles
-  m128 = m_tiles;
-  g.mh = (!pair && conv_variant() == 3 && ((m128 + 1) / 2) * g.n_tiles >= kNumSMs) ? 2 : 1;
-  if (const char* e = getenv("STEP_B200_MH")) { if (!pair) { if (e[0] == '1') g.mh = 1; else if (e[0] == '2') g.mh = 2; } }
-  {
-    int ncols = 32;
-    while (ncols < g.BN) ncols <<= 1;
-    g.tmem_bufs = (g.mh * ncols * 2 <= 512) ? 2 : 1;
-    g.res_tma = (persist && p->residual && g.mh == 1 && mode == A_LINEAR && g.BN % 64 == 0 && p->Cout % 64 == 0) ? 1 : 0;
-    g.res_bufs = g.BN > 128 ? 1 : 2;
-    const size_t res_bytes = g.res_tma ? (size_t)g.res_bufs * (g.BN / 64) * kBM * 128 + 1024 : 0;
-    const size_t budget = 227 * 1024 - kBookBytesP - 1024 - (size_t)kEpiWarps * kSlabBytes - res_bytes;
-    const size_t stage_bytes = (size_t)g.mh * kBM * BK * 2 + (size_t)(pair ? g.BN / 2 : g.BN) * BK * 2;
-    int st = (int)(budget / stage_bytes);
-    g.n_stages_p = st > kMaxStagesP ? kMaxStagesP : st;
-    if (const char* e = getenv("STEP_B200_STAGES")) { int v = atoi(e); if (v >= 2 && v < g.n_stages_p) g.n_stages_p = v; }
-    STEP_CHECK_ARG(g.n_stages_p >= 2, "conv3d(f16): tile does not fit shared memory");
-    g.cluster = 1;
-    {
-      const char* e = getenv("STEP_B200_CLUSTER");
-      // measured (tools/conv_bench.py, STEP_B200_CLUSTER=1|2): no gain on B200 -- the wide-N 1x1x1 layers are not
-      // bound by the weight traffic out of L2 -- so the multicast path is opt-in (validated by tests/test_gpu_conv.py)
-      const bool want = e ? (e[0] == '2') : false;
-      if (want && !pair && persist && g.mh == 1 && m128 >= 2 * 74 && g.BN >= 64 && (g.BN / 2) % 8 == 0) g.cluster = 2;
-    }
-    pl->persist_tiles = (pair || g.cluster == 2) ? (int)(((m128 + 1) / 2) * g.n_tiles) : (int)(((m128 + g.mh - 1) / g.mh) * g.n_tiles);
-    if (pair) g.idesc = (1u << 4) | ((uint32_t)(g.BN >> 3) << 17) | ((uint32_t)((2 * kBM) >> 4) << 24);   // M = 256 across the pair
-    // epilogue column split between the two warp groups (mh == 1) and the store path
-    {
-      const char* e = getenv("STEP_B200_TMAST");
-      g.tma_store = (persist && mode != A_BOX && !(e && e[0] == '0')) ? 1 : 0;
-      if (g.tma_store) {
-        g.col_split = g.BN < 32 ? g.BN : (g.BN / 2 + 31) / 32 * 32;   // 32-column passes: keep the 16-wide tail to one group
-      } else {
-        g.col_split = ((g.BN / 16 + 1) / 2) * 16;
-      }
-      // 32-column boxes (half the bulk-store requests) when no box can straddle a destination or the next N tile
-      g.st_w = 16;
-      if (g.tma_store && (g.n_tiles == 1 || g.BN % 32 == 0) && !(getenv("STEP_B200_STW") && atoi(getenv("STEP_B200_STW")) == 16)) {
-        bool ok = true;
-        for (int i = 0; i < p->n_splits; ++i) ok = ok && p->split[i] % 32 == 0;
-        if (ok) g.st_w = 32;
-      }
-      for (int d = 0; d < 3; ++d) pl->map_y[d] = pl->map_b;   // placeholders
-      if (g.tma_store) {
-        STEP_CHECK_ARG(g.M < (1LL << 31), "conv3d(f16): M too large");
-        for (int d = 0; d <= p->n_splits; ++d) {
-          const int ds = d ? p->split[d - 1] : 0, de = d < p->n_splits ? p->split[d] : p->Cout;
-          __half* base = d ? (__half*)p->y_extra[d - 1] + p->coff_extra[d - 1] : (__half*)p->y + p->out_coff;
-          const int ld = d ? p->ld_extra[d - 1] : p->out_ld;
-          cuuint64_t ydims[2] = {(cuuint64_t)(de - ds), (cuuint64_t)g.M};
-          cuuint64_t ystr[1] = {(cuuint64_t)ld * 2};
-          cuuint32_t ybox[2] = {(cuuint32_t)g.st_w, 32};
-          const cuuint32_t ones2[2] = {1, 1};
-          CUresult cy = g_encode_tiled(&pl->map_y[d], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, ydims, ystr, ybox, ones2,
-                                       CU_TENSOR_MAP_INTERLEAVE_NONE, g.st_w == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B,
-                                       CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-          if (cy != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(f16): tensor map (output %d) encode failed: CUresult %d", d, (int)cy);
-        }
-      }
-    }
-    pl->map_bh = pl->map_b;
-    if (g.cluster == 2 || pair) {
-      cuuint64_t bdims[3] = {(cuuint64_t)p->Cin, (cuuint64_t)taps, (cuuint64_t)p->Cout};
-      cuuint64_t bstr[2] = {(cuuint64_t)p->w_ld * 2, (cuuint64_t)taps * p->w_ld * 2};
-      cuuint32_t bbox[3] = {(cuuint32_t)BK, 1, (cuuint32_t)(g.BN / 2)};
-      const cuuint32_t ones3[3] = {1, 1, 1};
-      CUresult cr3 = g_encode_tiled(&pl->map_bh, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)p->w, bdims, bstr, bbox, ones3,
-                                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(BK), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (cr3 != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(f16): tensor map (B half) encode failed: CUresult %d", (int)cr3);
-    }
-    pl->persist_smem = kBookBytesP + 1024 + (size_t)g.n_stages_p * stage_bytes + (size_t)kEpiWarps * kSlabBytes + res_bytes;
-    if (g.res_tma) {
-      cuuint64_t rdims[2] = {(cuuint64_t)p->Cout, (cuuint64_t)g.M};
-      cuuint64_t rstr[1] = {(cuuint64_t)p->res_ld * 2};
-      cuuint32_t rbox[2] = {64, (cuuint32_t)kBM};
-      const cuuint32_t ones2[2] = {1, 1};
-      CUresult cr2 = g_encode_tiled(&pl->map_r, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)((const __half*)p->residual + p->res_coff),
-                                    rdims, rstr, rbox, ones2, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (cr2 != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(f16): tensor map (residual) encode failed: CUresult %d", (int)cr2);
-    } else {
-      pl->map_r = pl->map_b;   // unused placeholder
-    }
-  }
+  if (!two) st = (int)((227L * 1024 - fixed) / per_stage);
+  g.n_stages = st > kStages ? kStages : st;
+  STEP_CHECK_ARG(g.n_stages >= 2, "conv3d(f16): tile does not fit shared memory");
+  const long stage_area = g.n_stages * per_stage;
+  pl->smem_bytes = (size_t)(fixed + (stage_area > out_tile ? stage_area : out_tile));
   return 0;
 }
 
-template <int BK, bool kHasRes>
+template <int BK, int NCH>
 static int launch_bk(const ConvPlan& pl, const step_conv_params* p, cudaStream_t s) {
   static std::atomic<unsigned long long> attr_seen{0};
   if (first_use_on_device(attr_seen)) {
-    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BK, kHasRes>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BK, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return fail((int)e, "conv3d(f16): smem attribute: %s", cudaGetErrorString(e));
   }
   cudaLaunchConfig_t cfg = {};
@@ -1201,78 +488,31 @@ static int launch_bk(const ConvPlan& pl, const step_conv_params* p, cudaStream_t
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
   }
-  cudaError_t le = cudaLaunchKernelEx(&cfg, conv_umma_kernel<BK, kHasRes>, pl.map_a, pl.map_b, pl.g, p->scale, p->shift,
+  cudaError_t le = cudaLaunchKernelEx(&cfg, conv_umma_kernel<BK, NCH>, pl.map_a, pl.map_b, pl.g, p->scale, p->shift,
                                       (const __half*)p->residual, (__half*)p->y);
   if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "conv_umma_kernel launch: %s", cudaGetErrorString(le)); }
   STEP_LAUNCH_CHECK("conv_umma_kernel");
   return 0;
 }
 
-template <int BK, bool kHasRes, bool kPair>
-static int launch_persist(const ConvPlan& pl, const step_conv_params* p, cudaStream_t s) {
-  static std::atomic<unsigned long long> attr_seen{0};
-  if (first_use_on_device(attr_seen)) {
-    cudaError_t e = cudaFuncSetAttribute(conv_umma_persist_kernel<BK, kHasRes, kPair>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return fail((int)e, "conv3d(f16): smem attribute: %s", cudaGetErrorString(e));
-  }
-  const int total = pl.persist_tiles;
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (pl.g.cluster == 2 || kPair) {
-    const int pairs = total < kNumSMs / 2 ? total : kNumSMs / 2;
-    cfg.gridDim = dim3(2 * pairs);
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = 2; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-    ++na;
-  } else {
-    cfg.gridDim = dim3(total < kNumSMs ? total : kNumSMs);
-  }
-  if (pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr; cfg.numAttrs = na;
-  cfg.blockDim = dim3(kThreadsP);
-  cfg.dynamicSmemBytes = pl.persist_smem;
-  cfg.stream = s;
-  cudaError_t le = cudaLaunchKernelEx(&cfg, conv_umma_persist_kernel<BK, kHasRes, kPair>, pl.map_a, pl.map_b, pl.map_r, pl.map_bh, pl.map_y[0], pl.map_y[1],
-                                      pl.map_y[2], pl.g,
-                                      total, p->scale, p->shift, (const __half*)p->residual, (__half*)p->y);
-  if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "conv_umma_persist_kernel launch: %s", cudaGetErrorString(le)); }
-  STEP_LAUNCH_CHECK(kPair ? "conv_umma_persist_kernel(pair)" : "conv_umma_persist_kernel");
-  return 0;
+template <int NCH>
+static int launch_nch(const ConvPlan& pl, const step_conv_params* p, cudaStream_t s) {
+  if (pl.BK == 64) return launch_bk<64, NCH>(pl, p, s);
+  if (pl.BK == 32) return launch_bk<32, NCH>(pl, p, s);
+  return launch_bk<16, NCH>(pl, p, s);
 }
 
 int conv3d_umma_launch(const step_conv_params* p, step_stream_t stream) {
   ConvPlan pl;
   if (int rc = build_plan(p, &pl)) return rc;
-  const bool res = p->residual != nullptr;
-  // Measured per layer (tools/conv_bench.py, profiles/): the persistent kernel wins on 1x1x1 filters (short K
-  // loops: per-CTA setup + epilogue dominate, wide N tiles); for k > 1 the one-tile-per-CTA kernel with 2-5
-  // co-resident CTAs per SM keeps more TMA requests in flight and wins, by 2x on the BK=32 stem.
-  // STEP_B200_CONV=1 forces one-tile-per-CTA everywhere, =3 forces the persistent kernel everywhere.
-  if (pl.pair) {
-    if (pl.BK == 64) return res ? launch_persist<64, true, true>(pl, p, cu(stream)) : launch_persist<64, false, true>(pl, p, cu(stream));
-    if (pl.BK == 32) return res ? launch_persist<32, true, true>(pl, p, cu(stream)) : launch_persist<32, false, true>(pl, p, cu(stream));
-    return res ? launch_persist<16, true, true>(pl, p, cu(stream)) : launch_persist<16, false, true>(pl, p, cu(stream));
-  }
-  if (pl.persist) {
-    if (pl.BK == 64) return res ? launch_persist<64, true, false>(pl, p, cu(stream)) : launch_persist<64, false, false>(pl, p, cu(stream));
-    if (pl.BK == 32) return res ? launch_persist<32, true, false>(pl, p, cu(stream)) : launch_persist<32, false, false>(pl, p, cu(stream));
-    return res ? launch_persist<16, true, false>(pl, p, cu(stream)) : launch_persist<16, false, false>(pl, p, cu(stream));
-  }
-  if (pl.BK == 64) return res ? launch_bk<64, true>(pl, p, cu(stream)) : launch_bk<64, false>(pl, p, cu(stream));
-  if (pl.BK == 32) return res ? launch_bk<32, true>(pl, p, cu(stream)) : launch_bk<32, false>(pl, p, cu(stream));
-  return res ? launch_bk<16, true>(pl, p, cu(stream)) : launch_bk<16, false>(pl, p, cu(stream));
+  return pl.g.BN == 64 ? launch_nch<1>(pl, p, cu(stream)) : launch_nch<2>(pl, p, cu(stream));
 }
 
 }  // namespace step
 
 using namespace step;
 
-// Test hook (tests/test_conv_umma.py): raw bytes of one staged A tile -> out [128 * BK * 2].
+// Test hook (tests/test_gpu_conv.py): raw bytes of one staged A tile -> out [128 * BK * 2].
 extern "C" int step_debug_tma_tile(const step_conv_params* p, int m_tile, int kt, int kh, int kw, int c0, void* out,
                                    int* bk_out, int* box_out /*[3]*/, step_stream_t stream) {
   ConvPlan pl;

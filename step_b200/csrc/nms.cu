@@ -1,4 +1,4 @@
-// nms.cu -- bit-exact greedy NMS on sm_100a, fully device resident.
+// nms.cu -- bit-exact greedy NMS on sm_90a, fully device resident.
 //
 // Replaces _C.nms (external/maskrcnn_benchmark/csrc/nms.h:34-51).  The semantics every reference
 // driver exercises are the CPU ones (test.py:192 calls nms on CPU tensors): legacy "+1" areas,

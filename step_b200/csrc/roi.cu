@@ -1,4 +1,4 @@
-// roi.cu -- ROIAlign / ROIPool for sm_100a.
+// roi.cu -- ROIAlign / ROIPool for sm_90a.
 //
 // Replaces _C.roi_align_forward/backward and _C.roi_pool_forward/backward
 // (external/maskrcnn_benchmark/csrc/vision.cpp:32-35).  Arithmetic follows
@@ -290,7 +290,7 @@ __global__ void __launch_bounds__(256) roi_align_fwd_nhwc_kernel(const T* __rest
 }
 
 
-// fp16 "packed" fast path.  Two observations from the C3 profile (profiles/): the direct form is bound by
+// fp16 "packed" fast path.  Two observations from profiling the C3 shape: the direct form is bound by
 // instruction issue and by the L1 data path (4 taps x g^2 samples = ~10 sixteen-byte loads per 16-byte output).
 //  (1) the g^2 samples of a bin hit only <= (g+1)^2 distinct pixels: their bilinear weights are merged per
 //      pixel (in fp32, with the 1/count factor) when the per-ROI table is built -> ~5.5 instead of ~10 loads;
@@ -428,7 +428,6 @@ __global__ void __launch_bounds__(256) roi_align_fwd_nhwc_f16_packed_kernel(cons
   __syncthreads();
   // Gather: an item is (bin, V channel vectors a V-th of a row apart): the 8-byte table entry (pixel offset, merged
   // weight) is read once for V 16-byte vectors, and two entries are in flight per iteration (2V independent loads).
-  // (measured on C3: V = 2 -> 0.575 of HBM peak, V = 4 -> 0.564, V = 1 -> 0.46)
   if ((nvec & 1) == 0) roi_gather_items<2>(bins, nbins, nvec, fbase, obase, out_ld, part, parts);
   else roi_gather_items<1>(bins, nbins, nvec, fbase, obase, out_ld, part, parts);
 }
@@ -550,8 +549,8 @@ extern "C" int step_roi_align_fwd_nhwc(const void* feat, int dtype, int K, int H
   FrameMap fm{roi_T, feat_T, t_start};
   if (dtype == STEP_F16 && exact == 0 && (size_t)ph * pw * sizeof(MergedBin) <= 48 * 1024 &&
       (long long)H * W * feat_ld < (1LL << 31)) {   // table entries hold 32-bit element offsets inside one frame
-    // One CTA per ROI row.  Splitting a row's channels over several CTAs (STEP_B200_ROI_PARTS=2|4, kept for A/B) was measured on
-    // the 704-row in-pipeline call and is slower (45 -> 59 us): every part rebuilds the row's tap table.
+    // One CTA per ROI row by default.  Splitting a row's channels over several CTAs (STEP_B200_ROI_PARTS=2|4, kept for A/B)
+    // makes every part rebuild the row's tap table.
     int parts = 1;
     if (const char* e = getenv("STEP_B200_ROI_PARTS")) {
       const int nvec = C / 8, hv = (nvec & 1) == 0 ? nvec / 2 : nvec, v = atoi(e);

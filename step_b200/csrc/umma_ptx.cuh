@@ -1,5 +1,5 @@
-// umma_ptx.cuh -- thin PTX wrappers shared by the tcgen05 kernels (mbarrier, TMA loads / stores, UMMA descriptors,
-// tcgen05.mma / commit / ld).  sm_100a only.
+// umma_ptx.cuh -- thin PTX wrappers shared by the tensor-core kernels (mbarrier, TMA loads / stores, wgmma descriptors and
+// instructions).  sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -16,6 +16,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
@@ -27,8 +30,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// named barrier over the `n` threads of the consumer warpgroups (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -48,57 +51,48 @@ __device__ __forceinline__ void tma_load_im2col_5d(const CUtensorMap* map, uint6
   asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2], {%8, %9, %10};"
                ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(d), "r"(n), "h"(ow), "h"(oh), "h"(od) : "memory");
 }
-
-// smem matrix descriptor, K-major, swizzled (cute/arch/mma_sm100_desc.hpp bit layout):
-// [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major) | [32,46) SBO>>4 | [46,48) version=1 |
-// [49,52) base offset | [61,64) layout (2 = 128B, 4 = 64B, 6 = 32B swizzle)
-template <int BK>
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  constexpr uint32_t row_bytes = BK * 2;
-  constexpr uint64_t layout = row_bytes == 128 ? 2 : (row_bytes == 64 ? 4 : 6);
-  constexpr uint64_t sbo = (8 * row_bytes) >> 4;  // 8-row core-matrix group pitch
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (sbo << 32) | (1ULL << 46) | (layout << 61);
-}
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
 // bulk tensor store shared -> global (2-D map, coordinates {column, row}); out-of-range elements are not written
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+// wgmma shared-memory matrix descriptor (PTX ISA, "Matrix Descriptor Format" for wgmma):
+// [0,14) start >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4 | [62,64) swizzle
+// (0 none, 1 = 128B, 2 = 64B, 3 = 32B).  K-major swizzled tiles as TMA writes them: rows of BK fp16, SBO = 8-row group pitch,
+// LBO unused (1); advancing K by 16 elements inside the swizzle atom adds 32 bytes to the start address.
+template <int BK>
+__device__ __forceinline__ uint64_t desc_hi_kmajor() {
+  constexpr uint64_t sw = BK == 64 ? 1 : (BK == 32 ? 2 : 3);
+  return (1ULL << 16) | ((uint64_t)((8 * BK * 2) >> 4) << 32) | (sw << 62);
+}
+__device__ __forceinline__ uint64_t desc_lo(const void* p) { return (uint64_t)((smem_u32(p) & 0x3FFFF) >> 4); }
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp16 inputs, fp32 accumulator in 32 registers per thread of the warpgroup:
+// d[4 j + 2 i + c] = row (warp % 4) * 16 + lane / 4 + 8 i, column 8 j + 2 (lane % 4) + c.
+__device__ __forceinline__ void wgmma_64x64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
 
 // Programmatic dependent launch (cudaLaunchAttributeProgrammaticStreamSerialization): a kernel launched with the attribute
-// may start while its predecessor in the stream is still running; everything up to pdl_wait() (barrier init, TMEM
-// allocation, descriptor prefetch, constant loads) overlaps the predecessor's tail.  pdl_wait() returns once the
-// predecessor grid has completed and its writes are visible; pdl_launch_dependents() lets the NEXT kernel start early.
+// may start while its predecessor in the stream is still running; everything up to pdl_wait() (barrier init, descriptor
+// prefetch, constant loads) overlaps the predecessor's tail.  pdl_wait() returns once the predecessor grid has completed
+// and its writes are visible; pdl_launch_dependents() lets the NEXT kernel start early.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 

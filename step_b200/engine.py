@@ -31,7 +31,7 @@ STEM_HALO = os.environ.get("STEP_B200_STEM_HALO", "1") != "0"
 # side streams: at these shapes one branch often has < 148 tiles, so overlapping the four branches is what
 # fills the SMs.  Under CUDA-graph capture the fork/join events become graph edges.
 BRANCH_STREAMS = os.environ.get("STEP_B200_BRANCH_STREAMS", "1") != "0"
-FUSE_1X1 = os.environ.get("STEP_B200_FUSE_1X1", "1") != "0" and os.environ.get("STEP_B200_CONV", "2") != "1"
+FUSE_1X1 = os.environ.get("STEP_B200_FUSE_1X1", "1") != "0"
 _side_streams = {}
 
 

@@ -129,7 +129,7 @@ class _ROIAlign(Function):
         rois = roi.detach().to(torch.float32).contiguous()
         R = rois.shape[0]
         if input.dtype == torch.float64:
-            raise RuntimeError("roi_align: float64 is not supported by the sm_100a kernels")
+            raise RuntimeError("roi_align: float64 is not supported by the sm_90a kernels")
         if _is_channels_last(input) and input.dtype in (torch.float16, torch.float32) and C % 8 == 0:
             # channels-last storage (our own modules produce it): fast path, output keeps the layout
             ld = input.stride(3)

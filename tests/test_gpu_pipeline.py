@@ -3,7 +3,7 @@ unmodified reference on seeded synthetic inputs) and the oracle.
 
 Tolerances (SURVEY.md section 8c):
   fp32 path (cfg.fp16=False, SIMT):  atol = 1e-4 * max|ref|, rtol = 1e-4   (accumulation order only)
-  fp16 path (cfg.fp16=True, tcgen05, fp32 accumulate): max-abs <= 2e-2 * max|ref| at the trunk output,
+  fp16 path (cfg.fp16=True, wgmma, fp32 accumulate): max-abs <= 2e-2 * max|ref| at the trunk output,
       mean-relative <= 1e-2; sigmoid scores <= 5e-3 abs; boxes <= 1.5 px.
 """
 import numpy as np
@@ -237,8 +237,8 @@ def test_c4_bench_batch_matches_reference_golden(golden, fp16):
     """The exact batch bench.py times (B=8 clips of T=32 x 224 x 224, 11 proposals, 3 steps, seeded) against the
     reference's outputs for clips 0 and 7 (tests/golden/pipe_c4.npz): trunk features, scores, boxes, neighbour boxes
     and proposals of every refinement step.  At B=8 every conv layer takes the dispatch branch the benchmark takes
-    (persistent / pair kernels with one CTA per SM, the shared-memory patch kernel at grid 3136, deep single-CTA
-    pipelines, multiple N tiles), so a wrong branch fails here.  Through the CUDA-graph runner on the fp16 path."""
+    (the implicit-GEMM kernel in its LINEAR / IM2COL modes with one and several N tiles and horizontally fused outputs,
+    the shared-memory patch kernel of the stem, the fused bottleneck exit), so a wrong branch fails here.  Through the CUDA-graph runner on the fp16 path."""
     import step_b200
     g = golden("pipe_c4")
     cfg = synth.make_cfg(fp16=fp16, **C4)
@@ -445,8 +445,7 @@ def test_fused_bottleneck_exit_does_not_change_the_pipeline(golden):
 def test_bench_with_three_batches_in_flight_completes():
     """bench.py's measured configuration (CUDA graphs, three batches in flight on separate streams) runs to completion and
     prints its JSON line.  A kernel that only works when it has the GPU to itself shows up here as a timeout: an
-    experimental variant of the fused bottleneck exit passed every single-stream test and stalled exactly this run
-    (tools/experiments/README.md)."""
+    experimental variant of the fused bottleneck exit once passed every single-stream test and stalled exactly this run."""
     import json
     import os
     import subprocess

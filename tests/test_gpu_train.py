@@ -217,7 +217,7 @@ def test_linear_backward_matches_matmul():
 
 def test_head_backward_every_parameter_matches_reference_autograd(golden):
     """The whole head of one refinement step, forward + losses + backward on the device (training.head_forward_backward:
-    tcgen05 dgrad through the forward kernels on transposed filters, tensor-core wgrad, max-pool / ReLU / BatchNorm-scale /
+    wgmma dgrad through the forward kernels on transposed filters, tensor-core wgrad, max-pool / ReLU / BatchNorm-scale /
     temporal-mean / linear backward), against the gradients the reference's autograd produced for the same seeded case
     (tests/golden/head_grads.npz: loss, per-parameter gradient norm and leading values for every trainable tensor (34: BatchNorm affine is frozen), and
     the gradient w.r.t. the pooled ROI features).  fp16 activations and activation gradients: gradient norms within 1e-2, full tensors within 8e-2 relative L2 (measured worst 4.5e-2: rounding noise of fp16 operands in sums of ~10^3 products)."""

@@ -74,60 +74,55 @@ def test_oracle_same_pad_table():
     assert E.same_pad(7, 2) == (2, 3) and E.same_pad(1, 1) == (0, 0)
 
 
-@pytest.mark.refonly
-def test_compat_patch_substitutes_the_names_the_reference_drivers_import():
-    """Build container only (needs /root/reference): after compat.patch(<reference root>) the reference's own import
-    lines (test.py:19-25) resolve to step_b200, and its utils.utils.inference IS ours -- without editing a reference file."""
-    import os
+def _stub_reference_tree(root):
+    """The part of the reference tree (NVlabs/STEP) that compat.patch() and the drivers' import lines touch: a `utils`
+    package whose utils.py defines `inference` next to helpers the drivers keep, and a tube_utils.py of host helpers."""
+    u = root / "utils"
+    u.mkdir()
+    (u / "__init__.py").write_text("")
+    (u / "utils.py").write_text("def inference(*args, **kwargs):\n    raise NotImplementedError('reference inference')\n\n"
+                                "def get_gpu_memory():\n    return 0\n")
+    (u / "tube_utils.py").write_text("def flatten_tubes(tubes, batch_idx=False):\n    return tubes\n\n"
+                                     "def valid_tubes(tubes, width=400, height=400):\n    return tubes\n")
+
+
+def test_compat_patch_substitutes_the_names_the_reference_drivers_import(tmp_path):
+    """After compat.patch(<reference root>) the reference's own import lines (test.py:19-25) resolve to step_b200, its
+    utils.utils.inference IS ours while the rest of utils.utils and utils.tube_utils stay the reference's own -- without
+    editing a reference file.  The reference root is a stub tree with the same module layout."""
     import sys
-    if not os.path.isdir("/root/reference/models"):
-        pytest.skip("reference tree not present")
     import step_b200
     import step_b200.compat as compat
+    _stub_reference_tree(tmp_path)
     saved = dict(sys.modules)
     saved_path = list(sys.path)
     try:
         for k in [k for k in sys.modules if k == "models" or k.startswith("models.") or k.startswith("external") or k == "utils" or k.startswith("utils.")]:
             del sys.modules[k]
-        compat.patch("/root/reference")
+        compat.patch(str(tmp_path))
         ns = {}
         exec("from models import BaseNet, ROINet, TwoBranchNet, ContextNet\n"
              "from external.maskrcnn_benchmark.roi_layers import nms\n"
              "from utils.utils import inference\n"
              "from utils.tube_utils import flatten_tubes, valid_tubes", ns)          # the import lines of test.py:19-25
         assert ns["BaseNet"] is step_b200.BaseNet and ns["TwoBranchNet"] is step_b200.TwoBranchNet
+        assert ns["ROINet"] is step_b200.ROINet and ns["ContextNet"] is step_b200.ContextNet
         assert ns["nms"] is step_b200.roi_layers.nms and ns["inference"] is step_b200.inference
+        assert sys.modules["utils.utils"].__file__.startswith(str(tmp_path))        # the caller's utils.utils, patched
+        assert sys.modules["utils.utils"].get_gpu_memory() == 0                      # ... keeping its other names
         assert ns["valid_tubes"].__module__ == "utils.tube_utils"                    # host helpers stay the reference's own
-        cfg = __import__("step_b200.synth", fromlist=["x"]).make_cfg()
+        assert ns["flatten_tubes"].__module__ == "utils.tube_utils"
+        cfg = synth.make_cfg()
         net = ns["TwoBranchNet"](cfg)
-        net.load_state_dict(__import__("step_b200.synth", fromlist=["x"]).head_state_dict(100, cfg), strict=True)
+        net.load_state_dict(synth.head_state_dict(100, cfg), strict=True)
         with pytest.raises(RuntimeError):                                            # no CPU fallback on the hot path
-            net(__import__("torch").zeros(1, 8, 832, 7, 7))
+            net(torch.zeros(1, 8, 832, 7, 7))
     finally:
         sys.path[:] = saved_path
         for k in list(sys.modules):
             if k not in saved:
                 del sys.modules[k]
         sys.modules.update(saved)
-
-
-def test_fused_exit_barrier_protocol_survives_adversarial_interleavings():
-    """tools/protocol_sim.py replays the mbarrier protocol of the fused bottleneck-exit kernel (csrc/bottleneck_exit.cu: TMA
-    producers, two MMA-issuing threads, eight epilogue warps per CTA of the pair, asynchronous commit / complete_tx
-    deliveries) under random and skewed schedules: no schedule may end blocked (a deadlock or a parity overrun)."""
-    import importlib.util
-    import os
-    spec = importlib.util.spec_from_file_location(
-        "protocol_sim", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools", "protocol_sim.py"))
-    sim = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(sim)
-    slow_cta = lambda n: isinstance(n, tuple) and len(n) > 1 and n[1] == 1
-    for skew in (None, slow_cta):
-        for p_deliver in (0.25, 0.0):
-            for store_y in (True, False):
-                for seed in range(4):
-                    res, info = sim.simulate("v3", seed, tiles=2, store_y=store_y, skew=skew, p_deliver=p_deliver)
-                    assert res == "ok", (res, info)
 
 
 def test_fused_exit_dispatch_rule():

@@ -1,5 +1,5 @@
 """Time individual conv layers of the C4 workload through the C ABI (CUDA events, 20 reps after 3 warm-ups).
-Knobs via env: STEP_B200_CONV (1 = one tile per CTA, 2 = persistent), STEP_B200_MH, STEP_B200_STAGES, STEP_B200_AMODE."""
+Knobs via env: STEP_B200_AMODE."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -75,4 +75,4 @@ for name in names:
             ref = ref + r.buf[:n_s].float()
         ref = torch.relu(ref)
         err = float((out.buf[:n_s].float() - ref).abs().max() / ref.abs().max())
-    print("%-10s %8.1f us  %7.1f TFLOP/s  %4.1f%% of 1451 (algorithmic %.1f GFLOP)  rel_err %.1e" % (name, us, gf / us * 1e3, gf / us * 1e3 / 14.511, gf, err))
+    print("%-10s %8.1f us  %7.1f TFLOP/s  %4.1f%% of 989 (H100 SXM data sheet; algorithmic %.1f GFLOP)  rel_err %.1e" % (name, us, gf / us * 1e3, gf / us * 1e3 / 9.89, gf, err))

@@ -1,9 +1,9 @@
-"""BASELINE.json configs 2 and 3 on one B200 (CUDA events, >= 5 warm-ups, inputs larger than L2 or L2 flushed).
+"""BASELINE.json configs 2 and 3 on one H100 (CUDA events, >= 5 warm-ups, inputs larger than L2 or L2 flushed).
 
   C2  I3D trunk only, batch 4, T=32, 224x224, fp16 storage / fp32 accumulate      -> clips/s, TFLOP/s, frac of bf16 peak
   C3a ROIAlign, 10 000 tubes x T'=8 = 80 000 ROI rows over a [64,14,14,832] map     -> GB/s of algorithmic bytes, frac of HBM peak
   C3b NMS, the 10 000 tube boxes, thr 0.4 (bit-exact vs the oracle)                 -> ms, boxes/s
-Prints one JSON object; `python tools/microbench.py > profiles/microbench_r1.json`."""
+Prints one JSON object; `python tools/microbench.py > microbench.json`."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -15,7 +15,7 @@ from step_b200.roi_layers import nms
 
 PEAKS = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
     if os.path.exists(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")) else \
-    {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+    {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}   # H100 SXM data sheet (700 W)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 
 
