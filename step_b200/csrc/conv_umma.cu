@@ -15,10 +15,12 @@
 //       IM2COL  k>1: TMA im2col mode walks 128 consecutive output pixels (w->h->t->n) inside the
 //               padded bounding box; dense M tiles on any map size.
 //   B (weights, [Cout, taps, Cin] fp16, K-major rows = output channels): 3-D map, box (BK,1,BN).
-//   D: fp32 in registers; consumer warpgroup w owns rows [64 w, 64 w + 64) x BN columns (BN = 64 | 128: 32 | 64 registers).
+//   D: fp32 in registers; consumer warpgroup w owns rows [64 w, 64 w + 64) x BN columns (BN / 2 registers), and issues one
+//      m64nBNk16 wgmma per 16-element K step.  BN is sized to Cout (up to 256, see pick_tile).
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread of warp 0) and the epilogue constants,
-// warpgroups 1, 2 = wgmma consumers + epilogue.  Pipeline: n_stages smem stages with full / empty mbarriers; the
-// stage area is reused as the fp16 output staging tile once both consumers are done with it.
+// warpgroups 1, 2 = wgmma consumers + epilogue; for BN > 128 the producer warpgroup hands registers to the consumers
+// (setmaxnreg).  Pipeline: n_stages smem stages with full / empty mbarriers; the stage area is reused as the fp16 output
+// staging tile once both consumers are done with it.
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -31,17 +33,31 @@ namespace step {
 enum { A_LINEAR = 1, A_BOX = 2, A_IM2COL = 3 };
 
 constexpr int kBM = 128;       // two m64 warpgroups
-constexpr int kMaxBN = 128;    // 64 fp32 accumulator registers per consumer thread
+constexpr int kMaxBN = 256;    // 128 fp32 accumulator registers per consumer thread
 constexpr int kStages = 8;     // barrier slots
 constexpr int kThreads = 384;
 constexpr int kConsumers = 256;
 constexpr int kBookBytes = 2 * kStages * 8 + 2 * kMaxBN * 4;  // barriers, scale, shift
+// registers per thread after the hand-over of wide tiles: 128 x 40 + 256 x 232 = 384 x 168, the launch allocation
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+
+// (BK, BN) instantiations of conv_umma_kernel: exactly the tiles pick_bk / pick_tile choose for the C4 layer table
+// (DESIGN.md section 3.1), plus (16, 64) for Cin <= 16, which the C4 step sends to the patch kernel (conv_halo.cu).  The
+// 64-column tile of each BK serves every other Cout, with padded columns.
+#define STEP_CONV_TILES(X)                                                                                         \
+  X(64, 32) X(64, 64) X(64, 128) X(64, 144) X(64, 152) X(64, 176) X(64, 192) X(64, 208) X(64, 224) X(64, 256)      \
+  X(32, 64) X(32, 128) X(32, 144) X(32, 152) X(32, 160) X(32, 208) X(32, 224)                                      \
+  X(16, 64)
+
+// byte pitch of a row of the fp16 output staging tile: BN columns plus 16 bytes, rounded up to an odd multiple of 16
+// so that the 8 rows one store instruction touches spread over the banks
+__host__ __device__ constexpr int staging_pitch(int BN) { return ((BN / 8 + 1) | 1) * 16; }
 
 struct ConvGeom {
   int mode;
   int taps, KT, KH, KW, PT, PH, PW;
   int kblocks_per_tap;          // ceil(Cin / BK); the channel tail of a tap's last block is TMA zero fill in A and B
-  int BN, n_tiles;              // N tile (64 | 128) and count
+  int BN, n_tiles;              // N tile (a STEP_CONV_TILES width) and count
   int n_stages;                 // smem pipeline depth
   int n_splits, split[2], ld_extra[2], coff_extra[2];  // fused 1x1x1 layers: extra destinations by column range
   __half* y_extra[2];
@@ -70,12 +86,14 @@ __device__ __forceinline__ long long tile_row_pixel(const ConvGeom& g, int m_til
 }
 
 // ---- the kernel -----------------------------------------------------------------------------
-template <int BK, int NCH>
+template <int BK, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, ConvGeom g,
                  const float* __restrict__ scale, const float* __restrict__ shift, const __half* __restrict__ residual,
                  __half* __restrict__ y) {
-  constexpr int BN = NCH * 64;
+  static_assert(BN % 8 == 0 && BN <= kMaxBN, "wgmma N is a multiple of 8, at most 256");
+  // more than 64 accumulators per consumer thread do not fit the even share of the register file (168 per thread)
+  constexpr bool kRealloc = BN > 128;
   constexpr int kABytes = kBM * BK * 2;
   constexpr int kBBytes = BN * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -111,9 +129,10 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   pdl_wait();                 // the producer of x (the previous kernel in the stream) has finished
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    if constexpr (kRealloc) setmaxnreg_dec<kProducerRegs>();
+    if (warp == 0 && elect_one()) {
       long long m0 = (long long)m_tile * kBM;
       int bn = 0, bt0 = 0, bh0 = 0, bw0 = 0;  // BOX origin
       if (g.mode == A_BOX) {
@@ -153,26 +172,24 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         if (++kw == g.KW) { kw = 0; if (++kh == g.KH) { kh = 0; ++kt; } }
       }
     }
-  } else if (warp >= 4) {
+  } else {
     // ===================== consumers (warpgroups 1, 2) =====================
+    if constexpr (kRealloc) setmaxnreg_inc<kConsumerRegs>();
     const int wg = (warp >> 2) - 1;              // 64-row half of the tile
     const int ct = threadIdx.x - 128;            // 0..255
     const uint64_t hi = desc_hi_kmajor<BK>();
     const uint64_t a_lo0 = desc_lo(sA + wg * 64 * BK * 2), b_lo0 = desc_lo(sB);
-    float acc[NCH * 32];
+    float acc[BN / 2];
 #pragma unroll
-    for (int i = 0; i < NCH * 32; ++i) acc[i] = 0.0f;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
     int stage = 0, prev = -1; uint32_t phase = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(&full_bar[stage], phase);
       const uint64_t a_lo = a_lo0 + (uint64_t)(stage * (kABytes >> 4)), b_lo = b_lo0 + (uint64_t)(stage * (kBBytes >> 4));
       wg_fence();
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {        // 16 elements (32 bytes) along K inside the swizzle atom per step
-#pragma unroll
-        for (int c = 0; c < NCH; ++c)
-          wgmma_64x64(acc + c * 32, hi | (a_lo + 2 * k), hi | (b_lo + (uint64_t)(c * ((64 * BK * 2) >> 4)) + 2 * k), 1u);
-      }
+      for (int k = 0; k < BK / 16; ++k)          // 16 elements (32 bytes) along K inside the swizzle atom per step
+        wgmma_f16<BN>(acc, hi | (a_lo + 2 * k), hi | (b_lo + 2 * k), 1u);
       wg_commit();
       wg_wait<1>();                              // the previous k-block's MMAs have retired: free its stage
       if (prev >= 0 && ct % 128 == 0) mbar_arrive(&empty_bar[prev]);
@@ -182,9 +199,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     wg_wait<0>();
     // both consumers are done reading the stage area: it becomes the output staging tile
     named_sync(1, kConsumers);
-    // Phase 1: registers -> scale/shift (+residual) (+relu) -> fp16 -> staging row.  Row pitch 2*BN+16 bytes is an odd
-    // multiple of 16, so the rows of one store instruction spread over the banks.
-    const int pitch = BN * 2 + 16;
+    // Phase 1: registers -> scale/shift (+residual) (+relu) -> fp16 -> staging row.
+    constexpr int pitch = staging_pitch(BN);
     const int wrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -193,7 +209,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       const __half* rrow = pix >= 0 ? residual + (size_t)pix * g.res_ld + g.res_coff + n0 : nullptr;
       uint8_t* srow = smem + (size_t)row * pitch;
 #pragma unroll
-      for (int j = 0; j < NCH * 8; ++j) {
+      for (int j = 0; j < BN / 8; ++j) {
         const int col = 8 * j + 2 * (lane & 3);
         float f0 = fmaf(acc[4 * j + 2 * i], s_scale[col], s_shift[col]);
         float f1 = fmaf(acc[4 * j + 2 * i + 1], s_scale[col + 1], s_shift[col + 1]);
@@ -291,16 +307,34 @@ static CUtensorMapSwizzle swizzle_for(int BK) {
 }
 
 // Channel block width.  A tap's last block is zero-filled past Cin and its zero 16-channel steps are multiplied, not skipped
-// (a data-dependent guard around the wgmma issue makes ptxas serialise the whole sequence), so the width is chosen by the
-// padded K it costs: e.g. Cin = 96 -> 3 blocks of 32 (no padding) rather than 2 blocks of 64 (25 % zero steps).  The zero
-// steps add exact zeros, so the choice does not change the result.
+// (a data-dependent guard around the wgmma issue makes ptxas serialise the whole sequence), so the width is the one with
+// the least padded K, the wider one on a tie: Cin = 96, 144, 160, 480, 528 -> blocks of 32 (no or less padding), 112 or
+// 1088 -> 64.  Blocks of 16 only serve Cin <= 16.  The zero steps add exact zeros, so the choice does not change the result.
 static int pick_bk(int Cin) {
-  int best = 64; long best_cost = -1;
-  const int cands[3] = {64, 32, 16};
-  for (int i = 0; i < 3; ++i) {
-    int bk = cands[i];
-    long cost = (long)((Cin + bk - 1) / bk) * (bk + 16);  // padded K plus a per-k-block overhead term
-    if (best_cost < 0 || cost < best_cost) { best = bk; best_cost = cost; }
+  if (Cin <= 16) return 16;
+  const int k64 = (Cin + 63) / 64 * 64, k32 = (Cin + 31) / 32 * 32;
+  return k32 < k64 ? 32 : 64;
+}
+
+struct ConvTile {
+  int BK, BN;
+  void (*kernel)(CUtensorMap, CUtensorMap, ConvGeom, const float*, const float*, const __half*, __half*);
+};
+static const ConvTile kTiles[] = {
+#define STEP_TILE_ENTRY(bk, bn) {bk, bn, conv_umma_kernel<bk, bn>},
+    STEP_CONV_TILES(STEP_TILE_ENTRY)
+#undef STEP_TILE_ENTRY
+};
+constexpr int kNumTiles = (int)(sizeof(kTiles) / sizeof(kTiles[0]));
+
+// N tile for Cout among the instantiated widths of this BK: the fewest padded columns, then the fewest tiles
+// (every N tile re-reads the whole A operand through L2).  E.g. 320 -> 2 x 160, 384 -> 2 x 192, 1024 -> 4 x 256.
+static int pick_tile(int BK, int Cout) {
+  int best = -1; long best_pad = 0, best_n = 0;
+  for (int i = 0; i < kNumTiles; ++i) {
+    if (kTiles[i].BK != BK) continue;
+    const long n = (Cout + kTiles[i].BN - 1) / kTiles[i].BN, pad = n * kTiles[i].BN - Cout;
+    if (best < 0 || pad < best_pad || (pad == best_pad && n < best_n)) { best = i; best_pad = pad; best_n = n; }
   }
   return best;
 }
@@ -318,33 +352,31 @@ static void pick_box(int OW, int OH, int OT, int* bw, int* bh, int* bt) {
     }
 }
 
-// Do two CTAs of conv_umma_kernel<BK, NCH> with `smem` bytes of dynamic shared memory fit one SM?  The answer depends only on
-// the instantiation (the caller derives `smem` from BK and NCH), so it is asked once per instantiation.
-template <int BK, int NCH>
-static int two_ctas_fit_t(size_t smem, bool* two) {
-  static std::atomic<int> cached{-1};
-  int v = cached.load(std::memory_order_relaxed);
-  if (v < 0) {
-    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BK, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    int n = 0;
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, conv_umma_kernel<BK, NCH>, kThreads, smem);
-    if (e != cudaSuccess) { cudaGetLastError(); return fail((int)e, "conv3d(f16): occupancy query: %s", cudaGetErrorString(e)); }
-    v = n >= 2 ? 1 : 0;
-    cached.store(v, std::memory_order_relaxed);
-  }
-  *two = v == 1;
-  return 0;
-}
+// Do two CTAs of tile `t` with `smem` bytes of dynamic shared memory fit one SM (registers included: the wide tiles that
+// re-balance registers with setmaxnreg never do)?  The answer depends only on the instantiation (the caller derives `smem`
+// from BK and BN), so it is asked once per instantiation.
+static std::atomic<int> g_two_ctas[kNumTiles];                // 0 = not asked yet, 1 = no, 2 = yes
+static std::atomic<unsigned long long> g_attr_seen[kNumTiles];
 
-static int two_ctas_fit(int BK, int NCH, size_t smem, bool* two) {
-  if (NCH == 1) return BK == 64 ? two_ctas_fit_t<64, 1>(smem, two) : (BK == 32 ? two_ctas_fit_t<32, 1>(smem, two) : two_ctas_fit_t<16, 1>(smem, two));
-  return BK == 64 ? two_ctas_fit_t<64, 2>(smem, two) : (BK == 32 ? two_ctas_fit_t<32, 2>(smem, two) : two_ctas_fit_t<16, 2>(smem, two));
+static int two_ctas_fit(int t, size_t smem, bool* two) {
+  int v = g_two_ctas[t].load(std::memory_order_relaxed);
+  if (v == 0) {
+    cudaError_t e = cudaFuncSetAttribute(kTiles[t].kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    int n = 0;
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kTiles[t].kernel, kThreads, smem);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail((int)e, "conv3d(f16): occupancy query: %s", cudaGetErrorString(e)); }
+    v = n >= 2 ? 2 : 1;
+    g_two_ctas[t].store(v, std::memory_order_relaxed);
+  }
+  *two = v == 2;
+  return 0;
 }
 
 struct ConvPlan {
   CUtensorMap map_a, map_b;
   ConvGeom g;
   int BK;
+  int tile;                     // index into kTiles
   size_t smem_bytes;
   dim3 grid;
 };
@@ -371,8 +403,8 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   pl->BK = pick_bk(p->Cin);
   const int BK = pl->BK;
   g.kblocks_per_tap = (p->Cin + BK - 1) / BK;
-  // N tile: as wide as the register accumulator allows -- every N tile re-reads the whole A operand through L2
-  g.BN = p->Cout <= 64 ? 64 : kMaxBN;
+  pl->tile = pick_tile(BK, p->Cout);
+  g.BN = kTiles[pl->tile].BN;
   g.n_tiles = (p->Cout + g.BN - 1) / g.BN;
   g.Cout = p->Cout; g.out_ld = p->out_ld; g.out_coff = p->out_coff; g.res_ld = p->res_ld; g.res_coff = p->res_coff;
   g.relu = p->relu;
@@ -457,13 +489,13 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   // as deep as the 227 KB of one SM allow.
   const long per_stage = (long)kBM * BK * 2 + (long)g.BN * BK * 2;
   const long fixed = kBookBytes + 1024;
-  const long out_tile = (long)kBM * (g.BN * 2 + 16);
+  const long out_tile = (long)kBM * staging_pitch(g.BN);
   int st = (int)((113L * 1024 - fixed) / per_stage);
   if (st > kStages) st = kStages;
   bool two = false;
   if (st >= 4) {
     const long area = st * per_stage;
-    if (int rc = two_ctas_fit(BK, g.BN / 64, (size_t)(fixed + (area > out_tile ? area : out_tile)), &two)) return rc;
+    if (int rc = two_ctas_fit(pl->tile, (size_t)(fixed + (area > out_tile ? area : out_tile)), &two)) return rc;
   }
   if (!two) st = (int)((227L * 1024 - fixed) / per_stage);
   g.n_stages = st > kStages ? kStages : st;
@@ -473,13 +505,15 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   return 0;
 }
 
-template <int BK, int NCH>
-static int launch_bk(const ConvPlan& pl, const step_conv_params* p, cudaStream_t s) {
-  static std::atomic<unsigned long long> attr_seen{0};
-  if (first_use_on_device(attr_seen)) {
-    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BK, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+int conv3d_umma_launch(const step_conv_params* p, step_stream_t stream) {
+  ConvPlan pl;
+  if (int rc = build_plan(p, &pl)) return rc;
+  const ConvTile& t = kTiles[pl.tile];
+  if (first_use_on_device(g_attr_seen[pl.tile])) {
+    cudaError_t e = cudaFuncSetAttribute(t.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return fail((int)e, "conv3d(f16): smem attribute: %s", cudaGetErrorString(e));
   }
+  cudaStream_t s = cu(stream);
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   cfg.gridDim = pl.grid; cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = pl.smem_bytes; cfg.stream = s;
@@ -488,24 +522,11 @@ static int launch_bk(const ConvPlan& pl, const step_conv_params* p, cudaStream_t
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
   }
-  cudaError_t le = cudaLaunchKernelEx(&cfg, conv_umma_kernel<BK, NCH>, pl.map_a, pl.map_b, pl.g, p->scale, p->shift,
+  cudaError_t le = cudaLaunchKernelEx(&cfg, t.kernel, pl.map_a, pl.map_b, pl.g, p->scale, p->shift,
                                       (const __half*)p->residual, (__half*)p->y);
   if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "conv_umma_kernel launch: %s", cudaGetErrorString(le)); }
   STEP_LAUNCH_CHECK("conv_umma_kernel");
   return 0;
-}
-
-template <int NCH>
-static int launch_nch(const ConvPlan& pl, const step_conv_params* p, cudaStream_t s) {
-  if (pl.BK == 64) return launch_bk<64, NCH>(pl, p, s);
-  if (pl.BK == 32) return launch_bk<32, NCH>(pl, p, s);
-  return launch_bk<16, NCH>(pl, p, s);
-}
-
-int conv3d_umma_launch(const step_conv_params* p, step_stream_t stream) {
-  ConvPlan pl;
-  if (int rc = build_plan(p, &pl)) return rc;
-  return pl.g.BN == 64 ? launch_nch<1>(pl, p, cu(stream)) : launch_nch<2>(pl, p, cu(stream));
 }
 
 }  // namespace step

@@ -73,21 +73,123 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp16 inputs, fp32 accumulator in 32 registers per thread of the warpgroup:
-// d[4 j + 2 i + c] = row (warp % 4) * 16 + lane / 4 + 8 i, column 8 j + 2 (lane % 4) + c.
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 inputs, fp32 accumulator in N / 2 registers per thread of the warpgroup:
+// d[4 j + 2 i + c] = row (warp % 4) * 16 + lane / 4 + 8 i, column 8 j + 2 (lane % 4) + c, j < N / 8.  One instruction
+// covers the whole N extent, so the 64 x 16 A slice is read from shared memory once per k16 step.  Defined for the N tile
+// widths the kernels instantiate (conv_umma.cu STEP_CONV_TILES, and 64 for the patch and bottleneck-exit kernels); the
+// accumulator operand list is spelled out per N because inline PTX takes only literal operand numbers.
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t da, uint64_t db, uint32_t accumulate);
+
+#define STEP_D4(i) "+f"(d[4 * (i)]), "+f"(d[4 * (i) + 1]), "+f"(d[4 * (i) + 2]), "+f"(d[4 * (i) + 3])
+#define STEP_WGMMA_F16(N, IA, IB, IC, REGS, ...)                                                                        \
+  template <>                                                                                                          \
+  __device__ __forceinline__ void wgmma_f16<N>(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {              \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #IC ", 0;\n\t"                                              \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 {" REGS "}, %" #IA ", %" #IB ", p, 1, 1, 0, 0;\n\t}" \
+                 : __VA_ARGS__ : "l"(da), "l"(db), "r"(accumulate));                                                    \
+  }
+STEP_WGMMA_F16(32, 16, 17, 18,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3))
+STEP_WGMMA_F16(64, 32, 33, 34,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7))
+STEP_WGMMA_F16(128, 64, 65, 66,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15))
+STEP_WGMMA_F16(144, 72, 73, 74,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+               STEP_D4(16), STEP_D4(17))
+STEP_WGMMA_F16(152, 76, 77, 78,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+               STEP_D4(16), STEP_D4(17), STEP_D4(18))
+STEP_WGMMA_F16(160, 80, 81, 82,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+               STEP_D4(16), STEP_D4(17), STEP_D4(18), STEP_D4(19))
+STEP_WGMMA_F16(176, 88, 89, 90,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, "
+               "%86, %87",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+               STEP_D4(16), STEP_D4(17), STEP_D4(18), STEP_D4(19), STEP_D4(20), STEP_D4(21))
+STEP_WGMMA_F16(192, 96, 97, 98,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, "
+               "%86, %87, %88, %89, %90, %91, %92, %93, %94, %95",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+               STEP_D4(16), STEP_D4(17), STEP_D4(18), STEP_D4(19), STEP_D4(20), STEP_D4(21), STEP_D4(22), STEP_D4(23))
+STEP_WGMMA_F16(208, 104, 105, 106,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, "
+               "%86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+               STEP_D4(16), STEP_D4(17), STEP_D4(18), STEP_D4(19), STEP_D4(20), STEP_D4(21), STEP_D4(22), STEP_D4(23),
+               STEP_D4(24), STEP_D4(25))
+STEP_WGMMA_F16(224, 112, 113, 114,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, "
+               "%86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, "
+               "%105, %106, %107, %108, %109, %110, %111",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+               STEP_D4(16), STEP_D4(17), STEP_D4(18), STEP_D4(19), STEP_D4(20), STEP_D4(21), STEP_D4(22), STEP_D4(23),
+               STEP_D4(24), STEP_D4(25), STEP_D4(26), STEP_D4(27))
+STEP_WGMMA_F16(256, 128, 129, 130,
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, "
+               "%86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, "
+               "%105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, "
+               "%122, %123, %124, %125, %126, %127",
+               STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+               STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+               STEP_D4(16), STEP_D4(17), STEP_D4(18), STEP_D4(19), STEP_D4(20), STEP_D4(21), STEP_D4(22), STEP_D4(23),
+               STEP_D4(24), STEP_D4(25), STEP_D4(26), STEP_D4(27), STEP_D4(28), STEP_D4(29), STEP_D4(30), STEP_D4(31))
+#undef STEP_WGMMA_F16
+#undef STEP_D4
+
 __device__ __forceinline__ void wgmma_64x64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
-        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(accumulate));
+  wgmma_f16<64>(d, da, db, accumulate);
 }
+
+// Move registers between the warpgroups of a warp-specialised CTA (PTX setmaxnreg): every thread of the executing
+// warpgroup must run it, and the CTA's total stays what it was launched with.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // Programmatic dependent launch (cudaLaunchAttributeProgrammaticStreamSerialization): a kernel launched with the attribute
 // may start while its predecessor in the stream is still running; everything up to pdl_wait() (barrier init, descriptor

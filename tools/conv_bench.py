@@ -1,78 +1,156 @@
-"""Time individual conv layers of the C4 workload through the C ABI (CUDA events, 20 reps after 3 warm-ups).
-Knobs via env: STEP_B200_AMODE."""
-import os, sys
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import torch
-from step_b200 import _lib as L, engine as E
-from step_b200.engine import Act
+"""Per-layer times of every convolution of the C4 step (STEP inference, batch 8, T = 32, 224 x 224, 11 proposals,
+max_iter = 3), through the same entry points the pipeline uses (CUDA events, 20 reps after 3 warm-ups).
 
-LAYERS = {
-    # name: (N, T, H, W, Cin, Cout, k, pad, residual)
-    "stem_s2d":   (8, 16, 112, 112, 32, 64, (4, 4, 4), (1, 1, 1), False),
-    "conv2c":     (8, 16, 56, 56, 64, 192, (3, 3, 3), None, False),
-    "3b_b2b":     (8, 16, 28, 28, 16, 32, (3, 3, 3), None, False),
-    "3c_b2b":     (8, 16, 28, 28, 32, 96, (3, 3, 3), None, False),
-    "4e_b2b":     (8, 8, 14, 14, 32, 64, (3, 3, 3), None, False),
-    "4f_b2b":     (8, 8, 14, 14, 32, 128, (3, 3, 3), None, False),
-    "5b_b2b":     (88, 8, 7, 7, 32, 128, (3, 3, 3), None, False),
-    "3b_b1b":     (8, 16, 28, 28, 96, 128, (3, 3, 3), None, False),
-    "3c_b1b":     (8, 16, 28, 28, 128, 192, (3, 3, 3), None, False),
-    "4c_b1b":     (8, 8, 14, 14, 112, 224, (3, 3, 3), None, False),
-    "4e_b1b":     (8, 8, 14, 14, 144, 288, (3, 3, 3), None, False),
-    "5c_b2b":     (88, 8, 7, 7, 48, 128, (3, 3, 3), None, False),
-    "4f_b1b":     (8, 8, 14, 14, 160, 320, (3, 3, 3), None, False),
-    "5b_b1b":     (88, 8, 7, 7, 160, 320, (3, 3, 3), None, False),
-    "5c_b1b":     (88, 8, 7, 7, 192, 384, (3, 3, 3), None, False),
-    "loc_1088":   (704, 1, 7, 7, 1088, 1024, (1, 1, 1), None, False),
-    "loc_3x3":    (704, 1, 7, 7, 256, 256, (1, 3, 3), None, False),
-    "loc_res":    (704, 1, 7, 7, 256, 1024, (1, 1, 1), None, True),
-    "loc_nores":  (704, 1, 7, 7, 256, 1024, (1, 1, 1), None, False),
-    "loc_1024":   (704, 1, 7, 7, 1024, 256, (1, 1, 1), None, False),
-    "5b_fused":   (88, 8, 7, 7, 832, 448, (1, 1, 1), None, False),
-    "4b_fused":   (8, 8, 14, 14, 480, 304, (1, 1, 1), None, False),
-    "conv2b":     (8, 16, 56, 56, 64, 64, (1, 1, 1), None, False),
-    "3b_fused":   (8, 16, 28, 28, 192, 176, (1, 1, 1), None, False),
-    "3c_fused":   (8, 16, 28, 28, 256, 288, (1, 1, 1), None, False),
-    "3c_b3":      (8, 16, 28, 28, 256, 64, (1, 1, 1), None, False),
-    "4c_fused":   (8, 8, 14, 14, 512, 296, (1, 1, 1), None, False),
-    "5c_fused":   (88, 8, 7, 7, 832, 624, (1, 1, 1), None, False),
-    "5b_b3":      (88, 8, 7, 7, 832, 128, (1, 1, 1), None, False),
-    "4b_b1b":     (8, 8, 14, 14, 96, 208, (3, 3, 3), None, False),
-    "4d_b1b":     (8, 8, 14, 14, 128, 256, (3, 3, 3), None, False),
-}
-names = sys.argv[1:] or list(LAYERS)
-torch.manual_seed(0)
-for name in names:
-    N, T, H, W, Cin, Cout, k, pad, res = LAYERS[name]
-    x = Act(torch.randn(N, T, H, W, Cin, device="cuda").half())
-    w = (torch.randn(Cout, k[0] * k[1] * k[2], Cin, device="cuda") / (Cin * k[0] * k[1] * k[2]) ** 0.5).half()
-    out = Act(torch.empty(N, T, H, W, Cout, device="cuda", dtype=torch.float16))
-    r = Act(torch.randn(N, T, H, W, Cout, device="cuda").half()) if res else None
-    sc = torch.ones(Cout, device="cuda"); sh = torch.zeros(Cout, device="cuda")
-    am = int(os.environ['CB_AMODE']) if os.environ.get('CB_AMODE') and k != (1, 1, 1) else None
-    f = lambda: E.conv(x, w, sc, sh, out, k, (1, 1, 1), pad, True, r, a_mode=am)
-    for _ in range(3): f()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    reps = 20
-    e0.record()
-    for _ in range(reps): f()
-    e1.record(); torch.cuda.synchronize()
-    us = e0.elapsed_time(e1) / reps * 1e3
-    gf = 2.0 * N * T * H * W * Cin * Cout * k[0] * k[1] * k[2] / 1e9
-    # spot check against torch on a sample of output pixels (tool only: the parity tests live in tests/)
-    err = -1.0
-    if os.environ.get("CB_CHECK", "1") == "1":
-        import torch.nn.functional as F
-        n_s = min(N, 2)
-        xs = x.buf[:n_s].float().permute(0, 4, 1, 2, 3)
-        ws = w.float().view(Cout, k[0], k[1], k[2], Cin).permute(0, 4, 1, 2, 3)
-        pd = pad if pad is not None else tuple(E.same_pad(kk, 1)[0] for kk in k)
-        hi = tuple(kk - 1 - q for kk, q in zip(k, pd))
-        xp = F.pad(xs, (pd[2], hi[2], pd[1], hi[1], pd[0], hi[0]))
-        ref = F.conv3d(xp, ws).permute(0, 2, 3, 4, 1)
-        if res:
-            ref = ref + r.buf[:n_s].float()
-        ref = torch.relu(ref)
-        err = float((out.buf[:n_s].float() - ref).abs().max() / ref.abs().max())
-    print("%-10s %8.1f us  %7.1f TFLOP/s  %4.1f%% of 989 (H100 SXM data sheet; algorithmic %.1f GFLOP)  rel_err %.1e" % (name, us, gf / us * 1e3, gf / us * 1e3 / 9.89, gf, err))
+    python tools/conv_bench.py [--check] [name ...]
+
+For each layer: launches per step, the kernel that runs it, algorithmic and executed (zero-padded) GMAC per launch,
+the conv_umma tile (BK, BN, number of N tiles), time per launch and TFLOP/s on the algorithmic FLOPs.  The last line
+sums time x count over the step.  The tile columns mirror pick_bk / pick_tile in step_b200/csrc/conv_umma.cu and read
+the instantiated tiles from its STEP_CONV_TILES list.  A tool, not the benchmark (bench.py)."""
+import os
+import re
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import torch  # noqa: E402
+from step_b200 import _lib as L, engine as E  # noqa: E402
+from step_b200.engine import Act  # noqa: E402
+
+TRUNK_56, TRUNK_28, TRUNK_14 = (8, 16, 56, 56), (8, 16, 28, 28), (8, 8, 14, 14)
+HEAD, LOCAL = (88, 8, 7, 7), (704, 1, 7, 7)     # 8 clips x 11 tubes, T' = 8; the local branch runs on frames
+LAYERS = [
+    # name, count per step, (N, T, H, W), Cin, Cout, k     (fused 1x1 = the Mixed block's three 1x1 branches in one GEMM)
+    ("stem_s2d",   1, (8, 16, 112, 112), 32, 64, (4, 4, 4)),
+    ("conv2b",     1, TRUNK_56, 64, 64, (1, 1, 1)),
+    ("conv2c",     1, TRUNK_56, 64, 192, (3, 3, 3)),
+    ("3b_fused",   1, TRUNK_28, 192, 176, (1, 1, 1)),
+    ("3b_b1b",     1, TRUNK_28, 96, 128, (3, 3, 3)),
+    ("3b_b2b",     1, TRUNK_28, 16, 32, (3, 3, 3)),
+    ("3b_b3",      1, TRUNK_28, 192, 32, (1, 1, 1)),
+    ("3c_fused",   1, TRUNK_28, 256, 288, (1, 1, 1)),
+    ("3c_b1b",     1, TRUNK_28, 128, 192, (3, 3, 3)),
+    ("3c_b2b",     1, TRUNK_28, 32, 96, (3, 3, 3)),
+    ("3c_b3",      1, TRUNK_28, 256, 64, (1, 1, 1)),
+    ("4b_fused",   1, TRUNK_14, 480, 304, (1, 1, 1)),
+    ("4b_b1b",     1, TRUNK_14, 96, 208, (3, 3, 3)),
+    ("4b_b2b",     1, TRUNK_14, 16, 48, (3, 3, 3)),
+    ("4b_b3",      1, TRUNK_14, 480, 64, (1, 1, 1)),
+    ("4c_fused",   1, TRUNK_14, 512, 296, (1, 1, 1)),
+    ("4c_b1b",     1, TRUNK_14, 112, 224, (3, 3, 3)),
+    ("4c_b2b",     1, TRUNK_14, 24, 64, (3, 3, 3)),
+    ("4c_b3",      1, TRUNK_14, 512, 64, (1, 1, 1)),
+    ("4d_fused",   1, TRUNK_14, 512, 280, (1, 1, 1)),
+    ("4d_b1b",     1, TRUNK_14, 128, 256, (3, 3, 3)),
+    ("4d_b2b",     1, TRUNK_14, 24, 64, (3, 3, 3)),
+    ("4d_b3",      1, TRUNK_14, 512, 64, (1, 1, 1)),
+    ("4e_fused",   1, TRUNK_14, 512, 288, (1, 1, 1)),
+    ("4e_b1b",     1, TRUNK_14, 144, 288, (3, 3, 3)),
+    ("4e_b2b",     1, TRUNK_14, 32, 64, (3, 3, 3)),
+    ("4e_b3",      1, TRUNK_14, 512, 64, (1, 1, 1)),
+    ("4f_fused",   1, TRUNK_14, 528, 448, (1, 1, 1)),
+    ("4f_b1b",     1, TRUNK_14, 160, 320, (3, 3, 3)),
+    ("4f_b2b",     1, TRUNK_14, 32, 128, (3, 3, 3)),
+    ("4f_b3",      1, TRUNK_14, 528, 128, (1, 1, 1)),
+    ("5b_fused",   3, HEAD, 832, 448, (1, 1, 1)),
+    ("5b_b1b",     3, HEAD, 160, 320, (3, 3, 3)),
+    ("5b_b2b",     3, HEAD, 32, 128, (3, 3, 3)),
+    ("5b_b3",      3, HEAD, 832, 128, (1, 1, 1)),
+    ("5c_fused",   3, HEAD, 832, 624, (1, 1, 1)),
+    ("5c_b1b",     3, HEAD, 192, 384, (3, 3, 3)),
+    ("5c_b2b",     3, HEAD, 48, 128, (3, 3, 3)),
+    ("5c_b3",      3, HEAD, 832, 128, (1, 1, 1)),
+    ("downsample", 3, HEAD, 1024, 256, (1, 1, 1)),
+    ("loc_res",    3, LOCAL, 1088, 1024, (1, 1, 1)),
+    ("loc_conv2",  3, LOCAL, 1088, 256, (1, 1, 1)),
+    ("loc_3x3",    9, LOCAL, 256, 256, (1, 3, 3)),
+    ("loc_exit",   9, LOCAL, 256, 1024, "exit"),     # bottleneck_exit: 256 -> 1024 (+x, relu) -> 256
+]
+
+
+def conv_tiles():
+    """(BK, BN) pairs of STEP_CONV_TILES in conv_umma.cu, or None for a tree without the list."""
+    src = open(os.path.join(ROOT, "step_b200", "csrc", "conv_umma.cu")).read()
+    m = re.search(r"#define STEP_CONV_TILES\(X\)(.*?)\n\n", src, re.S)
+    return [(int(a), int(b)) for a, b in re.findall(r"X\((\d+),\s*(\d+)\)", m.group(1))] if m else None
+
+
+def plan(Cin, Cout, tiles):
+    """(BK, BN, n_tiles) as build_plan picks them."""
+    bk = 16 if Cin <= 16 else (32 if -(-Cin // 32) * 32 < -(-Cin // 64) * 64 else 64)
+    best = min((-(-Cout // bn) * bn - Cout, -(-Cout // bn), bn) for b, bn in tiles if b == bk)
+    return bk, best[2], best[1]
+
+
+def kernel_of(N, T, H, W, Cin, Cout, k):
+    taps = k[0] * k[1] * k[2]
+    halo = taps > 1 and Cin in (16, 32, 64) and Cout <= 256 and Cin <= 32 and min(H, W) >= 14
+    return "halo" if halo else "umma"
+
+
+def main():
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    check = "--check" in sys.argv
+    tiles = conv_tiles()
+    torch.manual_seed(0)
+    total_ms = 0.0
+    print("%-10s %3s %4s %9s %9s %3s %4s %3s %9s %8s" % ("layer", "n", "kern", "GMAC", "exec_GMAC", "BK", "BN", "nt",
+                                                         "us", "TFLOP/s"))
+    for name, count, (N, T, H, W), Cin, Cout, k in LAYERS:
+        if args and name not in args:
+            continue
+        M = N * T * H * W
+        if k == "exit":
+            h = Act(torch.randn(N, T, H, W, Cin, device="cuda").half())
+            w3 = (torch.randn(Cout, 1, Cin, device="cuda") / Cin ** 0.5).half()
+            x = Act(torch.randn(N, T, H, W, Cout, device="cuda").half())
+            w1 = (torch.randn(Cin, 1, Cout, device="cuda") / Cout ** 0.5).half()
+            z = Act(torch.empty(N, T, H, W, Cin, device="cuda", dtype=torch.float16))
+            y = Act(torch.empty(N, T, H, W, Cout, device="cuda", dtype=torch.float16))
+            f = lambda: E.bottleneck_exit(h, w3, x, w1, None, True, z, y)
+            gmac = 2.0 * M * Cin * Cout / 1e9
+            kern, exec_gmac, tile = "exit", gmac, ("-", "-", "-")
+        else:
+            taps = k[0] * k[1] * k[2]
+            x = Act(torch.randn(N, T, H, W, Cin, device="cuda").half())
+            w = (torch.randn(Cout, taps, Cin, device="cuda") / (Cin * taps) ** 0.5).half()
+            out = Act(torch.empty(N, T, H, W, Cout, device="cuda", dtype=torch.float16))
+            sc, sh = torch.ones(Cout, device="cuda"), torch.zeros(Cout, device="cuda")
+            pad = (1, 1, 1) if name == "stem_s2d" else None
+            f = lambda: E.conv(x, w, sc, sh, out, k, (1, 1, 1), pad, True, None)
+            gmac = M * Cin * Cout * taps / 1e9
+            kern = kernel_of(N, T, H, W, Cin, Cout, k)
+            if kern == "umma" and tiles:
+                bk, bn, nt = plan(Cin, Cout, tiles)
+                exec_gmac = M * (-(-Cin // bk) * bk) * (bn * nt) * taps / 1e9
+                tile = (bk, bn, nt)
+            else:
+                exec_gmac, tile = float("nan"), ("-", "-", "-")
+        for _ in range(3):
+            f()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        reps = 20
+        e0.record()
+        for _ in range(reps):
+            f()
+        e1.record()
+        torch.cuda.synchronize()
+        us = e0.elapsed_time(e1) / reps * 1e3
+        total_ms += us * count / 1e3
+        line = "%-10s %3d %4s %9.2f %9.2f %3s %4s %3s %9.1f %8.1f" % (name, count, kern, gmac, exec_gmac, tile[0], tile[1],
+                                                                     tile[2], us, 2 * gmac / us * 1e3)
+        if check and k != "exit":   # spot check against torch on two images (tool only: the parity tests live in tests/)
+            import torch.nn.functional as F
+            xs = x.buf[:2].float().permute(0, 4, 1, 2, 3)
+            ws = w.float().view(Cout, k[0], k[1], k[2], Cin).permute(0, 4, 1, 2, 3)
+            pd = pad if pad is not None else tuple(E.same_pad(kk, 1)[0] for kk in k)
+            hi = tuple(kk - 1 - q for kk, q in zip(k, pd))
+            ref = torch.relu(F.conv3d(F.pad(xs, (pd[2], hi[2], pd[1], hi[1], pd[0], hi[0])), ws).permute(0, 2, 3, 4, 1))
+            line += "  rel_err %.1e" % float((out.buf[:2].float() - ref).abs().max() / ref.abs().max())
+        print(line, flush=True)
+    print("sum over the step (time x count): %.3f ms" % total_ms)
+
+
+if __name__ == "__main__":
+    main()
