@@ -6,18 +6,25 @@
 //     Z[M,  256] = act(Y[M, 1024] * W1[256, 1024]^T + shift2)               next conv1 (ReLU) / downsample2 (bias, no ReLU)
 //
 // As two launches of the implicit-GEMM kernel the 1024-wide Y makes a round trip through HBM between them.  Here a CTA owns
-// 64 rows and walks the 1024 columns of Y in 16 chunks of 64: consumer warpgroup (chunk & 1) computes the GEMM1 chunk with
-// wgmma (registers), adds the residual, applies the ReLU, rounds to fp16 and writes the chunk as a K-major 128B-swizzled A
-// operand into shared memory (and to Y when it is stored); then both warpgroups accumulate Z += Y_chunk * W1[:, chunk]^T, each
-// for 128 of Z's 256 columns.  Y is rounded to fp16 before GEMM2 exactly as the two-launch path rounds it, and both GEMMs issue
-// the same m64n64k16 wgmma sequence in the same K order as conv_umma.cu, so the results are bit-identical to the unfused path.
+// 128 rows; consumer warpgroup wg owns rows [64 wg, 64 wg + 64) and walks the 1024 columns of Y in 16 chunks of 64:
+//   GEMM1   acc[64 x 64] = H * W3[chunk]^T                    16 x m64n64k16, both operands in shared memory
+//   epilogue acc + residual (X chunk, TMA-loaded), ReLU, fp16 -> written back over the X chunk for the TMA store of Y, and
+//           kept in registers: accumulator registers [8 kk, 8 kk + 8) are the A fragment of k-step kk of GEMM2
+//   GEMM2   Z[64 x 256] += Y_chunk * W1[:, chunk]^T            4 x m64n256k16, A in registers, Z in 128 registers
+// GEMM1 of chunk c + 1 is issued right behind GEMM2 of chunk c.  The two consumer warpgroups share the weight rings and no
+// other barrier (a staggered start and a 2-CTA weight multicast were measured and did not pay, DESIGN.md section 3.1).
+// Y is rounded to fp16 before GEMM2 exactly as the two-launch path rounds it, and both GEMMs accumulate K in ascending
+// 16-wide steps as conv_umma.cu does, so the results are bit-identical to the unfused path.  Z is staged in the warpgroup's (then finished) rows of the H tile and stored by TMA;
+// the tensor maps clip the ragged last tile.
 //
-// Per CTA (384 threads): warp 0 loads H and the W3 chunks (TMA, 3-slot ring), warp 1 loads the W1 slices (2-slot ring),
-// warpgroups 1 and 2 compute.
+// Per CTA (384 threads): warp 0 loads H and the W3 chunks, warp 1 the W1 slices, warps 2 and 3 the X chunks of consumer
+// warpgroup 0 and 1 (TMA, one thread per ring, two slots each); warpgroups 1 and 2 compute, with the producer warpgroup's
+// registers handed to them (setmaxnreg 40 / 232).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 #include "common.cuh"
 #include "umma_ptx.cuh"
 
@@ -25,35 +32,38 @@ namespace step {
 namespace bexit {
 
 constexpr int kThreads = 384;
-constexpr int BM = 64;                          // rows per CTA
+constexpr int BM = 128;                         // rows per CTA, 64 per consumer warpgroup
 constexpr int K1 = 256, N1 = 1024, N2 = 256, CH = 64, NCH = N1 / CH;   // 16 chunks of 64 columns of Y
-constexpr int kHBytes = 4 * BM * 128;           // H tile: 4 k-blocks x [64 rows x 128 B]
+constexpr int kHBytes = 4 * BM * 128;           // H tile: 4 k-blocks x [128 rows x 128 B]
 constexpr int kW3Bytes = 4 * CH * 128;          // W3 chunk: 4 k-blocks x [64 rows x 128 B]
 constexpr int kW1Bytes = N2 * 128;              // W1 slice: [256 rows x 128 B]
-constexpr int kYBytes = BM * 128;               // Y chunk: [64 rows x 128 B]
-constexpr int kW3Ring = 3, kW1Ring = 2;
+constexpr int kXBytes = 64 * 128;               // one warpgroup's X / Y chunk: [64 rows x 128 B]
+constexpr int kRing = 2;                        // slots of every ring
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 
 struct Geom {
-  int M, store_y, relu2, x_ld, y_ld, z_ld;
+  int M, store_y, relu2;
 };
 
 struct Bars {
   uint64_t h_full;
-  uint64_t w3_full[kW3Ring], w3_empty[kW3Ring];
-  uint64_t w1_full[kW1Ring], w1_empty[kW1Ring];
+  uint64_t w3_full[kRing], w3_empty[kRing];
+  uint64_t w1_full[kRing], w1_empty[kRing];
+  uint64_t x_full[2][kRing], x_empty[2][kRing];   // per consumer warpgroup
 };
 
 __global__ void __launch_bounds__(kThreads, 1)
 bottleneck_exit_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_w3,
-                       const __grid_constant__ CUtensorMap map_w1, Geom g, const float* __restrict__ shift2,
-                       const __half* __restrict__ x, __half* __restrict__ y, __half* __restrict__ z) {
+                       const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_x,
+                       const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_z, Geom g,
+                       const float* __restrict__ shift2) {
   extern __shared__ __align__(1024) uint8_t raw[];
   Bars* bars = (Bars*)raw;
   uint8_t* base = (uint8_t*)(((uintptr_t)raw + sizeof(Bars) + 1023) & ~(uintptr_t)1023);
   uint8_t* sH = base;
   uint8_t* sW3 = sH + kHBytes;
-  uint8_t* sW1 = sW3 + kW3Ring * kW3Bytes;
-  uint8_t* sY = sW1 + kW1Ring * kW1Bytes;        // [2][kYBytes]
+  uint8_t* sW1 = sW3 + kRing * kW3Bytes;
+  uint8_t* sX = sW1 + kRing * kW1Bytes;          // [slot][warpgroup][kXBytes]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * BM;
 
@@ -61,120 +71,169 @@ bottleneck_exit_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_c
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_h) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w3) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w1) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
+    if (g.store_y) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_y) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_z) : "memory");
     mbar_init(&bars->h_full, 1);
-    for (int i = 0; i < kW3Ring; ++i) { mbar_init(&bars->w3_full[i], 1); mbar_init(&bars->w3_empty[i], 1); }
-    for (int i = 0; i < kW1Ring; ++i) { mbar_init(&bars->w1_full[i], 1); mbar_init(&bars->w1_empty[i], 2); }
+    for (int i = 0; i < kRing; ++i) {
+      mbar_init(&bars->w3_full[i], 1); mbar_init(&bars->w3_empty[i], 2);
+      mbar_init(&bars->w1_full[i], 1); mbar_init(&bars->w1_empty[i], 2);
+      for (int w = 0; w < 2; ++w) { mbar_init(&bars->x_full[w][i], 1); mbar_init(&bars->x_empty[w][i], 1); }
+    }
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();
   pdl_launch_dependents();
 
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_expect_tx(&bars->h_full, kHBytes);
-      for (int kb = 0; kb < 4; ++kb) tma_load_2d(&map_h, &bars->h_full, sH + kb * BM * 128, kb * 64, m0);
-      for (int c = 0; c < NCH; ++c) {
-        const int s = c % kW3Ring;
-        mbar_wait(&bars->w3_empty[s], ((uint32_t)(c / kW3Ring) & 1u) ^ 1u);
-        mbar_expect_tx(&bars->w3_full[s], kW3Bytes);
-        for (int kb = 0; kb < 4; ++kb)
-          tma_load_2d(&map_w3, &bars->w3_full[s], sW3 + s * kW3Bytes + kb * CH * 128, kb * 64, c * CH);
+  if (warp < 4) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == 0) {
+      if (elect_one()) {
+        mbar_expect_tx(&bars->h_full, kHBytes);
+        for (int kb = 0; kb < 4; ++kb) tma_load_2d(&map_h, &bars->h_full, sH + kb * BM * 128, kb * 64, m0);
+        for (int c = 0; c < NCH; ++c) {
+          const int s = c % kRing;
+          mbar_wait(&bars->w3_empty[s], ((uint32_t)(c / kRing) & 1u) ^ 1u);
+          mbar_expect_tx(&bars->w3_full[s], kW3Bytes);
+          for (int kb = 0; kb < 4; ++kb)
+            tma_load_2d(&map_w3, &bars->w3_full[s], sW3 + s * kW3Bytes + kb * CH * 128, kb * 64, c * CH);
+        }
+      }
+    } else if (warp == 1) {
+      if (elect_one()) {
+        for (int c = 0; c < NCH; ++c) {
+          const int s = c % kRing;
+          mbar_wait(&bars->w1_empty[s], ((uint32_t)(c / kRing) & 1u) ^ 1u);
+          mbar_expect_tx(&bars->w1_full[s], kW1Bytes);
+          tma_load_2d(&map_w1, &bars->w1_full[s], sW1 + s * kW1Bytes, c * CH, 0);
+        }
+      }
+    } else {
+      const int wg = warp - 2;
+      if (m0 + 64 * wg < g.M && elect_one()) {    // the last tile's second warpgroup may have no rows: no X to load
+        for (int c = 0; c < NCH; ++c) {
+          const int s = c % kRing;
+          mbar_wait(&bars->x_empty[wg][s], ((uint32_t)(c / kRing) & 1u) ^ 1u);
+          mbar_expect_tx(&bars->x_full[wg][s], kXBytes);
+          tma_load_2d(&map_x, &bars->x_full[wg][s], sX + (s * 2 + wg) * kXBytes, c * CH, m0 + 64 * wg);
+        }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      for (int c = 0; c < NCH; ++c) {
-        const int s = c % kW1Ring;
-        mbar_wait(&bars->w1_empty[s], ((uint32_t)(c / kW1Ring) & 1u) ^ 1u);
-        mbar_expect_tx(&bars->w1_full[s], kW1Bytes);
-        tma_load_2d(&map_w1, &bars->w1_full[s], sW1 + s * kW1Bytes, c * CH, 0);
-      }
-    }
-  } else if (warp >= 4) {
+  } else {
+    setmaxnreg_inc<kConsumerRegs>();
     const int wg = (warp >> 2) - 1;
     const bool leader = (threadIdx.x & 127) == 0;
+    if (m0 + 64 * wg >= g.M) {
+      // No rows (the second half of a last tile of at most 64 rows): release every weight slot in the order the other
+      // warpgroup does, and compute nothing.  Waiting for each slot to fill first keeps these arrivals in the slot's
+      // current phase: the next fill of a slot needs the other warpgroup's release of it too.
+      if (leader)
+        for (int c = 0; c < NCH; ++c) {
+          const int s = c % kRing;
+          const uint32_t ph = (uint32_t)(c / kRing) & 1u;
+          mbar_wait(&bars->w3_full[s], ph);
+          mbar_arrive(&bars->w3_empty[s]);
+          mbar_wait(&bars->w1_full[s], ph);
+          mbar_arrive(&bars->w1_empty[s]);
+        }
+      return;
+    }
     const uint64_t hi = desc_hi_kmajor<64>();
-    const uint64_t h_lo = desc_lo(sH), w3_lo = desc_lo(sW3), w1_lo = desc_lo(sW1), y_lo = desc_lo(sY);
-    const int r0 = (warp & 3) * 16 + (lane >> 2);          // rows r0, r0 + 8 of the tile
-    float accz[64];
+    const uint64_t h_lo = desc_lo(sH + wg * 64 * 128), w3_lo = desc_lo(sW3), w1_lo = desc_lo(sW1);
+    const int r0 = (warp & 3) * 16 + (lane >> 2);          // rows r0, r0 + 8 of the warpgroup's 64
+    const int t4 = 4 * (lane & 3);                          // byte offset of the thread's column pair in a 16-byte chunk
+    float accz[128], acc[32];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) accz[i] = 0.0f;
-    mbar_wait(&bars->h_full, 0);
-    for (int p = 0; p < NCH / 2; ++p) {
-      // ---- GEMM1: this warpgroup's chunk c1 of Y ----
-      const int c1 = 2 * p + wg, s3 = c1 % kW3Ring;
-      float acc[32];
+    for (int i = 0; i < 128; ++i) accz[i] = 0.0f;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) acc[i] = 0.0f;
-      mbar_wait(&bars->w3_full[s3], (uint32_t)(c1 / kW3Ring) & 1u);
+    for (int i = 0; i < 32; ++i) acc[i] = 0.0f;
+    // GEMM1 of chunk c into acc: W3 chunk c sits in slot c % kRing
+    auto gemm1 = [&](int c) {
+      const int s3 = c % kRing;
+      mbar_wait(&bars->w3_full[s3], (uint32_t)(c / kRing) & 1u);
       wg_fence();
 #pragma unroll
       for (int kb = 0; kb < 4; ++kb)
 #pragma unroll
         for (int k = 0; k < 4; ++k)
-          wgmma_64x64(acc, hi | (h_lo + (uint64_t)((kb * BM * 128) >> 4) + 2 * k),
-                      hi | (w3_lo + (uint64_t)((s3 * kW3Bytes + kb * CH * 128) >> 4) + 2 * k), 1u);
+          wgmma_f16<64>(acc, hi | (h_lo + (uint64_t)((kb * BM * 128) >> 4) + 2 * k),
+                        hi | (w3_lo + (uint64_t)((s3 * kW3Bytes + kb * CH * 128) >> 4) + 2 * k), 1u);
       wg_commit();
-      wg_wait<0>();
-      if (leader) mbar_arrive(&bars->w3_empty[s3]);
-      // ---- residual + ReLU -> fp16 Y chunk (swizzled A operand; Y in global memory when stored) ----
-      uint8_t* ybuf = sY + wg * kYBytes;
+    };
+    mbar_wait(&bars->h_full, 0);
+    gemm1(0);
+    wg_wait<0>();
+    if (leader) mbar_arrive(&bars->w3_empty[0]);
+    for (int c = 0; c < NCH; ++c) {
+      const int s = c % kRing;
+      const uint32_t ph = (uint32_t)(c / kRing) & 1u;
+      uint8_t* xb = sX + (s * 2 + wg) * kXBytes;
+      // ---- residual + ReLU -> fp16 Y chunk: GEMM2's A fragments, and over the X chunk for the store ----
+      uint32_t a[16];
+      mbar_wait(&bars->x_full[wg][s], ph);
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int r = r0 + 8 * i;
-        const bool valid = m0 + r < g.M;
-        const __half* xrow = x + (size_t)(m0 + r) * g.x_ld + c1 * CH;
+      for (int j = 0; j < 8; ++j)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int col = 8 * j + 2 * (lane & 3);
+        for (int i = 0; i < 2; ++i) {
+          const int r = r0 + 8 * i;
+          __half2* px = reinterpret_cast<__half2*>(xb + r * 128 + ((j ^ (r & 7)) << 4) + t4);
           float f0 = fmaf(acc[4 * j + 2 * i], 1.0f, 0.0f), f1 = fmaf(acc[4 * j + 2 * i + 1], 1.0f, 0.0f);
-          if (valid) {
-            const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(xrow + col));
-            f0 += rf.x; f1 += rf.y;
-          }
+          const float2 rf = __half22float2(*px);
+          f0 += rf.x; f1 += rf.y;
           f0 = fmaxf(f0, 0.0f); f1 = fmaxf(f1, 0.0f);
           const __half2 hv = __floats2half2_rn(f0, f1);
-          *reinterpret_cast<__half2*>(ybuf + r * 128 + ((j ^ (r & 7)) << 4) + 4 * (lane & 3)) = hv;
-          if (valid && g.store_y) *reinterpret_cast<__half2*>(y + (size_t)(m0 + r) * g.y_ld + c1 * CH + col) = hv;
+          if (g.store_y) *px = hv;
+          a[4 * (j >> 1) + 2 * (j & 1) + i] = *reinterpret_cast<const uint32_t*>(&hv);
         }
+      if (g.store_y) fence_proxy_async();                 // generic-proxy writes of Y -> visible to the TMA store
+      named_sync(1 + wg, 128);                            // the whole warpgroup is done with the X chunk
+      if (leader) {
+        if (g.store_y) { tma_store_2d(&map_y, xb, c * CH, m0 + 64 * wg); bulk_commit(); }
+        else mbar_arrive(&bars->x_empty[wg][s]);
       }
-      fence_proxy_async();                                  // generic-proxy writes of Y -> visible to wgmma
-      named_sync(1, 256);
-      // ---- GEMM2: Z[:, 128 wg + (0..127)] += Y_chunk(c) * W1[:, chunk c]^T for c = 2p, 2p + 1, in K order ----
+      // ---- GEMM2: Z += Y_chunk(c) * W1[:, chunk c]^T, then GEMM1 of the next chunk behind it ----
+      mbar_wait(&bars->w1_full[s], ph);
+      wg_fence();
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int c = 2 * p + h, s1 = c % kW1Ring;
-        mbar_wait(&bars->w1_full[s1], (uint32_t)(c / kW1Ring) & 1u);
-        wg_fence();
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_f16_ra<256>(accz, a + 4 * kk, hi | (w1_lo + (uint64_t)((s * kW1Bytes) >> 4) + 2 * kk), 1u);
+      wg_commit();
+      if (c + 1 < NCH) {
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-#pragma unroll
-          for (int n = 0; n < 2; ++n)
-            wgmma_64x64(accz + n * 32, hi | (y_lo + (uint64_t)((h * kYBytes) >> 4) + 2 * k),
-                        hi | (w1_lo + (uint64_t)((s1 * kW1Bytes + (128 * wg + 64 * n) * 128) >> 4) + 2 * k), 1u);
-        wg_commit();
+        for (int i = 0; i < 32; ++i) acc[i] = 0.0f;
+        gemm1(c + 1);
       }
+      if (leader && g.store_y) { bulk_wait_read<0>(); mbar_arrive(&bars->x_empty[wg][s]); }
       wg_wait<0>();
-      if (leader) { mbar_arrive(&bars->w1_empty[0]); mbar_arrive(&bars->w1_empty[1]); }
-      named_sync(1, 256);                                   // both Y buffers are free for the next pair
+      if (leader) {
+        mbar_arrive(&bars->w1_empty[s]);
+        if (c + 1 < NCH) mbar_arrive(&bars->w3_empty[(c + 1) % kRing]);
+      }
     }
-    // ---- Z epilogue: + shift2, optional ReLU, fp16 ----
+    // ---- Z epilogue: + shift2, optional ReLU, fp16, staged as 4 column blocks of 64 in this warpgroup's rows of H ----
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int r = r0 + 8 * i;
-      if (m0 + r >= g.M) continue;
-      __half* zrow = z + (size_t)(m0 + r) * g.z_ld + 128 * wg;
+    for (int n = 0; n < 4; ++n) {
+      uint8_t* zb = sH + n * BM * 128 + wg * 64 * 128;
 #pragma unroll
-      for (int n = 0; n < 2; ++n)
+      for (int j = 0; j < 8; ++j) {
+        const int col = 64 * n + 8 * j + (t4 >> 1);
+        const float b0 = shift2 ? shift2[col] : 0.0f, b1 = shift2 ? shift2[col + 1] : 0.0f;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int col = 64 * n + 8 * j + 2 * (lane & 3);
-          const float b0 = shift2 ? shift2[128 * wg + col] : 0.0f, b1 = shift2 ? shift2[128 * wg + col + 1] : 0.0f;
-          float f0 = fmaf(accz[n * 32 + 4 * j + 2 * i], 1.0f, b0), f1 = fmaf(accz[n * 32 + 4 * j + 2 * i + 1], 1.0f, b1);
+        for (int i = 0; i < 2; ++i) {
+          const int r = r0 + 8 * i;
+          float f0 = fmaf(accz[4 * (8 * n + j) + 2 * i], 1.0f, b0), f1 = fmaf(accz[4 * (8 * n + j) + 2 * i + 1], 1.0f, b1);
           if (g.relu2) { f0 = fmaxf(f0, 0.0f); f1 = fmaxf(f1, 0.0f); }
-          *reinterpret_cast<__half2*>(zrow + col) = __floats2half2_rn(f0, f1);
+          *reinterpret_cast<__half2*>(zb + r * 128 + ((j ^ (r & 7)) << 4) + t4) = __floats2half2_rn(f0, f1);
         }
+      }
+    }
+    fence_proxy_async();
+    named_sync(1 + wg, 128);
+    if (leader) {
+      for (int n = 0; n < 4; ++n) tma_store_2d(&map_z, sH + n * BM * 128 + wg * 64 * 128, 64 * n, m0 + 64 * wg);
+      bulk_commit();
+      bulk_wait_read<0>();
     }
   }
 }
@@ -216,14 +275,18 @@ extern "C" int step_bottleneck_exit_f16(const void* h, long long h_ld, const voi
       return fail(STEP_E_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
     g_enc = (EncFn)f;
   }
-  CUtensorMap mh, mw3, mw1;
+  CUtensorMap mh, mw3, mw1, mx, my, mz;
+  memset(&my, 0, sizeof(my));
   int r;
   if ((r = enc2d(&mh, h, K1, M, h_ld, BM, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map h (%d)", r);
   if ((r = enc2d(&mw3, w3, K1, N1, K1, CH, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map w3 (%d)", r);
   if ((r = enc2d(&mw1, w1, N1, N2, N1, N2, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map w1 (%d)", r);
+  if ((r = enc2d(&mx, x, N1, M, x_ld, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map x (%d)", r);
+  if (y && (r = enc2d(&my, y, N1, M, y_ld, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map y (%d)", r);
+  if ((r = enc2d(&mz, z, N2, M, z_ld, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map z (%d)", r);
   Geom g;
-  g.M = (int)M; g.store_y = y ? 1 : 0; g.relu2 = relu2 ? 1 : 0; g.x_ld = (int)x_ld; g.y_ld = (int)y_ld; g.z_ld = (int)z_ld;
-  const size_t smem = sizeof(Bars) + 1024 + kHBytes + kW3Ring * kW3Bytes + kW1Ring * kW1Bytes + 2 * kYBytes;
+  g.M = (int)M; g.store_y = y ? 1 : 0; g.relu2 = relu2 ? 1 : 0;
+  const size_t smem = sizeof(Bars) + 1024 + kHBytes + kRing * (kW3Bytes + kW1Bytes + 2 * kXBytes);
   static std::atomic<unsigned long long> attr_seen{0};
   if (first_use_on_device(attr_seen)) {
     cudaError_t e = cudaFuncSetAttribute(bottleneck_exit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -242,7 +305,7 @@ extern "C" int step_bottleneck_exit_f16(const void* h, long long h_ld, const voi
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = cu(stream);
-  cudaError_t le = cudaLaunchKernelEx(&cfg, bottleneck_exit_kernel, mh, mw3, mw1, g, shift2, (const __half*)x, (__half*)y, (__half*)z);
+  cudaError_t le = cudaLaunchKernelEx(&cfg, bottleneck_exit_kernel, mh, mw3, mw1, mx, my, mz, g, shift2);
   if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "bottleneck_exit_kernel launch: %s", cudaGetErrorString(le)); }
   STEP_LAUNCH_CHECK("bottleneck_exit_kernel");
   return 0;

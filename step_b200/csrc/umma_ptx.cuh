@@ -56,6 +56,10 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
 }
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the newest N committed bulk stores have finished reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 
 // wgmma shared-memory matrix descriptor (PTX ISA, "Matrix Descriptor Format" for wgmma):
 // [0,14) start >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4 | [62,64) swizzle
@@ -178,6 +182,30 @@ STEP_WGMMA_F16(256, 128, 129, 130,
                STEP_D4(16), STEP_D4(17), STEP_D4(18), STEP_D4(19), STEP_D4(20), STEP_D4(21), STEP_D4(22), STEP_D4(23),
                STEP_D4(24), STEP_D4(25), STEP_D4(26), STEP_D4(27), STEP_D4(28), STEP_D4(29), STEP_D4(30), STEP_D4(31))
 #undef STEP_WGMMA_F16
+
+// As wgmma_f16<N>, with A taken from registers: a[q] packs the fp16 pair of row (warp % 4) * 16 + lane / 4 + 8 (q & 1),
+// columns 8 (q >> 1) + 2 (lane % 4) + {0, 1}.  That is the accumulator layout above, so accumulator registers
+// [8 kk, 8 kk + 8) rounded pairwise to fp16 are the A operand of k-step kk.  Registers written by ordinary instructions
+// need a wg_fence() before the first wgmma that reads them, and must not change until that wgmma has retired.
+template <int N>
+__device__ __forceinline__ void wgmma_f16_ra(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_f16_ra<256>(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+               "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+               "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+               "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "
+               "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, "
+               "%86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, "
+               "%105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, "
+               "%122, %123, %124, %125, %126, %127}, {%128, %129, %130, %131}, %132, p, 1, 1, 0;\n\t}"
+               : STEP_D4(0), STEP_D4(1), STEP_D4(2), STEP_D4(3), STEP_D4(4), STEP_D4(5), STEP_D4(6), STEP_D4(7),
+                 STEP_D4(8), STEP_D4(9), STEP_D4(10), STEP_D4(11), STEP_D4(12), STEP_D4(13), STEP_D4(14), STEP_D4(15),
+                 STEP_D4(16), STEP_D4(17), STEP_D4(18), STEP_D4(19), STEP_D4(20), STEP_D4(21), STEP_D4(22), STEP_D4(23),
+                 STEP_D4(24), STEP_D4(25), STEP_D4(26), STEP_D4(27), STEP_D4(28), STEP_D4(29), STEP_D4(30), STEP_D4(31)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
 #undef STEP_D4
 
 __device__ __forceinline__ void wgmma_64x64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {

@@ -64,7 +64,10 @@ LAYERS = [
     ("loc_res",    3, LOCAL, 1088, 1024, (1, 1, 1)),
     ("loc_conv2",  3, LOCAL, 1088, 256, (1, 1, 1)),
     ("loc_3x3",    9, LOCAL, 256, 256, (1, 3, 3)),
-    ("loc_exit",   9, LOCAL, 256, 1024, "exit"),     # bottleneck_exit: 256 -> 1024 (+x, relu) -> 256
+    # bottleneck_exit: 256 -> 1024 (+x, relu) -> 256.  Per refinement step two exits store Y and feed the next block's
+    # conv1 (ReLU); the last one feeds downsample2 (bias, no ReLU) and does not store Y.
+    ("loc_exit",   6, LOCAL, 256, 1024, "exit"),
+    ("loc_exit_ds", 3, LOCAL, 256, 1024, "exit_ds"),
 ]
 
 
@@ -94,20 +97,24 @@ def main():
     tiles = conv_tiles()
     torch.manual_seed(0)
     total_ms = 0.0
-    print("%-10s %3s %4s %9s %9s %3s %4s %3s %9s %8s" % ("layer", "n", "kern", "GMAC", "exec_GMAC", "BK", "BN", "nt",
+    print("%-11s %3s %4s %9s %9s %3s %4s %3s %9s %8s" % ("layer", "n", "kern", "GMAC", "exec_GMAC", "BK", "BN", "nt",
                                                          "us", "TFLOP/s"))
     for name, count, (N, T, H, W), Cin, Cout, k in LAYERS:
         if args and name not in args:
             continue
         M = N * T * H * W
-        if k == "exit":
+        if k in ("exit", "exit_ds"):
             h = Act(torch.randn(N, T, H, W, Cin, device="cuda").half())
             w3 = (torch.randn(Cout, 1, Cin, device="cuda") / Cin ** 0.5).half()
             x = Act(torch.randn(N, T, H, W, Cout, device="cuda").half())
             w1 = (torch.randn(Cin, 1, Cout, device="cuda") / Cout ** 0.5).half()
             z = Act(torch.empty(N, T, H, W, Cin, device="cuda", dtype=torch.float16))
-            y = Act(torch.empty(N, T, H, W, Cout, device="cuda", dtype=torch.float16))
-            f = lambda: E.bottleneck_exit(h, w3, x, w1, None, True, z, y)
+            if k == "exit":
+                y = Act(torch.empty(N, T, H, W, Cout, device="cuda", dtype=torch.float16))
+                f = lambda: E.bottleneck_exit(h, w3, x, w1, None, True, z, y)
+            else:
+                b = torch.randn(Cin, device="cuda")
+                f = lambda: E.bottleneck_exit(h, w3, x, w1, b, False, z)
             gmac = 2.0 * M * Cin * Cout / 1e9
             kern, exec_gmac, tile = "exit", gmac, ("-", "-", "-")
         else:
@@ -138,9 +145,9 @@ def main():
         torch.cuda.synchronize()
         us = e0.elapsed_time(e1) / reps * 1e3
         total_ms += us * count / 1e3
-        line = "%-10s %3d %4s %9.2f %9.2f %3s %4s %3s %9.1f %8.1f" % (name, count, kern, gmac, exec_gmac, tile[0], tile[1],
+        line = "%-11s %3d %4s %9.2f %9.2f %3s %4s %3s %9.1f %8.1f" % (name, count, kern, gmac, exec_gmac, tile[0], tile[1],
                                                                      tile[2], us, 2 * gmac / us * 1e3)
-        if check and k != "exit":   # spot check against torch on two images (tool only: the parity tests live in tests/)
+        if check and not isinstance(k, str):   # spot check against torch on two images (tool only: the parity tests live in tests/)
             import torch.nn.functional as F
             xs = x.buf[:2].float().permute(0, 4, 1, 2, 3)
             ws = w.float().view(Cout, k[0], k[1], k[2], Cin).permute(0, 4, 1, 2, 3)
