@@ -198,6 +198,10 @@ int step_maxpool3d_fwd(const void* x, int dtype, int N, int T, int H, int W, int
  * (the temporal mean of two_branch.py:249 taken before the classifier, which is linear). */
 int step_mean_mid(const void* x, int dtype, int A, int B, int P, int C, int ld, void* y, int out_dtype,
                   step_stream_t stream);
+/* step_mean_mid with row a of x at a * a_stride elements (a_stride >= B * P * ld): the mean over a slice of axis B of a
+ * wider tensor, e.g. ContextNet's [clips, T', 1024] output over one refinement step's frames (train.py:317-321). */
+int step_mean_mid_strided(const void* x, int dtype, int A, int B, int P, int C, int ld, long long a_stride, void* y,
+                          int out_dtype, step_stream_t stream);
 /* y[m, n] = act(sum_k x[m,k] * w[n,k] + bias[n]); small-N GEMM (N <= 64) for global_cls,
  * local_reg, neighbor_reg (two_branch.py:246,261,269-270).  x [M,K] (row stride x_ld) in dtype,
  * w [N,K] in dtype, y fp32 [M, y_ld].  act: 0 none, 1 sigmoid (applied after accumulation).
@@ -247,6 +251,22 @@ int step_head_losses_f32(const float* logits, const float* local_loc, const floa
 int step_roi_align_bwd_nhwc(const void* grad_out, int dtype, int out_ld, const float* rois, int R, float scale, int ph,
                             int pw, int K, int H, int W, int C, int sampling_ratio, float* grad_in, int in_ld,
                             step_stream_t stream);
+/* step_roi_align_bwd_nhwc for ROIs whose frame index f is relative to the slice conv_feat[:, t_start:t_start+roi_T] of a
+ * [K = clips * feat_T, H, W, C] map (the frame map of step_roi_align_fwd_nhwc).  The contribution of each ROI frame is formed
+ * completely, in the same order as step_roi_align_bwd_nhwc, in a workspace of
+ * step_roi_align_bwd_slice_workspace_bytes(K, H, W, C, roi_T, feat_T) bytes and then ADDED to grad_in frame
+ * (f / roi_T) * feat_T + t_start + f % roi_T; frames outside the slice are untouched.  Deterministic, no atomics: with
+ * t_start = 0 and roi_T = feat_T, calls on a zeroed grad_in give bit for bit the sum of the step_roi_align_bwd_nhwc results. */
+size_t step_roi_align_bwd_slice_workspace_bytes(int K, int H, int W, int C, int roi_T, int feat_T);
+int step_roi_align_bwd_slice_nhwc(const void* grad_out, int dtype, int out_ld, const float* rois, int R, float scale, int ph,
+                                  int pw, int K, int H, int W, int C, int sampling_ratio, int roi_T, int feat_T, int t_start,
+                                  float* grad_in, int in_ld, void* workspace, size_t ws_bytes, step_stream_t stream);
+/* Gradient of ContextNet's output from one refinement step (train.py:317-321): dctx [R, C] (row stride dctx_ld) is the
+ * gradient of each tube's context input of the classifier, tubes [R, T_len, 5] the step's flat tubes (frame index first).
+ * acc [B, feat_T, C] fp32 += (sum over the tubes of clip b = floor(frame / T_len), ascending tube order) / T_len on frames
+ * [t_start, t_start + T_len) of clip b.  Deterministic, no atomics. */
+int step_ctx_grad_reduce_f32(const float* dctx, int dctx_ld, const float* tubes, int R, int T_len, int B, int feat_T,
+                             int t_start, int C, float* acc, step_stream_t stream);
 /* Backward of y = x W^T + b for the small-N linears of the head (nn.Linear / global_cls, two_branch.py:246-270):
  * dx [M,K] (+)= dy W, dw [Nn,K] = dy^T x, db [Nn] = column sums of dy; any of dx / dw may be NULL.  Fixed summation order. */
 int step_linear_small_n_bwd(const void* x, int dtype, int M, int K, int x_ld, const float* w, const float* dy, int Nn,

@@ -62,6 +62,7 @@ def _declare(lib):
         "step_conv3d_fwd": ([ctypes.POINTER(ConvParams), S], c_int),
         "step_maxpool3d_fwd": ([P, I] + [I] * 21 + [P, I, S], c_int),
         "step_mean_mid": ([P, I, I, I, I, I, I, P, I, S], c_int),
+        "step_mean_mid_strided": ([P, I, I, I, I, I, I, ctypes.c_longlong, P, I, S], c_int),
         "step_linear_small_n_workspace_bytes": ([I, I, I], c_size_t),
         "step_linear_small_n": ([P, I, I, I, I, P, P, I, P, I, I, I, P, P, c_size_t, S], c_int),
         "step_head_regress": ([P, I, I, I, I, I, P, P, I, I, I, I, P, P, P, P, c_size_t, S], c_int),
@@ -69,6 +70,9 @@ def _declare(lib):
                                      ctypes.c_longlong, I, I, I, S], c_int),
         "step_head_losses_f32": ([P, P, P, P, P, P, I, I, I, I, I, Fl, Fl, P, P, P, P, P, P, P, P, P, S], c_int),
         "step_roi_align_bwd_nhwc": ([P, I, I, P, I, Fl, I, I, I, I, I, I, I, P, I, S], c_int),
+        "step_roi_align_bwd_slice_workspace_bytes": ([I, I, I, I, I, I], c_size_t),
+        "step_roi_align_bwd_slice_nhwc": ([P, I, I, P, I, Fl, I, I, I, I, I, I, I, I, I, I, P, I, P, c_size_t, S], c_int),
+        "step_ctx_grad_reduce_f32": ([P, I, P, I, I, I, I, I, I, P, S], c_int),
         "step_linear_small_n_bwd": ([P, I, I, I, I, P, P, I, P, I, P, P, S], c_int),
         "step_conv1x1_wgrad_workspace_bytes": ([I, I, I], c_size_t),
         "step_conv1x1_wgrad_f16": ([P, I, P, I, I, I, I, Fl, P, I, I, P, c_size_t, S], c_int),

@@ -296,22 +296,25 @@ __global__ void __launch_bounds__(128) maxpool3d_march_kernel(const T* __restric
   }
 }
 
-// x [A,B,P,C] (C contiguous, pixel stride ld) -> y [A, P*C]  (mean over B, fp32 accumulate in index order)
+// x [A,B,P,C] (C contiguous, pixel stride ld, row a at a * a_stride) -> y [A, P*C]  (mean over B, fp32 accumulate in
+// index order)
 template <typename TI, typename TO>
-__global__ void mean_mid_kernel(const TI* __restrict__ x, int A, int B, int P, int C, int ld, TO* __restrict__ y) {
+__global__ void mean_mid_kernel(const TI* __restrict__ x, int A, int B, int P, int C, int ld, long long a_stride,
+                                TO* __restrict__ y) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)A * P * C) return;
   int c = (int)(idx % C);
   int p = (int)((idx / C) % P);
   int a = (int)(idx / ((long long)C * P));
   float s = 0.0f;
-  for (int b = 0; b < B; ++b) s += to_f32<TI>(x[(((size_t)a * B + b) * P + p) * ld + c]);
+  for (int b = 0; b < B; ++b) s += to_f32<TI>(x[(size_t)a * a_stride + ((size_t)b * P + p) * ld + c]);
   y[idx] = from_f32<TO>(s / (float)B);
 }
 
 // fp16 input, 8 channels per thread (16-byte loads); the per-channel sums run in the same index order as above
 template <typename TO>
-__global__ void mean_mid_h8_kernel(const __half* __restrict__ x, int A, int B, int P, int C, int ld, TO* __restrict__ y) {
+__global__ void mean_mid_h8_kernel(const __half* __restrict__ x, int A, int B, int P, int C, int ld, long long a_stride,
+                                   TO* __restrict__ y) {
   const int cv = C >> 3;
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)A * P * cv) return;
@@ -323,7 +326,7 @@ __global__ void mean_mid_h8_kernel(const __half* __restrict__ x, int A, int B, i
   for (int k = 0; k < 8; ++k) s[k] = 0.0f;
   for (int b = 0; b < B; ++b) {
     float v[8];
-    load16(x + (((size_t)a * B + b) * P + p) * ld + c, v);
+    load16(x + (size_t)a * a_stride + ((size_t)b * P + p) * ld + c, v);
 #pragma unroll
     for (int k = 0; k < 8; ++k) s[k] += v[k];
   }
@@ -733,29 +736,35 @@ extern "C" int step_maxpool3d_fwd(const void* x, int dtype, int N, int T, int H,
   return 0;
 }
 
-extern "C" int step_mean_mid(const void* x, int dtype, int A, int B, int P, int C, int ld, void* y, int out_dtype,
-                             step_stream_t stream) {
+extern "C" int step_mean_mid_strided(const void* x, int dtype, int A, int B, int P, int C, int ld, long long a_stride, void* y,
+                                     int out_dtype, step_stream_t stream) {
   STEP_CHECK_ARG(x && y && A > 0 && B > 0 && P > 0 && C > 0 && ld >= C, "mean_mid: bad args");
+  STEP_CHECK_ARG(A == 1 || a_stride >= (long long)B * P * ld, "mean_mid: row stride %lld < B * P * ld", a_stride);
   long long total = (long long)A * P * C;
   int g = ceil_div(total, 256);
-  if (dtype == STEP_F16 && C % 8 == 0 && ld % 8 == 0 && ((uintptr_t)x & 15) == 0) {
+  if (dtype == STEP_F16 && C % 8 == 0 && ld % 8 == 0 && a_stride % 8 == 0 && ((uintptr_t)x & 15) == 0) {
     const int g8 = ceil_div(total / 8, 256);
-    if (out_dtype == STEP_F16) mean_mid_h8_kernel<__half><<<g8, 256, 0, cu(stream)>>>((const __half*)x, A, B, P, C, ld, (__half*)y);
-    else if (out_dtype == STEP_F32) mean_mid_h8_kernel<float><<<g8, 256, 0, cu(stream)>>>((const __half*)x, A, B, P, C, ld, (float*)y);
+    if (out_dtype == STEP_F16) mean_mid_h8_kernel<__half><<<g8, 256, 0, cu(stream)>>>((const __half*)x, A, B, P, C, ld, a_stride, (__half*)y);
+    else if (out_dtype == STEP_F32) mean_mid_h8_kernel<float><<<g8, 256, 0, cu(stream)>>>((const __half*)x, A, B, P, C, ld, a_stride, (float*)y);
     else return fail(STEP_E_UNSUPPORTED, "mean_mid: dtype combination %d -> %d", dtype, out_dtype);
     STEP_LAUNCH_CHECK("mean_mid_h8_kernel");
     return 0;
   }
   if (dtype == STEP_F16 && out_dtype == STEP_F16)
-    mean_mid_kernel<__half, __half><<<g, 256, 0, cu(stream)>>>((const __half*)x, A, B, P, C, ld, (__half*)y);
+    mean_mid_kernel<__half, __half><<<g, 256, 0, cu(stream)>>>((const __half*)x, A, B, P, C, ld, a_stride, (__half*)y);
   else if (dtype == STEP_F16 && out_dtype == STEP_F32)
-    mean_mid_kernel<__half, float><<<g, 256, 0, cu(stream)>>>((const __half*)x, A, B, P, C, ld, (float*)y);
+    mean_mid_kernel<__half, float><<<g, 256, 0, cu(stream)>>>((const __half*)x, A, B, P, C, ld, a_stride, (float*)y);
   else if (dtype == STEP_F32 && out_dtype == STEP_F32)
-    mean_mid_kernel<float, float><<<g, 256, 0, cu(stream)>>>((const float*)x, A, B, P, C, ld, (float*)y);
+    mean_mid_kernel<float, float><<<g, 256, 0, cu(stream)>>>((const float*)x, A, B, P, C, ld, a_stride, (float*)y);
   else
     return fail(STEP_E_UNSUPPORTED, "mean_mid: dtype combination %d -> %d", dtype, out_dtype);
   STEP_LAUNCH_CHECK("mean_mid_kernel");
   return 0;
+}
+
+extern "C" int step_mean_mid(const void* x, int dtype, int A, int B, int P, int C, int ld, void* y, int out_dtype,
+                             step_stream_t stream) {
+  return step_mean_mid_strided(x, dtype, A, B, P, C, ld, (long long)B * P * ld, y, out_dtype, stream);
 }
 
 extern "C" int step_clip_to_ndhwc(const float* clip, int N, int T, int Cc, int H, int W, void* out, int dtype, int ld,

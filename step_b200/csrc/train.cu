@@ -6,6 +6,10 @@
 //                              contributions in a fixed order (ROI index, bin, sample), so the result is bit-for-bit
 //                              repeatable -- the reference's RoIAlignBackwardFeature (cuda/ROIAlign_cuda.cu:201-278) scatters
 //                              with atomicAdd and is not;
+//   * roi_align_bwd_slice_nhwc the same backward for ROIs pooled from a temporal slice of conv_feat (temporal mode of
+//                              train.py:294-309), accumulated into the gradient of the whole feature map;
+//   * ctx_grad_reduce          the gradient of ContextNet's output from the per-tube context inputs of the classifier
+//                              (train.py:317-321), summed per clip in tube order and spread over the step's frames;
 //   * linear_bwd_*             backward of the small-N linears of the head (global_cls, local_reg, neighbor_reg*):
 //                              dx = dy W, dW = dy^T x, db = sum dy, fixed summation order;
 //   * conv1x1_wgrad_*          weight gradient of a 1x1(x1) convolution, dW[Cout, Cin] = dz^T x with the reduction over
@@ -178,24 +182,18 @@ __device__ __forceinline__ void bilinear_taps(int H, int W, float y, float x, in
   pix[0] = y_low * W + x_low; pix[1] = y_low * W + x_high; pix[2] = y_high * W + x_low; pix[3] = y_high * W + x_high;
 }
 
+// Adds the contributions of every ROI r with roi[0] == roi_frame to dst, this frame's [H*W, C] gradient (channel stride
+// dst_ld), which the caller has initialised: per ROI and element the samples are summed in a fixed order and the sum is
+// added to dst.  Called by the whole CTA; `tab` is the CTA's shared sample table.
 template <typename T>
-__global__ void __launch_bounds__(256) roi_align_bwd_nhwc_kernel(const T* __restrict__ grad_out, int out_ld,
-                                                                 const float* __restrict__ rois, int R, float scale, int H,
-                                                                 int W, int C, int ph, int pw, int sampling_ratio,
-                                                                 float* __restrict__ grad_in, int in_ld) {
-  __shared__ RoiBwdSample tab[kBwdMaxSamples];
-  __shared__ int n_s;
-  const int frame = blockIdx.x;
+__device__ __forceinline__ void roi_align_bwd_frame(const T* __restrict__ grad_out, int out_ld, const float* __restrict__ rois,
+                                                    int R, float scale, int H, int W, int C, int ph, int pw, int sampling_ratio,
+                                                    int roi_frame, float* __restrict__ dst, int dst_ld, RoiBwdSample* tab) {
   constexpr int VN = 4;
   const int nvec = C / VN, npix = H * W;
-  // this CTA owns grad_in[frame]: zero it, then accumulate ROI by ROI (ascending index: fixed order)
-  for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x) {
-    const int p = i / nvec, cv = i - p * nvec;
-    *reinterpret_cast<float4*>(grad_in + ((size_t)frame * npix + p) * in_ld + cv * VN) = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
   for (int r = 0; r < R; ++r) {
     const float* roi = rois + 5 * (size_t)r;
-    if ((int)roi[0] != frame) continue;                       // uniform across the CTA
+    if ((int)roi[0] != roi_frame) continue;                   // uniform across the CTA
     // ROIAlign_cuda.cu:214-233
     const float sw = __fmul_rn(roi[1], scale), sh = __fmul_rn(roi[2], scale), ew = __fmul_rn(roi[3], scale), eh = __fmul_rn(roi[4], scale);
     const float roi_w = fmaxf(__fsub_rn(ew, sw), 1.0f), roi_h = fmaxf(__fsub_rn(eh, sh), 1.0f);
@@ -220,7 +218,6 @@ __global__ void __launch_bounds__(256) roi_align_bwd_nhwc_kernel(const T* __rest
         e.bin = bin;
         tab[s] = e;
       }
-      if (threadIdx.x == 0) n_s = cnt;
       __syncthreads();
       const T* go = grad_out + (size_t)r * ph * pw * out_ld;
       for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x) {
@@ -250,14 +247,78 @@ __global__ void __launch_bounds__(256) roi_align_bwd_nhwc_kernel(const T* __rest
           }
         }
         if (hit) {
-          float4* dst = reinterpret_cast<float4*>(grad_in + ((size_t)frame * npix + p) * in_ld + cv * VN);
-          float4 cur = *dst;
+          float4* d = reinterpret_cast<float4*>(dst + (size_t)p * dst_ld + cv * VN);
+          float4 cur = *d;
           cur.x = __fadd_rn(cur.x, acc[0]); cur.y = __fadd_rn(cur.y, acc[1]); cur.z = __fadd_rn(cur.z, acc[2]); cur.w = __fadd_rn(cur.w, acc[3]);
-          *dst = cur;
+          *d = cur;
         }
       }
     }
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) roi_align_bwd_nhwc_kernel(const T* __restrict__ grad_out, int out_ld,
+                                                                 const float* __restrict__ rois, int R, float scale, int H,
+                                                                 int W, int C, int ph, int pw, int sampling_ratio,
+                                                                 float* __restrict__ grad_in, int in_ld) {
+  __shared__ RoiBwdSample tab[kBwdMaxSamples];
+  const int frame = blockIdx.x;
+  const int nvec = C / 4, npix = H * W;
+  float* dst = grad_in + (size_t)frame * npix * in_ld;
+  // this CTA owns grad_in[frame]: zero it, then accumulate ROI by ROI (ascending index: fixed order)
+  for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x) {
+    const int p = i / nvec, cv = i - p * nvec;
+    *reinterpret_cast<float4*>(dst + (size_t)p * in_ld + cv * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  roi_align_bwd_frame<T>(grad_out, out_ld, rois, R, scale, H, W, C, ph, pw, sampling_ratio, frame, dst, in_ld, tab);
+}
+
+// The same backward for ROIs whose frame index f is relative to the slice conv_feat[:, t_start:t_start+roi_T]
+// (ROINet.pool_into's frame map): one CTA per ROI frame f forms the frame's whole contribution in its [H*W, C] workspace
+// frame exactly as roi_align_bwd_nhwc_kernel does, then adds it to grad_in frame (f / roi_T) * feat_T + t_start + f % roi_T.
+// Frames outside the slice are not touched, so successive refinement steps accumulate into one [B*feat_T, H, W, C] buffer.
+template <typename T>
+__global__ void __launch_bounds__(256) roi_align_bwd_slice_nhwc_kernel(const T* __restrict__ grad_out, int out_ld,
+                                                                       const float* __restrict__ rois, int R, float scale, int H,
+                                                                       int W, int C, int ph, int pw, int sampling_ratio, int roi_T,
+                                                                       int feat_T, int t_start, float* __restrict__ ws,
+                                                                       float* __restrict__ grad_in, int in_ld) {
+  __shared__ RoiBwdSample tab[kBwdMaxSamples];
+  const int f = blockIdx.x;
+  const int nvec = C / 4, npix = H * W;
+  float* part = ws + (size_t)f * npix * C;
+  for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x)
+    *reinterpret_cast<float4*>(part + (size_t)i * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+  roi_align_bwd_frame<T>(grad_out, out_ld, rois, R, scale, H, W, C, ph, pw, sampling_ratio, f, part, C, tab);
+  __syncthreads();
+  float* dst = grad_in + ((size_t)(f / roi_T) * feat_T + t_start + f % roi_T) * npix * in_ld;
+  for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x) {
+    const int p = i / nvec, cv = i - p * nvec;
+    const float4 a = *reinterpret_cast<const float4*>(part + (size_t)i * 4);
+    float4* d = reinterpret_cast<float4*>(dst + (size_t)p * in_ld + cv * 4);
+    float4 cur = *d;
+    cur.x = __fadd_rn(cur.x, a.x); cur.y = __fadd_rn(cur.y, a.y); cur.z = __fadd_rn(cur.z, a.z); cur.w = __fadd_rn(cur.w, a.w);
+    *d = cur;
+  }
+}
+
+// ---- context-feature gradient (train.py:317-321: temp_context_feat[p] = context_feat[clip(p), :, t_start:t_start+T_len]) --
+// dctx[r, c] is the gradient of tube r's context input of the classifier (the slice mean the forward feeds to global_cls).
+// acc[b, t, c] += (sum over the tubes r of clip b, ascending r, of dctx[r, c]) / T_len for t in [t_start, t_start + T_len);
+// clip(r) = floor(frame(r) / T_len) with frame(r) = tubes[r, 0, 0].  One thread per (clip, channel): no atomics.
+__global__ void __launch_bounds__(256) ctx_grad_reduce_kernel(const float* __restrict__ dctx, int dctx_ld, const float* __restrict__ tubes,
+                                                              int R, int T_len, int B, int feat_T, int t_start, int C,
+                                                              float* __restrict__ acc) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)B * C) return;
+  const int b = (int)(i / C), c = (int)(i - (long long)b * C);
+  float s = 0.0f;
+  for (int r = 0; r < R; ++r)
+    if ((int)__fdiv_rn(tubes[(size_t)r * T_len * 5], (float)T_len) == b) s = __fadd_rn(s, dctx[(size_t)r * dctx_ld + c]);
+  const float v = __fdiv_rn(s, (float)T_len);
+  float* d = acc + ((size_t)b * feat_T + t_start) * C + c;
+  for (int t = 0; t < T_len; ++t) d[(size_t)t * C] = __fadd_rn(d[(size_t)t * C], v);
 }
 
 // ---- small-N linear backward -----------------------------------------------------------------------------------------
@@ -569,6 +630,48 @@ extern "C" int step_roi_align_bwd_nhwc(const void* grad_out, int dtype, int out_
     roi_align_bwd_nhwc_kernel<__half><<<K, 256, 0, cu(stream)>>>((const __half*)grad_out, out_ld, rois, R, scale, H, W, C, ph, pw,
                                                                   sampling_ratio, grad_in, in_ld);
   STEP_LAUNCH_CHECK("roi_align_bwd_nhwc_kernel");
+  return 0;
+}
+
+extern "C" size_t step_roi_align_bwd_slice_workspace_bytes(int K, int H, int W, int C, int roi_T, int feat_T) {
+  if (K <= 0 || H <= 0 || W <= 0 || C <= 0 || roi_T <= 0 || feat_T <= 0) return 0;
+  return (size_t)(K / feat_T) * roi_T * H * W * C * sizeof(float);
+}
+
+extern "C" int step_roi_align_bwd_slice_nhwc(const void* grad_out, int dtype, int out_ld, const float* rois, int R, float scale, int ph,
+                                             int pw, int K, int H, int W, int C, int sampling_ratio, int roi_T, int feat_T, int t_start,
+                                             float* grad_in, int in_ld, void* workspace, size_t ws_bytes, step_stream_t stream) {
+  STEP_CHECK_ARG(K > 0 && H > 0 && W > 0 && C > 0 && R >= 0 && ph > 0 && pw > 0, "roi_align_bwd_slice_nhwc: bad shape");
+  STEP_CHECK_ARG(dtype == STEP_F32 || dtype == STEP_F16, "roi_align_bwd_slice_nhwc: bad dtype");
+  STEP_CHECK_ARG(C % 4 == 0 && in_ld % 4 == 0 && out_ld % 4 == 0 && in_ld >= C && out_ld >= C,
+                 "roi_align_bwd_slice_nhwc: C / ld must be multiples of 4");
+  STEP_CHECK_ARG(feat_T > 0 && K % feat_T == 0 && roi_T > 0 && t_start >= 0 && t_start + roi_T <= feat_T,
+                 "roi_align_bwd_slice_nhwc: bad frame map roi_T=%d feat_T=%d t_start=%d K=%d", roi_T, feat_T, t_start, K);
+  STEP_CHECK_ARG(grad_in && workspace && (R == 0 || (grad_out && rois)), "roi_align_bwd_slice_nhwc: null pointer");
+  STEP_CHECK_ARG((((uintptr_t)grad_in | (uintptr_t)grad_out | (uintptr_t)workspace) & 15) == 0,
+                 "roi_align_bwd_slice_nhwc: pointers must be 16-byte aligned");
+  const size_t need = step_roi_align_bwd_slice_workspace_bytes(K, H, W, C, roi_T, feat_T);
+  if (ws_bytes < need) return fail(STEP_E_WORKSPACE, "roi_align_bwd_slice_nhwc: workspace %zu < %zu", ws_bytes, need);
+  const int frames = (K / feat_T) * roi_T;
+  if (dtype == STEP_F32)
+    roi_align_bwd_slice_nhwc_kernel<float><<<frames, 256, 0, cu(stream)>>>((const float*)grad_out, out_ld, rois, R, scale, H, W, C, ph, pw,
+                                                                            sampling_ratio, roi_T, feat_T, t_start, (float*)workspace,
+                                                                            grad_in, in_ld);
+  else
+    roi_align_bwd_slice_nhwc_kernel<__half><<<frames, 256, 0, cu(stream)>>>((const __half*)grad_out, out_ld, rois, R, scale, H, W, C, ph,
+                                                                             pw, sampling_ratio, roi_T, feat_T, t_start, (float*)workspace,
+                                                                             grad_in, in_ld);
+  STEP_LAUNCH_CHECK("roi_align_bwd_slice_nhwc_kernel");
+  return 0;
+}
+
+extern "C" int step_ctx_grad_reduce_f32(const float* dctx, int dctx_ld, const float* tubes, int R, int T_len, int B, int feat_T,
+                                        int t_start, int C, float* acc, step_stream_t stream) {
+  STEP_CHECK_ARG(B > 0 && C > 0 && R >= 0 && T_len > 0 && dctx_ld >= C && t_start >= 0 && t_start + T_len <= feat_T,
+                 "ctx_grad_reduce: bad shape B=%d C=%d R=%d T_len=%d feat_T=%d t_start=%d", B, C, R, T_len, feat_T, t_start);
+  STEP_CHECK_ARG(acc && (R == 0 || (dctx && tubes)), "ctx_grad_reduce: null pointer");
+  ctx_grad_reduce_kernel<<<ceil_div((long long)B * C, 256), 256, 0, cu(stream)>>>(dctx, dctx_ld, tubes, R, T_len, B, feat_T, t_start, C, acc);
+  STEP_LAUNCH_CHECK("ctx_grad_reduce_kernel");
   return 0;
 }
 

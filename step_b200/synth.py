@@ -202,3 +202,39 @@ def make_loss_case(name, num_classes):
         tg[0, :, 5] = 1.0
     tg[:, :, 6:] = (torch.rand(n, 3, num_classes, generator=g) > 0.9).float()
     return T_, chunks, feat, tubes, tg
+
+
+def make_train_case(cfg, B, N, W, H, seed=3):
+    """Seeded selected samples of one training step (what train_select, utils/utils.py:135-423, hands to train.py:300-333)
+    for refinement steps 1..cfg.max_iter: (step_tubes, step_targets), step_tubes[i] [B*N, T_length_i, 5] fp32 with the
+    frame index relative to the step's frame slice first (flatten_tubes(batch_idx=True)), step_targets[i]
+    [B*N, 3, 6 + classes].  Boxes lie inside a W x H image; every step has positive class and regression samples."""
+    g = torch.Generator().manual_seed(seed)
+    step_tubes, step_targets = [], []
+    for i in range(1, cfg.max_iter + 1):
+        t_len = cfg.NUM_CHUNKS[i] * cfg.T
+        R = B * N
+        x1 = torch.rand(R, 1, generator=g) * 0.3 * W
+        y1 = torch.rand(R, 1, generator=g) * 0.3 * H
+        w = (0.3 + torch.rand(R, 1, generator=g) * 0.3) * W
+        hh = (0.3 + torch.rand(R, 1, generator=g) * 0.3) * H
+        box = torch.cat([x1, y1, x1 + w, y1 + hh], 1)
+        frame = (torch.arange(R) // N).view(R, 1, 1) * t_len + torch.arange(t_len).view(1, t_len, 1)
+        jit = torch.rand(R, t_len, 4, generator=g) * 0.02 * W
+        tubes = torch.cat([frame.float(), box.view(R, 1, 4).expand(R, t_len, 4) + jit], 2)
+        tg = torch.zeros(R, 3, 6 + cfg.num_classes)
+        tg[:, :, :4] = box.view(R, 1, 4) + torch.rand(R, 3, 4, generator=g) * 0.06 * W
+        tg[:, :, 4] = (torch.rand(R, 3, generator=g) > 0.3).float()
+        tg[:, :, 5] = (torch.rand(R, 3, generator=g) > 0.3).float()
+        tg[0, :, 4:6] = 1.0
+        tg[:, :, 6:] = (torch.rand(R, 3, cfg.num_classes, generator=g) > 0.9).float()
+        step_tubes.append(tubes.contiguous())
+        step_targets.append(tg)
+    return step_tubes, step_targets
+
+
+def make_conv_feat(B, T, H, W, seed=2468):
+    """A seeded stand-in for the trunk's output [B, T', 832, H', W'] (post-ReLU: non-negative)."""
+    g = torch.Generator().manual_seed(seed)
+    return torch.relu(torch.randn(B, T, 832, H, W, generator=g))
+

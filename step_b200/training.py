@@ -1,10 +1,13 @@
-"""First pieces of the training step on the device (SURVEY.md section 8f rank 1; the reference: train.py:286-348).
+"""The training step on the device (SURVEY.md section 8f rank 1; the reference: train.py:263-348).
 
 What exists: the head's three losses and the gradient of the training objective with respect to the head outputs
 (`head_losses`), the backward of the head's small-N linears (`linear_backward`), a deterministic channels-last ROIAlign
-backward (`roi_align_backward_nhwc`) and the tensor-core weight gradient of 1x1 convolutions (`conv1x1_wgrad`).
-What does not exist yet: dgrad / wgrad of the k > 1 convolutions, max-pool backward, the optimizer step and the gradient
-all-reduce -- `BaseNet` / `TwoBranchNet` therefore still run without autograd (their outputs carry no grad_fn).
+backward (`roi_align_backward_nhwc`, and `roi_align_backward_slice` for the temporal slices of train.py:294-309), the
+tensor-core weight gradient of the convolutions, max-pool backward, the backward of the whole head including the context
+columns of `global_cls` (`head_forward_backward`), of ContextNet (`context_forward` / `context_backward`) and of the I3D
+trunk (`trunk_forward_backward`), the SGD update with the gradient all-reduce (`sgd_step`) and the whole step in spatial
+and temporal mode with or without the context branch (`train_step`).  `BaseNet` / `ContextNet` / `TwoBranchNet` still run
+without autograd (their outputs carry no grad_fn): the backward walks the tape their forward records.
 """
 import torch
 
@@ -256,12 +259,17 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
     with respect to every trainable parameter of the head and to the pooled ROI features.  fp16 activations / activation
     gradients with a static loss scale (apex-style), fp32 weight gradients.  Dropout is the identity (eval mode), like the
     reference's gradient goldens.
-    Returns dict(prob, loc, first, last, losses=(cls, loc, nb), loss, grads={param: grad}, feat_grad=[N,T',832,7,7] fp32)."""
+    context_feat (heads built with the context columns, cfg.no_context=False), in one of two forms:
+      * [N,1024,T',1,1], the per-tube context feature the reference passes (train.py:317-321, two_branch.py:242-249);
+      * (ctx_mean, row_map): ctx_mean fp32 [rows, 1024] is the mean of the context feature over the step's frames and
+        row_map int32 [N] (or None = identity) the row of each tube (ContextNet output per clip, as train_step feeds it).
+    Returns dict(prob, loc, first, last, losses=(cls, loc, nb), loss, grads={param: grad}, feat_grad=[N,T',832,7,7] fp32,
+    ctx_grad): grads holds the whole global_cls.weight (context columns included); ctx_grad is the gradient with respect to
+    the context input, [N,1024,T',1,1] for the first form and the per-tube [N,1024] gradient of the row each tube reads for
+    the second (None without context)."""
     from . import engine as E
     from .engine import Act
     from .networks import to_act
-    if context_feat is not None:
-        raise NotImplementedError("head_forward_backward: the context branch's backward is not built")
     if E.dtype_code(net.fp16) != L.F16:
         raise RuntimeError("head_forward_backward runs on the fp16 path (cfg.fp16=True)")
     fc, ps = net.fc_dim, net.pool_size
@@ -272,16 +280,31 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
     else:   # ROI features already pooled into the [ROI | downsample] concat buffer (ROINet.pool_into)
         dev = L.same_device(cat.buf, tubes, targets)
         N, Tl, Wd, Hd, C = cat.N, cat.T, cat.H, cat.W, cat.ld - fc
+    hw = net._head_weights()
+    if (context_feat is None) != (hw["ctx_w"] is None):
+        raise RuntimeError("head_forward_backward: global_cls has %d context columns but context_feat is %s"
+                           % (0 if hw["ctx_w"] is None else hw["ctx_w"].shape[1], "None" if context_feat is None else "given"))
     with torch.cuda.device(dev), torch.no_grad():
         if cat is None:
             cat = Act.empty(N, Tl, Wd, Hd, C + fc, L.F16, dev)
             src = to_act(global_feat, L.F16)
             cat.buf[..., :C].copy_(src.buf[..., src.coff:src.coff + C])
+        ctx_mean, row_map, ctx_module_form = None, None, False
+        if isinstance(context_feat, (tuple, list)):
+            ctx_mean, row_map = context_feat
+            L.same_device(ctx_mean, row_map, cat.buf)
+            ctx_mean = ctx_mean.float().contiguous()
+        elif context_feat is not None:
+            ctx_module_form = True
+            if tuple(context_feat.shape) != (N, 1024, Tl, 1, 1):
+                raise RuntimeError("head_forward_backward: context_feat %s, expected [%d,1024,%d,1,1]" % (tuple(context_feat.shape), N, Tl))
+            cf = context_feat.detach().to(dev).float().contiguous().view(N * 1024, Tl)
+            ctx_mean = E.mean_mid(cf.data_ptr(), L.F32, N * 1024, Tl, 1, 1, 1, dev).view(N, 1024)   # as TwoBranchNet.forward
         tape, keep = [], {}
         saved_tape, saved_bs = E.TAPE, E.BRANCH_STREAMS
         E.TAPE, E.BRANCH_STREAMS = tape, False          # one stream: the tape order is the execution order
         try:
-            prob, loc, first, last, logits = net.forward_act(cat, None, None, want_logits=True, keep=keep)
+            prob, loc, first, last, logits = net.forward_act(cat, ctx_mean, row_map, want_logits=True, keep=keep)
         finally:
             E.TAPE, E.BRANCH_STREAMS = saved_tape, saved_bs
         lc, ll, ln, g = head_losses(logits, loc, first, last, tubes, targets, net.T, lambda_reg, lambda_neighbor, want_grads=True)
@@ -290,11 +313,20 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
                 g[k_].mul_(objective_scale)
         grads = GradStore()
         out = {}
-        hw = net._head_weights()
         unperm = lambda w: w.view(-1, ps * ps, fc).permute(0, 2, 1).reshape(w.shape[0], -1)   # (p*fc + c) -> (c*49 + p)
-        # ---- classifier: logits = mean_t(gconv) . W^T + b   (two_branch.py:246-249)
+        # ---- classifier: logits = mean_t(gconv) . W^T + ctx . W_ctx^T + b   (two_branch.py:242-249)
         dxbar, dw, db = linear_backward(keep["xbar"], hw["cls_w"], g["logits"])
-        out[net.global_cls.weight] = unperm(dw).reshape(net.global_cls.weight.shape)
+        ctx_grad = None
+        if ctx_mean is not None:
+            # the context columns are not permuted; the rows each tube read (row_map) are gathered for dW_ctx
+            xc = ctx_mean if row_map is None else ctx_mean.index_select(0, row_map.long())
+            ctx_grad, dw_ctx, _ = linear_backward(xc, hw["ctx_w"], g["logits"])
+            dw = torch.cat([unperm(dw), dw_ctx], 1)
+            if ctx_module_form:   # the classifier averages its per-frame logits over T' (two_branch.py:249)
+                ctx_grad = (ctx_grad * (1.0 / Tl)).view(N, 1024, 1, 1, 1).expand(N, 1024, Tl, 1, 1).contiguous()
+        else:
+            dw = unperm(dw)
+        out[net.global_cls.weight] = dw.reshape(net.global_cls.weight.shape)
         out[net.global_cls.bias] = db
         gcat = grads.of(cat)
         L.check(L.lib().step_mean_mid_bwd(L.ptr(dxbar), N, Tl, ps * ps, fc, float(loss_scale),
@@ -320,7 +352,55 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
         fg = gcat.buf[..., :C].float().mul_(1.0 / loss_scale).permute(0, 1, 4, 2, 3).contiguous() if global_feat is not None else None
     loss = lc.mean() + lambda_reg * ll.mean() + lambda_neighbor * ln.mean()
     return dict(prob=prob, loc=loc, first=first, last=last, losses=(lc, ll, ln), loss=loss, grads=out, feat_grad=fg,
-                roi_grad=Act(gcat.buf, C, 0))
+                roi_grad=Act(gcat.buf, C, 0), ctx_grad=ctx_grad)
+
+
+def context_forward(context_net, feat):
+    """ContextNet.forward_act (two_branch.py:132-138) on the fp16 path with the tape on.  feat: the trunk's output Act
+    [B,T',H',W',832].  Returns (ctx [B,T',1024] fp32, state for context_backward)."""
+    from . import engine as E
+    if E.dtype_code(context_net.fp16) != L.F16:
+        raise RuntimeError("context_forward runs on the fp16 path (cfg.fp16=True)")
+    with torch.cuda.device(feat.device), torch.no_grad():
+        tape, keep = [], {}
+        saved_tape, saved_bs = E.TAPE, E.BRANCH_STREAMS
+        E.TAPE, E.BRANCH_STREAMS = tape, False
+        try:
+            ctx = context_net.forward_act(feat, keep=keep)
+        finally:
+            E.TAPE, E.BRANCH_STREAMS = saved_tape, saved_bs
+    return ctx, dict(tape=tape, x=keep["mixed_5c"], feat=feat)
+
+
+def context_backward(state, d_ctx, loss_scale=1024.0):
+    """Backward of context_forward from d_ctx = d(loss)/d(ctx), fp32 [B,T',1024]: the spatial mean's backward into the
+    gradient of Mixed_5c's output, then the tape (Mixed_5c, Mixed_5b, the (1,3,3)/(1,2,2) max-pool).  Returns
+    ({conv weight: fp32 gradient} for the 12 Unit3D convolutions -- BatchNorm stays frozen --, fp16 [B,T',H',W',832] (a
+    channel-slice view) holding loss_scale * d(loss)/d(conv_feat) through the context branch)."""
+    x = state["x"]
+    with torch.cuda.device(x.device), torch.no_grad():
+        grads = GradStore()
+        gx = grads.of(x)
+        d = d_ctx.float().contiguous()
+        L.check(L.lib().step_mean_mid_bwd(L.ptr(d), x.N * x.T, x.H * x.W, 1, x.C, float(loss_scale), L.c_void_p(gx.data_ptr()), gx.ld,
+                                          L.stream()))
+        out = tape_backward(state["tape"], grads, loss_scale)
+        gfeat = grads.of(state["feat"])
+    return out, gfeat.buf[..., gfeat.coff:gfeat.coff + gfeat.C]
+
+
+def context_grad_reduce(dctx, tubes, acc, t_start):
+    """acc [B, T', 1024] fp32 += the gradient of ContextNet's output from one refinement step: dctx [R, 1024] is each
+    tube's gradient of the context row it read, tubes [R, T_len, 5] the step's flat tubes (train.py:317-321: clip =
+    floor(frame / T_len), frames [t_start, t_start + T_len) of the clip, weight 1 / T_len).  Deterministic."""
+    dev = L.same_device(dctx, tubes, acc)
+    R, T_len = tubes.shape[0], tubes.shape[1]
+    B, T_all, C = acc.shape
+    d = dctx.float().contiguous()
+    tb = tubes.float().contiguous()
+    with torch.cuda.device(dev):
+        L.check(L.lib().step_ctx_grad_reduce_f32(L.ptr(d), C, L.ptr(tb), R, T_len, B, T_all, int(t_start), C, L.ptr(acc), L.stream()))
+    return acc
 
 
 def trunk_forward_backward(base_net, clips, d_feat_fn, loss_scale=1024.0):
@@ -379,44 +459,79 @@ def sgd_step(params_and_grads, lr, momentum=0.9, weight_decay=0.0, state=None, w
     return state
 
 
+def step_frames(cfg, i):
+    """(T_start, T_length) of refinement step i (1-based) -- train.py:294-298."""
+    chunks = cfg.NUM_CHUNKS[i]
+    return int((cfg.NUM_CHUNKS[cfg.max_iter] - chunks) / 2) * cfg.T, chunks * cfg.T
+
+
 def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9, weight_decay=0.0, lambda_reg=5.0,
                lambda_neighbor=1.0, loss_scale=1024.0, sgd_state=None, world_size=1):
-    """One optimisation step of train.py:286-348 on the device, for already selected training samples
+    """One optimisation step of train.py:263-348 on the device, for already selected training samples
     (`train_select`, utils/utils.py:135-423, is the host-side sampling of SURVEY.md section 8f rank 4 and is not built):
-        conv_feat = base_net(clips)                                   train.py:263
-        for each refinement step i: ROI-pool the step's flat tubes, run det_net[i-1] with targets,
-            loss_back += loss_cls.mean() + lambda_reg * loss_loc.mean() + lambda_neighbor * loss_nb.mean()   train.py:323-336
-        loss_back.backward(); optimizer.step()                         train.py:345-348
-    step_tubes[i]: [R_i, T', 5] fp32 (frame index first, as flatten_tubes(batch_idx=True) builds them), step_targets[i]:
-    [R_i, 3, 6 + classes].  Spatial mode only (every step pools the whole T' range).  Context branch off.
-    Returns dict(loss, losses=[(cls, loc, nb)], grads={param: fp32 grad}); updates the parameters when lr is given."""
-    from . import engine as E
+        conv_feat = base_net(clips); context_feat = context_net(conv_feat) unless cfg.no_context      train.py:266-269
+        for each refinement step i: T_start, T_length from cfg.NUM_CHUNKS / cfg.T / cfg.max_iter; ROI-pool the step's
+            flat tubes from conv_feat[:, T_start:T_start+T_length]; run det_net[i-1] with targets and each tube's clip
+            context over those frames;
+            loss_back += loss_cls.mean() + lambda_reg * loss_loc.mean() + lambda_neighbor * loss_nb.mean()   train.py:294-336
+        loss_back.backward(); optimizer.step()                                                             train.py:345-348
+    step_tubes[i]: [R_i, T_length_i, 5] fp32 (frame index first, relative to the step's frame slice, as
+    flatten_tubes(batch_idx=True) builds them), step_targets[i]: [R_i, 3, 6 + classes].
+    The gradient of conv_feat is, in this order, the ROIAlign backward of every step (each on its own frame slice) plus
+    the context branch's.  Returns dict(loss, losses=[(cls, loc, nb)], grads={param: fp32 grad} (trunk, heads and, with
+    the context branch, ContextNet's convolutions)); updates the parameters when lr is given."""
     from .engine import Act
     base, roi_net = nets["base_net"], nets["roi_net"]
+    use_ctx = not getattr(cfg, "no_context", True)
+    if use_ctx and nets.get("context_net") is None:
+        raise RuntimeError("train_step: cfg.no_context is False but nets has no 'context_net'")
     dev = clips.device
     n_steps = len(step_tubes)
-    results, roi_grads = [], []
+    results = []
     all_grads = {}
 
     def d_feat(feat):
-        # heads first (they need conv_feat), then the sum of their ROIAlign backward results is the trunk's output gradient
-        total = None
+        # ContextNet and the heads first (they need conv_feat), then the sum of their conv_feat gradients is the trunk's
+        # output gradient
+        B, T_all = feat.N, feat.T
+        ctx = ctx_state = d_ctx = None
+        if use_ctx:
+            ctx, ctx_state = context_forward(nets["context_net"], feat)                     # [B, T', 1024] fp32
+            d_ctx = torch.zeros_like(ctx)
+        total = torch.zeros((B * T_all, feat.H, feat.W, feat.C), dtype=torch.float32, device=dev)
+        ws = None
         for i in range(n_steps):
             head = nets["det_net%d" % i]
+            t_start, t_len = step_frames(cfg, i + 1)
             flat = step_tubes[i].to(dev).float().contiguous()
-            R, Tl = flat.shape[0], flat.shape[1]
-            if Tl != feat.T:
-                raise NotImplementedError("train_step: temporal chunking of the training step is not built (spatial mode)")
-            cat = Act.empty(R, Tl, head.pool_size, head.pool_size, 832 + head.fc_dim, L.F16, dev)
-            roi_net.pool_into(feat, flat, cat.frames().slice(0, 832), Tl, feat.T, 0)
-            r = head_forward_backward(head, None, flat, step_targets[i].to(dev), lambda_reg=lambda_reg, lambda_neighbor=lambda_neighbor,
-                                      loss_scale=loss_scale, cat=cat)
+            R = flat.shape[0]
+            if flat.shape[1] != t_len or t_start + t_len > T_all:
+                raise RuntimeError("train_step: step %d pools frames [%d, %d) of T'=%d (cfg.T=%d, NUM_CHUNKS=%s) but its tubes have %d frames"
+                                   % (i + 1, t_start, t_start + t_len, T_all, cfg.T, cfg.NUM_CHUNKS, flat.shape[1]))
+            cat = Act.empty(R, t_len, head.pool_size, head.pool_size, 832 + head.fc_dim, L.F16, dev)
+            roi_net.pool_into(feat, flat, cat.frames().slice(0, 832), t_len, T_all, t_start)
+            context = None
+            if use_ctx:
+                # per-clip mean of the context over the step's frames; row_map = clip of each tube (train.py:317-321)
+                sl = ctx[:, t_start:]
+                ctx_mean = torch.empty((B, ctx.shape[2]), dtype=torch.float32, device=dev)
+                L.check(L.lib().step_mean_mid_strided(L.c_void_p(sl.data_ptr()), L.F32, B, t_len, 1, ctx.shape[2], ctx.shape[2],
+                                                      T_all * ctx.shape[2], L.ptr(ctx_mean), L.F32, L.stream()))
+                row_map = torch.div(flat[:, 0, 0], float(t_len), rounding_mode="floor").to(torch.int32)
+                context = (ctx_mean, row_map)
+            r = head_forward_backward(head, None, flat, step_targets[i].to(dev), context_feat=context, lambda_reg=lambda_reg,
+                                      lambda_neighbor=lambda_neighbor, loss_scale=loss_scale, cat=cat)
             results.append(r)
             all_grads.update(r["grads"])
-            rg = r["roi_grad"]                                     # fp16, scaled by loss_scale, [R, T', 7, 7, ld] slice [0, 832)
-            gin = roi_align_backward_nhwc_strided(rg, flat.view(-1, 5), 1.0 / 16.0, feat.N * feat.T, feat.H, feat.W)
-            total = gin if total is None else total.add_(gin)
-        return total.mul_(1.0 / loss_scale).view(feat.N, feat.T, feat.H, feat.W, feat.C)
+            if use_ctx:
+                context_grad_reduce(r["ctx_grad"], flat, d_ctx, t_start)
+            with _Phase("roi_bwd"):
+                ws = roi_align_backward_slice(r["roi_grad"], flat.view(-1, 5), 1.0 / 16.0, total, t_len, T_all, t_start, ws=ws)
+        if use_ctx:
+            cg, gfeat = context_backward(ctx_state, d_ctx, loss_scale)
+            all_grads.update(cg)
+            total.add_(gfeat.reshape(B * T_all, feat.H, feat.W, feat.C).float())             # scaled by loss_scale too
+        return total.mul_(1.0 / loss_scale).view(B, T_all, feat.H, feat.W, feat.C)
 
     feat, tg = trunk_forward_backward(base, clips, d_feat, loss_scale)
     all_grads.update(tg)
@@ -424,6 +539,27 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     if lr is not None:
         sgd_state = sgd_step(all_grads, lr, momentum, weight_decay, sgd_state, world_size)
     return dict(loss=loss, losses=[r["losses"] for r in results], grads=all_grads, sgd_state=sgd_state)
+
+
+def roi_align_backward_slice(grad_act, rois, spatial_scale, grad_in, roi_T, feat_T, t_start, sampling_ratio=0, ws=None):
+    """grad_in [B*feat_T, H, W, C] fp32 += ROIAlign backward of grad_act (Act [R, roi_T, ph, pw, ld] slice of C channels,
+    fp16 | fp32) for ROIs whose frame index is relative to the frames [t_start, t_start + roi_T) of every clip (the frame map
+    of ROINet.pool_into).  Frames outside the slice are untouched.  ws: optional fp32 workspace tensor, reused when large
+    enough; the one used is returned."""
+    ph, pw, C = grad_act.H, grad_act.W, grad_act.C
+    R = grad_act.N * grad_act.T
+    dev = L.same_device(grad_act.buf, rois, grad_in)
+    K, H, W = grad_in.shape[0], grad_in.shape[1], grad_in.shape[2]
+    r = rois.detach().float().contiguous()
+    with torch.cuda.device(dev):
+        nbytes = L.lib().step_roi_align_bwd_slice_workspace_bytes(K, H, W, C, roi_T, feat_T)
+        if ws is None or ws.numel() * 4 < nbytes:
+            ws = torch.empty((max(nbytes, 16) // 4,), dtype=torch.float32, device=dev)
+        L.check(L.lib().step_roi_align_bwd_slice_nhwc(L.c_void_p(grad_act.data_ptr()), grad_act.code, grad_act.ld, L.ptr(r), R,
+                                                      float(spatial_scale), ph, pw, K, H, W, C, int(sampling_ratio), int(roi_T),
+                                                      int(feat_T), int(t_start), L.ptr(grad_in), grad_in.shape[3], L.ptr(ws),
+                                                      ws.numel() * 4, L.stream()))
+    return ws
 
 
 def roi_align_backward_nhwc_strided(grad_act, rois, spatial_scale, K, H, W, sampling_ratio=0):

@@ -5,7 +5,9 @@ TwoBranchNet.forward(global_feat[R,T',832,7,7], context_feat=None|[R,1024,T',1,1
   -> (global_prob[R,cls], local_loc[R,T',4], first_loc[R,T,4], last_loc[R,T,4], loss x3)
 With targets=None the three losses are returned as zeros exactly as the reference does
 (two_branch.py:278-280, 338-340); with targets they are computed on the device (step_b200/training.py::head_losses,
-eval-mode dropout).  The outputs carry no grad_fn: the backward of the convolutions is not built yet.
+eval-mode dropout).  The outputs carry no grad_fn: the backward of the head (with or without the context columns) and of
+ContextNet runs explicitly on the forward's tape (step_b200/training.py: head_forward_backward, context_backward,
+train_step).
 
 Layout tricks (none changes results beyond fp rounding):
   * ROI features and the 1x1x1 `downsample` output share one [R*T',7,7,1088] buffer, so the concat
@@ -144,11 +146,14 @@ class ContextNet(nn.Module):
             ctx = self.forward_act(to_act(conv_feat, E.dtype_code(self.fp16)))  # [N, T', 1024] fp32
         return ctx.permute(0, 2, 1).unsqueeze(-1).unsqueeze(-1)
 
-    def forward_act(self, a):
-        """Act [N,T',H',W',832] -> fp32 tensor [N, T', 1024] (spatial mean)."""
+    def forward_act(self, a, keep=None):
+        """Act [N,T',H',W',832] -> fp32 tensor [N, T', 1024] (spatial mean).  keep: dict that receives Mixed_5c's output
+        Act under "mixed_5c" (the input of the spatial mean, for the backward in step_b200/training.py)."""
         x = self.i3d_conv_context[0](a)
         x = self.i3d_conv_context[1](x)
         x = self.i3d_conv_context[2](x)
+        if keep is not None:
+            keep["mixed_5c"] = x
         # mean over the H*W pixels of every (n, t): [A = N*T', B = H*W, P = 1, C]
         y = E.mean_mid(x.data_ptr(), x.code, x.N * x.T, x.H * x.W, 1, x.C, x.ld, x.device)
         return y.view(x.N, x.T, x.C)
@@ -252,7 +257,7 @@ class TwoBranchNet(nn.Module):
         if targets is None:
             return prob, loc, first, last, z.view(-1), z.view(-1), z.view(-1)
         # training-time outputs (two_branch.py:276-341), eval-mode dropout; the losses are computed on the device.
-        # NOTE: the outputs carry no grad_fn -- the backward of the convolutions is not built yet (step_b200/training.py).
+        # NOTE: the outputs carry no grad_fn -- the backward runs explicitly (step_b200/training.py::head_forward_backward).
         from . import training
         if tubes is None:
             raise RuntimeError("TwoBranchNet.forward: targets need tubes")
