@@ -299,6 +299,52 @@ int step_maxpool3d_bwd_f16(const void* x, int x_ld, const void* dy, int dy_ld, i
                            int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
                            int pad_hi_w, int OT, int OH, int OW, void* dx, int dx_ld, uint8_t* argmax_ws, step_stream_t stream);
 
+/* ------------------------------------------------------------------ optimizer ------------ */
+/* Multi-tensor parameter update (train.py:123-128, 345-348): one launch over every tensor of a parameter set, described by a
+ * device table of step_optim_tensor rows and a device block map.  Row r describes one fp32 tensor of `numel` contiguous
+ * elements; block b of a launch works on elements [chunk * step_multi_tensor_chunk(), + step_multi_tensor_chunk()) of row
+ * blocks[b].tensor, so a tensor of n elements needs ceil(n / step_multi_tensor_chunk()) map entries.  The per-row scalars are
+ * the ones torch's single-tensor optimizers pass to their kernels, computed on the host in double and rounded to float:
+ *   Adam: step_size = lr / (1 - beta1^t), inv_bias_correction2_sqrt = 1 / sqrt(1 - beta2^t), one_minus_beta1 = 1 - beta1,
+ *         one_minus_beta2 = 1 - beta2 (exp_avg_sq non-null);
+ *   SGD:  step_size = lr, momentum (exp_avg = momentum buffer, NULL when momentum == 0), buf_uninit = 1 on the buffer's first
+ *         step (the buffer is then set to the gradient, as torch.optim.SGD does).
+ * Every tensor pointer that is 16-byte aligned together with the others of its row takes vector loads and stores. */
+typedef struct {
+  float* param;
+  const float* grad;
+  float* exp_avg;            /* Adam exp_avg | SGD momentum buffer (nullable for SGD) */
+  float* exp_avg_sq;         /* Adam only */
+  long long numel;
+  float step_size;
+  float inv_bias_correction2_sqrt;
+  float weight_decay;        /* L2, added to the gradient (torch's weight_decay, not AdamW) */
+  float one_minus_beta1;
+  float beta2;
+  float one_minus_beta2;
+  float eps;
+  float momentum;
+  int buf_uninit;
+} step_optim_tensor;
+typedef struct {
+  int tensor;                /* row of the table */
+  int chunk;                 /* chunk of that tensor */
+} step_optim_block;
+/* Elements of one tensor one block map entry covers. */
+int step_multi_tensor_chunk(void);
+/* *flag (device int) = 1 if any gradient element of the table is inf or NaN, else 0 (the call clears it first).  Plain stores:
+ * the result is deterministic. */
+int step_multi_tensor_nonfinite_f32(const step_optim_tensor* table, int n_tensors, const step_optim_block* blocks, int n_blocks,
+                                    int* flag, step_stream_t stream);
+/* torch.optim.Adam (amsgrad=False, maximize=False), per element:  g += wd * p;  m = lerp(m, g, 1 - beta1);
+ * v = v * beta2 + (1 - beta2) * g * g;  p -= step_size * m / (sqrt(v) * inv_bias_correction2_sqrt + eps). */
+int step_multi_tensor_adam_f32(const step_optim_tensor* table, int n_tensors, const step_optim_block* blocks, int n_blocks,
+                               step_stream_t stream);
+/* torch.optim.SGD (dampening=0, nesterov=False), per element:  g += wd * p;  buf = buf_uninit ? g : buf * momentum + g;
+ * p -= step_size * (momentum ? buf : g). */
+int step_multi_tensor_sgd_f32(const step_optim_tensor* table, int n_tensors, const step_optim_block* blocks, int n_blocks,
+                              step_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,6 +11,6 @@ from .networks import BaseNet, ROINet  # noqa: F401
 from .two_branch import ContextNet, TwoBranchNet  # noqa: F401
 from .inference import inference  # noqa: F401
 from .runner import StepRunner  # noqa: F401
-from . import postprocess, roi_layers, tube_utils  # noqa: F401
+from . import optim, postprocess, roi_layers, tube_utils  # noqa: F401
 
 __all__ = ["BaseNet", "ROINet", "TwoBranchNet", "ContextNet", "inference", "StepRunner", "roi_layers", "tube_utils", "postprocess"]

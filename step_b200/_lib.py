@@ -32,6 +32,19 @@ class ConvParams(ctypes.Structure):
                 ("ld_extra", c_int * 2), ("coff_extra", c_int * 2), ("zero_cin_last_kt", c_int)]
 
 
+class OptimTensor(ctypes.Structure):
+    """mirror of step_optim_tensor (include/step_b200.h)"""
+    _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p),
+                ("numel", ctypes.c_longlong)] + \
+               [(n, c_float) for n in ("step_size", "inv_bias_correction2_sqrt", "weight_decay", "one_minus_beta1", "beta2",
+                                       "one_minus_beta2", "eps", "momentum")] + [("buf_uninit", c_int)]
+
+
+class OptimBlock(ctypes.Structure):
+    """mirror of step_optim_block (include/step_b200.h)"""
+    _fields_ = [("tensor", c_int), ("chunk", c_int)]
+
+
 def _declare(lib):
     P, I, Fl, S = c_void_p, c_int, c_float, c_void_p  # S = stream
     sigs = {
@@ -83,6 +96,10 @@ def _declare(lib):
         "step_mean_mid_bwd": ([P, I, I, I, I, Fl, P, I, S], c_int),
         "step_f32_accum_f16": ([P, ctypes.c_longlong, I, Fl, P, I, S], c_int),
         "step_maxpool3d_bwd_f16": ([P, I, P, I] + [I] * 20 + [P, I, P, S], c_int),
+        "step_multi_tensor_chunk": ([], c_int),
+        "step_multi_tensor_nonfinite_f32": ([P, I, P, I, P, S], c_int),
+        "step_multi_tensor_adam_f32": ([P, I, P, I, S], c_int),
+        "step_multi_tensor_sgd_f32": ([P, I, P, I, S], c_int),
         "step_debug_tma_tile": ([ctypes.POINTER(ConvParams), I, I, I, I, I, P, P, P, S], c_int),
     }
     for name, (argtypes, restype) in sigs.items():

@@ -6,7 +6,8 @@ backward (`roi_align_backward_nhwc`, and `roi_align_backward_slice` for the temp
 tensor-core weight gradient of the convolutions, max-pool backward, the backward of the whole head including the context
 columns of `global_cls` (`head_forward_backward`), of ContextNet (`context_forward` / `context_backward`) and of the I3D
 trunk (`trunk_forward_backward`), the SGD update with the gradient all-reduce (`sgd_step`) and the whole step in spatial
-and temporal mode with or without the context branch (`train_step`).  `BaseNet` / `ContextNet` / `TwoBranchNet` still run
+and temporal mode with or without the context branch (`train_step`), which can also update through the optimizers of
+`optim` with dynamic loss scaling.  `BaseNet` / `ContextNet` / `TwoBranchNet` still run
 without autograd (their outputs carry no grad_fn): the backward walks the tape their forward records.
 """
 import torch
@@ -427,12 +428,9 @@ def trunk_forward_backward(base_net, clips, d_feat_fn, loss_scale=1024.0):
     return feat, out
 
 
-def sgd_step(params_and_grads, lr, momentum=0.9, weight_decay=0.0, state=None, world_size=1):
-    """optim.SGD(momentum, weight_decay) (train.py:124) on the fp32 master parameters, after an optional gradient
-    all-reduce over the clip-parallel ranks (NCCL; one flat bucket).  state: dict param -> momentum buffer.
-    Host-side glue over torch.distributed + elementwise updates; the parameters change in place (their packed fp16
-    copies are rebuilt by the modules' version-keyed caches on the next forward)."""
-    state = {} if state is None else state
+def _average_gradients(params_and_grads, world_size):
+    """[(param, grad)] of the trainable parameters, the gradients averaged in place over the clip-parallel ranks (NCCL
+    all-reduce of one flat bucket; an inf or NaN on any rank reaches every rank through the sum)."""
     items = [(p, g) for p, g in params_and_grads.items() if p.requires_grad]
     if world_size > 1 and items:
         import torch.distributed as dist
@@ -443,6 +441,16 @@ def sgd_step(params_and_grads, lr, momentum=0.9, weight_decay=0.0, state=None, w
         for _, g in items:
             g.copy_(flat[off:off + g.numel()].view_as(g))
             off += g.numel()
+    return items
+
+
+def sgd_step(params_and_grads, lr, momentum=0.9, weight_decay=0.0, state=None, world_size=1):
+    """optim.SGD(momentum, weight_decay) (train.py:124) on the fp32 master parameters, after an optional gradient
+    all-reduce over the clip-parallel ranks (NCCL; one flat bucket).  state: dict param -> momentum buffer.
+    Host-side glue over torch.distributed + elementwise updates; the parameters change in place (their packed fp16
+    copies are rebuilt by the modules' version-keyed caches on the next forward)."""
+    state = {} if state is None else state
+    items = _average_gradients(params_and_grads, world_size)
     with torch.no_grad():
         for p, g in items:
             g = g.to(p.device, p.dtype)
@@ -466,7 +474,7 @@ def step_frames(cfg, i):
 
 
 def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9, weight_decay=0.0, lambda_reg=5.0,
-               lambda_neighbor=1.0, loss_scale=1024.0, sgd_state=None, world_size=1):
+               lambda_neighbor=1.0, loss_scale=1024.0, sgd_state=None, world_size=1, optimizer=None, scaler=None):
     """One optimisation step of train.py:263-348 on the device, for already selected training samples
     (`train_select`, utils/utils.py:135-423, is the host-side sampling of SURVEY.md section 8f rank 4 and is not built):
         conv_feat = base_net(clips); context_feat = context_net(conv_feat) unless cfg.no_context      train.py:266-269
@@ -479,8 +487,18 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     flatten_tubes(batch_idx=True) builds them), step_targets[i]: [R_i, 3, 6 + classes].
     The gradient of conv_feat is, in this order, the ROIAlign backward of every step (each on its own frame slice) plus
     the context branch's.  Returns dict(loss, losses=[(cls, loc, nb)], grads={param: fp32 grad} (trunk, heads and, with
-    the context branch, ContextNet's convolutions)); updates the parameters when lr is given."""
+    the context branch, ContextNet's convolutions), skipped, loss_scale).
+    Parameter update: with lr, `sgd_step` (one global rate); with optimizer (a step_b200.optim.Adam / SGD over the nets'
+    parameters, e.g. built from the reference's get_params, and lr None), the gradients, averaged over the ranks, become
+    p.grad and optimizer.step() runs -- it skips the update when a gradient is inf or NaN (skipped=True).  scaler (a
+    step_b200.optim.LossScaler; needs optimizer) replaces loss_scale by its dynamic scale and is updated from the step."""
     from .engine import Act
+    if optimizer is not None and lr is not None:
+        raise ValueError("train_step: give either lr (sgd_step) or optimizer, not both")
+    if scaler is not None:
+        if optimizer is None:
+            raise ValueError("train_step: scaler needs an optimizer (it is updated from optimizer.found_inf)")
+        loss_scale = scaler.scale
     base, roi_net = nets["base_net"], nets["roi_net"]
     use_ctx = not getattr(cfg, "no_context", True)
     if use_ctx and nets.get("context_net") is None:
@@ -536,9 +554,18 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     feat, tg = trunk_forward_backward(base, clips, d_feat, loss_scale)
     all_grads.update(tg)
     loss = sum(r["loss"] for r in results)
-    if lr is not None:
+    skipped = False
+    if optimizer is not None:
+        for p, g in _average_gradients(all_grads, world_size):
+            p.grad = g
+        optimizer.step()
+        skipped = bool(optimizer.found_inf)
+        if scaler is not None:
+            scaler.update(skipped)
+    elif lr is not None:
         sgd_state = sgd_step(all_grads, lr, momentum, weight_decay, sgd_state, world_size)
-    return dict(loss=loss, losses=[r["losses"] for r in results], grads=all_grads, sgd_state=sgd_state)
+    return dict(loss=loss, losses=[r["losses"] for r in results], grads=all_grads, sgd_state=sgd_state, skipped=skipped,
+                loss_scale=loss_scale)
 
 
 def roi_align_backward_slice(grad_act, rois, spatial_scale, grad_in, roi_T, feat_T, t_start, sampling_ratio=0, ws=None):
