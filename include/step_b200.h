@@ -245,6 +245,13 @@ int step_head_losses_f32(const float* logits, const float* local_loc, const floa
                          const float* tubes, const float* targets, int N, int cls, int T_len, int T, int Tc, float w_loc,
                          float w_nb, float* loss_cls, float* loss_loc, float* loss_nb, int* flags, float* dlogits,
                          float* dloc, float* dfirst, float* dlast, float* scratch, step_stream_t stream);
+/* The loss of a class-only head (TwoBranchNet(cls_only=True), models/two_branch.py:291-297; train_cls.py:310-311) and, when
+ * dlogits is given, d mean(loss_cls) / d logits, with the arithmetic of step_head_losses_f32's classification part (bit for
+ * bit the same loss_cls and dlogits).  logits [N,cls] (pre-sigmoid), targets [N,3,6+cls] (only the centre row is read).
+ * loss_cls [N*cls] is the element-wise BCE; flags[0] = 0 when the centre rows' classification masks sum to zero, and then
+ * loss_cls and dlogits are zeros (the reference returns a [1] zero loss). */
+int step_cls_loss_f32(const float* logits, const float* targets, int N, int cls, float* loss_cls, int* flags, float* dlogits,
+                      step_stream_t stream);
 /* Channels-last ROIAlign backward without atomics (replaces _C.roi_align_backward, vision.cpp:33 /
  * cuda/ROIAlign_cuda.cu:201-278, whose atomicAdd scatter is not repeatable): grad_out [R,ph,pw,C] (channel stride
  * out_ld, STEP_F32 / STEP_F16) -> grad_in [K,H,W,C] fp32 (channel stride in_ld), written completely by the call. */

@@ -82,6 +82,7 @@ def _declare(lib):
         "step_bottleneck_exit_f16": ([P, ctypes.c_longlong, P, P, ctypes.c_longlong, P, P, I, P, ctypes.c_longlong, P, ctypes.c_longlong,
                                      ctypes.c_longlong, I, I, I, S], c_int),
         "step_head_losses_f32": ([P, P, P, P, P, P, I, I, I, I, I, Fl, Fl, P, P, P, P, P, P, P, P, P, S], c_int),
+        "step_cls_loss_f32": ([P, P, I, I, P, P, P, S], c_int),
         "step_roi_align_bwd_nhwc": ([P, I, I, P, I, Fl, I, I, I, I, I, I, I, P, I, S], c_int),
         "step_roi_align_bwd_slice_workspace_bytes": ([I, I, I, I, I, I], c_size_t),
         "step_roi_align_bwd_slice_nhwc": ([P, I, I, P, I, Fl, I, I, I, I, I, I, I, I, I, I, P, I, P, c_size_t, S], c_int),

@@ -2,6 +2,9 @@
 //   * head_losses_kernel       TwoBranchNet's three losses (models/two_branch.py:276-333) and, in the same pass, the
 //                              gradient of the training objective  mean(loss_cls) + w_loc * loss_loc + w_nb * loss_nb
 //                              (train.py:323-347) with respect to the head outputs;
+//   * cls_loss_kernel          the loss of class-only heads (TwoBranchNet(cls_only=True), the first training stage of
+//                              train_cls.py) and d mean(loss_cls) / d logits, with the classification arithmetic of
+//                              head_losses_kernel (one shared device function);
 //   * roi_align_bwd_nhwc       channels-last ROIAlign backward WITHOUT float atomics: every feature pixel gathers its
 //                              contributions in a fixed order (ROI index, bin, sample), so the result is bit-for-bit
 //                              repeatable -- the reference's RoIAlignBackwardFeature (cuda/ROIAlign_cuda.cu:201-278) scatters
@@ -52,6 +55,38 @@ __device__ __forceinline__ float smooth_l1(float d, float* grad) {
   return __fsub_rn(ad, 0.5f);
 }
 
+// Sum of the centre rows' classification masks, targets[n][1][4], in tube order (two_branch.py:291-293).  One thread.
+__device__ __forceinline__ float cls_mask_sum(const float* __restrict__ targets, int N, int tgt_ld) {
+  float mc = 0.0f;
+  for (int n = 0; n < N; ++n) mc = __fadd_rn(mc, targets[((size_t)n * 3 + 1) * tgt_ld + 4]);
+  return mc;
+}
+
+// Classification loss of the centre chunk (two_branch.py:291-297) over the [N, cls] logits, block-strided: BCE with logits
+// against the labels masked by the centre row's classification flag, and d mean(loss_cls) / d logit.  Without any
+// classification sample (has_cls false) both are zero.  Shared by head_losses_kernel and cls_loss_kernel so that the two
+// agree bit for bit.
+__device__ __forceinline__ void cls_loss_pass(const float* __restrict__ logits, const float* __restrict__ targets, int N, int cls,
+                                              int tgt_ld, bool has_cls, float* __restrict__ loss_cls, float* __restrict__ dlogits) {
+  const float inv_ncls = 1.0f / (float)((long long)N * cls);
+  for (int i = threadIdx.x; i < N * cls; i += blockDim.x) {
+    const int n = i / cls, c = i - n * cls;
+    const float x = logits[i];
+    float l = 0.0f, gx = 0.0f;
+    if (has_cls) {
+      const float* tc = targets + ((size_t)n * 3 + 1) * tgt_ld;
+      const float t = __fmul_rn(tc[6 + c], tc[4]);
+      // ATen: (1 - t) * x - log_sigmoid(x),  log_sigmoid(x) = min(x, 0) - log1p(exp(-|x|))
+      const float ls = __fsub_rn(fminf(x, 0.0f), log1pf(expf(-fabsf(x))));
+      l = __fsub_rn(__fmul_rn(__fsub_rn(1.0f, t), x), ls);
+      const float sg = 1.0f / (1.0f + expf(-x));
+      gx = __fmul_rn(__fsub_rn(sg, t), inv_ncls);              // d mean(loss_cls) / d logit
+    }
+    loss_cls[i] = l;
+    if (dlogits) dlogits[i] = gx;
+  }
+}
+
 struct LossGeom {
   int N, cls, T_len, Tc;     // tubes, classes, frames of local_loc, frames of first/last_loc (= T)
   int centre, first_idx, last_idx, half_T;   // chunk_idx[chunks/2], chunk_idx[0], chunk_idx[-1] (two_branch.py:226-228)
@@ -76,8 +111,8 @@ __global__ void __launch_bounds__(256) head_losses_kernel(LossGeom g, const floa
   // targets[n][j] with j = 0 first, 1 centre, 2 last (two_branch.py:283-285: [:, 0], [:, 1], [:, -1])
   auto tgt = [&](int n, int j) { return targets + ((size_t)n * 3 + j) * g.tgt_ld; };
   if (threadIdx.x == 0) {
-    float mc = 0.0f, ml = 0.0f, mn = 0.0f;
-    for (int n = 0; n < N; ++n) mc = __fadd_rn(mc, tgt(n, 1)[4]);
+    const float mc = cls_mask_sum(targets, N, g.tgt_ld);
+    float ml = 0.0f, mn = 0.0f;
     for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) ml = __fadd_rn(ml, tgt(n, 1)[5]);
     for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) mn = __fadd_rn(mn, tgt(n, 0)[5]);
     for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) mn = __fadd_rn(mn, tgt(n, 2)[5]);
@@ -87,22 +122,7 @@ __global__ void __launch_bounds__(256) head_losses_kernel(LossGeom g, const floa
   __syncthreads();
   const bool has_cls = s_sum[0] != 0.0f, has_loc = s_sum[1] != 0.0f, has_nb = s_sum[2] != 0.0f;
   // ---- classification: BCE with logits on the centre chunk, background samples masked (two_branch.py:291-297)
-  const float inv_ncls = 1.0f / (float)((long long)N * g.cls);
-  for (int i = threadIdx.x; i < N * g.cls; i += blockDim.x) {
-    const int n = i / g.cls, c = i - n * g.cls;
-    const float x = logits[i];
-    float l = 0.0f, gx = 0.0f;
-    if (has_cls) {
-      const float t = __fmul_rn(tgt(n, 1)[6 + c], tgt(n, 1)[4]);
-      // ATen: (1 - t) * x - log_sigmoid(x),  log_sigmoid(x) = min(x, 0) - log1p(exp(-|x|))
-      const float ls = __fsub_rn(fminf(x, 0.0f), log1pf(expf(-fabsf(x))));
-      l = __fsub_rn(__fmul_rn(__fsub_rn(1.0f, t), x), ls);
-      const float sg = 1.0f / (1.0f + expf(-x));
-      gx = __fmul_rn(__fsub_rn(sg, t), inv_ncls);              // d mean(loss_cls) / d logit
-    }
-    loss_cls[i] = l;
-    if (dlogits) dlogits[i] = gx;
-  }
+  cls_loss_pass(logits, targets, N, g.cls, g.tgt_ld, has_cls, loss_cls, dlogits);
   // ---- regression: per-tube smooth-L1 terms staged in `scratch` [N][3][4] (loss) and gradients written in place
   if (dloc) for (int i = threadIdx.x; i < N * g.T_len * 4; i += blockDim.x) dloc[i] = 0.0f;
   if (dfirst) for (int i = threadIdx.x; i < N * g.Tc * 4; i += blockDim.x) { dfirst[i] = 0.0f; dlast[i] = 0.0f; }
@@ -158,6 +178,20 @@ __global__ void __launch_bounds__(256) head_losses_kernel(LossGeom g, const floa
       if (b != 0.0f) dloc[((size_t)n * g.T_len + g.e0) * 4 + r] += b;
     }
   }
+}
+
+// The loss of class-only heads (TwoBranchNet(cls_only=True), two_branch.py:291-297): the classification part of
+// head_losses_kernel alone, with no regression inputs.  One CTA.
+__global__ void __launch_bounds__(256) cls_loss_kernel(int N, int cls, const float* __restrict__ logits,
+                                                       const float* __restrict__ targets, float* __restrict__ loss_cls,
+                                                       int* __restrict__ flags, float* __restrict__ dlogits) {
+  __shared__ float s_mc;
+  if (threadIdx.x == 0) {
+    s_mc = cls_mask_sum(targets, N, 6 + cls);
+    flags[0] = s_mc != 0.0f;
+  }
+  __syncthreads();
+  cls_loss_pass(logits, targets, N, cls, 6 + cls, s_mc != 0.0f, loss_cls, dlogits);
 }
 
 // ---- ROIAlign backward, channels-last, deterministic ----------------------------------------------------------------
@@ -612,6 +646,15 @@ extern "C" int step_head_losses_f32(const float* logits, const float* local_loc,
   head_losses_kernel<<<1, 256, 0, cu(stream)>>>(g, logits, local_loc, first_loc, last_loc, tubes, targets, loss_cls, loss_loc, loss_nb,
                                                 flags, dlogits, dloc, dfirst, dlast, scratch);
   STEP_LAUNCH_CHECK("head_losses_kernel");
+  return 0;
+}
+
+extern "C" int step_cls_loss_f32(const float* logits, const float* targets, int N, int cls, float* loss_cls, int* flags,
+                                 float* dlogits, step_stream_t stream) {
+  STEP_CHECK_ARG(N > 0 && cls > 0, "cls_loss: bad shape N=%d cls=%d", N, cls);
+  STEP_CHECK_ARG(logits && targets && loss_cls && flags, "cls_loss: null pointer");
+  cls_loss_kernel<<<1, 256, 0, cu(stream)>>>(N, cls, logits, targets, loss_cls, flags, dlogits);
+  STEP_LAUNCH_CHECK("cls_loss_kernel");
   return 0;
 }
 

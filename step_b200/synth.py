@@ -120,6 +120,15 @@ def head_state_dict(seed, cfg, reg_std=5e-5, cls_std=2e-3):
     return sd
 
 
+CLS_HEAD_PREFIXES = ("i3d_conv.", "downsample.", "global_cls.")
+
+
+def cls_head_state_dict(seed, cfg, **kw):
+    """Keys of TwoBranchNet(cfg, cls_only=True).state_dict() (two_branch.py:181-189): head_state_dict without the local
+    branch, so the shared tensors equal those of the full head of the same seed."""
+    return {k: v for k, v in head_state_dict(seed, cfg, **kw).items() if k.startswith(CLS_HEAD_PREFIXES)}
+
+
 def make_clips(B, T_in, H, W, seed=1234):
     """[B, T_in, 3, H, W] fp32 in [-1, 1] (the layout BaseNet.forward takes, networks.py:69-76)."""
     g = torch.Generator().manual_seed(seed)
@@ -231,6 +240,38 @@ def make_train_case(cfg, B, N, W, H, seed=3):
         step_tubes.append(tubes.contiguous())
         step_targets.append(tg)
     return step_tubes, step_targets
+
+
+def make_cls_case(cfg, B, N, W, H, seed=3):
+    """Seeded samples of one step of the classification pre-training stage, shaped as train_cls.py:260-297 builds them:
+    (flat_tubes [B*N, cfg.T, 5] fp32 with the frame index b * T + t first (flatten_tubes(batch_idx=True)), flat_targets
+    [B*N, 3, 6 + classes]).  Each clip has min(5, (N + 3) // 4) positives (select_proposals(..., 0.75, 5, 'uniform', 3)
+    keeps at most 5) followed by negatives; with B > 1 the last clip has negatives only.  A positive row holds its ground
+    truth box in columns :4 and its labels in 6:; every row has the classification flag (column 4) set and none the
+    regression flag (column 5); the one target frame is tiled three times.  Boxes lie inside a W x H image."""
+    g = torch.Generator().manual_seed(seed)
+    T_, C = cfg.T, cfg.num_classes
+    n_pos = min(5, (N + 3) // 4)
+    tubes, targets = [], []
+    for b in range(B):
+        pos = 0 if (B > 1 and b == B - 1) else n_pos
+        x1 = torch.rand(N, 1, generator=g) * 0.4 * W
+        y1 = torch.rand(N, 1, generator=g) * 0.4 * H
+        w = (0.2 + torch.rand(N, 1, generator=g) * 0.35) * W
+        hh = (0.2 + torch.rand(N, 1, generator=g) * 0.35) * H
+        box = torch.cat([x1, y1, x1 + w, y1 + hh], 1)
+        jit = torch.rand(N, T_, 4, generator=g) * 0.02 * W
+        frame = (b * T_ + torch.arange(T_, dtype=torch.float32)).view(1, T_, 1).expand(N, T_, 1)
+        tubes.append(torch.cat([frame, box.view(N, 1, 4) + jit], 2))
+        tg = torch.zeros(N, 1, 6 + C)
+        if pos:
+            tg[:pos, 0, :4] = box[:pos] + (torch.rand(pos, 4, generator=g) - 0.5) * 0.04 * W
+            lab = (torch.rand(pos, C, generator=g) > 0.9).float()
+            lab[torch.arange(pos), torch.randint(0, C, (pos,), generator=g)] = 1.0
+            tg[:pos, 0, 6:] = lab
+        tg[:, 0, 4] = 1.0
+        targets.append(tg.repeat(1, 3, 1))
+    return torch.cat(tubes).contiguous(), torch.cat(targets).contiguous()
 
 
 def make_conv_feat(B, T, H, W, seed=2468):

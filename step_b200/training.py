@@ -53,6 +53,30 @@ def head_losses(logits, local_loc, first_loc, last_loc, tubes, targets, T, lambd
     return (loss_cls, loss_loc, loss_nb) if not want_grads else (loss_cls, loss_loc, loss_nb, g)
 
 
+def cls_loss(logits, targets, want_grads=False):
+    """The loss of a class-only head (TwoBranchNet(cls_only=True), models/two_branch.py:291-297) on the device: logits
+    [N,cls] (pre-sigmoid), targets [N,3,6+cls] (train_cls.py:260-297 tiles one frame three times; the centre row is read).
+    Returns loss_cls, the element-wise BCE [N*cls] or the [1] zero of the reference when no row has the classification flag,
+    and with want_grads also d mean(loss_cls) / d logits [N,cls] (zeros in that case).  Bit for bit the classification part
+    of `head_losses`."""
+    dev = L.same_device(logits, targets)
+    logits = logits.detach().to(torch.float32).contiguous()
+    targets = targets.detach().to(torch.float32).contiguous()
+    N, cls = logits.shape
+    if targets.shape != (N, 3, 6 + cls):
+        raise RuntimeError("cls_loss: targets %s do not match N=%d, classes=%d" % (tuple(targets.shape), N, cls))
+    with torch.cuda.device(dev):
+        loss_cls = torch.empty((N * cls,), dtype=torch.float32, device=dev)
+        flags = torch.empty((1,), dtype=torch.int32, device=dev)
+        dlogits = torch.empty_like(logits) if want_grads else None
+        L.check(L.lib().step_cls_loss_f32(L.ptr(logits), L.ptr(targets), N, cls, L.ptr(loss_cls), L.ptr(flags), L.ptr(dlogits),
+                                          L.stream()))
+        # `if mask.sum():` in the reference is the same host read-back (two_branch.py:293)
+        if int(flags[0].item()) == 0:
+            loss_cls = torch.zeros((1,), dtype=torch.float32, device=dev)
+    return (loss_cls, dlogits) if want_grads else loss_cls
+
+
 def linear_backward(x, w, dy, need_dx=True, need_dw=True, dx_out=None, accumulate_dx=False):
     """Backward of y = x W^T + b (nn.Linear, or the 1x1x1 `global_cls` on flattened features) for the head's small-N
     layers: x [M,K] fp16|fp32, w [Nn,K] fp32, dy [M,Nn] fp32 -> (dx [M,K] fp32 | None, dw [Nn,K] | None, db [Nn] | None)."""
@@ -260,6 +284,9 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
     with respect to every trainable parameter of the head and to the pooled ROI features.  fp16 activations / activation
     gradients with a static loss scale (apex-style), fp32 weight gradients.  Dropout is the identity (eval mode), like the
     reference's gradient goldens.
+    Class-only heads (TwoBranchNet(cls_only=True), the first training stage of train_cls.py) have no local branch: the
+    objective is mean(loss_cls) alone (`cls_loss`), the regression losses are the reference's [1] zeros and grads holds the
+    16 tensors of Mixed_5b / Mixed_5c, `downsample` and `global_cls`.
     context_feat (heads built with the context columns, cfg.no_context=False), in one of two forms:
       * [N,1024,T',1,1], the per-tube context feature the reference passes (train.py:317-321, two_branch.py:242-249);
       * (ctx_mean, row_map): ctx_mean fp32 [rows, 1024] is the mean of the context feature over the step's frames and
@@ -308,7 +335,13 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
             prob, loc, first, last, logits = net.forward_act(cat, ctx_mean, row_map, want_logits=True, keep=keep)
         finally:
             E.TAPE, E.BRANCH_STREAMS = saved_tape, saved_bs
-        lc, ll, ln, g = head_losses(logits, loc, first, last, tubes, targets, net.T, lambda_reg, lambda_neighbor, want_grads=True)
+        if net.cls_only:
+            # class-only heads: the regression losses are the reference's zeros (two_branch.py:252,276-280)
+            lc, dlogits = cls_loss(logits, targets, want_grads=True)
+            ll, ln = torch.zeros((1,), dtype=torch.float32, device=dev), torch.zeros((1,), dtype=torch.float32, device=dev)
+            g = {"logits": dlogits}
+        else:
+            lc, ll, ln, g = head_losses(logits, loc, first, last, tubes, targets, net.T, lambda_reg, lambda_neighbor, want_grads=True)
         if objective_scale != 1.0:
             for k_ in g:
                 g[k_].mul_(objective_scale)
@@ -332,21 +365,23 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
         gcat = grads.of(cat)
         L.check(L.lib().step_mean_mid_bwd(L.ptr(dxbar), N, Tl, ps * ps, fc, float(loss_scale),
                                           L.c_void_p(gcat.data_ptr() + 2 * C), gcat.ld, L.stream()))
-        # ---- regressors (two_branch.py:261-270): local_reg on every frame, neighbor_reg1 / 2 on the first / last chunk
-        lf2 = keep["local_feat2"]
-        lf2v = lf2.buf.view(N, Tl, D)
-        s0, s1, e0, e1 = keep["slices"]
-        dlf2 = torch.zeros((N, Tl, D), dtype=torch.float32, device=dev)
-        dx, dw, db = linear_backward(lf2v.reshape(N * Tl, D), hw["local_reg_w32"], g["local_loc"].reshape(N * Tl, 4), dx_out=dlf2.view(N * Tl, D))
-        out[net.local_reg.weight], out[net.local_reg.bias] = unperm(dw), db
-        for mod, nm, (a, b), gk in ((net.neighbor_reg1, "neighbor_reg1", (s0, s1), "first_loc"), (net.neighbor_reg2, "neighbor_reg2", (e0, e1), "last_loc")):
-            xs = lf2v[:, a:b].reshape(-1, D).contiguous()
-            dx, dw, db = linear_backward(xs, hw[nm + "_w32"], g[gk].reshape(-1, 4))
-            dlf2[:, a:b] += dx.view(N, b - a, D)                      # disjoint frame ranges of one buffer (host-side glue)
-            out[mod.weight], out[mod.bias] = unperm(dw), db
-        glf2 = grads.of(lf2)
-        L.check(L.lib().step_f32_accum_f16(L.ptr(dlf2), N * Tl * ps * ps, fc, float(loss_scale), L.c_void_p(glf2.data_ptr()), glf2.ld,
-                                           L.stream()))
+        # ---- regressors (two_branch.py:261-270): local_reg on every frame, neighbor_reg1 / 2 on the first / last chunk.
+        # Class-only heads have no local branch: their tape ends at `downsample`.
+        if not net.cls_only:
+            lf2 = keep["local_feat2"]
+            lf2v = lf2.buf.view(N, Tl, D)
+            s0, s1, e0, e1 = keep["slices"]
+            dlf2 = torch.zeros((N, Tl, D), dtype=torch.float32, device=dev)
+            dx, dw, db = linear_backward(lf2v.reshape(N * Tl, D), hw["local_reg_w32"], g["local_loc"].reshape(N * Tl, 4), dx_out=dlf2.view(N * Tl, D))
+            out[net.local_reg.weight], out[net.local_reg.bias] = unperm(dw), db
+            for mod, nm, (a, b), gk in ((net.neighbor_reg1, "neighbor_reg1", (s0, s1), "first_loc"), (net.neighbor_reg2, "neighbor_reg2", (e0, e1), "last_loc")):
+                xs = lf2v[:, a:b].reshape(-1, D).contiguous()
+                dx, dw, db = linear_backward(xs, hw[nm + "_w32"], g[gk].reshape(-1, 4))
+                dlf2[:, a:b] += dx.view(N, b - a, D)                      # disjoint frame ranges of one buffer (host-side glue)
+                out[mod.weight], out[mod.bias] = unperm(dw), db
+            glf2 = grads.of(lf2)
+            L.check(L.lib().step_f32_accum_f16(L.ptr(dlf2), N * Tl * ps * ps, fc, float(loss_scale), L.c_void_p(glf2.data_ptr()), glf2.ld,
+                                               L.stream()))
         # ---- every convolution and pool of the head, in reverse
         out.update(tape_backward(tape, grads, loss_scale))
         gcat = grads.of(cat)
@@ -485,6 +520,8 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
         loss_back.backward(); optimizer.step()                                                             train.py:345-348
     step_tubes[i]: [R_i, T_length_i, 5] fp32 (frame index first, relative to the step's frame slice, as
     flatten_tubes(batch_idx=True) builds them), step_targets[i]: [R_i, 3, 6 + classes].
+    Heads built with cls_only=True run the first training stage (train_cls.py:253-322, one step of T_length = cfg.T): their
+    objective is loss_cls.mean() alone, and their gradients are those of Mixed_5b / Mixed_5c, `downsample` and `global_cls`.
     The gradient of conv_feat is, in this order, the ROIAlign backward of every step (each on its own frame slice) plus
     the context branch's.  Returns dict(loss, losses=[(cls, loc, nb)], grads={param: fp32 grad} (trunk, heads and, with
     the context branch, ContextNet's convolutions), skipped, loss_scale).

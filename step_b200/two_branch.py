@@ -5,9 +5,9 @@ TwoBranchNet.forward(global_feat[R,T',832,7,7], context_feat=None|[R,1024,T',1,1
   -> (global_prob[R,cls], local_loc[R,T',4], first_loc[R,T,4], last_loc[R,T,4], loss x3)
 With targets=None the three losses are returned as zeros exactly as the reference does
 (two_branch.py:278-280, 338-340); with targets they are computed on the device (step_b200/training.py::head_losses,
-eval-mode dropout).  The outputs carry no grad_fn: the backward of the head (with or without the context columns) and of
-ContextNet runs explicitly on the forward's tape (step_b200/training.py: head_forward_backward, context_backward,
-train_step).
+eval-mode dropout; heads built with cls_only=True compute the classification loss alone, training.cls_loss).  The outputs
+carry no grad_fn: the backward of the head (with or without the context columns) and of ContextNet runs explicitly on the
+forward's tape (step_b200/training.py: head_forward_backward, context_backward, train_step).
 
 Layout tricks (none changes results beyond fp rounding):
   * ROI features and the 1x1x1 `downsample` output share one [R*T',7,7,1088] buffer, so the concat
@@ -261,9 +261,10 @@ class TwoBranchNet(nn.Module):
         from . import training
         if tubes is None:
             raise RuntimeError("TwoBranchNet.forward: targets need tubes")
-        if self.cls_only:
-            raise NotImplementedError("TwoBranchNet(cls_only=True).forward(targets=...) is not built")
         tb, tg = tubes.to(prob.device), targets.to(prob.device)
+        if self.cls_only:
+            # train_cls.py:310: only the classification loss; the regression losses are zeros (two_branch.py:276-280)
+            return prob, loc, first, last, training.cls_loss(logits, tg), z.view(-1), z.view(-1)
         lc, ll, ln = training.head_losses(logits, loc, first, last, tb, tg, self.T)
         return prob, loc, first, last, lc, ll, ln
 
@@ -298,6 +299,8 @@ class TwoBranchNet(nn.Module):
                 E.linear_small_n(ctx_mean, R, 1024, 1024, hw["ctx_w"], None, self.num_classes, y=raw, act=0,
                                  accumulate=True, row_map=ctx_row_map)
         if self.cls_only:
+            if keep is not None:
+                keep.update(xbar=xbar)
             z = torch.tensor([0.], device=prob.device)
             return (prob, z, z, z, raw) if want_logits else (prob, z, z, z)
         # local branch on frames (two_branch.py:253-262)
