@@ -170,7 +170,8 @@ typedef struct {
   int res_ld, res_coff;
   void* y;
   int a_mode;                /* f16 path: 0 auto, 1 linear (1x1x1 only), 2 box tiles, 3 TMA im2col,
-                                4 input patch staged in shared memory (stride 1, Cin in {16,32,64}, Cout <= 256),
+                                4 input patch staged in shared memory (stride 1, Cin in {16,32,64}, Cout <= 256;
+                                  or the s2d stem, see zero_cin_last_kt),
                                 5 best of 3 / 4 per layer shape, 9 SIMT */
   /* Horizontally fused 1x1x1 layers that share an input (Mixed.branch_0 / branch_1[0] / branch_2[0],
    * i3dpt.py:133-147): output channels [0, split[0]) go to y, [split[0], split[1]) to y_extra[0],
@@ -182,9 +183,10 @@ typedef struct {
   int ld_extra[2];
   int coff_extra[2];
   /* Structured zeros of the weights (a_mode 4 only): for the filter taps of the LAST t plane (kt == KT-1) the input
-   * channels [zero_cin_last_kt, Cin) carry zero weights.  0 = no such structure.  Advisory: the kernels multiply the
-   * zeros (exactly) rather than skip them.  The space-to-depth stem has it: tap plane qt = 2 only holds the rt = 0 sub-position (k = 2(q+1)+r <= 6),
-   * engine.pack_stem_s2d. */
+   * channels [zero_cin_last_kt, Cin) carry zero weights.  0 = no such structure.  The space-to-depth stem has it: tap plane
+   * qt = 2 only holds the rt = 0 sub-position (k = 2(q+1)+r <= 6), engine.pack_stem_s2d.  The stem kernel (a_mode 4,
+   * Cin = 24, Cout = 64, 4x4x4, pad 1) is chosen only when 0 < zero_cin_last_kt <= 16 and skips channels 16..23 of that
+   * plane; the generic patch kernel multiplies the zeros. */
   int zero_cin_last_kt;
 } step_conv_params;
 int step_conv3d_fwd(const step_conv_params* p, step_stream_t stream);

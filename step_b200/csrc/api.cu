@@ -28,6 +28,8 @@ int conv3d_simt_launch(const step_conv_params* p, step_stream_t stream);
 int conv3d_umma_launch(const step_conv_params* p, step_stream_t stream);
 int conv3d_halo_launch(const step_conv_params* p, step_stream_t stream);
 bool conv3d_halo_supported(const step_conv_params* p);
+int conv3d_stem_launch(const step_conv_params* p, step_stream_t stream);
+bool conv3d_stem_supported(const step_conv_params* p);
 
 }  // namespace step
 
@@ -52,7 +54,8 @@ extern "C" int step_conv3d_fwd(const step_conv_params* p, step_stream_t stream) 
   STEP_CHECK_ARG((p->OT - 1) * p->ST - p->PT < p->T && (p->OH - 1) * p->SH - p->PH < p->H && (p->OW - 1) * p->SW - p->PW < p->W,
                  "conv3d: output extent inconsistent with input/stride/pad");
   if (p->dtype == STEP_F32 || p->a_mode == 9) return conv3d_simt_launch(p, stream);
-  if (p->a_mode == 4) {   // explicit request: patch-in-shared-memory kernel (conv_halo.cu)
+  if (p->a_mode == 4) {   // explicit request: a patch-in-shared-memory kernel (conv_stem.cu for the s2d stem, else conv_halo.cu)
+    if (conv3d_stem_supported(p)) return conv3d_stem_launch(p, stream);
     STEP_CHECK_ARG(p->ST == 1 && p->SH == 1 && p->SW == 1 && conv3d_halo_supported(p), "conv3d: a_mode 4 (halo) does not fit this problem");
     return conv3d_halo_launch(p, stream);
   }

@@ -1,5 +1,5 @@
-// conv_halo.cu -- stride-1 k>1 convolution on thin inputs (Cin <= 64 channels: the space-to-depth I3D stem,
-// models/i3dpt.py:184-190 after engine.pack_stem_s2d) with the input neighbourhood staged ONCE in shared memory.
+// conv_halo.cu -- stride-1 k>1 convolution on thin inputs (Cin <= 64 channels: the 3x3x3 layers of the Mixed blocks'
+// second branch; the space-to-depth I3D stem runs in conv_stem.cu) with the input neighbourhood staged ONCE in shared memory.
 //
 // The im2col path of conv_umma.cu fetches a fresh 128-row A tile from L2 for every filter tap; with 32 input channels a tap
 // is a K=32 sliver and the kernel is bound by the bytes it pulls through TMA for each of them.  Here a CTA owns an output

@@ -56,6 +56,12 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
 }
+// Four 8 x 8 fp16 matrices stored transposed: v[m] holds this thread's pair (row lane / 4, columns 2 (lane % 4) + {0, 1})
+// of matrix m; lanes 8 m .. 8 m + 7 give the addresses of its memory rows 0..7, and memory row c receives column c.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t* v) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all but the newest N committed bulk stores have finished reading their shared-memory source
 template <int N>

@@ -71,10 +71,12 @@ class Unit3Dpy(torch.nn.Module):
         """fp16 stem: x_s2d is the space-to-depth clip [N, T/2, H/2, W/2, 32]; 4x4x4 filter, pad 1."""
         w, scale, shift = self.packed(L.F16, s2d=True)
         out = Act.empty(x_s2d.N, x_s2d.T, x_s2d.H, x_s2d.W, self.conv3d.out_channels, L.F16, x_s2d.device)
-        # patch-in-shared-memory kernel (csrc/conv_halo.cu) unless STEP_B200_STEM_HALO=0
+        # only the 8 * Cin live channels of the s2d buffer are convolved (the rest of its row is padding)
+        x = x_s2d.slice(0, 8 * self.conv3d.in_channels)
+        # the stem's patch-in-shared-memory kernel (csrc/conv_stem.cu) unless STEP_B200_STEM_HALO=0
         # tap plane qt = 2 is k_t = 6 + rt: only the rt = 0 sub-position (channels [0, 4 Cin)) has weights there, the
-        # rt = 1 half is structurally zero (engine.pack_stem_s2d) -> its MMA steps are skipped by the patch kernel
-        return E.conv(x_s2d, w, scale, shift, out, (4, 4, 4), (1, 1, 1), (1, 1, 1), self.activation is not None,
+        # rt = 1 half is structurally zero (engine.pack_stem_s2d) -> the stem kernel skips its channel group 16..23
+        return E.conv(x, w, scale, shift, out, (4, 4, 4), (1, 1, 1), (1, 1, 1), self.activation is not None,
                       a_mode=L.A_HALO if E.STEM_HALO else None, out_dims=(x_s2d.T, x_s2d.H, x_s2d.W),
                       zero_cin_last_kt=4 * self.conv3d.in_channels, tag=("s2d", self))
 

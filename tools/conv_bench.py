@@ -21,7 +21,7 @@ TRUNK_56, TRUNK_28, TRUNK_14 = (8, 16, 56, 56), (8, 16, 28, 28), (8, 8, 14, 14)
 HEAD, LOCAL = (88, 8, 7, 7), (704, 1, 7, 7)     # 8 clips x 11 tubes, T' = 8; the local branch runs on frames
 LAYERS = [
     # name, count per step, (N, T, H, W), Cin, Cout, k     (fused 1x1 = the Mixed block's three 1x1 branches in one GEMM)
-    ("stem_s2d",   1, (8, 16, 112, 112), 32, 64, (4, 4, 4)),
+    ("stem_s2d",   1, (8, 16, 112, 112), 24, 64, (4, 4, 4)),    # the 24 live channels of the 32-channel s2d row
     ("conv2b",     1, TRUNK_56, 64, 64, (1, 1, 1)),
     ("conv2c",     1, TRUNK_56, 64, 192, (3, 3, 3)),
     ("3b_fused",   1, TRUNK_28, 192, 176, (1, 1, 1)),
@@ -86,6 +86,8 @@ def plan(Cin, Cout, tiles):
 
 
 def kernel_of(N, T, H, W, Cin, Cout, k):
+    if Cin == 24 and k == (4, 4, 4):
+        return "stem"
     taps = k[0] * k[1] * k[2]
     halo = taps > 1 and Cin in (16, 32, 64) and Cout <= 256 and Cin <= 32 and min(H, W) >= 14
     return "halo" if halo else "umma"
@@ -117,6 +119,19 @@ def main():
                 f = lambda: E.bottleneck_exit(h, w3, x, w1, b, False, z)
             gmac = 2.0 * M * Cin * Cout / 1e9
             kern, exec_gmac, tile = "exit", gmac, ("-", "-", "-")
+        elif name == "stem_s2d":
+            # Unit3Dpy.forward_s2d's problem: 24 live channels in rows of 32 and pack_stem_s2d weights, whose zero last t
+            # tap plane channels 16..23 the stem kernel does not multiply (88 k16 steps per pixel)
+            buf = torch.randn(N, T, H, W, 32, device="cuda").half()
+            buf[..., 24:] = 0
+            x = Act(buf, Cin)
+            w = E.pack_stem_s2d(torch.randn(Cout, 3, 7, 7, 7, device="cuda") / 1029 ** 0.5)
+            out = Act(torch.empty(N, T, H, W, Cout, device="cuda", dtype=torch.float16))
+            sc, sh = torch.ones(Cout, device="cuda"), torch.zeros(Cout, device="cuda")
+            pad = (1, 1, 1)
+            f = lambda: E.conv(x, w, sc, sh, out, k, (1, 1, 1), pad, True, None, a_mode=L.A_HALO, zero_cin_last_kt=12)
+            gmac = M * Cout * 3 * 7 ** 3 / 1e9
+            kern, exec_gmac, tile = kernel_of(N, T, H, W, Cin, Cout, k), M * Cout * 88 * 16 / 1e9, ("-", "-", "-")
         else:
             taps = k[0] * k[1] * k[2]
             x = Act(torch.randn(N, T, H, W, Cin, device="cuda").half())
@@ -150,7 +165,7 @@ def main():
         if check and not isinstance(k, str):   # spot check against torch on two images (tool only: the parity tests live in tests/)
             import torch.nn.functional as F
             xs = x.buf[:2].float().permute(0, 4, 1, 2, 3)
-            ws = w.float().view(Cout, k[0], k[1], k[2], Cin).permute(0, 4, 1, 2, 3)
+            ws = w.float().view(Cout, k[0], k[1], k[2], w.shape[2]).permute(0, 4, 1, 2, 3)
             pd = pad if pad is not None else tuple(E.same_pad(kk, 1)[0] for kk in k)
             hi = tuple(kk - 1 - q for kk, q in zip(k, pd))
             ref = torch.relu(F.conv3d(F.pad(xs, (pd[2], hi[2], pd[1], hi[1], pd[0], hi[0])), ws).permute(0, 2, 3, 4, 1))
