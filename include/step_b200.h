@@ -110,6 +110,13 @@ int step_roi_align_fwd_nhwc(const void* feat, int dtype, int K, int H, int W, in
 int step_roi_pool_fwd_nhwc(const void* feat, int dtype, int K, int H, int W, int C, int feat_ld,
                            const float* rois, int R, float scale, int ph, int pw, void* out, int out_ld,
                            int roi_T, int feat_T, int t_start, step_stream_t stream);
+/* step_roi_pool_fwd_nhwc for training: the same pooled values bit for bit, plus argmax [R,ph,pw,C] int32 (channel
+ * stride C, 16-byte aligned) holding the frame-local pixel h*W + w of each maximum as cuda/ROIPool_cuda.cu:40-101 picks it
+ * (strict `>` from -FLT_MAX, h outer, w inner: on ties the first pixel in scan order wins), -1 for an empty bin.
+ * H*W must not exceed the 6400 pixels step_roi_pool_bwd_slice_nhwc accepts (STEP_E_ARG otherwise). */
+int step_roi_pool_fwd_argmax_nhwc(const void* feat, int dtype, int K, int H, int W, int C, int feat_ld,
+                                  const float* rois, int R, float scale, int ph, int pw, void* out, int out_ld,
+                                  int roi_T, int feat_T, int t_start, int32_t* argmax, step_stream_t stream);
 
 /* ------------------------------------------------------------------ tube arithmetic ------ */
 /* boxes are rows of 4 floats with a row stride (in floats) so the [.,5] flat-tube layout
@@ -270,6 +277,17 @@ size_t step_roi_align_bwd_slice_workspace_bytes(int K, int H, int W, int C, int 
 int step_roi_align_bwd_slice_nhwc(const void* grad_out, int dtype, int out_ld, const float* rois, int R, float scale, int ph,
                                   int pw, int K, int H, int W, int C, int sampling_ratio, int roi_T, int feat_T, int t_start,
                                   float* grad_in, int in_ld, void* workspace, size_t ws_bytes, step_stream_t stream);
+/* Channels-last ROIPool backward without atomics (replaces _C.roi_pool_backward, vision.cpp:35 / cuda/ROIPool_cuda.cu:103-132,
+ * whose atomicAdd scatter is not repeatable), with the frame contract of step_roi_align_bwd_slice_nhwc: grad_out [R,ph,pw,C]
+ * (channel stride out_ld, STEP_F32 / STEP_F16) and argmax [R,ph,pw,C] of step_roi_pool_fwd_argmax_nhwc for ROIs whose frame
+ * index f is relative to the slice conv_feat[:, t_start:t_start+roi_T] of a [K = clips * feat_T, H, W, C] map; the
+ * contribution is ADDED to grad_in (fp32, channel stride in_ld) frame (f / roi_T) * feat_T + t_start + f % roi_T, frames
+ * outside the slice are untouched.  Every element sums its contributions in ascending (ROI row, ph, pw) order, the loop order
+ * of torchvision's CPU roi_pool backward: with fp32 grad_out on a zeroed grad_in the result is bit-identical to it.  The
+ * per-frame accumulator lives in shared memory: H*W must not exceed 6400 (STEP_E_ARG otherwise). */
+int step_roi_pool_bwd_slice_nhwc(const void* grad_out, int dtype, int out_ld, const int32_t* argmax, const float* rois, int R,
+                                 int ph, int pw, int K, int H, int W, int C, int roi_T, int feat_T, int t_start,
+                                 float* grad_in, int in_ld, step_stream_t stream);
 /* Gradient of ContextNet's output from one refinement step (train.py:317-321): dctx [R, C] (row stride dctx_ld) is the
  * gradient of each tube's context input of the classifier, tubes [R, T_len, 5] the step's flat tubes (frame index first).
  * acc [B, feat_T, C] fp32 += (sum over the tubes of clip b = floor(frame / T_len), ascending tube order) / T_len on frames

@@ -62,6 +62,7 @@ def _declare(lib):
         "step_roi_pool_bwd_nchw_f32": ([P, P, P, I, I, I, I, I, I, I, P, S], c_int),
         "step_roi_align_fwd_nhwc": ([P, I, I, I, I, I, I, P, I, Fl, I, I, I, P, I, I, I, I, I, S], c_int),
         "step_roi_pool_fwd_nhwc": ([P, I, I, I, I, I, I, P, I, Fl, I, I, P, I, I, I, I, S], c_int),
+        "step_roi_pool_fwd_argmax_nhwc": ([P, I, I, I, I, I, I, P, I, Fl, I, I, P, I, I, I, I, P, S], c_int),
         "step_tube_decode_f32": ([P, I, P, I, P, S], c_int),
         "step_tube_encode_f32": ([P, P, I, I, P, S], c_int),
         "step_tube_valid_f32": ([P, I, Fl, Fl, S], c_int),
@@ -86,6 +87,7 @@ def _declare(lib):
         "step_roi_align_bwd_nhwc": ([P, I, I, P, I, Fl, I, I, I, I, I, I, I, P, I, S], c_int),
         "step_roi_align_bwd_slice_workspace_bytes": ([I, I, I, I, I, I], c_size_t),
         "step_roi_align_bwd_slice_nhwc": ([P, I, I, P, I, Fl, I, I, I, I, I, I, I, I, I, I, P, I, P, c_size_t, S], c_int),
+        "step_roi_pool_bwd_slice_nhwc": ([P, I, I, P, P, I, I, I, I, I, I, I, I, I, I, P, I, S], c_int),
         "step_ctx_grad_reduce_f32": ([P, I, P, I, I, I, I, I, I, P, S], c_int),
         "step_linear_small_n_bwd": ([P, I, I, I, I, P, P, I, P, I, P, P, S], c_int),
         "step_conv1x1_wgrad_workspace_bytes": ([I, I, I], c_size_t),

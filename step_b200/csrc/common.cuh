@@ -48,6 +48,13 @@ inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 constexpr int kNumSMs = 132;  // H100 SXM
 
+// The ROIPool backward (train.cu) accumulates one frame's [H*W, chunk] fp32 tile in shared memory, chunk >= 8 channels:
+// maps of up to 6400 pixels (80x80, inputs up to ~1280x1280).  The argmax forward (roi.cu) checks the same limit, so a
+// training step fails before its forward rather than after it.
+constexpr int kPoolBwdSmem = 200 * 1024;
+constexpr int kPoolBwdMinChunk = 8;
+constexpr int kPoolBwdMaxPixels = kPoolBwdSmem / (kPoolBwdMinChunk * (int)sizeof(float));
+
 // Function attributes (dynamic shared memory limit) are per device: a process driving several GPUs (nn.DataParallel,
 // test.py:79-95 of the reference) must set them once on each.  `seen` is a per-kernel bitmask owned by the caller.
 inline bool first_use_on_device(std::atomic<unsigned long long>& seen) {

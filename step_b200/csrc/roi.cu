@@ -432,11 +432,15 @@ __global__ void __launch_bounds__(256) roi_align_fwd_nhwc_f16_packed_kernel(cons
   else roi_gather_items<1>(bins, nbins, nvec, fbase, obase, out_ld, part, parts);
 }
 
-template <typename T>
+// kArgmax (training): also record, per output element, the frame-local pixel h*W + w of the maximum in `argmax`
+// [R, ph, pw, C] (channel stride C), -1 for an empty bin.  The rule of ROIPool_cuda.cu:79-96: strict `>` against the running
+// maximum, h outer / w inner, so on ties the first pixel in scan order wins.  The pooled value is the same fmaxf chain as
+// without the flag (`v > m` and fmaxf agree on which value is largest; only the index is added), so outputs are bit-identical.
+template <typename T, bool kArgmax>
 __global__ void __launch_bounds__(256) roi_pool_fwd_nhwc_kernel(const T* __restrict__ feat, int H, int W, int C,
                                                                 int feat_ld, const float* __restrict__ rois,
                                                                 float scale, int ph, int pw, T* __restrict__ out,
-                                                                int out_ld, FrameMap fm) {
+                                                                int out_ld, FrameMap fm, int32_t* __restrict__ argmax) {
   constexpr int VN = Vec16<T>::N;
   const int r = blockIdx.x, nbins = ph * pw, nvec = C / VN;
   T* obase = out + (size_t)r * nbins * out_ld;
@@ -446,17 +450,31 @@ __global__ void __launch_bounds__(256) roi_pool_fwd_nhwc_kernel(const T* __restr
     PoolWin o = pool_window(rois + 5 * (size_t)r, scale, ph, pw, p, q, H, W);
     const bool empty = (o.he <= o.hs) || (o.we <= o.ws);
     float m[VN];
+    int idx[kArgmax ? VN : 1];
 #pragma unroll
     for (int k = 0; k < VN; ++k) m[k] = empty ? 0.0f : -3.402823466e+38f;
+    if constexpr (kArgmax) {
+#pragma unroll
+      for (int k = 0; k < VN; ++k) idx[k] = -1;
+    }
     const T* fbase = feat + (size_t)fm.map(o.batch) * H * W * feat_ld + cv * VN;
     for (int h = o.hs; h < o.he; ++h)
       for (int w = o.ws; w < o.we; ++w) {
         float v[VN];
         load16(fbase + (size_t)(h * W + w) * feat_ld, v);
+        if constexpr (kArgmax) {
+#pragma unroll
+          for (int k = 0; k < VN; ++k) idx[k] = v[k] > m[k] ? h * W + w : idx[k];
+        }
 #pragma unroll
         for (int k = 0; k < VN; ++k) m[k] = fmaxf(m[k], v[k]);
       }
     store16(obase + (size_t)bin * out_ld + cv * VN, m);
+    if constexpr (kArgmax) {
+      int4* a = reinterpret_cast<int4*>(argmax + ((size_t)r * nbins + bin) * C + cv * VN);
+#pragma unroll
+      for (int k = 0; k < VN / 4; ++k) a[k] = make_int4(idx[4 * k], idx[4 * k + 1], idx[4 * k + 2], idx[4 * k + 3]);
+    }
   }
 }
 
@@ -584,11 +602,35 @@ extern "C" int step_roi_pool_fwd_nhwc(const void* feat, int dtype, int K, int H,
   STEP_CHECK_ARG(roi_T == 0 || (roi_T > 0 && t_start >= 0 && t_start + roi_T <= feat_T), "roi_pool_fwd_nhwc: bad frame map");
   FrameMap fm{roi_T, feat_T, t_start};
   if (dtype == STEP_F16)
-    roi_pool_fwd_nhwc_kernel<__half><<<R, 256, 0, cu(stream)>>>((const __half*)feat, H, W, C, feat_ld, rois, scale,
-                                                                 ph, pw, (__half*)out, out_ld, fm);
+    roi_pool_fwd_nhwc_kernel<__half, false><<<R, 256, 0, cu(stream)>>>((const __half*)feat, H, W, C, feat_ld, rois, scale,
+                                                                        ph, pw, (__half*)out, out_ld, fm, nullptr);
   else
-    roi_pool_fwd_nhwc_kernel<float><<<R, 256, 0, cu(stream)>>>((const float*)feat, H, W, C, feat_ld, rois, scale,
-                                                                ph, pw, (float*)out, out_ld, fm);
+    roi_pool_fwd_nhwc_kernel<float, false><<<R, 256, 0, cu(stream)>>>((const float*)feat, H, W, C, feat_ld, rois, scale,
+                                                                       ph, pw, (float*)out, out_ld, fm, nullptr);
   STEP_LAUNCH_CHECK("roi_pool_fwd_nhwc_kernel");
+  return 0;
+}
+
+extern "C" int step_roi_pool_fwd_argmax_nhwc(const void* feat, int dtype, int K, int H, int W, int C, int feat_ld,
+                                             const float* rois, int R, float scale, int ph, int pw, void* out, int out_ld,
+                                             int roi_T, int feat_T, int t_start, int32_t* argmax, step_stream_t stream) {
+  STEP_CHECK_ARG(K >= 0 && H > 0 && W > 0 && R >= 0 && ph > 0 && pw > 0, "roi_pool_fwd_argmax_nhwc: bad shape");
+  if (R == 0) return 0;
+  STEP_CHECK_ARG(feat && rois && out && argmax, "roi_pool_fwd_argmax_nhwc: null pointer");
+  if (int rc = check_nhwc("roi_pool_fwd_argmax_nhwc", dtype, C, feat_ld, out_ld, feat, out)) return rc;
+  STEP_CHECK_ARG(((uintptr_t)argmax & 15) == 0, "roi_pool_fwd_argmax_nhwc: argmax must be 16-byte aligned");
+  STEP_CHECK_ARG((long long)H * W <= kPoolBwdMaxPixels,
+                 "roi_pool_fwd_argmax_nhwc: H*W=%lld exceeds the %d-pixel limit of the ROIPool backward's shared-memory accumulator "
+                 "(inputs up to ~1280x1280)", (long long)H * W, kPoolBwdMaxPixels);
+  STEP_CHECK_ARG(roi_T == 0 || (roi_T > 0 && t_start >= 0 && t_start + roi_T <= feat_T),
+                 "roi_pool_fwd_argmax_nhwc: bad frame map roi_T=%d feat_T=%d t_start=%d", roi_T, feat_T, t_start);
+  FrameMap fm{roi_T, feat_T, t_start};
+  if (dtype == STEP_F16)
+    roi_pool_fwd_nhwc_kernel<__half, true><<<R, 256, 0, cu(stream)>>>((const __half*)feat, H, W, C, feat_ld, rois, scale,
+                                                                       ph, pw, (__half*)out, out_ld, fm, argmax);
+  else
+    roi_pool_fwd_nhwc_kernel<float, true><<<R, 256, 0, cu(stream)>>>((const float*)feat, H, W, C, feat_ld, rois, scale,
+                                                                      ph, pw, (float*)out, out_ld, fm, argmax);
+  STEP_LAUNCH_CHECK("roi_pool_fwd_argmax_nhwc_kernel");
   return 0;
 }

@@ -337,6 +337,80 @@ __global__ void __launch_bounds__(256) roi_align_bwd_slice_nhwc_kernel(const T* 
   }
 }
 
+// ---- ROIPool backward on a frame slice (the reference's ROIPool_cuda.cu:103-132 scatters with atomicAdd) -----------------
+// One CTA per (ROI frame f, chunk of `blockDim.x` channels) holds the frame's [H*W, chunk] fp32 accumulator in shared
+// memory; thread t owns channel c0 + t (and, at 32 channels or more, shared-memory bank t % 32).  The CTA streams the ROI rows in ascending order,
+// compacts those of frame f (in order, blockDim.x rows at a time: no cap on R, no workspace), and every thread adds
+// grad_out[row, bin, c] into acc[argmax[row, bin, c], c] bin by bin.  So each element sums its contributions in ascending
+// (row, ph, pw) order -- the loop order of torchvision's CPU roi_pool backward -- with no atomics and no bank conflicts.
+// The tile is then added into grad_in frame (f / roi_T) * feat_T + t_start + f % roi_T with 16-byte accesses; frames
+// without a ROI are not touched.
+constexpr int kPoolBwdMaxChunk = 64;           // the smallest chunk and the shared-memory budget: common.cuh
+constexpr int kPoolBwdBins = 16;               // bins whose (argmax, gradient) loads are in flight together
+
+template <typename T>
+__global__ void __launch_bounds__(kPoolBwdMaxChunk) roi_pool_bwd_slice_nhwc_kernel(const T* __restrict__ grad_out, int out_ld,
+                                                                                   const int32_t* __restrict__ argmax,
+                                                                                   const float* __restrict__ rois, int R, int nbins,
+                                                                                   int npix, int C, int roi_T, int feat_T, int t_start,
+                                                                                   float* __restrict__ grad_in, int in_ld) {
+  extern __shared__ float acc[];                // [npix][chunk]
+  __shared__ int rows[kPoolBwdMaxChunk];
+  __shared__ int warp_rows[kPoolBwdMaxChunk / 32];
+  const int chunk = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = (chunk + 31) >> 5;
+  const unsigned mask = chunk >= 32 ? 0xffffffffu : (1u << chunk) - 1u;
+  const int f = blockIdx.x, c0 = blockIdx.y * chunk, c = c0 + tid;
+  for (int i = tid; i < npix * chunk; i += chunk) acc[i] = 0.0f;
+  int seen = 0;                                 // rows of frame f so far (uniform across the CTA)
+  for (int base = 0; base < R; base += chunk) {
+    const int r = base + tid;
+    const bool keep = r < R && (int)rois[5 * (size_t)r] == f;
+    const unsigned bal = __ballot_sync(mask, keep);
+    __syncthreads();                            // the previous batch's rows have been consumed
+    if (lane == 0) warp_rows[warp] = __popc(bal);
+    __syncthreads();
+    int off = 0, n = 0;
+    for (int w = 0; w < nwarps; ++w) { off += w < warp ? warp_rows[w] : 0; n += warp_rows[w]; }
+    if (keep) rows[off + __popc(bal & ((1u << lane) - 1u))] = r;
+    __syncthreads();
+    seen += n;
+    if (c >= C) continue;
+    for (int j = 0; j < n; ++j) {
+      const int row = rows[j];
+      const T* g = grad_out + (size_t)row * nbins * out_ld + c;
+      const int32_t* a = argmax + (size_t)row * nbins * C + c;
+      for (int b0 = 0; b0 < nbins; b0 += kPoolBwdBins) {
+        int av[kPoolBwdBins];
+        float gv[kPoolBwdBins];
+#pragma unroll
+        for (int k = 0; k < kPoolBwdBins; ++k) {
+          const bool in = b0 + k < nbins;
+          av[k] = in ? a[(size_t)(b0 + k) * C] : -1;
+          gv[k] = in ? to_f32<T>(g[(size_t)(b0 + k) * out_ld]) : 0.0f;
+        }
+#pragma unroll
+        for (int k = 0; k < kPoolBwdBins; ++k)
+          if ((unsigned)av[k] < (unsigned)npix) {   // -1: empty bin, no contribution
+            float* s = acc + av[k] * chunk + tid;
+            *s = __fadd_rn(*s, gv[k]);
+          }
+      }
+    }
+  }
+  if (seen == 0) return;
+  __syncthreads();
+  float* dst = grad_in + ((size_t)(f / roi_T) * feat_T + t_start + f % roi_T) * npix * in_ld + c0;
+  const int nv = min(chunk, C - c0) / 4;
+  for (int i = tid; i < npix * nv; i += chunk) {
+    const int p = i / nv, v = i - p * nv;
+    const float4 s = *reinterpret_cast<const float4*>(acc + p * chunk + v * 4);
+    float4* d = reinterpret_cast<float4*>(dst + (size_t)p * in_ld + v * 4);
+    float4 cur = *d;
+    cur.x = __fadd_rn(cur.x, s.x); cur.y = __fadd_rn(cur.y, s.y); cur.z = __fadd_rn(cur.z, s.z); cur.w = __fadd_rn(cur.w, s.w);
+    *d = cur;
+  }
+}
+
 // ---- context-feature gradient (train.py:317-321: temp_context_feat[p] = context_feat[clip(p), :, t_start:t_start+T_len]) --
 // dctx[r, c] is the gradient of tube r's context input of the classifier (the slice mean the forward feeds to global_cls).
 // acc[b, t, c] += (sum over the tubes r of clip b, ascending r, of dctx[r, c]) / T_len for t in [t_start, t_start + T_len);
@@ -705,6 +779,47 @@ extern "C" int step_roi_align_bwd_slice_nhwc(const void* grad_out, int dtype, in
                                                                              pw, sampling_ratio, roi_T, feat_T, t_start, (float*)workspace,
                                                                              grad_in, in_ld);
   STEP_LAUNCH_CHECK("roi_align_bwd_slice_nhwc_kernel");
+  return 0;
+}
+
+extern "C" int step_roi_pool_bwd_slice_nhwc(const void* grad_out, int dtype, int out_ld, const int32_t* argmax, const float* rois, int R,
+                                            int ph, int pw, int K, int H, int W, int C, int roi_T, int feat_T, int t_start,
+                                            float* grad_in, int in_ld, step_stream_t stream) {
+  STEP_CHECK_ARG(K > 0 && H > 0 && W > 0 && C > 0 && R >= 0 && ph > 0 && pw > 0, "roi_pool_bwd_slice_nhwc: bad shape");
+  STEP_CHECK_ARG(dtype == STEP_F32 || dtype == STEP_F16, "roi_pool_bwd_slice_nhwc: bad dtype");
+  STEP_CHECK_ARG(C % 4 == 0 && in_ld % 4 == 0 && in_ld >= C && out_ld >= C,
+                 "roi_pool_bwd_slice_nhwc: C=%d in_ld=%d must be multiples of 4, out_ld=%d >= C", C, in_ld, out_ld);
+  STEP_CHECK_ARG(feat_T > 0 && K % feat_T == 0 && roi_T > 0 && t_start >= 0 && t_start + roi_T <= feat_T,
+                 "roi_pool_bwd_slice_nhwc: bad frame map roi_T=%d feat_T=%d t_start=%d K=%d", roi_T, feat_T, t_start, K);
+  STEP_CHECK_ARG(grad_in && (R == 0 || (grad_out && argmax && rois)), "roi_pool_bwd_slice_nhwc: null pointer");
+  STEP_CHECK_ARG(((uintptr_t)grad_in & 15) == 0, "roi_pool_bwd_slice_nhwc: grad_in must be 16-byte aligned");
+  const long long npix = (long long)H * W;
+  STEP_CHECK_ARG(npix <= kPoolBwdMaxPixels,
+                 "roi_pool_bwd_slice_nhwc: H*W=%lld exceeds the %d-pixel limit of the shared-memory accumulator (inputs up to ~1280x1280)",
+                 npix, kPoolBwdMaxPixels);
+  if (R == 0) return 0;
+  // the widest channel chunk whose accumulator fits, no wider than C needs
+  int chunk = kPoolBwdMaxChunk;
+  while (chunk > kPoolBwdMinChunk && (npix * chunk * (long long)sizeof(float) > kPoolBwdSmem || chunk >= 2 * C)) chunk /= 2;
+  const size_t smem = (size_t)npix * chunk * sizeof(float);
+  const dim3 grid((K / feat_T) * roi_T, ceil_div(C, chunk));
+  static std::atomic<unsigned long long> seen32{0}, seen16{0};
+  if (dtype == STEP_F32) {
+    if (first_use_on_device(seen32)) {
+      cudaError_t e = cudaFuncSetAttribute(roi_pool_bwd_slice_nhwc_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPoolBwdSmem);
+      if (e != cudaSuccess) return fail((int)e, "roi_pool_bwd_slice_nhwc: shared memory attribute: %s", cudaGetErrorString(e));
+    }
+    roi_pool_bwd_slice_nhwc_kernel<float><<<grid, chunk, smem, cu(stream)>>>((const float*)grad_out, out_ld, argmax, rois, R, ph * pw,
+                                                                             (int)npix, C, roi_T, feat_T, t_start, grad_in, in_ld);
+  } else {
+    if (first_use_on_device(seen16)) {
+      cudaError_t e = cudaFuncSetAttribute(roi_pool_bwd_slice_nhwc_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPoolBwdSmem);
+      if (e != cudaSuccess) return fail((int)e, "roi_pool_bwd_slice_nhwc: shared memory attribute: %s", cudaGetErrorString(e));
+    }
+    roi_pool_bwd_slice_nhwc_kernel<__half><<<grid, chunk, smem, cu(stream)>>>((const __half*)grad_out, out_ld, argmax, rois, R, ph * pw,
+                                                                              (int)npix, C, roi_T, feat_T, t_start, grad_in, in_ld);
+  }
+  STEP_LAUNCH_CHECK("roi_pool_bwd_slice_nhwc_kernel");
   return 0;
 }
 

@@ -84,13 +84,27 @@ class ROINet(nn.Module):
             feat = conv_feat.reshape(-1, C, W, H)
         return self.pool_layer(feat, tubes.view(-1, 5).detach())
 
-    def pool_into(self, feat, flat_tubes, out, roi_T, feat_T, t_start):
+    def pool_into(self, feat, flat_tubes, out, roi_T, feat_T, t_start, argmax=None):
         """Pipeline entry: feat Act [B, feat_T, H, W, C]; flat_tubes [R, roi_T, 5] fp32 CUDA;
         out Act [R*roi_T, 1, 7, 7, ld] channel slice.  Frame indices are relative to the slice
-        conv_feat[:, t_start:t_start+roi_T] exactly as utils/utils.py:48 builds it."""
+        conv_feat[:, t_start:t_start+roi_T] exactly as utils/utils.py:48 builds it.
+        argmax ('pool' mode only, for training): int32 CUDA tensor of R*roi_T*7*7*C elements that receives the
+        frame-local pixel of every maximum ([R*roi_T, 7, 7, C], -1 for an empty bin), the input of
+        training.roi_pool_backward_slice; the pooled values are the same with or without it."""
         R = flat_tubes.shape[0] * flat_tubes.shape[1]
         ps = self.pool_size
-        fn = L.lib().step_roi_align_fwd_nhwc if self.pool_mode == 'align' else L.lib().step_roi_pool_fwd_nhwc
+        if argmax is not None:
+            if self.pool_mode != 'pool':
+                raise RuntimeError("ROINet.pool_into: argmax is recorded in 'pool' mode only, this ROINet is %r" % self.pool_mode)
+            if argmax.dtype != torch.int32 or not argmax.is_contiguous() or argmax.numel() < R * ps * ps * feat.C:
+                raise RuntimeError("ROINet.pool_into: argmax must be a contiguous int32 tensor of >= %d elements"
+                                   % (R * ps * ps * feat.C))
+            L.same_device(argmax, flat_tubes)
+            fn = L.lib().step_roi_pool_fwd_argmax_nhwc
+        elif self.pool_mode == 'align':
+            fn = L.lib().step_roi_align_fwd_nhwc
+        else:
+            fn = L.lib().step_roi_pool_fwd_nhwc
         args = [L.c_void_p(feat.data_ptr()), feat.code, feat.N * feat.T, feat.H, feat.W, feat.C, feat.ld,
                 L.ptr(flat_tubes), R, 1.0 / 16.0, ps, ps]
         if self.pool_mode == 'align':
@@ -98,6 +112,8 @@ class ROINet(nn.Module):
         args += [L.c_void_p(out.data_ptr()), out.ld, roi_T, feat_T, t_start]
         if self.pool_mode == 'align':
             args.append(0 if feat.code == L.F16 else 1)   # fp16 pipeline: FMA fast path (within 1 fp16 ulp)
+        if argmax is not None:
+            args.append(L.ptr(argmax))
         args.append(L.stream())
         L.check(fn(*args))
         return out

@@ -2,7 +2,8 @@
 
 What exists: the head's three losses and the gradient of the training objective with respect to the head outputs
 (`head_losses`), the backward of the head's small-N linears (`linear_backward`), a deterministic channels-last ROIAlign
-backward (`roi_align_backward_nhwc`, and `roi_align_backward_slice` for the temporal slices of train.py:294-309), the
+backward (`roi_align_backward_nhwc`, and `roi_align_backward_slice` for the temporal slices of train.py:294-309), its
+ROIPool counterpart through the recorded maxima (`roi_pool_backward_slice`), the
 tensor-core weight gradient of the convolutions, max-pool backward, the backward of the whole head including the context
 columns of `global_cls` (`head_forward_backward`), of ContextNet (`context_forward` / `context_backward`) and of the I3D
 trunk (`trunk_forward_backward`), the SGD update with the gradient all-reduce (`sgd_step`) and the whole step in spatial
@@ -522,8 +523,10 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     flatten_tubes(batch_idx=True) builds them), step_targets[i]: [R_i, 3, 6 + classes].
     Heads built with cls_only=True run the first training stage (train_cls.py:253-322, one step of T_length = cfg.T): their
     objective is loss_cls.mean() alone, and their gradients are those of Mixed_5b / Mixed_5c, `downsample` and `global_cls`.
-    The gradient of conv_feat is, in this order, the ROIAlign backward of every step (each on its own frame slice) plus
-    the context branch's.  Returns dict(loss, losses=[(cls, loc, nb)], grads={param: fp32 grad} (trunk, heads and, with
+    The gradient of conv_feat is, in this order, the ROI pooling backward of every step (each on its own frame slice) plus
+    the context branch's; the pooling is nets['roi_net'].pool_mode's: ROIAlign ('align') or ROIPool ('pool', the
+    reference's default, config.py:67), whose backward routes each gradient to the pixel of the maximum recorded by the
+    step's forward.  Returns dict(loss, losses=[(cls, loc, nb)], grads={param: fp32 grad} (trunk, heads and, with
     the context branch, ContextNet's convolutions), skipped, loss_scale).
     Parameter update: with lr, `sgd_step` (one global rate); with optimizer (a step_b200.optim.Adam / SGD over the nets'
     parameters, e.g. built from the reference's get_params, and lr None), the gradients, averaged over the ranks, become
@@ -537,6 +540,9 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
             raise ValueError("train_step: scaler needs an optimizer (it is updated from optimizer.found_inf)")
         loss_scale = scaler.scale
     base, roi_net = nets["base_net"], nets["roi_net"]
+    pool_mode = roi_net.pool_mode
+    if pool_mode not in ("align", "pool"):
+        raise RuntimeError("train_step: ROINet pool_mode %r is neither 'align' nor 'pool'" % pool_mode)
     use_ctx = not getattr(cfg, "no_context", True)
     if use_ctx and nets.get("context_net") is None:
         raise RuntimeError("train_step: cfg.no_context is False but nets has no 'context_net'")
@@ -564,7 +570,10 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
                 raise RuntimeError("train_step: step %d pools frames [%d, %d) of T'=%d (cfg.T=%d, NUM_CHUNKS=%s) but its tubes have %d frames"
                                    % (i + 1, t_start, t_start + t_len, T_all, cfg.T, cfg.NUM_CHUNKS, flat.shape[1]))
             cat = Act.empty(R, t_len, head.pool_size, head.pool_size, 832 + head.fc_dim, L.F16, dev)
-            roi_net.pool_into(feat, flat, cat.frames().slice(0, 832), t_len, T_all, t_start)
+            argmax = None
+            if pool_mode == "pool":   # the pixel of every maximum, for this step's ROIPool backward
+                argmax = torch.empty((R * t_len * head.pool_size * head.pool_size * feat.C,), dtype=torch.int32, device=dev)
+            roi_net.pool_into(feat, flat, cat.frames().slice(0, 832), t_len, T_all, t_start, argmax=argmax)
             context = None
             if use_ctx:
                 # per-clip mean of the context over the step's frames; row_map = clip of each tube (train.py:317-321)
@@ -581,7 +590,11 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
             if use_ctx:
                 context_grad_reduce(r["ctx_grad"], flat, d_ctx, t_start)
             with _Phase("roi_bwd"):
-                ws = roi_align_backward_slice(r["roi_grad"], flat.view(-1, 5), 1.0 / 16.0, total, t_len, T_all, t_start, ws=ws)
+                if pool_mode == "pool":
+                    roi_pool_backward_slice(r["roi_grad"], flat.view(-1, 5), argmax, total, t_len, T_all, t_start)
+                else:
+                    ws = roi_align_backward_slice(r["roi_grad"], flat.view(-1, 5), 1.0 / 16.0, total, t_len, T_all, t_start, ws=ws)
+            argmax = None
         if use_ctx:
             cg, gfeat = context_backward(ctx_state, d_ctx, loss_scale)
             all_grads.update(cg)
@@ -624,6 +637,25 @@ def roi_align_backward_slice(grad_act, rois, spatial_scale, grad_in, roi_T, feat
                                                       int(feat_T), int(t_start), L.ptr(grad_in), grad_in.shape[3], L.ptr(ws),
                                                       ws.numel() * 4, L.stream()))
     return ws
+
+
+def roi_pool_backward_slice(grad_act, rois, argmax, grad_in, roi_T, feat_T, t_start):
+    """grad_in [B*feat_T, H, W, C] fp32 += ROIPool backward of grad_act (Act [R, roi_T, ph, pw, ld] slice of C channels,
+    fp16 | fp32) through argmax (int32 [R*roi_T, ph, pw, C], as ROINet.pool_into records it) for ROIs whose frame index is
+    relative to the frames [t_start, t_start + roi_T) of every clip.  Frames outside the slice are untouched.
+    Deterministic, no atomics: every element sums its contributions in ascending (ROI row, ph, pw) order."""
+    ph, pw, C = grad_act.H, grad_act.W, grad_act.C
+    R = grad_act.N * grad_act.T
+    if argmax.dtype != torch.int32 or not argmax.is_contiguous() or argmax.numel() < R * ph * pw * C:
+        raise RuntimeError("roi_pool_backward_slice: argmax must be a contiguous int32 tensor of >= %d elements" % (R * ph * pw * C))
+    dev = L.same_device(grad_act.buf, rois, argmax, grad_in)
+    K, H, W = grad_in.shape[0], grad_in.shape[1], grad_in.shape[2]
+    r = rois.detach().float().contiguous()
+    with torch.cuda.device(dev):
+        L.check(L.lib().step_roi_pool_bwd_slice_nhwc(L.c_void_p(grad_act.data_ptr()), grad_act.code, grad_act.ld, L.ptr(argmax), L.ptr(r),
+                                                     R, ph, pw, K, H, W, C, int(roi_T), int(feat_T), int(t_start), L.ptr(grad_in),
+                                                     grad_in.shape[3], L.stream()))
+    return grad_in
 
 
 def roi_align_backward_nhwc_strided(grad_act, rois, spatial_scale, K, H, W, sampling_ratio=0):

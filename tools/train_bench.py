@@ -8,7 +8,10 @@
                                                  36 x 400 x 400, 20 tubes per clip (5 positives; the last clip negatives
                                                  only), one class-only head over T=9 frames, ContextNet on, Adam with a
                                                  LossScaler
-Correctness is covered by tests/test_gpu_train.py, tests/test_gpu_train_context.py and tests/test_gpu_train_cls.py; this only
+    --pool (with any of the above)               ROINet("pool", 7), the reference's default pool_mode (config.py:67): ROIPool
+                                                 forward with argmax and its deterministic backward instead of ROIAlign
+Correctness is covered by tests/test_gpu_train.py, tests/test_gpu_train_context.py, tests/test_gpu_train_cls.py and
+tests/test_gpu_train_pool.py; this only
 reports where the (not yet optimised) step stands."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -17,6 +20,7 @@ import step_b200
 from step_b200 import optim, synth, training
 shipped = "--shipped" in sys.argv
 cls = "--cls" in sys.argv
+pool_mode = "pool" if "--pool" in sys.argv else "align"
 pos = [a for a in sys.argv[1:] if not a.startswith("--")]
 if cls:
     B = int(pos[0]) if pos else 4
@@ -30,7 +34,7 @@ else:
     B = int(pos[0]) if pos else 8
     N, T_in, HW = 11, 32, 224
     cfg = synth.make_cfg(fp16=True, T=8, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 1}, image_size=(HW, HW))
-nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet("align", 7)}
+nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet(pool_mode, 7)}
 nets["base_net"].load_state_dict(synth.base_net_state_dict())
 if shipped or cls:
     nets["context_net"] = step_b200.ContextNet(cfg)
@@ -79,6 +83,6 @@ for it in range(4):
             if pn > 0 and gn > 0:
                 training.sgd_step({p: g}, lr=3e-4 * pn / gn, momentum=0.0)
     torch.cuda.synchronize(); dt = time.perf_counter() - t0
-    print(json.dumps({"iter": it, "config": "cls" if cls else "shipped" if shipped else "c4", "B": B, "train_step_ms": round(dt * 1e3, 1), "loss": round(float(r["loss"]), 5),
+    print(json.dumps({"iter": it, "config": "cls" if cls else "shipped" if shipped else "c4", "pool_mode": pool_mode, "B": B, "train_step_ms": round(dt * 1e3, 1), "loss": round(float(r["loss"]), 5),
                       "clips_per_s": round(B / dt, 1), "peak_mem_gb": round(torch.cuda.max_memory_allocated() / 2**30, 2)}), flush=True)
 print(json.dumps({"device_ms_by_phase_of_the_backward_tape": training.timing_summary()}))
