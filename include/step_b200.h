@@ -157,6 +157,27 @@ int step_nhwc_to_nchw_f32(const void* in, int dtype, int N, int S, int C, int ld
 int step_nchw_to_nhwc(const float* in, int N, int S, int C, void* out, int dtype, int ld,
                       step_stream_t stream);
 
+/* ------------------------------------------------------------------ input -------------- */
+/* One source clip of step_frames_to_clip_u8: uint8 frames of H0 x W0 pixels, 3 channels, addressed as
+ * data[t*stride_t + c*stride_c + y*stride_h + x*stride_w] (strides in elements; any sign).  A stacked [B,T,3,H0,W0]
+ * tensor, a per-clip view and cv2's HWC-BGR frames (stride_c = -1 from the last channel) are all just strides. */
+typedef struct {
+  const uint8_t* data;
+  int H0, W0;
+  long long stride_t, stride_c, stride_h, stride_w;
+} step_frame_src;
+/* The reference's BaseTransform (data/augmentations.py:601-615: ConvertFromInts(scale), cv2.resize INTER_LINEAR on float32,
+ * SubtractMeans, DivideStds) followed by its dataset's permute, for B clips of T frames in one launch:
+ * out [B,T,3,H,W] fp32 contiguous, channel c of the output reading channel c of the source.
+ *   scale_mode 2: u*2/255 - 1, 1: u/255, 0: u; each step rounded in fp32 and applied before interpolation.
+ *   Resize: cv2 4.x's generic (non-IPP) INTER_LINEAR arithmetic bit for bit, including its unclamped row weights at the
+ *   border rows and its switch to INTER_AREA for an exact 2x downscale in both axes.
+ *   mean3 / std3: HOST arrays indexed by output channel; out = (resized - mean3[c]) / std3[c].
+ * `table` is a DEVICE array of B entries, read by the kernel: it is not validated here.  Each entry needs H0, W0 > 0 and
+ * W0 <= 48 * W (a tile's source columns must fit shared memory; tiles of an entry beyond that are written as NaN). */
+int step_frames_to_clip_u8(const step_frame_src* table, int B, int T, int H, int W, int scale_mode, const float* mean3,
+                           const float* std3, float* out, step_stream_t stream);
+
 /* ------------------------------------------------------------------ conv / pool / linear - */
 typedef struct {
   int dtype;                 /* STEP_F32: SIMT fp32 path.  STEP_F16: wgmma implicit GEMM, fp32 accumulate */

@@ -45,6 +45,12 @@ class OptimBlock(ctypes.Structure):
     _fields_ = [("tensor", c_int), ("chunk", c_int)]
 
 
+class FrameSrc(ctypes.Structure):
+    """mirror of step_frame_src (include/step_b200.h)"""
+    _fields_ = [("data", c_void_p), ("H0", c_int), ("W0", c_int)] + \
+               [(n, ctypes.c_longlong) for n in ("stride_t", "stride_c", "stride_h", "stride_w")]
+
+
 def _declare(lib):
     P, I, Fl, S = c_void_p, c_int, c_float, c_void_p  # S = stream
     sigs = {
@@ -103,6 +109,7 @@ def _declare(lib):
         "step_multi_tensor_nonfinite_f32": ([P, I, P, I, P, S], c_int),
         "step_multi_tensor_adam_f32": ([P, I, P, I, S], c_int),
         "step_multi_tensor_sgd_f32": ([P, I, P, I, S], c_int),
+        "step_frames_to_clip_u8": ([P, I, I, I, I, I, P, P, P, S], c_int),
         "step_debug_tma_tile": ([ctypes.POINTER(ConvParams), I, I, I, I, I, P, P, P, S], c_int),
     }
     for name, (argtypes, restype) in sigs.items():
