@@ -945,6 +945,11 @@ extern "C" int step_maxpool3d_bwd_f16(const void* x, int x_ld, const void* dy, i
                                       int pad_hi_w, int OT, int OH, int OW, void* dx /* accumulated in place */, int dx_ld, uint8_t* argmax_ws /* N*OT*OH*OW*C bytes */,
                                       step_stream_t stream) {
   STEP_CHECK_ARG(x && dy && dx && argmax_ws && N > 0 && T > 0 && H > 0 && W > 0 && C > 0 && KT * KH * KW < 254, "maxpool3d_bwd: bad arguments");
+  // the argmax pass divides by the strides, and a window must start inside its padding for every tap index to fit a byte
+  STEP_CHECK_ARG(KT > 0 && KH > 0 && KW > 0 && ST > 0 && SH > 0 && SW > 0 && OT > 0 && OH > 0 && OW > 0,
+                 "maxpool3d_bwd: kernel %dx%dx%d, stride %dx%dx%d, output %dx%dx%d must be positive", KT, KH, KW, ST, SH, SW, OT, OH, OW);
+  STEP_CHECK_ARG(PT >= 0 && PT < KT && PH >= 0 && PH < KH && PW >= 0 && PW < KW && pad_hi_t >= 0 && pad_hi_h >= 0 && pad_hi_w >= 0,
+                 "maxpool3d_bwd: bad padding (%d,%d,%d) / (%d,%d,%d) for kernel %dx%dx%d", PT, PH, PW, pad_hi_t, pad_hi_h, pad_hi_w, KT, KH, KW);
   PoolGeom g = {N, T, H, W, C, KT, KH, KW, ST, SH, SW, PT, PH, PW, OT, OH, OW, pad_hi_t, pad_hi_h, pad_hi_w};
   const long long n_out = (long long)N * OT * OH * OW * C, n_in = (long long)N * T * H * W * C;
   maxpool_argmax_kernel<<<ceil_div(n_out, 256), 256, 0, cu(stream)>>>(g, (const __half*)x, x_ld, argmax_ws);

@@ -160,6 +160,15 @@ def _dgrad_weights(entry):
     return c
 
 
+def stem_s2d_wgrad(dw, cin):
+    """Weight gradient of the stride-2 7x7x7 stem from that of the 4x4x4 filter it runs as over the space-to-depth clip
+    (engine.pack_stem_s2d): dw [Cout, 64 taps (qt, qh, qw), >= 8 cin channels (rt, rh, rw, c)] -> [Cout, cin, 7, 7, 7].
+    Tap q and sub-position r hold filter position k = 2 q + r; k = 7 is padding and is dropped."""
+    n = dw.shape[0]
+    g8 = dw[:, :, :8 * cin].reshape(n, 4, 4, 4, 2, 2, 2, cin).permute(0, 7, 1, 4, 2, 5, 3, 6).reshape(n, cin, 8, 8, 8)
+    return g8[:, :, :7, :7, :7].contiguous()
+
+
 TIMING = None     # set to {} to collect per-phase device times of tape_backward (tools/train_bench.py)
 
 
@@ -239,13 +248,9 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
           L.check(lib.step_conv_wgrad_f16(L.ptr(dz), n_total, L.c_void_p(x.data_ptr()), x.ld, x.N, x.T, x.H, x.W, n_total, x.C, k[0], k[1],
                                         k[2], pl[0], pl[1], pl[2], inv, L.ptr(dw), x.C, 0, L.ptr(ws), nbytes, L.stream()))
         if isinstance(e["tag"], tuple) and e["tag"][0] == "s2d":
-            # the stride-2 7x7x7 stem runs as a 4x4x4 filter over the space-to-depth clip (engine.pack_stem_s2d):
-            # tap q and sub-position r hold filter position k = 2 q + r (k = 7 is padding) -- undo that packing
             unit = e["tag"][1]
-            cin = unit.conv3d.in_channels
-            g8 = dw[:, :, :8 * cin].reshape(n_total, 4, 4, 4, 2, 2, 2, cin).permute(0, 7, 1, 4, 2, 5, 3, 6).reshape(n_total, cin, 8, 8, 8)
             if unit.conv3d.weight.requires_grad:
-                add(unit.conv3d.weight, g8[:, :, :7, :7, :7].contiguous())
+                add(unit.conv3d.weight, stem_s2d_wgrad(dw, unit.conv3d.in_channels))
             continue                                   # the clip itself needs no gradient
         tags = e["tag"] if isinstance(e["tag"], (list, tuple)) else [e["tag"]]
         row = 0

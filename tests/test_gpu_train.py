@@ -322,8 +322,14 @@ def test_trunk_backward_matches_reference_autograd(golden):
     """Backward of the whole I3D trunk (45 Unit3D convolutions incl. the space-to-depth stem, 10 max-pools, BatchNorm in
     eval with frozen affine) on the device against the reference's autograd for the same seeded clip and the same linear
     functional of conv_feat (tests/golden/trunk_grads.npz: per-weight gradient norms) and against the oracle's torch-CPU
-    autograd tensors (relative L2).  45 layers of fp16 activations / activation gradients: the error grows smoothly with depth (relative L2 0.1 % at
-    Mixed_4f, 12 % at the stem): norms within 1e-1 (40+ of 45 within 2e-2), tensors within 1.5e-1."""
+    autograd tensors (relative L2).  The oracle keeps fp32 activations; the device stores activations and activation
+    gradients in fp16, and every layer's backward matches a float64 reference on its own fp16 operands to within its
+    accumulation bound (tests/test_gpu_backward_layers.py).  The difference is therefore fp16 storage: each stored
+    activation and gradient carries a 2^-11 rounding, and ReLU masks of near-zero activations flip, compounding through
+    the layers below.  Measured on an H100 (tools/trunk_loss_scale.py): relative L2 0.07 % at Mixed_4f growing to 11 % at
+    Mixed_3b's 16-channel bottleneck and 12.7 % at the stem.  The error is the same to five digits at loss scale 1024 and
+    65536, with <= 0.3 % of the gradients subnormal at 1024 and none at 65536, so fp16 underflow plays no part.  Norms
+    within 1e-1 (40+ of 45 within 2e-2), tensors within 1.5e-1."""
     import step_b200
     from step_b200 import training
     g = golden("trunk_grads")
@@ -360,7 +366,7 @@ def test_trunk_backward_matches_reference_autograd(golden):
         rel = float((got[k].cpu().double() - ref.double()).norm() / ref.double().norm())
         assert rel <= 1.5e-1, (k, rel)
         checked += 1
-    assert checked == 45 and within2 >= 40     # measured: 44 of 45 norms within 2 %, the 16-channel Mixed_3b bottleneck +7.3 %
+    assert checked == 45 and within2 >= 40     # measured: 44 of 45 norms within 2 % (fp16 storage, see the docstring)
 
 
 def test_train_step_end_to_end_matches_oracle_autograd():
