@@ -149,9 +149,37 @@ def check_params(grads, ref, what):
     assert len(grads) == n, what
 
 
+def entry_shift(e):
+    """The fp32 shift the forward launch of a conv entry read: the folded BatchNorm of its Unit3Dpy container(s), or the
+    bias of an nn.Conv container (engine.conv keeps the scale on the tape, not the shift)."""
+    from step_b200 import _lib as L
+    parts = []
+    for tg, o in zip(R.tags_of(e), [e["out"]] + e["extra_outs"]):
+        if isinstance(tg, tuple):                              # ("s2d", stem unit)
+            parts.append(tg[1].packed(L.F16, s2d=True)[2])
+        elif hasattr(tg, "packed"):
+            parts.append(tg.packed(L.F16)[2])
+        else:
+            parts.append(tg.bias.detach().float() if tg.bias is not None else torch.zeros(o.C, device="cuda"))
+    return torch.cat(parts) if any(p is not None for p in parts) else None
+
+
+def check_conv_forward(e, what):
+    """The entry's forward outputs against conv_fwd (tests/test_gpu_forward_layers.py derives the bound)."""
+    outs = [e["out"]] + e["extra_outs"]
+    o0 = outs[0]
+    res = R.act_view(e["residual"]) if e["residual"] is not None else None
+    ys, xws, epis = R.conv_fwd(R.act_view(e["x"]), e["w"], e["scale"], entry_shift(e), res, e["k"], e["stride"], e["pad_lo"],
+                               (o0.T, o0.H, o0.W), e["relu"], [o.C for o in outs])
+    steps = R.conv_steps(e["k"], e["x"].C)
+    for j, (o, y, xw, epi) in enumerate(zip(outs, ys, xws, epis)):
+        R.check_fwd(R.act_view(o), y, xw, epi, steps, (what, "forward", j))
+
+
 def isolate_conv(e, gen, loss_scale, what):
     from step_b200 import training
     outs = [e["out"]] + e["extra_outs"]
+    check_conv_forward(e, what)
     gs = training.GradStore()
     dys = []
     for o in outs:
@@ -193,8 +221,9 @@ def isolate_pool(e, gen, what):
 
 @pytest.mark.parametrize("name", ["trunk_shipped", "context_shipped", "head_T3", "head_T9", "cls_head", "trunk_odd", "context_odd"])
 def test_every_tape_entry_in_isolation(tapes, name):
-    """Each conv / pool entry of the tape alone: a fresh GradStore seeded with a random fp16 output gradient,
-    tape_backward([entry]), then dz, dres, dW / db, dx against the float64 reference."""
+    """Each conv / pool entry of the tape alone: its forward output against conv_fwd / the pool reference, then a fresh
+    GradStore seeded with a random fp16 output gradient, tape_backward([entry]), and dz, dres, dW / db, dx against the
+    float64 reference."""
     tape = tapes[name]
     kind = name.rsplit("_", 1)[0] if name.startswith(("trunk", "context")) else ("cls_head" if name == "cls_head" else "head")
     assert counts(tape) == COUNTS[kind], (name, counts(tape))

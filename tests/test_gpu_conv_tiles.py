@@ -1,9 +1,10 @@
 """GPU: every (BK, BN) tile of the wgmma convolution (STEP_CONV_TILES in step_b200/csrc/conv_umma.cu) against the SIMT
-kernel on identical fp16 inputs: a Cout that leaves the last N tile ragged, a residual, a destination split inside an N
-tile, and M not a multiple of the 128-row tile (98 M tiles).  Tolerance as in test_gpu_conv.py
-(accumulation order only)."""
+kernel on identical fp16 inputs and against the float64 convolution (bound derived in test_gpu_forward_layers.py): a Cout
+that leaves the last N tile ragged, a residual, a destination split inside an N tile, and M not a multiple of the 128-row
+tile (98 M tiles)."""
 import os
 import re
+import sys
 
 import pytest
 import torch
@@ -11,6 +12,9 @@ import torch
 from step_b200 import _lib as L
 from step_b200 import engine as E
 from step_b200.engine import Act
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import _tape_reference as R  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -72,6 +76,10 @@ def test_every_tile_matches_simt(bk, bn):
         err = float((got.float() - ref.float()).abs().max())
         assert err <= tol, (k, Cin, Cout, err, tol)
         assert float(got[..., :8].abs().max()) == 0 and float(got[..., 8 + Cout:].abs().max()) == 0
+        pad = tuple(E.same_pad(kk, 1)[0] for kk in k)
+        (y,), (xw,), (epi,) = R.conv_fwd(x, E.pack_conv_weight(w, L.F16), scale, shift, res, k, (1, 1, 1), pad, (T, H, W),
+                                         True)
+        R.check_fwd(got[..., 8:8 + Cout], y, xw, epi, R.conv_steps(k, Cin), (bk, bn, k))
     # destination split inside the first N tile (and a second one further on when Cout allows), 1x1x1, no residual
     s0 = 16
     s1 = s0 + 16 * max(1, (Cout - s0) // 32) if Cout - s0 > 16 else None
@@ -85,3 +93,8 @@ def test_every_tile_matches_simt(bk, bn):
     for b, c0, c1 in zip(bufs, cuts, cuts[1:]):
         assert float((b[..., 8:].float() - ref[..., c0:c1].float()).abs().max()) <= tol, (c0, c1)
         assert float(b[..., :8].abs().max()) == 0
+    widths = [c1 - c0 for c0, c1 in zip(cuts, cuts[1:])]
+    ys, xws, epis = R.conv_fwd(x, E.pack_conv_weight(w, L.F16), scale, shift, None, (1, 1, 1), (1, 1, 1), (0, 0, 0), (T, H, W),
+                               True, widths)
+    for b, y, xw, epi in zip(bufs, ys, xws, epis):
+        R.check_fwd(b[..., 8:], y, xw, epi, R.conv_steps((1, 1, 1), Cin), (bk, bn, "split", b.shape[-1]))

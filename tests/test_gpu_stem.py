@@ -1,5 +1,8 @@
 """GPU: the space-to-depth stem kernel (csrc/conv_stem.cu) -- the stride-2 7x7x7 stem as a 4x4x4 filter over the 24 live
 channels of the s2d clip, with pack_stem_s2d weights and folded BatchNorm."""
+import os
+import sys
+
 import pytest
 import torch
 from torch.profiler import ProfilerActivity, profile
@@ -8,6 +11,9 @@ from step_b200 import _lib as L
 from step_b200 import engine as E
 from step_b200.engine import Act
 from step_b200.i3d import Unit3Dpy
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import _tape_reference as R  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -80,6 +86,10 @@ def test_stem_kernel_matches_32_channel_patch_kernel(shape):
     ref = ref.buf.float()
     err = float((got - ref).abs().max())
     assert err <= 2e-3 * float(ref.abs().max()), err
+    # and against the float64 4x4x4 / pad-1 convolution of the 24 live channels (bound: test_gpu_forward_layers.py)
+    (y,), (xw,), (epi,) = R.conv_fwd(s2d.buf[..., :24], w, scale, shift, None, (4, 4, 4), (1, 1, 1), (1, 1, 1),
+                                     (s2d.T, s2d.H, s2d.W), True)
+    R.check_fwd(got, y, xw, epi, R.conv_steps((4, 4, 4), 24), shape)
 
 
 def test_stem_shape_reaches_the_stem_kernel():

@@ -5,6 +5,7 @@ The reference rounds dz = dy * [y > 0] * scale to fp16 as act_bwd_kernel does; a
 That rounding moves each dz by at most half an fp16 ulp, 2^-11 |dz|, so a weight or input gradient moves by at most
 2^-11 (|dz|^T |x|) or 2^-11 (|dz| * |w|): the bound every comparison below uses.  Everything else is float64."""
 import ctypes
+import math
 import os
 import sys
 
@@ -326,3 +327,238 @@ def test_maxpool_bwd_rejects_oversized_windows_zero_strides_and_padding_outside_
     expect(lib, pool_bwd(lib, p, out=(4, 0, 5)), "must be positive")
     for lo, hi in (((3, 1, 1), (1, 1, 1)), ((1, -1, 1), (1, 1, 1)), ((1, 1, 1), (1, 1, -1))):
         expect(lib, pool_bwd(lib, p, lo=lo, hi=hi), "maxpool3d_bwd: bad padding")
+
+
+# ---- the forward helpers ----------------------------------------------------------------------------------------------
+def _bn_unit(cin, cout, k, stride=(1, 1, 1), seed=0):
+    from step_b200.i3d import Unit3Dpy
+    gen = torch.Generator().manual_seed(seed)
+    u = Unit3Dpy(cin, cout, kernel_size=k, stride=stride).eval()
+    with torch.no_grad():
+        u.conv3d.weight.copy_(torch.randn(u.conv3d.weight.shape, generator=gen) * 0.2)
+        u.batch3d.weight.copy_(torch.rand(cout, generator=gen) + 0.5)
+        u.batch3d.bias.copy_(torch.randn(cout, generator=gen) * 0.2)
+        u.batch3d.running_mean.copy_(torch.randn(cout, generator=gen) * 0.1)
+        u.batch3d.running_var.copy_(torch.rand(cout, generator=gen) + 0.5)
+    return u, gen
+
+
+def _module_fwd(u, x16, stride, residual=None):
+    """relu(batch_norm(conv3d(SAME pad(x), w)) + residual) in float64 on the module's fp16-rounded weight."""
+    k = u.kernel_size
+    lo, hi = zip(*(E.same_pad(kk, ss) for kk, ss in zip(k, stride)))
+    bn = u.batch3d
+    z = F.conv3d(F.pad(R.ncdhw(x16.double()), fpad(lo, hi)), u.conv3d.weight.detach().half().double(), stride=stride)
+    z = F.batch_norm(z, bn.running_mean.double(), bn.running_var.double(), bn.weight.double(), bn.bias.double(), False, 0.0,
+                     bn.eps)
+    if residual is not None:
+        z = z + R.ncdhw(residual.double())
+    return R.ndhwc(torch.relu(z))
+
+
+def _fold_within(got, ref, scale_err):
+    """conv_fwd uses engine.fold_bn's fp32 scale / shift: within a few fp32 ulps of the float64 BatchNorm."""
+    err = (got - ref).abs()
+    assert bool((err <= scale_err).all()), float((err - scale_err).max())
+
+
+@pytest.mark.parametrize("k,stride,residual", [((3, 3, 3), (1, 1, 1), False), ((1, 1, 1), (1, 1, 1), True),
+                                               ((3, 3, 3), (2, 2, 2), False), ((1, 3, 3), (1, 1, 1), True)])
+def test_conv_fwd_matches_the_module(k, stride, residual):
+    """conv_fwd (packed fp16 filter, fp32 folded scale / shift, fp16 residual) against the Unit3Dpy's meaning in float64:
+    SAME padding (asymmetric at stride 2 on odd extents), BatchNorm eval, residual, ReLU; and its magnitude terms."""
+    u, gen = _bn_unit(8, 16, k, stride, seed=sum(k) + stride[0])
+    N, T, H, W = 2, 5, 7, 6
+    x16 = half_values(N, T, H, W, 8, gen=gen)
+    w, scale, shift = u.packed(L.F16)
+    od = E.same_out_dims((T, H, W), k, stride)
+    lo = tuple(E.same_pad(kk, ss)[0] for kk, ss in zip(k, stride))
+    res = half_values(N, *od, 16, gen=gen) if residual else None
+    (y,), (xw,), (epi,) = R.conv_fwd(x16, w, scale, shift, res, k, stride, lo, od, True)
+    ref = _module_fwd(u, x16, stride, res)
+    assert y.shape == ref.shape
+    _fold_within(y, ref, 2.0 ** -20 * (epi + 1.0))
+    # the magnitude terms bound what they claim to: |acc * scale| <= xw, |y| <= epi
+    assert bool((y.abs() <= epi + 1e-12).all())
+    assert bool((xw >= 0).all()) and bool((epi >= 0).all())
+
+
+def test_conv_fwd_splits_the_fused_1x1_and_runs_the_stem_and_frame_convs():
+    """The three-way fused 1x1 (one packed filter, outputs split by width) equals three separate conv_fwd calls; the s2d
+    stem (4x4x4 pad 1 over the 24 live channels, pack_stem_s2d filter) equals the stride-2 7x7x7 module; a biased (1,3,3)
+    frame conv (nn.Conv2d on frames) equals F.conv2d."""
+    units = [_bn_unit(24, c, (1, 1, 1), seed=c)[0] for c in (16, 8, 24)]
+    gen = torch.Generator().manual_seed(9)
+    x16 = half_values(1, 3, 4, 5, 24, gen=gen)
+    parts = [u.packed(L.F16) for u in units]
+    w = torch.cat([p[0] for p in parts], 0)
+    sc = torch.cat([p[1] for p in parts])
+    sh = torch.cat([p[2] for p in parts])
+    ys, xws, epis = R.conv_fwd(x16, w, sc, sh, None, (1, 1, 1), (1, 1, 1), (0, 0, 0), (3, 4, 5), True, [16, 8, 24])
+    assert [y.shape[-1] for y in ys] == [16, 8, 24]
+    for (wp, s, b), y, xw in zip(parts, ys, xws):
+        (y1,), (xw1,), _ = R.conv_fwd(x16, wp, s, b, None, (1, 1, 1), (1, 1, 1), (0, 0, 0), (3, 4, 5), True)
+        assert torch.equal(y, y1) and torch.equal(xw, xw1)
+    # the stem
+    from step_b200.i3d import Unit3Dpy
+    stem = Unit3Dpy(3, 64, kernel_size=(7, 7, 7), stride=(2, 2, 2)).eval()
+    with torch.no_grad():
+        stem.conv3d.weight.copy_(torch.randn(stem.conv3d.weight.shape, generator=gen) * 0.05)
+    clip = torch.randn(1, 3, 6, 10, 8, generator=gen).half()
+    xs = s2d_pack(clip.double()).half()
+    ws, ss, bs = stem.packed(L.F16, s2d=True)
+    (y,), _, _ = R.conv_fwd(xs[..., :24], ws, ss, bs, None, (4, 4, 4), (1, 1, 1), (1, 1, 1), (3, 5, 4), True)
+    ref = _module_fwd(stem, R.ndhwc(clip), (2, 2, 2))
+    _fold_within(y, ref, 2.0 ** -20 * (ref.abs() + 1.0))
+    # a frame conv with bias, no BatchNorm, no activation
+    conv = torch.nn.Conv2d(16, 8, 3, padding=1, bias=True)
+    xf = half_values(4, 1, 6, 5, 16, gen=gen)
+    wp = E.pack_conv_weight(conv.weight, L.F16)
+    (y,), _, _ = R.conv_fwd(xf, wp, None, conv.bias.detach().float(), None, (1, 3, 3), (1, 1, 1), (0, 1, 1), (1, 6, 5), False)
+    ref = F.conv2d(R.ncdhw(xf.double())[:, :, 0], conv.weight.detach().half().double(), conv.bias.detach().float().double(),
+                   padding=1)
+    assert float((y[:, 0] - ref.permute(0, 2, 3, 1)).abs().max()) <= 1e-12
+
+
+@pytest.mark.parametrize("relu2,bias", [(True, False), (False, True)])
+def test_exit_fwd_equals_two_conv_fwd(relu2, bias):
+    """y and z of exit_fwd are two conv_fwd calls: the 1x1 with residual and ReLU, then the 1x1 on fp16(y); z_carry is
+    |w1| applied to y's full tolerance."""
+    gen = torch.Generator().manual_seed(5)
+    M = 37
+    h = half_values(M, 64, gen=gen)
+    w3 = half_values(128, 1, 64, gen=gen, scale=0.125)
+    x = half_values(M, 128, gen=gen)
+    w1 = half_values(32, 1, 128, gen=gen, scale=0.1)
+    b = torch.randn(32, generator=gen) if bias else None
+    r = R.exit_fwd(h, w3, x, w1, b, relu2)
+    rows = lambda t: t.reshape(M, 1, 1, 1, t.shape[-1])
+    (y,), (yxw,), (yepi,) = R.conv_fwd(rows(h), w3, None, None, rows(x), (1, 1, 1), (1, 1, 1), (0, 0, 0), (1, 1, 1), True)
+    assert torch.equal(y.reshape(M, -1), r["y"]) and torch.equal(yxw.reshape(M, -1), r["y_xw"])
+    assert torch.equal(yepi.reshape(M, -1), r["y_epi"])
+    y16 = r["y"].half()
+    (z,), (zxw,), (zepi,) = R.conv_fwd(rows(y16), w1, None, b, None, (1, 1, 1), (1, 1, 1), (0, 0, 0), (1, 1, 1), relu2)
+    for a, key in ((z, "z"), (zxw, "z_xw"), (zepi, "z_epi")):
+        assert float((a.reshape(M, -1) - r[key]).abs().max()) <= 1e-12 * (1.0 + float(r[key].abs().max())), key
+    my = R.fwd_margin(r["y_xw"], r["y_epi"])
+    carry = (my + R.ulp16(r["y"].abs() + my)) @ w1[:, 0].double().abs().t()
+    assert torch.allclose(carry, r["z_carry"], rtol=1e-12, atol=0)
+
+
+def test_check_fwd_accepts_rounding_and_rejects_a_scaled_or_truncated_output():
+    """check_fwd on a synthetic 1x1 layer: the float64 result rounded to nearest passes; the same scaled by 1 + 2^-8 fails;
+    rounded toward zero it stays inside the elementwise bound and fails the bias test."""
+    gen = torch.Generator().manual_seed(11)
+    x16 = half_values(4, 4, 14, 14, 256, gen=gen)
+    w = half_values(64, 1, 256, gen=gen, scale=1.0 / 16)
+    (ref,), (xw,), (epi,) = R.conv_fwd(x16, w, None, None, None, (1, 1, 1), (1, 1, 1), (0, 0, 0), (4, 14, 14), False)
+    steps = R.conv_steps((1, 1, 1), 256)
+    n, d, thr = R.check_fwd(ref.half(), ref, xw, epi, steps, "nearest")
+    assert n > 10000 and abs(d) < thr < 0.5
+    with pytest.raises(AssertionError, match="scaled"):
+        R.check_fwd((ref * (1.0 + 2.0 ** -8)).half(), ref, xw, epi, steps, "scaled")
+    rtz = ref.half().double()
+    rtz = torch.where(rtz.abs() > ref.abs(), rtz - rtz.sign() * R.ulp16(rtz - rtz.sign() * R.ulp16(rtz) / 2), rtz)
+    assert bool(((rtz - ref).abs() < R.ulp16(ref) + 1e-30).all()) and bool((rtz.abs() <= ref.abs()).all())
+    with pytest.raises(AssertionError, match="bias"):
+        R.check_fwd(rtz, ref, xw, epi, steps, "toward zero")
+
+
+def test_mean_mid_and_linear_references():
+    """mean_mid is the mean over B; linear is x[row_map] w^T + bias (+ y0), sigmoid on request."""
+    gen = torch.Generator().manual_seed(12)
+    x = torch.randn(3, 5, 2, 8, generator=gen).half()
+    m, mabs = R.mean_mid(x)
+    assert torch.allclose(m, x.double().permute(0, 2, 3, 1).reshape(3, 16, 5).mean(-1), rtol=0, atol=1e-15)
+    assert bool((m.abs() <= mabs).all())
+    xs = torch.randn(7, 40, generator=gen)
+    w = torch.randn(5, 40, generator=gen)
+    b = torch.randn(5, generator=gen)
+    y0 = torch.randn(4, 5, generator=gen)
+    rows = torch.tensor([6, 0, 3, 3], dtype=torch.int32)
+    y, v, a = R.linear(xs, w, b, y0, rows, act=1)
+    ref = xs.double()[rows.long()] @ w.double().t() + b.double() + y0.double()
+    assert torch.allclose(v, ref, rtol=1e-14, atol=0) and torch.allclose(y, torch.sigmoid(ref), rtol=1e-14, atol=0)
+    assert bool((v.abs() <= a).all())
+
+
+def test_head_regress_matches_nn_linear_on_the_nchw_flatten():
+    """head_regress from the three nn.Linear modules equals nn.Linear on the reference's (c, h, w) flatten of the
+    downsample2 output, chunk slices included; and the channels-last product with two_branch._perm_flat's weight is the
+    same number (what the kernel computes)."""
+    from step_b200.two_branch import _perm_flat
+    gen = torch.Generator().manual_seed(13)
+    C, ps, R_, T, Tc = 16, 7, 3, 9, 3
+    mods = [torch.nn.Linear(C * ps * ps, 4) for _ in range(3)]
+    feat = half_values(R_ * T, ps, ps, C, gen=gen)
+    r = R.head_regress(feat, *mods, Tc, T)
+    flat = feat.double().permute(0, 3, 1, 2).reshape(R_ * T, -1)                # NCHW flatten (two_branch.py:261)
+    outs = [(flat @ m.weight.detach().half().double().t() + m.bias.detach().double()).view(R_, T, 4) for m in mods]
+    s0, s1, e0, e1 = R.head_chunks(Tc, T)
+    assert (s0, s1, e0, e1) == (0, 3, 6, 9)
+    assert torch.allclose(r["local"], outs[0], rtol=1e-13, atol=1e-13)
+    assert torch.allclose(r["first"], (outs[0] + outs[1])[:, s0:s1], rtol=1e-13, atol=1e-13)
+    assert torch.allclose(r["last"], (outs[0] + outs[2])[:, e0:e1], rtol=1e-13, atol=1e-13)
+    cl = feat.double().reshape(R_ * T, -1) @ _perm_flat(mods[0].weight, C, ps).half().double().t()
+    assert torch.allclose(cl.view(R_, T, 4) + mods[0].bias.detach().double(), outs[0], rtol=1e-13, atol=1e-13)
+    assert bool((r["local_tol"] > 0).all())
+
+
+def _roi_align_loops(feat, roi, scale, ph, pw):
+    """ROIAlign of one roi, written as the loops of the reference's CPU op (float32 coordinates, float64 sums)."""
+    f32 = lambda v: float(torch.tensor(float(v), dtype=torch.float32))
+    K, H, W, C = feat.shape
+    b = int(roi[0])
+    sw, sh, ew, eh = (f32(f32(roi[j]) * f32(scale)) for j in (1, 2, 3, 4))
+    rw, rh = max(f32(ew - sw), 1.0), max(f32(eh - sh), 1.0)
+    bh, bw = f32(rh / ph), f32(rw / pw)
+    gh, gw = int(math.ceil(f32(rh / ph))), int(math.ceil(f32(rw / pw)))
+    out = torch.zeros(ph, pw, C, dtype=torch.float64)
+    fd = feat.double()
+    for p in range(ph):
+        for q in range(pw):
+            for iy in range(gh):
+                y = f32(f32(sh + f32(p * bh)) + f32(f32(f32(iy + 0.5) * bh) / gh))
+                for ix in range(gw):
+                    x = f32(f32(sw + f32(q * bw)) + f32(f32(f32(ix + 0.5) * bw) / gw))
+                    if y < -1.0 or y > H or x < -1.0 or x > W:
+                        continue
+                    yy, xx = max(y, 0.0), max(x, 0.0)
+                    yl, xl = int(yy), int(xx)
+                    if yl >= H - 1:
+                        yh = yl = H - 1
+                        yy = float(yl)
+                    else:
+                        yh = yl + 1
+                    if xl >= W - 1:
+                        xh = xl = W - 1
+                        xx = float(xl)
+                    else:
+                        xh = xl + 1
+                    ly, lx = f32(yy - yl), f32(xx - xl)
+                    hy, hx = f32(1.0 - ly), f32(1.0 - lx)
+                    out[p, q] += (f32(hy * hx) * fd[b, yl, xl] + f32(hy * lx) * fd[b, yl, xh] + f32(ly * hx) * fd[b, yh, xl]
+                                  + f32(ly * lx) * fd[b, yh, xh])
+    return out / (gh * gw)
+
+
+def test_roi_align_reference_matches_the_loop_rule():
+    """R.roi_align (vectorised) against the per-sample loops on ROIs inside, across and past the map edge (samples beyond
+    [-1, H] dropped, the last row / column clamped), a small ROI (grid 1x1) and a large one (grid 3x3), with the
+    roi_T / feat_T / t_start frame map."""
+    gen = torch.Generator().manual_seed(14)
+    K, H, W, C = 6, 9, 11, 8
+    feat = half_values(K, H, W, C, gen=gen)
+    rois = torch.tensor([[0, 10.0, 20.0, 90.0, 100.0], [1, -30.0, -20.0, 60.0, 40.0], [2, 100.0, 90.0, 200.0, 170.0],
+                         [3, 40.0, 40.0, 44.0, 47.0], [4, 0.0, 0.0, 175.0, 143.0]], dtype=torch.float32)
+    out, out_abs = R.roi_align(feat, rois, 1.0 / 16.0, 7, 7)
+    for r in range(rois.shape[0]):
+        ref = _roi_align_loops(feat, rois[r], 1.0 / 16.0, 7, 7)
+        assert torch.allclose(out[r], ref, rtol=1e-12, atol=1e-12), r
+    assert bool((out.abs() <= out_abs + 1e-15).all())
+    # frame map: roi frame f of a 2-frame slice starting at t 1 of 3-frame clips -> (f // 2) * 3 + 1 + f % 2
+    fm, _ = R.roi_align(feat, rois[:4], 1.0 / 16.0, 7, 7, roi_T=2, feat_T=3, t_start=1)
+    direct = rois[:4].clone()
+    direct[:, 0] = torch.tensor([1.0, 2.0, 4.0, 5.0])
+    ref, _ = R.roi_align(feat, direct, 1.0 / 16.0, 7, 7)
+    assert torch.equal(fm, ref)
