@@ -2,6 +2,7 @@
 (`Act`), weight packing / BatchNorm folding, and thin launch helpers.  No arithmetic happens here;
 torch supplies device memory and the current stream only.
 """
+import contextlib
 import math
 import os
 
@@ -33,6 +34,21 @@ STEM_HALO = os.environ.get("STEP_B200_STEM_HALO", "1") != "0"
 BRANCH_STREAMS = os.environ.get("STEP_B200_BRANCH_STREAMS", "1") != "0"
 FUSE_1X1 = os.environ.get("STEP_B200_FUSE_1X1", "1") != "0"
 _side_streams = {}
+
+
+@contextlib.contextmanager
+def recording(tape):
+    """Set TAPE to `tape` for the block and restore TAPE and BRANCH_STREAMS on exit.  A list turns BRANCH_STREAMS off
+    too, so that every launch runs on one stream and the tape order is the execution order; None only stops recording."""
+    global TAPE, BRANCH_STREAMS
+    saved = TAPE, BRANCH_STREAMS
+    TAPE = tape
+    if tape is not None:
+        BRANCH_STREAMS = False
+    try:
+        yield tape
+    finally:
+        TAPE, BRANCH_STREAMS = saved
 
 
 def side_streams(device, n=3):

@@ -11,6 +11,8 @@ and temporal mode with or without the context branch (`train_step`), which can a
 `optim` with dynamic loss scaling.  `BaseNet` / `ContextNet` / `TwoBranchNet` still run
 without autograd (their outputs carry no grad_fn): the backward walks the tape their forward records.
 """
+import contextlib
+
 import torch
 
 from . import _lib as L
@@ -102,15 +104,65 @@ def linear_backward(x, w, dy, need_dx=True, need_dw=True, dx_out=None, accumulat
 
 def roi_align_backward_nhwc(grad_out, rois, spatial_scale, K, H, W, sampling_ratio=0):
     """grad_out [R,ph,pw,C] (channels-last, fp16|fp32) -> grad_in [K,H,W,C] fp32.  Deterministic: no atomics."""
-    dev = L.same_device(grad_out, rois)
-    R, ph, pw, C = grad_out.shape
+    from .engine import Act
     go = grad_out.detach().contiguous()
+    R, ph, pw, C = go.shape
+    return roi_align_backward_nhwc_strided(Act(go.view(R, 1, ph, pw, C)), rois, spatial_scale, K, H, W, sampling_ratio)
+
+
+def roi_align_backward_nhwc_strided(grad_act, rois, spatial_scale, K, H, W, sampling_ratio=0):
+    """ROIAlign backward from a channel slice of a wider buffer: grad_act (Act [R, T', ph, pw, ld] slice of C channels,
+    fp16 | fp32; its R * T' rows are the rows of rois) -> grad_in [K,H,W,C] fp32.  Deterministic: no atomics."""
+    ph, pw, C = grad_act.H, grad_act.W, grad_act.C
+    R = grad_act.N * grad_act.T
+    dev = L.same_device(grad_act.buf, rois)
     r = rois.detach().float().contiguous()
     with torch.cuda.device(dev):
         gin = torch.empty((K, H, W, C), dtype=torch.float32, device=dev)
-        L.check(L.lib().step_roi_align_bwd_nhwc(L.ptr(go), L.dt(go), C, L.ptr(r), R, float(spatial_scale), ph, pw, K, H, W, C,
-                                                int(sampling_ratio), L.ptr(gin), C, L.stream()))
+        L.check(L.lib().step_roi_align_bwd_nhwc(L.c_void_p(grad_act.data_ptr()), grad_act.code, grad_act.ld, L.ptr(r), R,
+                                                float(spatial_scale), ph, pw, K, H, W, C, int(sampling_ratio), L.ptr(gin), C,
+                                                L.stream()))
     return gin
+
+
+def roi_align_backward_slice(grad_act, rois, spatial_scale, grad_in, roi_T, feat_T, t_start, sampling_ratio=0, ws=None):
+    """grad_in [B*feat_T, H, W, C] fp32 += ROIAlign backward of grad_act (Act [R, roi_T, ph, pw, ld] slice of C channels,
+    fp16 | fp32) for ROIs whose frame index is relative to the frames [t_start, t_start + roi_T) of every clip (the frame map
+    of ROINet.pool_into).  Frames outside the slice are untouched.  ws: optional fp32 workspace tensor, reused when large
+    enough; the one used is returned."""
+    ph, pw, C = grad_act.H, grad_act.W, grad_act.C
+    R = grad_act.N * grad_act.T
+    dev = L.same_device(grad_act.buf, rois, grad_in)
+    K, H, W = grad_in.shape[0], grad_in.shape[1], grad_in.shape[2]
+    r = rois.detach().float().contiguous()
+    with torch.cuda.device(dev):
+        nbytes = L.lib().step_roi_align_bwd_slice_workspace_bytes(K, H, W, C, roi_T, feat_T)
+        if ws is None or ws.numel() * 4 < nbytes:
+            ws = torch.empty((max(nbytes, 16) // 4,), dtype=torch.float32, device=dev)
+        L.check(L.lib().step_roi_align_bwd_slice_nhwc(L.c_void_p(grad_act.data_ptr()), grad_act.code, grad_act.ld, L.ptr(r), R,
+                                                      float(spatial_scale), ph, pw, K, H, W, C, int(sampling_ratio), int(roi_T),
+                                                      int(feat_T), int(t_start), L.ptr(grad_in), grad_in.shape[3], L.ptr(ws),
+                                                      ws.numel() * 4, L.stream()))
+    return ws
+
+
+def roi_pool_backward_slice(grad_act, rois, argmax, grad_in, roi_T, feat_T, t_start):
+    """grad_in [B*feat_T, H, W, C] fp32 += ROIPool backward of grad_act (Act [R, roi_T, ph, pw, ld] slice of C channels,
+    fp16 | fp32) through argmax (int32 [R*roi_T, ph, pw, C], as ROINet.pool_into records it) for ROIs whose frame index is
+    relative to the frames [t_start, t_start + roi_T) of every clip.  Frames outside the slice are untouched.
+    Deterministic, no atomics: every element sums its contributions in ascending (ROI row, ph, pw) order."""
+    ph, pw, C = grad_act.H, grad_act.W, grad_act.C
+    R = grad_act.N * grad_act.T
+    if argmax.dtype != torch.int32 or not argmax.is_contiguous() or argmax.numel() < R * ph * pw * C:
+        raise RuntimeError("roi_pool_backward_slice: argmax must be a contiguous int32 tensor of >= %d elements" % (R * ph * pw * C))
+    dev = L.same_device(grad_act.buf, rois, argmax, grad_in)
+    K, H, W = grad_in.shape[0], grad_in.shape[1], grad_in.shape[2]
+    r = rois.detach().float().contiguous()
+    with torch.cuda.device(dev):
+        L.check(L.lib().step_roi_pool_bwd_slice_nhwc(L.c_void_p(grad_act.data_ptr()), grad_act.code, grad_act.ld, L.ptr(argmax), L.ptr(r),
+                                                     R, ph, pw, K, H, W, C, int(roi_T), int(feat_T), int(t_start), L.ptr(grad_in),
+                                                     grad_in.shape[3], L.stream()))
+    return grad_in
 
 
 def conv1x1_wgrad(dz, x, scale=1.0, out=None, accumulate=False):
@@ -172,19 +224,19 @@ def stem_s2d_wgrad(dw, cin):
 TIMING = None     # set to {} to collect per-phase device times of tape_backward (tools/train_bench.py)
 
 
-class _Phase:
-    def __init__(self, name):
-        self.name = name
-
-    def __enter__(self):
-        if TIMING is not None:
-            self.e0 = torch.cuda.Event(enable_timing=True); self.e1 = torch.cuda.Event(enable_timing=True)
-            self.e0.record()
-
-    def __exit__(self, *a):
-        if TIMING is not None:
-            self.e1.record()
-            TIMING.setdefault(self.name, []).append((self.e0, self.e1))
+@contextlib.contextmanager
+def _phase(name):
+    """Adds the block's device time to TIMING[name] when TIMING is a dict."""
+    if TIMING is None:
+        yield
+        return
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    try:
+        yield
+    finally:
+        e1.record()
+        TIMING.setdefault(name, []).append((e0, e1))
 
 
 def timing_summary():
@@ -213,10 +265,10 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
             gy, gx = grads.of(y), grads.of(x)
             k, s, pl, ph = e["k"], e["stride"], e["pad_lo"], e["pad_hi"]
             ws = torch.empty((y.N * y.T * y.H * y.W * y.C,), dtype=torch.uint8, device=x.device)
-            with _Phase("pool_bwd"):
-              L.check(lib.step_maxpool3d_bwd_f16(L.c_void_p(x.data_ptr()), x.ld, L.c_void_p(gy.data_ptr()), gy.ld, x.N, x.T, x.H, x.W,
-                                               x.C, k[0], k[1], k[2], s[0], s[1], s[2], pl[0], pl[1], pl[2], ph[0], ph[1], ph[2],
-                                               y.T, y.H, y.W, L.c_void_p(gx.data_ptr()), gx.ld, L.ptr(ws), L.stream()))
+            with _phase("pool_bwd"):
+                L.check(lib.step_maxpool3d_bwd_f16(L.c_void_p(x.data_ptr()), x.ld, L.c_void_p(gy.data_ptr()), gy.ld, x.N, x.T, x.H,
+                                                   x.W, x.C, k[0], k[1], k[2], s[0], s[1], s[2], pl[0], pl[1], pl[2], ph[0], ph[1],
+                                                   ph[2], y.T, y.H, y.W, L.c_void_p(gx.data_ptr()), gx.ld, L.ptr(ws), L.stream()))
             continue
         x, w, k = e["x"], e["w"], e["k"]
         if e["stride"] != (1, 1, 1):
@@ -226,27 +278,27 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
         n_total = sum(o.C for o in outs)
         dz = torch.empty((x.N, x.T, x.H, x.W, n_total), dtype=torch.float16, device=x.device)
         col = 0
-        ph_act = _Phase("act_bwd"); ph_act.__enter__()
-        for o in outs:
-            gy = grads.of(o)
-            sc = e["scale"][col:col + o.C] if e["scale"] is not None else None
-            res = e["residual"]
-            gres = grads.of(res) if res is not None else None
-            L.check(lib.step_act_bwd_f16(L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, L.ptr(sc), 1 if e["relu"] else 0,
-                                         M, o.C, L.c_void_p(dz.data_ptr() + 2 * col), n_total,
-                                         L.c_void_p(gres.data_ptr()) if gres is not None else None, gres.ld if gres is not None else 0,
-                                         L.stream()))
-            col += o.C
-        ph_act.__exit__()
+        with _phase("act_bwd"):
+            for o in outs:
+                gy = grads.of(o)
+                sc = e["scale"][col:col + o.C] if e["scale"] is not None else None
+                res = e["residual"]
+                gres = grads.of(res) if res is not None else None
+                L.check(lib.step_act_bwd_f16(L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, L.ptr(sc),
+                                             1 if e["relu"] else 0, M, o.C, L.c_void_p(dz.data_ptr() + 2 * col), n_total,
+                                             L.c_void_p(gres.data_ptr()) if gres is not None else None,
+                                             gres.ld if gres is not None else 0, L.stream()))
+                col += o.C
         # ---- weight (and bias) gradients
         taps = k[0] * k[1] * k[2]
         dw = torch.empty((n_total, taps, x.C), dtype=torch.float32, device=x.device)
         nbytes = lib.step_conv_wgrad_workspace_bytes(M, n_total, x.C, taps)
         ws = torch.empty((nbytes // 4,), dtype=torch.float32, device=x.device)
         pl = e["pad_lo"]
-        with _Phase("wgrad_k%d" % taps):
-          L.check(lib.step_conv_wgrad_f16(L.ptr(dz), n_total, L.c_void_p(x.data_ptr()), x.ld, x.N, x.T, x.H, x.W, n_total, x.C, k[0], k[1],
-                                        k[2], pl[0], pl[1], pl[2], inv, L.ptr(dw), x.C, 0, L.ptr(ws), nbytes, L.stream()))
+        with _phase("wgrad_k%d" % taps):
+            L.check(lib.step_conv_wgrad_f16(L.ptr(dz), n_total, L.c_void_p(x.data_ptr()), x.ld, x.N, x.T, x.H, x.W, n_total, x.C,
+                                            k[0], k[1], k[2], pl[0], pl[1], pl[2], inv, L.ptr(dw), x.C, 0, L.ptr(ws), nbytes,
+                                            L.stream()))
         if isinstance(e["tag"], tuple) and e["tag"][0] == "s2d":
             unit = e["tag"][1]
             if unit.conv3d.weight.requires_grad:
@@ -274,12 +326,8 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
             gx = grads.of(x)
             wT = _dgrad_weights(e)
             pad = tuple(kk - 1 - p for kk, p in zip(k, pl))
-            saved, E.TAPE = E.TAPE, None
-            try:
-                with _Phase("dgrad"):
-                    E.conv(Act(dz), wT, None, None, gx, k, (1, 1, 1), pad, relu=False, residual=gx, out_dims=(x.T, x.H, x.W))
-            finally:
-                E.TAPE = saved
+            with E.recording(None), _phase("dgrad"):
+                E.conv(Act(dz), wT, None, None, gx, k, (1, 1, 1), pad, relu=False, residual=gx, out_dims=(x.T, x.H, x.W))
     return out
 
 
@@ -335,12 +383,8 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
             cf = context_feat.detach().to(dev).float().contiguous().view(N * 1024, Tl)
             ctx_mean = E.mean_mid(cf.data_ptr(), L.F32, N * 1024, Tl, 1, 1, 1, dev).view(N, 1024)   # as TwoBranchNet.forward
         tape, keep = [], {}
-        saved_tape, saved_bs = E.TAPE, E.BRANCH_STREAMS
-        E.TAPE, E.BRANCH_STREAMS = tape, False          # one stream: the tape order is the execution order
-        try:
+        with E.recording(tape):
             prob, loc, first, last, logits = net.forward_act(cat, ctx_mean, row_map, want_logits=True, keep=keep)
-        finally:
-            E.TAPE, E.BRANCH_STREAMS = saved_tape, saved_bs
         if net.cls_only:
             # class-only heads: the regression losses are the reference's zeros (two_branch.py:252,276-280)
             lc, dlogits = cls_loss(logits, targets, want_grads=True)
@@ -405,12 +449,8 @@ def context_forward(context_net, feat):
         raise RuntimeError("context_forward runs on the fp16 path (cfg.fp16=True)")
     with torch.cuda.device(feat.device), torch.no_grad():
         tape, keep = [], {}
-        saved_tape, saved_bs = E.TAPE, E.BRANCH_STREAMS
-        E.TAPE, E.BRANCH_STREAMS = tape, False
-        try:
+        with E.recording(tape):
             ctx = context_net.forward_act(feat, keep=keep)
-        finally:
-            E.TAPE, E.BRANCH_STREAMS = saved_tape, saved_bs
     return ctx, dict(tape=tape, x=keep["mixed_5c"], feat=feat)
 
 
@@ -454,12 +494,8 @@ def trunk_forward_backward(base_net, clips, d_feat_fn, loss_scale=1024.0):
     dev = clips.device
     with torch.cuda.device(dev), torch.no_grad():
         tape = []
-        saved_tape, saved_bs = E.TAPE, E.BRANCH_STREAMS
-        E.TAPE, E.BRANCH_STREAMS = tape, False
-        try:
+        with E.recording(tape):
             feat = base_net.forward_act(clips)
-        finally:
-            E.TAPE, E.BRANCH_STREAMS = saved_tape, saved_bs
         grads = GradStore()
         gfeat = grads.of(feat)
         d = d_feat_fn(feat).to(torch.float32).contiguous()
@@ -594,7 +630,7 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
             all_grads.update(r["grads"])
             if use_ctx:
                 context_grad_reduce(r["ctx_grad"], flat, d_ctx, t_start)
-            with _Phase("roi_bwd"):
+            with _phase("roi_bwd"):
                 if pool_mode == "pool":
                     roi_pool_backward_slice(r["roi_grad"], flat.view(-1, 5), argmax, total, t_len, T_all, t_start)
                 else:
@@ -621,55 +657,3 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
         sgd_state = sgd_step(all_grads, lr, momentum, weight_decay, sgd_state, world_size)
     return dict(loss=loss, losses=[r["losses"] for r in results], grads=all_grads, sgd_state=sgd_state, skipped=skipped,
                 loss_scale=loss_scale)
-
-
-def roi_align_backward_slice(grad_act, rois, spatial_scale, grad_in, roi_T, feat_T, t_start, sampling_ratio=0, ws=None):
-    """grad_in [B*feat_T, H, W, C] fp32 += ROIAlign backward of grad_act (Act [R, roi_T, ph, pw, ld] slice of C channels,
-    fp16 | fp32) for ROIs whose frame index is relative to the frames [t_start, t_start + roi_T) of every clip (the frame map
-    of ROINet.pool_into).  Frames outside the slice are untouched.  ws: optional fp32 workspace tensor, reused when large
-    enough; the one used is returned."""
-    ph, pw, C = grad_act.H, grad_act.W, grad_act.C
-    R = grad_act.N * grad_act.T
-    dev = L.same_device(grad_act.buf, rois, grad_in)
-    K, H, W = grad_in.shape[0], grad_in.shape[1], grad_in.shape[2]
-    r = rois.detach().float().contiguous()
-    with torch.cuda.device(dev):
-        nbytes = L.lib().step_roi_align_bwd_slice_workspace_bytes(K, H, W, C, roi_T, feat_T)
-        if ws is None or ws.numel() * 4 < nbytes:
-            ws = torch.empty((max(nbytes, 16) // 4,), dtype=torch.float32, device=dev)
-        L.check(L.lib().step_roi_align_bwd_slice_nhwc(L.c_void_p(grad_act.data_ptr()), grad_act.code, grad_act.ld, L.ptr(r), R,
-                                                      float(spatial_scale), ph, pw, K, H, W, C, int(sampling_ratio), int(roi_T),
-                                                      int(feat_T), int(t_start), L.ptr(grad_in), grad_in.shape[3], L.ptr(ws),
-                                                      ws.numel() * 4, L.stream()))
-    return ws
-
-
-def roi_pool_backward_slice(grad_act, rois, argmax, grad_in, roi_T, feat_T, t_start):
-    """grad_in [B*feat_T, H, W, C] fp32 += ROIPool backward of grad_act (Act [R, roi_T, ph, pw, ld] slice of C channels,
-    fp16 | fp32) through argmax (int32 [R*roi_T, ph, pw, C], as ROINet.pool_into records it) for ROIs whose frame index is
-    relative to the frames [t_start, t_start + roi_T) of every clip.  Frames outside the slice are untouched.
-    Deterministic, no atomics: every element sums its contributions in ascending (ROI row, ph, pw) order."""
-    ph, pw, C = grad_act.H, grad_act.W, grad_act.C
-    R = grad_act.N * grad_act.T
-    if argmax.dtype != torch.int32 or not argmax.is_contiguous() or argmax.numel() < R * ph * pw * C:
-        raise RuntimeError("roi_pool_backward_slice: argmax must be a contiguous int32 tensor of >= %d elements" % (R * ph * pw * C))
-    dev = L.same_device(grad_act.buf, rois, argmax, grad_in)
-    K, H, W = grad_in.shape[0], grad_in.shape[1], grad_in.shape[2]
-    r = rois.detach().float().contiguous()
-    with torch.cuda.device(dev):
-        L.check(L.lib().step_roi_pool_bwd_slice_nhwc(L.c_void_p(grad_act.data_ptr()), grad_act.code, grad_act.ld, L.ptr(argmax), L.ptr(r),
-                                                     R, ph, pw, K, H, W, C, int(roi_T), int(feat_T), int(t_start), L.ptr(grad_in),
-                                                     grad_in.shape[3], L.stream()))
-    return grad_in
-
-
-def roi_align_backward_nhwc_strided(grad_act, rois, spatial_scale, K, H, W, sampling_ratio=0):
-    """ROIAlign backward from a channel slice of a wider fp16 buffer (Act [R, T', ph, pw, ld] slice of C channels)."""
-    ph, pw, C = grad_act.H, grad_act.W, grad_act.C
-    R = grad_act.N * grad_act.T
-    dev = grad_act.device
-    r = rois.detach().float().contiguous()
-    gin = torch.empty((K, H, W, C), dtype=torch.float32, device=dev)
-    L.check(L.lib().step_roi_align_bwd_nhwc(L.c_void_p(grad_act.data_ptr()), grad_act.code, grad_act.ld, L.ptr(r), R, float(spatial_scale),
-                                            ph, pw, K, H, W, C, int(sampling_ratio), L.ptr(gin), C, L.stream()))
-    return gin

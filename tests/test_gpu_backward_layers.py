@@ -29,10 +29,10 @@ from step_b200 import synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import _tape_reference as R  # noqa: E402
+from _train_case import SHIPPED, device_nets  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-SHIPPED = dict(T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False)
 U12 = 2.0 ** -12
 # (conv entries, pool entries) of each tape, from the module structure: a Mixed block records its fused 1x1 triple, two
 # 3x3x3 convs, the branch-3 pool and its 1x1; the trunk adds the stem, conv3d_2b / 2c and three strided pools; ContextNet a
@@ -45,16 +45,11 @@ def counts(tape):
 
 
 def record(fn):
-    """Run fn with the tape on and the Inception branches on one stream, as training.trunk_forward_backward does."""
+    """Run fn with the tape on, as training.trunk_forward_backward does."""
     from step_b200 import engine as E
     tape = []
-    saved = E.TAPE, E.BRANCH_STREAMS
-    E.TAPE, E.BRANCH_STREAMS = tape, False
-    try:
-        with torch.no_grad():
-            fn()
-    finally:
-        E.TAPE, E.BRANCH_STREAMS = saved
+    with E.recording(tape), torch.no_grad():
+        fn()
     return tape
 
 
@@ -243,10 +238,8 @@ def chain():
     steps of 3, 3 and 9 frames) with tape_backward wrapped so that each call's tape, GradStore, the gradients seeded
     before it and its parameter gradients are kept: three heads, then ContextNet, then the trunk."""
     from step_b200 import training
-    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    from test_gpu_train_context import shipped_nets
     cfg = synth.make_cfg(fp16=True, **SHIPPED, image_size=(66, 82))
-    nets_ = shipped_nets(cfg)
+    nets_ = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], context=True)
     x = synth.make_clips(2, 36, 66, 82, seed=13).cuda()
     st, tg = synth.make_train_case(cfg, 2, 3, 82, 66, seed=5)
     calls, orig = [], training.tape_backward

@@ -12,7 +12,7 @@ import torch
 from step_b200 import optim, synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_gpu_train_context import SHIPPED, shipped_nets  # noqa: E402
+from _train_case import SHIPPED, device_nets  # noqa: E402
 from test_optim_cpu import fixture_groups  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -216,7 +216,7 @@ def test_update_invalidates_the_modules_weight_caches():
     updated weights (the packed fp16 / permuted caches are keyed on the parameters' _version)."""
     import step_b200
     cfg = synth.make_cfg(fp16=True, **SHIPPED, image_size=(64, 64))
-    nets = shipped_nets(cfg)
+    nets = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], context=True)
     x = synth.make_clips(1, 36, 64, 64, seed=3).cuda()
     g = torch.Generator().manual_seed(4)
     feat = (torch.randn(4, 3, 832, 7, 7, generator=g) * 0.5).cuda()
@@ -255,7 +255,8 @@ def trainable(nets):
 def test_train_step_with_adam_matches_torch_adam_on_the_returned_gradients():
     from step_b200 import training
     cfg, batch = shipped_case()
-    nets_a, nets_b = shipped_nets(cfg), shipped_nets(cfg)
+    heads_sd = [synth.head_state_dict(100 + i, cfg) for i in range(3)]
+    nets_a, nets_b = device_nets(cfg, heads_sd, context=True), device_nets(cfg, heads_sd, context=True)
     p0 = {k: p.detach().clone() for k, p in trainable(nets_a).items()}
     opt = optim.Adam(fixture_groups(nets_a))
     ra = training.train_step(cfg, nets_a, *batch, optimizer=opt)
@@ -278,7 +279,7 @@ def test_train_step_with_adam_matches_torch_adam_on_the_returned_gradients():
 def test_overflowing_loss_scale_skips_then_backs_off_to_an_applied_step():
     from step_b200 import training
     cfg, batch = shipped_case()
-    nets = shipped_nets(cfg)
+    nets = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], context=True)
     opt = optim.Adam(fixture_groups(nets))
     scaler = optim.LossScaler(init_scale=2.0 ** 40)
     before = {k: p.detach().clone() for k, p in trainable(nets).items()}
@@ -310,7 +311,7 @@ def test_adam_steps_descend_shipped_config():
     5e-5 next to O(0.05) conv weights."""
     from step_b200 import training
     cfg, batch = shipped_case(seed=7)
-    nets = shipped_nets(cfg)
+    nets = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], context=True)
     opt = optim.Adam(fixture_groups(nets, DESCENT_LR_SCALE))
     losses = []
     for _ in range(5):

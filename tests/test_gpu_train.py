@@ -4,6 +4,9 @@ torch-CPU autograd of the oracle, and torchvision's ROIAlign backward (tests/gol
 
 Tolerances: fp32 losses 1e-4 relative (expf / log1pf / logf are not bit-exact); gradients through fp16 activations
 2e-2 of the tensor norm."""
+import os
+import sys
+
 import numpy as np
 import pytest
 import torch
@@ -11,20 +14,14 @@ import torch
 from oracle import model as om
 from step_b200 import synth
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from _train_case import compare_grads, device_head, device_nets, spatial_case, trainable  # noqa: E402
+
 pytestmark = pytest.mark.gpu
 
 
 def cu(a):
     return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def head(cfg):
-    import step_b200
-    h = step_b200.TwoBranchNet(cfg)
-    h.load_state_dict(synth.head_state_dict(100, cfg), strict=True)
-    h = h.cuda().eval()
-    h.set_device("cuda:0")
-    return h
 
 
 @pytest.mark.parametrize("name", list(synth.LOSS_CASES))
@@ -35,7 +32,7 @@ def test_forward_with_targets_matches_reference(golden, name):
     T_, chunks, _, _ = synth.LOSS_CASES[name]
     cfg = synth.make_cfg(fp16=False, T=T_, max_iter=1, NUM_CHUNKS={1: chunks}, image_size=(112, 112))
     _, _, feat, tb, tg = synth.make_loss_case(name, cfg.num_classes)
-    net = head(cfg)
+    net = device_head(cfg, synth.head_state_dict(100, cfg))
     with torch.no_grad():
         prob, loc, first, last, lc, ll, ln = net(feat.cuda(), None, tubes=tb.cuda(), targets=tg.cuda())
     torch.cuda.synchronize()
@@ -100,7 +97,7 @@ def test_head_weight_gradients_match_reference_autograd(golden):
     T_, chunks, n, _ = synth.LOSS_CASES[name]
     cfg = synth.make_cfg(fp16=True, T=T_, max_iter=1, NUM_CHUNKS={1: chunks}, image_size=(112, 112))
     _, _, feat, tb, tg = synth.make_loss_case(name, cfg.num_classes)
-    net = head(cfg)
+    net = device_head(cfg, synth.head_state_dict(100, cfg))
     N, Tl = feat.shape[0], feat.shape[1]
     keep = {}
     with torch.no_grad():
@@ -227,7 +224,7 @@ def test_head_backward_every_parameter_matches_reference_autograd(golden):
     T_, chunks, n, _ = synth.LOSS_CASES[name]
     cfg = synth.make_cfg(fp16=True, T=T_, max_iter=1, NUM_CHUNKS={1: chunks}, image_size=(112, 112))
     _, _, feat, tb, tg = synth.make_loss_case(name, cfg.num_classes)
-    net = head(cfg)
+    net = device_head(cfg, synth.head_state_dict(100, cfg))
     r = training.head_forward_backward(net, feat.cuda(), tb.cuda(), tg.cuda(), lambda_reg=5.0, lambda_neighbor=1.0)
     torch.cuda.synchronize()
     assert abs(float(r["loss"]) - float(g["loss"][0])) <= 2e-3 * abs(float(g["loss"][0]))
@@ -374,47 +371,19 @@ def test_train_step_end_to_end_matches_oracle_autograd():
     backward into conv_feat, trunk backward, SGD(momentum, weight decay) update -- against torch-CPU autograd through the
     oracle's functional model (oracle/model.py, pinned to the reference) with torchvision's roi_align (bit-identical to the
     reference's forward) for the same seeded clips, tubes and targets (train.py:263-348 without train_select)."""
-    import step_b200
     from torchvision.ops import roi_align as tv_roi_align
     from step_b200 import training
-    cfg = synth.make_cfg(fp16=True, T=2, max_iter=2, NUM_CHUNKS={1: 1, 2: 1}, image_size=(64, 64))
-    B, N = 2, 3
-    x = synth.make_clips(B, 8, 64, 64, seed=11)
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet("align", 7)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict())
+    cfg, x, step_tubes, step_targets = spatial_case()
     heads_sd = [synth.head_state_dict(100 + i, cfg) for i in range(2)]
-    for i in range(2):
-        h = step_b200.TwoBranchNet(cfg)
-        h.load_state_dict(heads_sd[i])
-        nets["det_net%d" % i] = h
-    for k in nets:
-        nets[k] = nets[k].cuda().eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device("cuda:0")
-    gen = torch.Generator().manual_seed(3)
-    step_tubes, step_targets = [], []
-    for i in range(2):
-        R = B * N
-        x1 = torch.rand(R, 1, generator=gen) * 20; y1 = torch.rand(R, 1, generator=gen) * 20
-        w = 20 + torch.rand(R, 1, generator=gen) * 20; hh = 20 + torch.rand(R, 1, generator=gen) * 20
-        box = torch.cat([x1, y1, x1 + w, y1 + hh], 1)
-        frame = (torch.arange(R) // N).view(R, 1, 1) * 2 + torch.arange(2).view(1, 2, 1)
-        tubes = torch.cat([frame.float(), box.view(R, 1, 4).expand(R, 2, 4) + torch.rand(R, 2, 4, generator=gen)], 2)
-        tg = torch.zeros(R, 3, 66)
-        tg[:, :, :4] = box.view(R, 1, 4) + torch.rand(R, 3, 4, generator=gen) * 4
-        tg[:, :, 4] = (torch.rand(R, 3, generator=gen) > 0.3).float(); tg[:, :, 5] = (torch.rand(R, 3, generator=gen) > 0.3).float()
-        tg[0, :, 4:6] = 1.0
-        tg[:, :, 6:] = (torch.rand(R, 3, 60, generator=gen) > 0.9).float()
-        step_tubes.append(tubes); step_targets.append(tg)
+    nets = device_nets(cfg, heads_sd)
     # ---- oracle: torch-CPU autograd
     sd_b = {k: v.clone().requires_grad_(k.endswith("conv3d.weight")) for k, v in synth.base_net_state_dict().items()}
-    sds = [{k: v.clone().requires_grad_(v.is_floating_point() and "running_" not in k and "batch3d" not in k) for k, v in sd.items()}
-           for sd in heads_sd]
+    sds = [trainable(sd) for sd in heads_sd]
     cf = om.base_net(x.clone(), sd_b)                                   # [B, T', 832, H', W']
     total = 0.0
     for i in range(2):
         fm = cf.reshape(-1, 832, cf.shape[3], cf.shape[4])
-        pooled = tv_roi_align(fm, step_tubes[i].view(-1, 5), (7, 7), 1.0 / 16.0, 0, aligned=False).view(B * N, 2, 832, 7, 7)
+        pooled = tv_roi_align(fm, step_tubes[i].view(-1, 5), (7, 7), 1.0 / 16.0, 0, aligned=False).view(-1, 2, 832, 7, 7)
         prob, loc, first, last, logits = om.two_branch(pooled, sds[i], cfg.T, None, cfg.fc_dim, cfg.pool_size, return_logits=True)
         lc, ll, ln = om.two_branch_losses(logits, loc, first, last, step_tubes[i], step_targets[i], cfg.T)
         total = total + lc.mean() + 5.0 * ll.mean() + 1.0 * ln.mean()
@@ -425,21 +394,9 @@ def test_train_step_end_to_end_matches_oracle_autograd():
                             momentum=0.9, weight_decay=1e-4)
     torch.cuda.synchronize()
     assert abs(float(r["loss"]) - float(total)) <= 5e-3 * abs(float(total))
-
-    def cmp(module, sd_ref, ntol, ttol):
-        names = {p: k for k, p in module.named_parameters()}
-        n = 0
-        for p, gdev in r["grads"].items():
-            if p not in names:
-                continue
-            ref = sd_ref[names[p]].grad
-            rn = float(ref.double().norm())
-            assert abs(float(gdev.double().norm()) - rn) <= ntol * rn, (names[p], float(gdev.double().norm()), rn)
-            assert float((gdev.cpu().double() - ref.double()).norm()) <= ttol * rn, names[p]
-            n += 1
-        return n
-    assert cmp(nets["det_net0"], sds[0], 3e-2, 1e-1) == 34 and cmp(nets["det_net1"], sds[1], 3e-2, 1e-1) == 34
-    assert cmp(nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45
+    assert compare_grads(r, nets["det_net0"], sds[0], 3e-2, 1e-1) == 34
+    assert compare_grads(r, nets["det_net1"], sds[1], 3e-2, 1e-1) == 34
+    assert compare_grads(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45
     # the SGD update itself (first step: momentum buffer = gradient): p_new = p - lr * (g + wd * p)
     names = {p: k for k, p in nets["base_net"].named_parameters()}
     for p, gdev in r["grads"].items():

@@ -16,8 +16,8 @@ from oracle import model as om
 from step_b200 import optim, synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_gpu_train_context import SHIPPED, rel_l2, shipped_nets  # noqa: E402
-from test_oracle_cls import CLS_CFG, cls_objective, golden_case, trainable, transfer_pretrained  # noqa: E402
+from _train_case import SHIPPED, compare_grads, device_head, device_nets, rel_l2, trainable  # noqa: E402
+from test_oracle_cls import CLS_CFG, cls_objective, golden_case, transfer_pretrained  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -84,15 +84,6 @@ def test_cls_loss_without_classification_flag_and_bad_arguments():
         training.cls_loss(x, t[:, :, :-1])
 
 
-def device_cls_head(cfg, seed=100):
-    import step_b200
-    h = step_b200.TwoBranchNet(cfg, cls_only=True)
-    h.load_state_dict(synth.cls_head_state_dict(seed, cfg), strict=True)
-    h = h.cuda().eval()
-    h.set_device("cuda:0")
-    return h
-
-
 @pytest.fixture(scope="module")
 def cls_oracle():
     """The golden case through the oracle on the CPU, with the per-tube context copy as a leaf: the gradients of the pooled
@@ -117,7 +108,7 @@ def test_cls_forward_with_targets_returns_the_reference_outputs(golden, cls_orac
     outputs of the reference (probabilities, three [1] zeros, loss_cls, two [1] zero regression losses)."""
     g, o = golden("cls_grads"), cls_oracle
     cfg = synth.make_cfg(fp16=False, **CLS_CFG, image_size=(400, 400))
-    net = device_cls_head(cfg)
+    net = device_head(cfg, synth.cls_head_state_dict(100, cfg), cls_only=True)
     with torch.no_grad():
         outs = net(o["pooled"].detach().cuda(), o["tctx"].detach().cuda(), tubes=o["tubes"].cuda(), targets=o["targets"].cuda())
     torch.cuda.synchronize()
@@ -143,7 +134,7 @@ def test_cls_head_backward_matches_reference_and_oracle(golden, cls_oracle, form
     from step_b200 import training
     g, o = golden("cls_grads"), cls_oracle
     dcfg = synth.make_cfg(fp16=True, **CLS_CFG, image_size=(400, 400))
-    net = device_cls_head(dcfg)
+    net = device_head(dcfg, synth.cls_head_state_dict(100, dcfg), cls_only=True)
     if form == "per_tube":
         context = o["tctx"].detach().cuda()
     else:
@@ -170,19 +161,6 @@ def test_cls_head_backward_matches_reference_and_oracle(golden, cls_oracle, form
         assert rel_l2(r["ctx_grad"], o["tctx"].grad.sum(2).view(-1, 1024)) <= 8e-2
 
 
-def cls_nets(cfg, seed=100):
-    import step_b200
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet("align", 7), "context_net": step_b200.ContextNet(cfg)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict())
-    nets["context_net"].load_state_dict(synth.context_net_state_dict())
-    for k in nets:
-        nets[k] = nets[k].cuda().eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device("cuda:0")
-    nets["det_net0"] = device_cls_head(cfg, seed)
-    return nets
-
-
 def cls_case(seed=3, B=2, N=6):
     cfg = synth.make_cfg(fp16=True, **CLS_CFG, image_size=(64, 64))
     tubes, targets = synth.make_cls_case(cfg, B, N, 64, 64, seed=seed)
@@ -195,7 +173,7 @@ def test_train_step_cls_config_matches_oracle_autograd():
     head tensors."""
     from step_b200 import training
     cfg, x, tubes, targets = cls_case()
-    nets = cls_nets(cfg)
+    nets = device_nets(cfg, [synth.cls_head_state_dict(100, cfg)], context=True, cls_only=True)
     sd_b = {k: v.clone().requires_grad_(k.endswith("conv3d.weight")) for k, v in synth.base_net_state_dict().items()}
     sd_ctx = trainable(synth.context_net_state_dict())
     sd_h = trainable(synth.cls_head_state_dict(100, cfg))
@@ -207,28 +185,15 @@ def test_train_step_cls_config_matches_oracle_autograd():
     torch.cuda.synchronize()
     assert abs(float(r["loss"]) - total) <= 5e-3 * abs(total)
     assert len(r["losses"]) == 1 and len(r["grads"]) == 45 + 12 + 16
-
-    def cmp(module, sd_ref, ntol, ttol):
-        names = {p: k for k, p in module.named_parameters()}
-        n = 0
-        for p, gdev in r["grads"].items():
-            if p not in names:
-                continue
-            ref = sd_ref[names[p]].grad
-            rn = float(ref.double().norm())
-            assert abs(float(gdev.double().norm()) - rn) <= ntol * rn, (names[p], float(gdev.double().norm()), rn)
-            assert float((gdev.cpu().double() - ref.double()).norm()) <= ttol * rn, (names[p], rel_l2(gdev, ref))
-            n += 1
-        return n
-    assert cmp(nets["det_net0"], sd_h, 3e-2, 1e-1) == 16
-    assert cmp(nets["context_net"], sd_ctx, 3e-2, 1e-1) == 12
-    assert cmp(nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45
+    assert compare_grads(r, nets["det_net0"], sd_h, 3e-2, 1e-1) == 16
+    assert compare_grads(r, nets["context_net"], sd_ctx, 3e-2, 1e-1) == 12
+    assert compare_grads(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45
 
 
 def test_train_step_cls_config_keeps_the_frame_and_context_checks():
     from step_b200 import training
     cfg, x, tubes, targets = cls_case()
-    nets = cls_nets(cfg)
+    nets = device_nets(cfg, [synth.cls_head_state_dict(100, cfg)], context=True, cls_only=True)
     with pytest.raises(RuntimeError, match="step 1 pools frames"):
         training.train_step(cfg, nets, x.cuda(), [tubes[:, :3].contiguous().cuda()], [targets.cuda()])
     del nets["context_net"]
@@ -255,7 +220,7 @@ def test_adam_steps_descend_then_checkpoint_trains_the_shipped_heads():
     and a shipped-configuration train_step runs on them."""
     from step_b200 import training
     cfg, x, tubes, targets = cls_case(seed=7)
-    nets = cls_nets(cfg)
+    nets = device_nets(cfg, [synth.cls_head_state_dict(100, cfg)], context=True, cls_only=True)
     opt = optim.Adam(cls_groups(nets, DESCENT_LR_SCALE))
     scaler = optim.LossScaler()
     batch = (x.cuda(), [tubes.cuda()], [targets.cuda()])
@@ -268,7 +233,7 @@ def test_adam_steps_descend_then_checkpoint_trains_the_shipped_heads():
     assert all(b <= a for a, b in zip(losses, losses[1:])) and losses[-1] < losses[0], losses
     ckpt = {k: {n: v.detach().clone() for n, v in nets[k].state_dict().items()} for k in ("base_net", "context_net", "det_net0")}
     scfg = synth.make_cfg(fp16=True, **SHIPPED, image_size=(64, 64))
-    full = shipped_nets(scfg)
+    full = device_nets(scfg, [synth.head_state_dict(100 + i, scfg) for i in range(3)], context=True)
     transfer_pretrained(ckpt, full, 3)
     moved = [k for k in ckpt["det_net0"] if "global_cls" not in k]
     for i in range(3):

@@ -14,15 +14,10 @@ from oracle import model as om
 from step_b200 import synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_oracle_context import golden_case, oracle_objective, trainable  # noqa: E402
+from _train_case import SHIPPED, compare_grads, device_head, device_nets, rel_l2, trainable  # noqa: E402
+from test_oracle_context import golden_case, oracle_objective  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-
-SHIPPED = dict(T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False)
-
-
-def rel_l2(got, ref):
-    return float((got.detach().cpu().double() - ref.double()).norm() / ref.double().norm())
 
 
 def slice_case(dtype=torch.float16, seed=5):
@@ -134,15 +129,6 @@ def golden_oracle():
                 pooled=pooled, ctx=ctx)
 
 
-def device_head(cfg, i):
-    import step_b200
-    h = step_b200.TwoBranchNet(cfg)
-    h.load_state_dict(synth.head_state_dict(100 + i, cfg), strict=True)
-    h = h.cuda().eval()
-    h.set_device("cuda:0")
-    return h
-
-
 def test_head_with_context_matches_reference_and_oracle(golden, golden_oracle):
     """head_forward_backward with the reference's per-tube context feature [R,1024,T',1,1] for the three heads of the
     shipped configuration (steps of 3, 3 and 9 frames): the 34 trainable tensors of each head, the gradient of the pooled
@@ -165,7 +151,7 @@ def test_head_with_context_matches_reference_and_oracle(golden, golden_oracle):
         _, loc, first, last, logits = om.two_branch(pl, sd, cfg.T, tctx, cfg.fc_dim, cfg.pool_size, return_logits=True)
         lc, ll, ln = om.two_branch_losses(logits, loc, first, last, flat, o["step_targets"][i], cfg.T)
         (lc.mean() + 5.0 * ll.mean() + 1.0 * ln.mean()).backward()
-        net = device_head(dcfg, i)
+        net = device_head(dcfg, synth.head_state_dict(100 + i, dcfg))
         r = training.head_forward_backward(net, pooled.cuda(), flat.cuda(), o["step_targets"][i].cuda(), context_feat=tctx.detach().cuda())
         torch.cuda.synchronize()
         total += float(r["loss"])
@@ -215,22 +201,6 @@ def test_context_net_backward_matches_reference_and_oracle(golden, golden_oracle
     assert rel_l2(gf, o["cf"].grad) <= 8e-2, rel_l2(gf, o["cf"].grad)
 
 
-def shipped_nets(cfg):
-    import step_b200
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet("align", 7), "context_net": step_b200.ContextNet(cfg)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict())
-    nets["context_net"].load_state_dict(synth.context_net_state_dict())
-    for i in range(3):
-        h = step_b200.TwoBranchNet(cfg)
-        h.load_state_dict(synth.head_state_dict(100 + i, cfg))
-        nets["det_net%d" % i] = h
-    for k in nets:
-        nets[k] = nets[k].cuda().eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device("cuda:0")
-    return nets
-
-
 def test_train_step_shipped_config_matches_oracle_autograd():
     """train_step in the shipped configuration at reduced resolution (2 clips of 36x64x64, T'=9: steps pool frames [3, 6),
     [3, 6) and [0, 9)) against the oracle's autograd with torchvision's roi_align: 45 trunk, 12 ContextNet and 3 x 34 head
@@ -240,7 +210,7 @@ def test_train_step_shipped_config_matches_oracle_autograd():
     B, N = 2, 3
     x = synth.make_clips(B, 36, 64, 64, seed=11)
     step_tubes, step_targets = synth.make_train_case(cfg, B, N, 64, 64, seed=3)
-    nets = shipped_nets(cfg)
+    nets = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], context=True)
     sd_b = {k: v.clone().requires_grad_(k.endswith("conv3d.weight")) for k, v in synth.base_net_state_dict().items()}
     sd_ctx = trainable(synth.context_net_state_dict())
     sds = [trainable(synth.head_state_dict(100 + i, cfg)) for i in range(3)]
@@ -253,23 +223,10 @@ def test_train_step_shipped_config_matches_oracle_autograd():
     torch.cuda.synchronize()
     assert abs(float(r["loss"]) - float(total)) <= 5e-3 * abs(float(total))
     assert len(r["losses"]) == 3
-
-    def cmp(module, sd_ref, ntol, ttol):
-        names = {p: k for k, p in module.named_parameters()}
-        n = 0
-        for p, gdev in r["grads"].items():
-            if p not in names:
-                continue
-            ref = sd_ref[names[p]].grad
-            rn = float(ref.double().norm())
-            assert abs(float(gdev.double().norm()) - rn) <= ntol * rn, (names[p], float(gdev.double().norm()), rn)
-            assert float((gdev.cpu().double() - ref.double()).norm()) <= ttol * rn, (names[p], rel_l2(gdev, ref))
-            n += 1
-        return n
     for i in range(3):
-        assert cmp(nets["det_net%d" % i], sds[i], 3e-2, 1e-1) == 34
-    assert cmp(nets["context_net"], sd_ctx, 3e-2, 1e-1) == 12
-    assert cmp(nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45
+        assert compare_grads(r, nets["det_net%d" % i], sds[i], 3e-2, 1e-1) == 34
+    assert compare_grads(r, nets["context_net"], sd_ctx, 3e-2, 1e-1) == 12
+    assert compare_grads(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45
     names = {p: k for k, p in nets["context_net"].named_parameters()}
     for p, gdev in r["grads"].items():
         if p in names and names[p].endswith("2.branch_0.conv3d.weight"):
@@ -281,7 +238,7 @@ def test_train_step_shipped_config_rejects_mismatched_tubes_and_missing_context_
     from step_b200 import training
     cfg = synth.make_cfg(fp16=True, **SHIPPED, image_size=(64, 64))
     step_tubes, step_targets = synth.make_train_case(cfg, 1, 2, 64, 64)
-    nets = shipped_nets(cfg)
+    nets = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], context=True)
     x = synth.make_clips(1, 36, 64, 64).cuda()
     bad = [step_tubes[0], step_tubes[2], step_tubes[2]]                   # step 2 pools 3 frames, not 9
     with pytest.raises(RuntimeError, match="step 2 pools frames"):
@@ -297,7 +254,7 @@ def test_sgd_steps_descend_shipped_config():
     tests/test_gpu_train.py::test_sgd_steps_descend."""
     from step_b200 import training
     cfg = synth.make_cfg(fp16=True, **SHIPPED, image_size=(64, 64))
-    nets = shipped_nets(cfg)
+    nets = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], context=True)
     step_tubes, step_targets = synth.make_train_case(cfg, 2, 3, 64, 64, seed=7)
     args = (cfg, nets, synth.make_clips(2, 36, 64, 64, seed=5).cuda(), [t.cuda() for t in step_tubes], [t.cuda() for t in step_targets])
     losses = []

@@ -23,6 +23,7 @@ from step_b200 import synth
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import test_oracle_cls  # noqa: E402
 import test_oracle_context  # noqa: E402
+from _train_case import SHIPPED, compare_grads, device_nets, spatial_case, trainable  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -211,52 +212,12 @@ def test_edge_cases_match_torchvision(size):
 
 
 # ---- 5. routing inside train_step -------------------------------------------------------------------------------------
-def spatial_case(B=2, N=3, seed=3):
-    """The two-step spatial case of tests/test_gpu_train.py::test_train_step_end_to_end_matches_oracle_autograd."""
-    cfg = synth.make_cfg(fp16=True, T=2, max_iter=2, NUM_CHUNKS={1: 1, 2: 1}, image_size=(64, 64))
-    x = synth.make_clips(B, 8, 64, 64, seed=11)
-    gen = torch.Generator().manual_seed(seed)
-    step_tubes, step_targets = [], []
-    for i in range(2):
-        R = B * N
-        x1 = torch.rand(R, 1, generator=gen) * 20; y1 = torch.rand(R, 1, generator=gen) * 20
-        w = 20 + torch.rand(R, 1, generator=gen) * 20; hh = 20 + torch.rand(R, 1, generator=gen) * 20
-        box = torch.cat([x1, y1, x1 + w, y1 + hh], 1)
-        frame = (torch.arange(R) // N).view(R, 1, 1) * 2 + torch.arange(2).view(1, 2, 1)
-        tubes = torch.cat([frame.float(), box.view(R, 1, 4).expand(R, 2, 4) + torch.rand(R, 2, 4, generator=gen)], 2)
-        tg = torch.zeros(R, 3, 66)
-        tg[:, :, :4] = box.view(R, 1, 4) + torch.rand(R, 3, 4, generator=gen) * 4
-        tg[:, :, 4] = (torch.rand(R, 3, generator=gen) > 0.3).float(); tg[:, :, 5] = (torch.rand(R, 3, generator=gen) > 0.3).float()
-        tg[0, :, 4:6] = 1.0
-        tg[:, :, 6:] = (torch.rand(R, 3, 60, generator=gen) > 0.9).float()
-        step_tubes.append(tubes); step_targets.append(tg)
-    return cfg, x, step_tubes, step_targets
-
-
-def build_nets(cfg, heads_sd, context=False, cls_only=False):
-    import step_b200
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet("pool", 7)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict())
-    if context:
-        nets["context_net"] = step_b200.ContextNet(cfg)
-        nets["context_net"].load_state_dict(synth.context_net_state_dict())
-    for i, sd in enumerate(heads_sd):
-        h = step_b200.TwoBranchNet(cfg, cls_only=cls_only)
-        h.load_state_dict(sd)
-        nets["det_net%d" % i] = h
-    for k in nets:
-        nets[k] = nets[k].cuda().eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device("cuda:0")
-    return nets
-
-
 def test_train_step_feeds_the_trunk_the_roi_pool_backward(monkeypatch):
     """The conv_feat gradient train_step hands to the trunk is torchvision's CPU ROIPool backward of the step's own fp16
     conv_feat, its pooled-feature gradients and its tubes (summed over the steps, divided by the loss scale)."""
     from step_b200 import training
     cfg, x, step_tubes, step_targets = spatial_case()
-    nets = build_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(2)])
+    nets = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(2)], "pool")
     cap = {"roi_grad": []}
     head_fb, trunk_fb = training.head_forward_backward, training.trunk_forward_backward
 
@@ -321,21 +282,6 @@ def argmax_flips(nets, x, cf, cfg, step_tubes):
     return flips, pos, total
 
 
-def compare(r, module, sd_ref, ntol, ttol):
-    names = {p: k for k, p in module.named_parameters()}
-    n = 0
-    for p, gdev in r["grads"].items():
-        if p not in names:
-            continue
-        ref = sd_ref[names[p]].grad
-        rn = float(ref.double().norm())
-        rel = float((gdev.cpu().double() - ref.double()).norm()) / rn
-        assert abs(float(gdev.double().norm()) - rn) <= ntol * rn, (names[p], float(gdev.double().norm()), rn)
-        assert rel <= ttol, (names[p], rel)
-        n += 1
-    return n
-
-
 # At most 1 % of the pooled elements may take another pixel than the fp32 oracle's: the ROIAlign tests' tolerances below
 # are kept unchanged on that condition (a failing comparison reports the counts).
 MAX_FLIP_FRACTION = 1e-2
@@ -345,9 +291,9 @@ def test_train_step_pool_end_to_end_matches_oracle_autograd():
     from step_b200 import training
     cfg, x, step_tubes, step_targets = spatial_case()
     heads_sd = [synth.head_state_dict(100 + i, cfg) for i in range(2)]
-    nets = build_nets(cfg, heads_sd)
+    nets = device_nets(cfg, heads_sd, "pool")
     sd_b = {k: v.clone().requires_grad_(k.endswith("conv3d.weight")) for k, v in synth.base_net_state_dict().items()}
-    sds = [test_oracle_context.trainable(sd) for sd in heads_sd]
+    sds = [trainable(sd) for sd in heads_sd]
     cf = om.base_net(x.clone(), sd_b)
     total = 0.0
     for i in range(2):
@@ -365,8 +311,8 @@ def test_train_step_pool_end_to_end_matches_oracle_autograd():
                             momentum=0.9, weight_decay=1e-4)
     torch.cuda.synchronize()
     assert abs(float(r["loss"]) - total) <= 5e-3 * abs(total)
-    assert compare(r, nets["det_net0"], sds[0], 3e-2, 1e-1) == 34 and compare(r, nets["det_net1"], sds[1], 3e-2, 1e-1) == 34
-    assert compare(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45, (flips, pos, n)
+    assert compare_grads(r, nets["det_net0"], sds[0], 3e-2, 1e-1) == 34 and compare_grads(r, nets["det_net1"], sds[1], 3e-2, 1e-1) == 34
+    assert compare_grads(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45, (flips, pos, n)
     names = {p: k for k, p in nets["base_net"].named_parameters()}
     for p, gdev in r["grads"].items():
         if p in names and names[p].endswith("12.branch_0.conv3d.weight"):
@@ -377,15 +323,14 @@ def test_train_step_pool_end_to_end_matches_oracle_autograd():
 def test_train_step_pool_shipped_config_matches_oracle_autograd(monkeypatch):
     from step_b200 import training
     monkeypatch.setattr(test_oracle_context, "tv_roi_align", pool_as_align)
-    shipped = dict(T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False)
-    cfg = synth.make_cfg(fp16=True, **shipped, image_size=(64, 64))
+    cfg = synth.make_cfg(fp16=True, **SHIPPED, image_size=(64, 64))
     B, N = 2, 3
     x = synth.make_clips(B, 36, 64, 64, seed=11)
     step_tubes, step_targets = synth.make_train_case(cfg, B, N, 64, 64, seed=3)
-    nets = build_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], context=True)
+    nets = device_nets(cfg, [synth.head_state_dict(100 + i, cfg) for i in range(3)], "pool", context=True)
     sd_b = {k: v.clone().requires_grad_(k.endswith("conv3d.weight")) for k, v in synth.base_net_state_dict().items()}
-    sd_ctx = test_oracle_context.trainable(synth.context_net_state_dict())
-    sds = [test_oracle_context.trainable(synth.head_state_dict(100 + i, cfg)) for i in range(3)]
+    sd_ctx = trainable(synth.context_net_state_dict())
+    sds = [trainable(synth.head_state_dict(100 + i, cfg)) for i in range(3)]
     cf = om.base_net(x.clone(), sd_b)
     total, _, _ = test_oracle_context.oracle_objective(cf, sd_ctx, sds, cfg, step_tubes, step_targets)
     total.backward()
@@ -398,9 +343,9 @@ def test_train_step_pool_shipped_config_matches_oracle_autograd(monkeypatch):
     assert abs(float(r["loss"]) - float(total)) <= 5e-3 * abs(float(total))
     assert len(r["losses"]) == 3
     for i in range(3):
-        assert compare(r, nets["det_net%d" % i], sds[i], 3e-2, 1e-1) == 34
-    assert compare(r, nets["context_net"], sd_ctx, 3e-2, 1e-1) == 12
-    assert compare(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45, (flips, pos, n)
+        assert compare_grads(r, nets["det_net%d" % i], sds[i], 3e-2, 1e-1) == 34
+    assert compare_grads(r, nets["context_net"], sd_ctx, 3e-2, 1e-1) == 12
+    assert compare_grads(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45, (flips, pos, n)
     names = {p: k for k, p in nets["context_net"].named_parameters()}
     for p, gdev in r["grads"].items():
         if p in names and names[p].endswith("2.branch_0.conv3d.weight"):
@@ -414,10 +359,10 @@ def test_train_step_pool_cls_config_matches_oracle_autograd(monkeypatch):
     cfg = synth.make_cfg(fp16=True, **test_oracle_cls.CLS_CFG, image_size=(64, 64))
     tubes, targets = synth.make_cls_case(cfg, 2, 6, 64, 64, seed=3)
     x = synth.make_clips(2, 36, 64, 64, seed=11)
-    nets = build_nets(cfg, [synth.cls_head_state_dict(100, cfg)], context=True, cls_only=True)
+    nets = device_nets(cfg, [synth.cls_head_state_dict(100, cfg)], "pool", context=True, cls_only=True)
     sd_b = {k: v.clone().requires_grad_(k.endswith("conv3d.weight")) for k, v in synth.base_net_state_dict().items()}
-    sd_ctx = test_oracle_cls.trainable(synth.context_net_state_dict())
-    sd_h = test_oracle_cls.trainable(synth.cls_head_state_dict(100, cfg))
+    sd_ctx = trainable(synth.context_net_state_dict())
+    sd_h = trainable(synth.cls_head_state_dict(100, cfg))
     cf = om.base_net(x.clone(), sd_b)
     total, _, _, _, _ = test_oracle_cls.cls_objective(cf, sd_ctx, sd_h, cfg, tubes, targets)
     total.backward()
@@ -428,6 +373,6 @@ def test_train_step_pool_cls_config_matches_oracle_autograd(monkeypatch):
     torch.cuda.synchronize()
     assert abs(float(r["loss"]) - total) <= 5e-3 * abs(total)
     assert len(r["losses"]) == 1 and len(r["grads"]) == 45 + 12 + 16
-    assert compare(r, nets["det_net0"], sd_h, 3e-2, 1e-1) == 16
-    assert compare(r, nets["context_net"], sd_ctx, 3e-2, 1e-1) == 12
-    assert compare(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45, (flips, pos, n)
+    assert compare_grads(r, nets["det_net0"], sd_h, 3e-2, 1e-1) == 16
+    assert compare_grads(r, nets["context_net"], sd_ctx, 3e-2, 1e-1) == 12
+    assert compare_grads(r, nets["base_net"], sd_b, 1.5e-1, 2.5e-1) == 45, (flips, pos, n)

@@ -134,15 +134,34 @@ def test_fused_exit_dispatch_rule():
     assert not E.can_fuse_exit(L.F32, 256, 1024, 256)
     assert not E.can_fuse_exit(L.F16, 128, 1024, 256)
     assert not E.can_fuse_exit(L.F16, 256, 1024, 512)
-    old = E.TAPE
-    try:
-        E.TAPE = []
+    with E.recording([]):
         assert not E.can_fuse_exit(L.F16, 256, 1024, 256)
-    finally:
-        E.TAPE = old
     old = E.FUSE_EXIT
     try:
         E.FUSE_EXIT = False
         assert not E.can_fuse_exit(L.F16, 256, 1024, 256)
     finally:
         E.FUSE_EXIT = old
+
+
+def test_recording_restores_tape_and_branch_streams(monkeypatch):
+    """engine.recording: a list is recorded into with the Inception branches on one stream, None only stops recording, and
+    both switches come back after a normal exit, an exception and a nested recording(None)."""
+    monkeypatch.setattr(E, "TAPE", None)
+    monkeypatch.setattr(E, "BRANCH_STREAMS", True)
+    tape = []
+    with E.recording(tape) as t:
+        assert t is tape and E.TAPE is tape and E.BRANCH_STREAMS is False
+    assert E.TAPE is None and E.BRANCH_STREAMS is True
+    with pytest.raises(ValueError):
+        with E.recording(tape):
+            raise ValueError
+    assert E.TAPE is None and E.BRANCH_STREAMS is True
+    with E.recording(tape):
+        with E.recording(None):
+            assert E.TAPE is None and E.BRANCH_STREAMS is False
+        assert E.TAPE is tape and E.BRANCH_STREAMS is False
+    assert E.TAPE is None and E.BRANCH_STREAMS is True
+    with E.recording(None):
+        assert E.TAPE is None and E.BRANCH_STREAMS is True
+    assert E.TAPE is None and E.BRANCH_STREAMS is True

@@ -5,6 +5,7 @@ the element-level checker of the device's class-only training step.  The step_b2
 state_dict, the reference's get_params groups its nets as its own (tests/golden/cls_param_groups.npz), and its checkpoint
 transfers into full heads as train.py:153-166 loads it."""
 import os
+import sys
 from types import SimpleNamespace
 
 import numpy as np
@@ -15,14 +16,13 @@ from torchvision.ops import roi_align as tv_roi_align
 from oracle import model as om
 from step_b200 import synth
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from _train_case import trainable  # noqa: E402
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "cls_param_groups.npz")
 # scripts/train_cls.sh (rgb input, context on, one refinement step) and config.py's default weight_decay
 CLS_ARGS = dict(base_lr=5e-5, det_lr0=1e-4, det_lr=5e-4, weight_decay=1e-7, input_type="rgb", no_context=False, max_iter=1)
 CLS_CFG = dict(T=9, max_iter=1, NUM_CHUNKS={1: 1}, no_context=False)
-
-
-def trainable(sd):
-    return {k: v.clone().requires_grad_(v.is_floating_point() and "running_" not in k and "batch3d" not in k) for k, v in sd.items()}
 
 
 def cls_objective(cf, sd_ctx, sd, cfg, flat_tubes, flat_targets, pooled_leaf=False):

@@ -2,6 +2,9 @@
 two_branch_losses) reproduces the reference's autograd for the shipped training configuration (scripts/train_step.sh:
 T=3, temporal mode NUM_CHUNKS {1:1, 2:1, 3:3}, context on) -- tests/golden/ctx_temporal_grads.npz.  Once pinned here,
 the oracle is the element-level checker of the device's context / temporal training step at any resolution."""
+import os
+import sys
+
 import numpy as np
 import torch
 from torchvision.ops import roi_align as tv_roi_align
@@ -9,9 +12,8 @@ from torchvision.ops import roi_align as tv_roi_align
 from oracle import model as om
 from step_b200 import synth
 
-
-def trainable(sd):
-    return {k: v.clone().requires_grad_(v.is_floating_point() and "running_" not in k and "batch3d" not in k) for k, v in sd.items()}
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from _train_case import trainable  # noqa: E402
 
 
 def oracle_objective(cf, sd_ctx, sds, cfg, step_tubes, step_targets, pooled_leaves=False):
