@@ -178,6 +178,35 @@ typedef struct {
 int step_frames_to_clip_u8(const step_frame_src* table, int B, int T, int H, int W, int scale_mode, const float* mean3,
                            const float* std3, float* out, step_stream_t stream);
 
+/* What the reference's TubeAugmentation (data/augmentations.py:540-589) drew for one clip, in source pixels.  The host
+ * stage (step_b200.transforms.TubeAugmentation) fills it in the DataLoader workers. */
+typedef struct {
+  int x0, y0, w, h;          /* RandomSampleCrop's rect: source columns x0..x0+w-1, rows y0..y0+h-1 (the whole frame if none) */
+  int flip;                  /* RandomMirror: the crop is mirrored horizontally */
+  int photometric;           /* PhotometricDistort ran: the program below, with its HSV round trip, precedes the rest */
+  int brightness, contrast, contrast_first, saturation, hue;  /* the ops' gates; contrast_first: before the HSV round trip */
+  float brightness_delta, contrast_alpha, saturation_alpha, hue_delta;  /* fp32, as applied */
+  int perm[3];               /* RandomLightingNoise: BGR channel k of the result is channel perm[k] (identity: 0,1,2) */
+  int erase_begin, erase_count;  /* this clip's RandomErase regions: erase[erase_begin .. erase_begin+erase_count-1] */
+} step_clip_aug;
+/* One RandomErase region, in the coordinates of the mirrored crop; later regions of a clip cover earlier ones.  Its values
+ * are noise[noise .. noise + (y2-y1)*(x2-x1)*3 - 1], fp32 [y2-y1, x2-x1, 3] in BGR order, the same for every frame. */
+typedef struct {
+  int x1, y1, x2, y2;
+  long long noise;
+} step_aug_erase;
+/* The reference's TubeAugmentation followed by its dataset's swap to RGB and permute, for B clips of T frames in one launch:
+ * out [B,T,3,H,W] fp32 contiguous.  Per pixel, in the reference's order: u8 BGR -> f32; PhotometricDistort (brightness,
+ * contrast, cv2's float BGR2HSV, saturation, hue with its wrap, cv2's HSV2BGR, contrast; cv2 4.x's arithmetic bit for bit,
+ * DESIGN.md); the channel permutation; ConvertFromInts(scale_mode) (np.clip to [0, 255] first when scale_mode
+ * is 2 and the clip is distorted); the erase regions.  Then the crop, mirrored when flipped, is resized and normalised as
+ * step_frames_to_clip_u8 resizes and normalises the whole frame.
+ * `table`, `params` (B entries), `erase` and `noise` are DEVICE arrays read by the kernel and are not validated here; erase
+ * and noise may both be NULL when no clip erases.  Each entry needs its crop inside the frame, w, h > 0 and w <= 48 * W. */
+int step_frames_to_clip_aug_u8(const step_frame_src* table, const step_clip_aug* params, const step_aug_erase* erase,
+                               const float* noise, int B, int T, int H, int W, int scale_mode, const float* mean3,
+                               const float* std3, float* out, step_stream_t stream);
+
 /* ------------------------------------------------------------------ conv / pool / linear - */
 typedef struct {
   int dtype;                 /* STEP_F32: SIMT fp32 path.  STEP_F16: wgmma implicit GEMM, fp32 accumulate */

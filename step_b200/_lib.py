@@ -51,6 +51,19 @@ class FrameSrc(ctypes.Structure):
                [(n, ctypes.c_longlong) for n in ("stride_t", "stride_c", "stride_h", "stride_w")]
 
 
+class ClipAug(ctypes.Structure):
+    """mirror of step_clip_aug (include/step_b200.h)"""
+    _fields_ = [(n, c_int) for n in ("x0", "y0", "w", "h", "flip", "photometric", "brightness", "contrast",
+                                     "contrast_first", "saturation", "hue")] + \
+               [(n, c_float) for n in ("brightness_delta", "contrast_alpha", "saturation_alpha", "hue_delta")] + \
+               [("perm", c_int * 3), ("erase_begin", c_int), ("erase_count", c_int)]
+
+
+class AugErase(ctypes.Structure):
+    """mirror of step_aug_erase (include/step_b200.h)"""
+    _fields_ = [(n, c_int) for n in ("x1", "y1", "x2", "y2")] + [("noise", ctypes.c_longlong)]
+
+
 def _declare(lib):
     P, I, Fl, S = c_void_p, c_int, c_float, c_void_p  # S = stream
     sigs = {
@@ -110,6 +123,7 @@ def _declare(lib):
         "step_multi_tensor_adam_f32": ([P, I, P, I, S], c_int),
         "step_multi_tensor_sgd_f32": ([P, I, P, I, S], c_int),
         "step_frames_to_clip_u8": ([P, I, I, I, I, I, P, P, P, S], c_int),
+        "step_frames_to_clip_aug_u8": ([P, P, P, P, I, I, I, I, I, P, P, P, S], c_int),
         "step_debug_tma_tile": ([ctypes.POINTER(ConvParams), I, I, I, I, I, P, P, P, S], c_int),
     }
     for name, (argtypes, restype) in sigs.items():
