@@ -17,10 +17,14 @@
 //   B (weights, [Cout, taps, Cin] fp16, K-major rows = output channels): 3-D map, box (BK,1,BN).
 //   D: fp32 in registers; consumer warpgroup w owns rows [64 w, 64 w + 64) x BN columns (BN / 2 registers), and issues one
 //      m64nBNk16 wgmma per 16-element K step.  BN is sized to Cout (up to 256, see pick_tile).
-// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread of warp 0) and the epilogue constants,
-// warpgroups 1, 2 = wgmma consumers + epilogue; for BN > 128 the producer warpgroup hands registers to the consumers
-// (setmaxnreg).  Pipeline: n_stages smem stages with full / empty mbarriers; the stage area is reused as the fp16 output
-// staging tile once both consumers are done with it.
+// Persistent: CTA b runs tiles b, b + grid, b + 2 grid, ... with no CTA waiting on another (tiles with long K loops get one
+// CTA each, see build_plan).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread of warp 0) and, in warps 1-3, the copy-out of
+// the fp16 output staging tile to global plus the next tile's epilogue constants; warpgroups 1, 2 = wgmma consumers and
+// the register half of the epilogue; for BN > 128 warpgroup 0 hands registers to the consumers (setmaxnreg).  Pipeline:
+// n_stages smem stages with full / empty mbarriers, carried across tiles, so the producer loads the next tile while the
+// epilogue of this one runs.  The staging tile is a buffer of its own, handed between consumers and copy warps by one
+// full / empty mbarrier pair.
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -37,7 +41,10 @@ constexpr int kMaxBN = 256;    // 128 fp32 accumulator registers per consumer th
 constexpr int kStages = 8;     // barrier slots
 constexpr int kThreads = 384;
 constexpr int kConsumers = 256;
-constexpr int kBookBytes = 2 * kStages * 8 + 2 * kMaxBN * 4;  // barriers, scale, shift
+constexpr int kCopyThreads = 96;  // warps 1-3
+constexpr int kPersistMaxKBlocks = 100;  // longer K loops run one tile per CTA (build_plan)
+// stage barriers, staging-tile barriers, scale and shift of two consecutive tiles
+constexpr int kBookBytes = 2 * kStages * 8 + 2 * 8 + 2 * 2 * kMaxBN * 4;
 // registers per thread after the hand-over of wide tiles: 128 x 40 + 256 x 232 = 384 x 168, the launch allocation
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 
@@ -64,6 +71,7 @@ struct ConvGeom {
   int Cout, out_ld, out_coff, res_ld, res_coff, relu;
   int OT, OH, OW, Nimg;
   long long M;                  // Nimg*OT*OH*OW
+  int tiles;                    // M tiles x n_tiles
   int bw, bh, bt, tiles_w, tiles_h, tiles_t;  // BOX mode
   int a_bytes;                  // bytes TMA writes for A per stage
 };
@@ -85,6 +93,13 @@ __device__ __forceinline__ long long tile_row_pixel(const ConvGeom& g, int m_til
   return m < g.M ? m : -1;
 }
 
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t done;
+  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+               : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+  return done != 0;
+}
+
 // ---- the kernel -----------------------------------------------------------------------------
 template <int BK, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -94,82 +109,170 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   static_assert(BN % 8 == 0 && BN <= kMaxBN, "wgmma N is a multiple of 8, at most 256");
   // more than 64 accumulators per consumer thread do not fit the even share of the register file (168 per thread)
   constexpr bool kRealloc = BN > 128;
+  // rows of more than 256 bytes leave the staging tile as bulk copies; per-copy overhead makes narrower rows faster as
+  // 16-byte stores
+  constexpr bool kBulkOut = BN > 128;
   constexpr int kABytes = kBM * BK * 2;
   constexpr int kBBytes = BN * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [barriers | scale | shift] (kBookBytes) then the 1024-aligned stage area [A stages][B stages], re-used by the
-  // epilogue as the fp16 output staging tile.
+  // carve: [stage barriers | staging barriers | scale, shift x 2] (kBookBytes) then the 1024-aligned stage area
+  // [A stages][B stages], then the fp16 output staging tile (kBM rows of staging_pitch(BN) bytes).
   uint64_t* full_bar = (uint64_t*)smem_raw;
   uint64_t* empty_bar = full_bar + kStages;
-  float* s_scale = (float*)(empty_bar + kStages);
-  float* s_shift = s_scale + kMaxBN;
+  uint64_t* out_full = empty_bar + kStages;     // phase 1 of the CTA's i-th tile has written the staging tile
+  uint64_t* out_empty = out_full + 1;           // the copy warps have read the i-th tile out of it
+  // scale and shift of the CTA's i-th tile live in buffer i & 1: the copy warps stage tile i + 1 while tile i's
+  // epilogue may still read buffer i & 1
+  float* s_consts = (float*)(out_empty + 1);    // [2][scale BN | shift BN] with kMaxBN pitch
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + kBookBytes + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = smem;
   uint8_t* sB = smem + g.n_stages * kABytes;
+  uint8_t* stg = smem + g.n_stages * (kABytes + kBBytes);
+  constexpr int pitch = staging_pitch(BN);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tile = blockIdx.x / g.n_tiles, n_tile = blockIdx.x - m_tile * g.n_tiles;
-  const int n0 = n_tile * BN;
   const int num_kb = g.taps * g.kblocks_per_tap;
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
     for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+    mbar_init(out_full, kConsumers / 32);
+    mbar_init(out_empty, kCopyThreads / 32);
     fence_barrier_init();
   }
-  if (threadIdx.x < 128) {  // stage the per-channel epilogue constants
-    for (int i = threadIdx.x; i < BN; i += 128) {
-      const int c = n0 + i;
+  // the per-channel epilogue constants of N tile n_tile into buffer `buf`, by `nthr` threads starting at `t`
+  auto stage_consts = [&](int n_tile, int buf, int t, int nthr) {
+    float* s_scale = s_consts + buf * 2 * kMaxBN;
+    float* s_shift = s_scale + kMaxBN;
+    for (int i = t; i < BN; i += nthr) {
+      const int c = n_tile * BN + i;
       s_scale[i] = (scale && c < g.Cout) ? scale[c] : 1.0f;
       s_shift[i] = (shift && c < g.Cout) ? shift[c] : 0.0f;
     }
-  }
+  };
+  if (threadIdx.x < 128) stage_consts(blockIdx.x % g.n_tiles, 0, threadIdx.x, 128);
   __syncthreads();
   pdl_wait();                 // the producer of x (the previous kernel in the stream) has finished
   pdl_launch_dependents();
 
   if (warp < 4) {
-    // ===================== TMA producer =====================
     if constexpr (kRealloc) setmaxnreg_dec<kProducerRegs>();
-    if (warp == 0 && elect_one()) {
-      long long m0 = (long long)m_tile * kBM;
-      int bn = 0, bt0 = 0, bh0 = 0, bw0 = 0;  // BOX origin
-      if (g.mode == A_BOX) {
-        int r = m_tile;
-        bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
-        bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
-        bt0 = (r % g.tiles_t) * g.bt; bn = r / g.tiles_t;
-      }
-      // IM2COL start coordinates: output pixel m0 -> (w,h,t,n) + lower corner (= -pad)
-      int iw = 0, ih = 0, it = 0, in_ = 0;
-      if (g.mode == A_IM2COL) {
-        long long r = m0;
-        iw = (int)(r % g.OW); r /= g.OW;
-        ih = (int)(r % g.OH); r /= g.OH;
-        it = (int)(r % g.OT); in_ = (int)(r / g.OT);
-        iw -= g.PW; ih -= g.PH; it -= g.PT;
-      }
-      const uint32_t tx_bytes = (uint32_t)(g.a_bytes + kBBytes);
-      int stage = 0; uint32_t phase = 0;
-      int kw = 0, kh = 0, kt = 0;                  // filter tap, advanced incrementally (no divisions in the loop)
-      for (int tap = 0; tap < g.taps; ++tap) {
-        for (int kc = 0; kc < g.kblocks_per_tap; ++kc) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], tx_bytes);
-          const int c0 = kc * BK;
-          uint8_t* a_dst = sA + stage * kABytes;
-          if (g.mode == A_LINEAR) {
-            tma_load_2d(&map_a, &full_bar[stage], a_dst, c0, (int)m0);
-          } else if (g.mode == A_BOX) {
-            tma_load_5d(&map_a, &full_bar[stage], a_dst, c0, bw0 + kw - g.PW, bh0 + kh - g.PH, bt0 + kt - g.PT, bn);
-          } else {
-            tma_load_im2col_5d(&map_a, &full_bar[stage], a_dst, c0, iw, ih, it, in_, (uint16_t)kw, (uint16_t)kh, (uint16_t)kt);
+    if (warp == 0) {
+      // ===================== TMA producer =====================
+      if (elect_one()) {
+        const uint32_t tx_bytes = (uint32_t)(g.a_bytes + kBBytes);
+        int stage = 0; uint32_t phase = 0;       // carried from each tile's last k-block into the next tile's first
+        for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x) {
+          const int m_tile = tile / g.n_tiles, n0 = (tile - m_tile * g.n_tiles) * BN;
+          long long m0 = (long long)m_tile * kBM;
+          int bn = 0, bt0 = 0, bh0 = 0, bw0 = 0;  // BOX origin
+          if (g.mode == A_BOX) {
+            int r = m_tile;
+            bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
+            bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
+            bt0 = (r % g.tiles_t) * g.bt; bn = r / g.tiles_t;
           }
-          tma_load_3d(&map_b, &full_bar[stage], sB + stage * kBBytes, c0, tap, n0);
-          if (++stage == g.n_stages) { stage = 0; phase ^= 1; }
+          // IM2COL start coordinates: output pixel m0 -> (w,h,t,n) + lower corner (= -pad)
+          int iw = 0, ih = 0, it = 0, in_ = 0;
+          if (g.mode == A_IM2COL) {
+            long long r = m0;
+            iw = (int)(r % g.OW); r /= g.OW;
+            ih = (int)(r % g.OH); r /= g.OH;
+            it = (int)(r % g.OT); in_ = (int)(r / g.OT);
+            iw -= g.PW; ih -= g.PH; it -= g.PT;
+          }
+          int kw = 0, kh = 0, kt = 0;                // filter tap, advanced incrementally (no divisions in the loop)
+          for (int tap = 0; tap < g.taps; ++tap) {
+            for (int kc = 0; kc < g.kblocks_per_tap; ++kc) {
+              mbar_wait(&empty_bar[stage], phase ^ 1);
+              mbar_expect_tx(&full_bar[stage], tx_bytes);
+              const int c0 = kc * BK;
+              uint8_t* a_dst = sA + stage * kABytes;
+              if (g.mode == A_LINEAR) {
+                tma_load_2d(&map_a, &full_bar[stage], a_dst, c0, (int)m0);
+              } else if (g.mode == A_BOX) {
+                tma_load_5d(&map_a, &full_bar[stage], a_dst, c0, bw0 + kw - g.PW, bh0 + kh - g.PH, bt0 + kt - g.PT, bn);
+              } else {
+                tma_load_im2col_5d(&map_a, &full_bar[stage], a_dst, c0, iw, ih, it, in_, (uint16_t)kw, (uint16_t)kh,
+                                   (uint16_t)kt);
+              }
+              tma_load_3d(&map_b, &full_bar[stage], sB + stage * kBBytes, c0, tap, n0);
+              if (++stage == g.n_stages) { stage = 0; phase ^= 1; }
+            }
+            if (++kw == g.KW) { kw = 0; if (++kh == g.KH) { kh = 0; ++kt; } }
+          }
         }
-        if (++kw == g.KW) { kw = 0; if (++kh == g.KH) { kh = 0; ++kt; } }
+      }
+    } else {
+      // ===================== copy-out (warps 1-3) =====================
+      const int ct = threadIdx.x - 32;           // 0..95
+      int i_tile = 0;
+      for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x, ++i_tile) {
+        const int m_tile = tile / g.n_tiles, n0 = (tile - m_tile * g.n_tiles) * BN;
+        // tile i - 1's phase 1, the last reader of buffer (i + 1) & 1, completed out_full before this thread's last wait
+        if (tile + (int)gridDim.x < g.tiles) stage_consts((tile + gridDim.x) % g.n_tiles, (i_tile + 1) & 1, ct, kCopyThreads);
+        // the copy warps sleep through the K loop instead of taking issue slots from the consumers
+        while (!mbar_try_wait(out_full, i_tile & 1)) __nanosleep(128);
+        if constexpr (!kBulkOut) {
+          // Phase 2, narrow rows: coalesced copy-out, consecutive threads write consecutive 16-byte chunks of an output
+          // row, kUnroll shared-memory loads in flight per thread
+          constexpr int cpr = BN / 8;  // 16-byte chunks per row
+          constexpr int kUnroll = 4;
+          for (int i0 = ct; i0 < kBM * cpr; i0 += kUnroll * kCopyThreads) {
+            uint4 val[kUnroll];
+#pragma unroll
+            for (int u = 0; u < kUnroll; ++u) {
+              const int i = i0 + u * kCopyThreads, rr = i / cpr, ch = i - rr * cpr;
+              if (i < kBM * cpr) val[u] = *reinterpret_cast<const uint4*>(stg + (size_t)rr * pitch + ch * 16);
+            }
+#pragma unroll
+            for (int u = 0; u < kUnroll; ++u) {
+              const int i = i0 + u * kCopyThreads, rr = i / cpr, ch = i - rr * cpr;
+              const int col = n0 + ch * 8;
+              if (i >= kBM * cpr || col >= g.Cout) continue;
+              const long long rp = tile_row_pixel(g, m_tile, rr);
+              if (rp < 0) continue;
+              __half* dst = y + (size_t)rp * g.out_ld + g.out_coff + col;
+              if (g.n_splits > 0 && col >= g.split[0]) {
+                const int d = (g.n_splits > 1 && col >= g.split[1]) ? 1 : 0;
+                dst = g.y_extra[d] + (size_t)rp * g.ld_extra[d] + g.coff_extra[d] + (col - g.split[d]);
+              }
+              *reinterpret_cast<uint4*>(dst) = val[u];
+            }
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(out_empty);
+          continue;
+        }
+        // Phase 2, wide rows: one bulk copy (TMA engine) per output row and destination: the row's columns
+        // [n0, min(n0 + BN, Cout)) cut at the split columns (multiples of 16, so every piece stays 16-byte aligned); box
+        // overhang rows are skipped.
+        const int end = min(n0 + BN, g.Cout);
+        for (int rr = ct; rr < kBM; rr += kCopyThreads) {
+          const long long rp = tile_row_pixel(g, m_tile, rr);
+          if (rp < 0) continue;
+          for (int col = n0; col < end;) {
+            __half* dst = y + (size_t)rp * g.out_ld + g.out_coff + col;
+            int next = end;
+            if (g.n_splits > 0) {
+              if (col >= g.split[0]) {
+                const int d = (g.n_splits > 1 && col >= g.split[1]) ? 1 : 0;
+                dst = g.y_extra[d] + (size_t)rp * g.ld_extra[d] + g.coff_extra[d] + (col - g.split[d]);
+                if (d == 0 && g.n_splits > 1) next = min(end, g.split[1]);
+              } else {
+                next = min(end, g.split[0]);
+              }
+            }
+            bulk_store(dst, stg + (size_t)rr * pitch + (col - n0) * 2, (uint32_t)(next - col) * 2);
+            col = next;
+          }
+        }
+        bulk_commit();
+        bulk_wait_read<0>();                     // the staging tile has been read
+        // staging reads and the next tile's constants are ordered before the arrival
+        __syncwarp();
+        if (lane == 0) mbar_arrive(out_empty);
       }
     }
   } else {
@@ -179,64 +282,59 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     const int ct = threadIdx.x - 128;            // 0..255
     const uint64_t hi = desc_hi_kmajor<BK>();
     const uint64_t a_lo0 = desc_lo(sA + wg * 64 * BK * 2), b_lo0 = desc_lo(sB);
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
-    int stage = 0, prev = -1; uint32_t phase = 0;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint64_t a_lo = a_lo0 + (uint64_t)(stage * (kABytes >> 4)), b_lo = b_lo0 + (uint64_t)(stage * (kBBytes >> 4));
-      wg_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k)          // 16 elements (32 bytes) along K inside the swizzle atom per step
-        wgmma_f16<BN>(acc, hi | (a_lo + 2 * k), hi | (b_lo + 2 * k), 1u);
-      wg_commit();
-      wg_wait<1>();                              // the previous k-block's MMAs have retired: free its stage
-      if (prev >= 0 && ct % 128 == 0) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == g.n_stages) { stage = 0; phase ^= 1; }
-    }
-    wg_wait<0>();
-    // both consumers are done reading the stage area: it becomes the output staging tile
-    named_sync(1, kConsumers);
-    // Phase 1: registers -> scale/shift (+residual) (+relu) -> fp16 -> staging row.
-    constexpr int pitch = staging_pitch(BN);
     const int wrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    float acc[BN / 2];
+    int stage = 0; uint32_t phase = 0;           // carried across tiles, as in the producer
+    int i_tile = 0;
+    for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x, ++i_tile) {
+      const int m_tile = tile / g.n_tiles, n0 = (tile - m_tile * g.n_tiles) * BN;
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int row = wrow + 8 * i;
-      const long long pix = residual ? tile_row_pixel(g, m_tile, row) : -1;
-      const __half* rrow = pix >= 0 ? residual + (size_t)pix * g.res_ld + g.res_coff + n0 : nullptr;
-      uint8_t* srow = smem + (size_t)row * pitch;
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t a_lo = a_lo0 + (uint64_t)(stage * (kABytes >> 4)), b_lo = b_lo0 + (uint64_t)(stage * (kBBytes >> 4));
+        wg_fence();
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = 8 * j + 2 * (lane & 3);
-        float f0 = fmaf(acc[4 * j + 2 * i], s_scale[col], s_shift[col]);
-        float f1 = fmaf(acc[4 * j + 2 * i + 1], s_scale[col + 1], s_shift[col + 1]);
-        if (rrow && n0 + col < g.Cout) {
-          const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(rrow + col));
-          f0 += rf.x; f1 += rf.y;
+        for (int k = 0; k < BK / 16; ++k)        // 16 elements (32 bytes) along K inside the swizzle atom per step
+          wgmma_f16<BN>(acc, hi | (a_lo + 2 * k), hi | (b_lo + 2 * k), 1u);
+        wg_commit();
+        wg_wait<1>();                            // the previous k-block's MMAs have retired: free its stage
+        if (prev >= 0 && ct % 128 == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == g.n_stages) { stage = 0; phase ^= 1; }
+      }
+      wg_wait<0>();
+      if (ct % 128 == 0) mbar_arrive(&empty_bar[prev]);  // the last stage too: the producer is filling the next tile
+      // the copy warps have read the previous tile out of the staging tile
+      mbar_wait(out_empty, (i_tile & 1) ^ 1);
+      // Phase 1: registers -> scale/shift (+residual) (+relu) -> fp16 -> staging row.
+      const float* s_scale = s_consts + (i_tile & 1) * 2 * kMaxBN;
+      const float* s_shift = s_scale + kMaxBN;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int row = wrow + 8 * i;
+        const long long pix = residual ? tile_row_pixel(g, m_tile, row) : -1;
+        const __half* rrow = pix >= 0 ? residual + (size_t)pix * g.res_ld + g.res_coff + n0 : nullptr;
+        uint8_t* srow = stg + (size_t)row * pitch;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = 8 * j + 2 * (lane & 3);
+          float f0 = fmaf(acc[4 * j + 2 * i], s_scale[col], s_shift[col]);
+          float f1 = fmaf(acc[4 * j + 2 * i + 1], s_scale[col + 1], s_shift[col + 1]);
+          if (rrow && n0 + col < g.Cout) {
+            const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(rrow + col));
+            f0 += rf.x; f1 += rf.y;
+          }
+          if (g.relu) { f0 = fmaxf(f0, 0.0f); f1 = fmaxf(f1, 0.0f); }
+          *reinterpret_cast<__half2*>(srow + col * 2) = __floats2half2_rn(f0, f1);
         }
-        if (g.relu) { f0 = fmaxf(f0, 0.0f); f1 = fmaxf(f1, 0.0f); }
-        *reinterpret_cast<__half2*>(srow + col * 2) = __floats2half2_rn(f0, f1);
       }
-    }
-    named_sync(1, kConsumers);
-    // Phase 2: coalesced copy-out: consecutive threads write consecutive 16-byte chunks of an output row.
-    constexpr int cpr = BN / 8;  // 16-byte chunks per row
-    for (int i = ct; i < kBM * cpr; i += kConsumers) {
-      const int rr = i / cpr, ch = i - rr * cpr;
-      const int col = n0 + ch * 8;
-      if (col >= g.Cout) continue;
-      const long long rp = tile_row_pixel(g, m_tile, rr);
-      if (rp < 0) continue;
-      const uint4 val = *reinterpret_cast<const uint4*>(smem + (size_t)rr * pitch + ch * 16);
-      __half* dst = y + (size_t)rp * g.out_ld + g.out_coff + col;
-      if (g.n_splits > 0 && col >= g.split[0]) {
-        const int d = (g.n_splits > 1 && col >= g.split[1]) ? 1 : 0;
-        dst = g.y_extra[d] + (size_t)rp * g.ld_extra[d] + g.coff_extra[d] + (col - g.split[d]);
-      }
-      *reinterpret_cast<uint4*>(dst) = val;
+      // hand the staging tile to the copy warps (Phase 2: bulk copies, which read it through the async proxy) and go on
+      // with the next tile's K loop
+      if constexpr (kBulkOut) fence_proxy_async();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(out_full);
     }
   }
 }
@@ -372,6 +470,23 @@ static int two_ctas_fit(int t, size_t smem, bool* two) {
   return 0;
 }
 
+// Streaming multiprocessors of the current device, asked once per device.
+static std::atomic<int> g_sm_count[64];
+
+static int sm_count(int* n) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) { cudaGetLastError(); return fail((int)e, "conv3d(f16): cudaGetDevice: %s", cudaGetErrorString(e)); }
+  int v = g_sm_count[dev & 63].load(std::memory_order_relaxed);
+  if (v == 0) {
+    e = cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail((int)e, "conv3d(f16): SM count: %s", cudaGetErrorString(e)); }
+    g_sm_count[dev & 63].store(v, std::memory_order_relaxed);
+  }
+  *n = v;
+  return 0;
+}
+
 struct ConvPlan {
   CUtensorMap map_a, map_b;
   ConvGeom g;
@@ -483,25 +598,34 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
     if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(f16): tensor map (B) encode failed: CUresult %d", (int)cr);
   }
   STEP_CHECK_ARG(m_tiles * g.n_tiles < (1LL << 31), "conv3d(f16): grid too large");
-  pl->grid = dim3((unsigned)(m_tiles * g.n_tiles));
-  // Pipeline depth: at least four stages within half of an SM's shared memory (<= 113 KB) when the occupancy calculator says
-  // two such CTAs really fit an SM (registers included), so that one CTA's epilogue overlaps the other's main loop; otherwise
-  // as deep as the 227 KB of one SM allow.
+  g.tiles = (int)(m_tiles * g.n_tiles);
+  // Pipeline depth: at least three stages and the output staging tile within half of an SM's shared memory (<= 113 KB) when
+  // the occupancy calculator says two such CTAs really fit an SM (registers included), so that one CTA's epilogue overlaps
+  // the other's main loop (BK 64 / BN 64, a thin 1x1x1 layer bound by memory, ran 45 % slower as one 8-stage CTA per SM);
+  // otherwise as deep as the 227 KB of one SM allow.
   const long per_stage = (long)kBM * BK * 2 + (long)g.BN * BK * 2;
-  const long fixed = kBookBytes + 1024;
-  const long out_tile = (long)kBM * staging_pitch(g.BN);
+  const long fixed = kBookBytes + 1024 + (long)kBM * staging_pitch(g.BN);
   int st = (int)((113L * 1024 - fixed) / per_stage);
   if (st > kStages) st = kStages;
   bool two = false;
-  if (st >= 4) {
-    const long area = st * per_stage;
-    if (int rc = two_ctas_fit(pl->tile, (size_t)(fixed + (area > out_tile ? area : out_tile)), &two)) return rc;
+  if (st >= 3) {
+    if (int rc = two_ctas_fit(pl->tile, (size_t)(fixed + st * per_stage), &two)) return rc;
   }
   if (!two) st = (int)((227L * 1024 - fixed) / per_stage);
   g.n_stages = st > kStages ? kStages : st;
   STEP_CHECK_ARG(g.n_stages >= 2, "conv3d(f16): tile does not fit shared memory");
-  const long stage_area = g.n_stages * per_stage;
-  pl->smem_bytes = (size_t)(fixed + (stage_area > out_tile ? stage_area : out_tile));
+  pl->smem_bytes = (size_t)(fixed + g.n_stages * per_stage);
+  // Persistent grid: as many CTAs as fit the device at once, each walking the tiles with a stride of the grid, in tile order
+  // (the N tiles of one M tile run on neighbouring CTAs and share A in L2).  A tile with a K loop of more than
+  // kPersistMaxKBlocks k-blocks already hides its fixed cost (prologue, pipeline fill, epilogue) behind its own MMAs, and the
+  // hardware's dispatch of one tile per CTA to whichever SM frees first balances unequal tile times better than a fixed
+  // stride: one CTA per tile there (Mixed 4e/4f/5b 3x3x3 at BK 32, 135 k-blocks, ran 6-12 % slower with the stride;
+  // layers of up to 81 k-blocks run faster with it).
+  int sms = 0;
+  if (int rc = sm_count(&sms)) return rc;
+  const long resident = (long)sms * (two ? 2 : 1);
+  const bool persist = g.taps * g.kblocks_per_tap <= kPersistMaxKBlocks && g.tiles > resident;
+  pl->grid = dim3((unsigned)(persist ? resident : g.tiles));
   return 0;
 }
 

@@ -56,6 +56,11 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
 }
+// bulk copy of `bytes` contiguous bytes shared -> global (both 16-byte aligned, bytes a multiple of 16)
+__device__ __forceinline__ void bulk_store(void* dst, const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+               ::"l"(dst), "r"(smem_u32(src)), "r"(bytes) : "memory");
+}
 // Four 8 x 8 fp16 matrices stored transposed: v[m] holds this thread's pair (row lane / 4, columns 2 (lane % 4) + {0, 1})
 // of matrix m; lanes 8 m .. 8 m + 7 give the addresses of its memory rows 0..7, and memory row c receives column c.
 __device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t* v) {

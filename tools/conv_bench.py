@@ -2,11 +2,15 @@
 max_iter = 3), through the same entry points the pipeline uses (CUDA events, 20 reps after 3 warm-ups).
 
     python tools/conv_bench.py [--check] [name ...]
+    python tools/conv_bench.py --ksweep
 
 For each layer: launches per step, the kernel that runs it, algorithmic and executed (zero-padded) GMAC per launch,
 the conv_umma tile (BK, BN, number of N tiles), time per launch and TFLOP/s on the algorithmic FLOPs.  The last line
 sums time x count over the step.  The tile columns mirror pick_bk / pick_tile in step_b200/csrc/conv_umma.cu and read
-the instantiated tiles from its STEP_CONV_TILES list.  A tool, not the benchmark (bench.py)."""
+the instantiated tiles from its STEP_CONV_TILES list.  A tool, not the benchmark (bench.py).
+
+--ksweep times a 1x1x1 conv at the head shape (M = 34,496, Cout = 256: BK 64 / BN 256, 270 tiles) for Cin = 256 ... 2048
+and fits the time of one wave of tiles against K: the intercept is the part of a tile's time outside the K loop."""
 import os
 import re
 import sys
@@ -93,7 +97,49 @@ def kernel_of(N, T, H, W, Cin, Cout, k):
     return "halo" if halo else "umma"
 
 
+def time_us(f, reps=20):
+    for _ in range(3):
+        f()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        f()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps * 1e3
+
+
+def ksweep():
+    N, T, H, W = HEAD
+    M, Cout = N * T * H * W, 256
+    tiles = -(-M // 128)
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    waves = -(-tiles // sms)
+    print("ksweep: 1x1x1 conv, M = %d, Cout = %d, %d tiles of 128 x 256 on %d SMs (%d waves)" % (M, Cout, tiles, sms, waves))
+    ks, per_wave = [], []
+    for Cin in (256, 512, 1024, 2048):
+        x = Act(torch.randn(N, T, H, W, Cin, device="cuda").half())
+        w = (torch.randn(Cout, 1, Cin, device="cuda") / Cin ** 0.5).half()
+        out = Act(torch.empty(N, T, H, W, Cout, device="cuda", dtype=torch.float16))
+        sc, sh = torch.ones(Cout, device="cuda"), torch.zeros(Cout, device="cuda")
+        us = time_us(lambda: E.conv(x, w, sc, sh, out, (1, 1, 1), (1, 1, 1), None, True, None), reps=50)
+        ks.append(Cin)
+        per_wave.append(us / waves)
+        print("K %5d  %8.1f us  %6.2f us per wave  %6.1f TFLOP/s" % (Cin, us, us / waves, 2.0 * M * Cin * Cout / us / 1e6))
+    n = len(ks)
+    mk, mt = sum(ks) / n, sum(per_wave) / n
+    slope = sum((k - mk) * (t - mt) for k, t in zip(ks, per_wave)) / sum((k - mk) ** 2 for k in ks)
+    icept = mt - slope * mk
+    t1024 = icept + slope * 1024
+    print("fit per wave: %.2f us + %.4f us per K (%.2f us per 64-channel block); intercept = %.0f %% of a K = 1024 tile"
+          % (icept, slope, slope * 64, 100.0 * icept / t1024))
+
+
 def main():
+    if "--ksweep" in sys.argv:
+        ksweep()
+        return
     args = [a for a in sys.argv[1:] if not a.startswith("--")]
     check = "--check" in sys.argv
     tiles = conv_tiles()
@@ -148,17 +194,7 @@ def main():
                 tile = (bk, bn, nt)
             else:
                 exec_gmac, tile = float("nan"), ("-", "-", "-")
-        for _ in range(3):
-            f()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        reps = 20
-        e0.record()
-        for _ in range(reps):
-            f()
-        e1.record()
-        torch.cuda.synchronize()
-        us = e0.elapsed_time(e1) / reps * 1e3
+        us = time_us(f)
         total_ms += us * count / 1e3
         line = "%-11s %3d %4s %9.2f %9.2f %3s %4s %3s %9.1f %8.1f" % (name, count, kern, gmac, exec_gmac, tile[0], tile[1],
                                                                      tile[2], us, 2 * gmac / us * 1e3)
