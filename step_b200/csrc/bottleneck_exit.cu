@@ -68,12 +68,12 @@ bottleneck_exit_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_c
   const int m0 = blockIdx.x * BM;
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_h) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w3) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w1) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-    if (g.store_y) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_y) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_z) : "memory");
+    prefetch_tensormap(&map_h);
+    prefetch_tensormap(&map_w3);
+    prefetch_tensormap(&map_w1);
+    prefetch_tensormap(&map_x);
+    if (g.store_y) prefetch_tensormap(&map_y);
+    prefetch_tensormap(&map_z);
     mbar_init(&bars->h_full, 1);
     for (int i = 0; i < kRing; ++i) {
       mbar_init(&bars->w3_full[i], 1); mbar_init(&bars->w3_empty[i], 2);
@@ -238,19 +238,6 @@ bottleneck_exit_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_c
   }
 }
 
-typedef CUresult (*EncFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                          const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncFn g_enc = nullptr;
-
-// [rows, cols] fp16, row pitch ld elements; box [box_r rows x 64 columns] = 128-byte rows, 128B swizzle
-static int enc2d(CUtensorMap* m, const void* base, int cols, long long rows, long long ld, int box_r, CUtensorMapL2promotion pr) {
-  cuuint64_t d[2] = {(cuuint64_t)cols, (cuuint64_t)rows}, st[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64u, (cuuint32_t)box_r}, es[2] = {1, 1};
-  CUresult r = g_enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), d, st, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, pr, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)r;
-}
-
 }  // namespace bexit
 }  // namespace step
 
@@ -268,45 +255,24 @@ extern "C" int step_bottleneck_exit_f16(const void* h, long long h_ld, const voi
   STEP_CHECK_ARG(h_ld % 8 == 0 && x_ld % 8 == 0 && z_ld % 8 == 0 && (!y || y_ld % 8 == 0), "bottleneck_exit: row pitches must keep 16-byte alignment");
   STEP_CHECK_ARG(((uintptr_t)h | (uintptr_t)w3 | (uintptr_t)w1 | (uintptr_t)y | (uintptr_t)x | (uintptr_t)z) % 16 == 0,
                  "bottleneck_exit: pointers must be 16-byte aligned");
-  if (!g_enc) {
-    cudaDriverEntryPointQueryResult q;
-    void* f = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || !f)
-      return fail(STEP_E_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
-    g_enc = (EncFn)f;
-  }
   CUtensorMap mh, mw3, mw1, mx, my, mz;
   memset(&my, 0, sizeof(my));
-  int r;
-  if ((r = enc2d(&mh, h, K1, M, h_ld, BM, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map h (%d)", r);
-  if ((r = enc2d(&mw3, w3, K1, N1, K1, CH, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map w3 (%d)", r);
-  if ((r = enc2d(&mw1, w1, N1, N2, N1, N2, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map w1 (%d)", r);
-  if ((r = enc2d(&mx, x, N1, M, x_ld, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map x (%d)", r);
-  if (y && (r = enc2d(&my, y, N1, M, y_ld, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map y (%d)", r);
-  if ((r = enc2d(&mz, z, N2, M, z_ld, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return fail(STEP_E_DRIVER, "bottleneck_exit: tensor map z (%d)", r);
+  // row matrices in boxes of 64 columns = 128-byte rows, 128B swizzle
+  const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B;
+  const CUtensorMapL2promotion act = CU_TENSOR_MAP_L2_PROMOTION_L2_128B, wgt = CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
+  int rc;
+  if ((rc = encode_rows2d(&mh, h, M, K1, h_ld, 64, BM, sw, act, "bottleneck_exit: h")) ||
+      (rc = encode_rows2d(&mw3, w3, N1, K1, K1, 64, CH, sw, wgt, "bottleneck_exit: w3")) ||
+      (rc = encode_rows2d(&mw1, w1, N2, N1, N1, 64, N2, sw, wgt, "bottleneck_exit: w1")) ||
+      (rc = encode_rows2d(&mx, x, M, N1, x_ld, 64, 64, sw, act, "bottleneck_exit: x")) ||
+      (y && (rc = encode_rows2d(&my, y, M, N1, y_ld, 64, 64, sw, act, "bottleneck_exit: y"))) ||
+      (rc = encode_rows2d(&mz, z, M, N2, z_ld, 64, 64, sw, act, "bottleneck_exit: z")))
+    return rc;
   Geom g;
   g.M = (int)M; g.store_y = y ? 1 : 0; g.relu2 = relu2 ? 1 : 0;
   const size_t smem = sizeof(Bars) + 1024 + kHBytes + kRing * (kW3Bytes + kW1Bytes + 2 * kXBytes);
   static std::atomic<unsigned long long> attr_seen{0};
-  if (first_use_on_device(attr_seen)) {
-    cudaError_t e = cudaFuncSetAttribute(bottleneck_exit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail((int)e, "bottleneck_exit: smem attribute: %s", cudaGetErrorString(e));
-  }
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  int na = 0;
-  if (pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr; cfg.numAttrs = na;
-  cfg.gridDim = dim3((unsigned)((M + BM - 1) / BM));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = cu(stream);
-  cudaError_t le = cudaLaunchKernelEx(&cfg, bottleneck_exit_kernel, mh, mw3, mw1, mx, my, mz, g, shift2);
-  if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "bottleneck_exit_kernel launch: %s", cudaGetErrorString(le)); }
-  STEP_LAUNCH_CHECK("bottleneck_exit_kernel");
-  return 0;
+  if ((rc = allow_dynamic_smem(bottleneck_exit_kernel, attr_seen, (int)smem, "bottleneck_exit_kernel"))) return rc;
+  return launch_tc("bottleneck_exit_kernel", bottleneck_exit_kernel, dim3((unsigned)((M + BM - 1) / BM)), kThreads, smem,
+                   cu(stream), mh, mw3, mw1, mx, my, mz, g, shift2);
 }

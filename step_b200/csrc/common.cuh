@@ -64,6 +64,15 @@ inline bool first_use_on_device(std::atomic<unsigned long long>& seen) {
   return (seen.fetch_or(bit, std::memory_order_relaxed) & bit) == 0;
 }
 
+// Raise `kernel`'s dynamic shared-memory limit to `bytes`, once per device (`seen` as above).
+template <typename Kernel>
+inline int allow_dynamic_smem(Kernel kernel, std::atomic<unsigned long long>& seen, int bytes, const char* label) {
+  if (!first_use_on_device(seen)) return 0;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return fail((int)e, "%s: shared memory attribute: %s", label, cudaGetErrorString(e));
+  return 0;
+}
+
 // ---- device helpers -----------------------------------------------------------------------
 template <typename T>
 struct Vec16;  // 16-byte vector of T

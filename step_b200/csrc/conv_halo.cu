@@ -60,8 +60,8 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   const int n = b / g.tiles_t;
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
+    prefetch_tensormap(&map_a);
+    prefetch_tensormap(&map_b);
     for (int s = 0; s < g.n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     mbar_init(pfull_bar, 1);
     fence_barrier_init();
@@ -149,11 +149,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 }
 
 // ---- host -------------------------------------------------------------------------------------
-typedef CUresult (*HaloEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                      const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static HaloEncodeTiledFn g_halo_encode = nullptr;
-
 // Does this problem fit the kernel?  (stride 1 is checked by the caller)
 bool conv3d_halo_supported(const step_conv_params* p) {
   const int taps = p->KT * p->KH * p->KW;
@@ -166,22 +161,9 @@ template <int BK, int NCH, int TT>
 static int launch_halo_tt(const CUtensorMap& ma, const CUtensorMap& mb, const HaloGeom& g, size_t smem, unsigned grid,
                           const step_conv_params* p, const float* scale, const float* shift, __half* y, cudaStream_t s) {
   static std::atomic<unsigned long long> attr_seen{0};
-  if (first_use_on_device(attr_seen)) {
-    cudaError_t e = cudaFuncSetAttribute(conv_halo_kernel<BK, NCH, TT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHaloSmemMax);
-    if (e != cudaSuccess) return fail((int)e, "conv_halo_kernel attribute: %s", cudaGetErrorString(e));
-  }
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kHaloThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  if (pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-  }
-  cudaError_t le = cudaLaunchKernelEx(&cfg, conv_halo_kernel<BK, NCH, TT>, ma, mb, g, scale, shift, y);
-  if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "conv_halo_kernel launch: %s", cudaGetErrorString(le)); }
-  STEP_LAUNCH_CHECK("conv_halo_kernel");
-  return 0;
+  if (int rc = allow_dynamic_smem(conv_halo_kernel<BK, NCH, TT>, attr_seen, kHaloSmemMax, "conv_halo_kernel")) return rc;
+  return launch_tc("conv_halo_kernel", conv_halo_kernel<BK, NCH, TT>, dim3(grid), kHaloThreads, smem, s, ma, mb, g, scale,
+                   shift, y);
 }
 
 template <int BK>
@@ -234,31 +216,17 @@ static int halo_launch_cols(const step_conv_params* p, int c0, int cout, step_st
   g.tiles_w = (p->OW + kHaloTW - 1) / kHaloTW; g.tiles_h = (p->OH + kHaloTH - 1) / kHaloTH; g.tiles_t = (p->OT + TT - 1) / TT;
   const long long ctas = (long long)p->N * g.tiles_t * g.tiles_h * g.tiles_w;
   STEP_CHECK_ARG(ctas < (1LL << 31), "conv3d(halo): grid too large");
-  const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
-  CUtensorMap ma, mb;
-  {
-    cuuint64_t dims[5] = {(cuuint64_t)p->Cin, (cuuint64_t)p->W, (cuuint64_t)p->H, (cuuint64_t)p->T, (cuuint64_t)p->N};
-    cuuint64_t strides[4] = {(cuuint64_t)p->in_ld * 2, (cuuint64_t)p->W * p->in_ld * 2, (cuuint64_t)p->H * p->W * p->in_ld * 2,
-                             (cuuint64_t)p->T * p->H * p->W * p->in_ld * 2};
-    cuuint32_t box[5] = {8, (cuuint32_t)g.hp_w, (cuuint32_t)g.hp_h, (cuuint32_t)g.hp_t, 1};
-    CUresult cr = g_halo_encode(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, (void*)p->x, dims, strides, box, ones,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(halo): tensor map (patch) encode failed: CUresult %d", (int)cr);
-  }
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)p->Cin, (cuuint64_t)g.taps, (cuuint64_t)cout};
-    cuuint64_t strides[2] = {(cuuint64_t)p->w_ld * 2, (cuuint64_t)g.taps * p->w_ld * 2};
-    cuuint32_t box[3] = {(cuuint32_t)BK, 1, (cuuint32_t)BN};
-    const __half* w = (const __half*)p->w + (size_t)c0 * g.taps * p->w_ld;
-    CUresult cr = g_halo_encode(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)w, dims, strides, box, ones,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B),
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(halo): tensor map (weights) encode failed: CUresult %d", (int)cr);
-  }
   const size_t smem = kHaloBook + 1024 + (size_t)g.n_stages * g.b_bytes + (size_t)g.patch_bytes;
   STEP_CHECK_ARG(smem <= (size_t)kHaloSmemMax, "conv3d(halo): %zu bytes of shared memory", smem);
+  CUtensorMap ma, mb;
+  const cuuint32_t box[5] = {8, (cuuint32_t)g.hp_w, (cuuint32_t)g.hp_h, (cuuint32_t)g.hp_t, 1};
+  if (int rc = encode_act5d(&ma, p->x, ActLayout(p->N, p->T, p->H, p->W, p->Cin, p->in_ld), box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "conv3d(halo): patch"))
+    return rc;
+  const __half* w = (const __half*)p->w + (size_t)c0 * g.taps * p->w_ld;
+  if (int rc = encode_weights3d(&mb, w, cout, g.taps, p->Cin, p->w_ld, BK, BN, swizzle_for(BK),
+                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "conv3d(halo): weights"))
+    return rc;
   step_conv_params q = *p;
   q.scale = p->scale ? p->scale + c0 : nullptr;
   q.shift = p->shift ? p->shift + c0 : nullptr;
@@ -271,13 +239,6 @@ int conv3d_halo_launch(const step_conv_params* p, step_stream_t stream) {
   STEP_CHECK_ARG(conv3d_halo_supported(p) && p->ST == 1 && p->SH == 1 && p->SW == 1, "conv3d(halo): unsupported problem");
   STEP_CHECK_ARG((((uintptr_t)p->x | (uintptr_t)p->w | (uintptr_t)p->y) & 15) == 0 && p->w_ld % 8 == 0 && p->w_ld >= p->Cin &&
                  p->out_ld % 8 == 0 && p->out_coff % 8 == 0, "conv3d(halo): alignment");
-  if (!g_halo_encode) {
-    cudaDriverEntryPointQueryResult q;
-    void* f = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || !f)
-      return fail(STEP_E_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
-    g_halo_encode = (HaloEncodeTiledFn)f;
-  }
   // more than 128 output channels: launches of 128-column tiles (registers hold at most 64 accumulators per thread)
   for (int c0 = 0; c0 < p->Cout; c0 += 128) {
     const int cout = p->Cout - c0 < 128 ? p->Cout - c0 : 128;

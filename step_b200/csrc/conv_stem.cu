@@ -103,8 +103,8 @@ conv_stem_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   const int n = b / g.tiles_t;
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
+    prefetch_tensormap(&map_x);
+    prefetch_tensormap(&map_w);
     for (int s = 0; s < kStemStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     mbar_init(pfull_bar, 1);
     fence_barrier_init();
@@ -192,11 +192,6 @@ conv_stem_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
 }
 
 // ---- host -------------------------------------------------------------------------------------
-typedef CUresult (*StemEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                      const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static StemEncodeTiledFn g_stem_encode = nullptr;
-
 // The s2d stem: 24 input channels, 64 output channels, 4x4x4 taps, pad 1, stride 1, and the zero weights of the last t tap
 // plane's channels >= 16 that the kernel does not multiply.
 bool conv3d_stem_supported(const step_conv_params* p) {
@@ -209,13 +204,6 @@ int conv3d_stem_launch(const step_conv_params* p, step_stream_t stream) {
   STEP_CHECK_ARG(conv3d_stem_supported(p), "conv3d(stem): unsupported problem");
   STEP_CHECK_ARG((((uintptr_t)p->x | (uintptr_t)p->w | (uintptr_t)p->y) & 15) == 0 && p->in_ld % 8 == 0 && p->in_ld >= 24 &&
                  p->w_ld % 8 == 0 && p->w_ld >= 24 && p->out_ld % 8 == 0 && p->out_coff % 8 == 0, "conv3d(stem): alignment");
-  if (!g_stem_encode) {
-    cudaDriverEntryPointQueryResult q;
-    void* f = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || !f)
-      return fail(STEP_E_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
-    g_stem_encode = (StemEncodeTiledFn)f;
-  }
   StemGeom g;
   memset(&g, 0, sizeof(g));
   g.OT = p->OT; g.OH = p->OH; g.OW = p->OW;
@@ -224,45 +212,20 @@ int conv3d_stem_launch(const step_conv_params* p, step_stream_t stream) {
   g.tiles_t = (p->OT + kStemTT - 1) / kStemTT;
   const long long ctas = (long long)p->N * g.tiles_t * g.tiles_h * g.tiles_w;
   STEP_CHECK_ARG(ctas < (1LL << 31), "conv3d(stem): grid too large");
-  const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
   CUtensorMap mx, mw;
-  {
-    // channels 24.. of the buffer lie outside the map: never read
-    cuuint64_t dims[5] = {24, (cuuint64_t)p->W, (cuuint64_t)p->H, (cuuint64_t)p->T, (cuuint64_t)p->N};
-    cuuint64_t strides[4] = {(cuuint64_t)p->in_ld * 2, (cuuint64_t)p->W * p->in_ld * 2, (cuuint64_t)p->H * p->W * p->in_ld * 2,
-                             (cuuint64_t)p->T * p->H * p->W * p->in_ld * 2};
-    cuuint32_t box[5] = {8, (cuuint32_t)kStemHpW, (cuuint32_t)kStemHpH, (cuuint32_t)kStemHpT, 1};
-    CUresult cr = g_stem_encode(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, (void*)p->x, dims, strides, box, ones,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(stem): tensor map (patch) encode failed: CUresult %d", (int)cr);
-  }
-  {
-    cuuint64_t dims[3] = {24, 64, 64};                  // channels, taps, output channels
-    cuuint64_t strides[2] = {(cuuint64_t)p->w_ld * 2, (cuuint64_t)64 * p->w_ld * 2};
-    cuuint32_t box[3] = {8, 1, 64};
-    CUresult cr = g_stem_encode(&mw, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)p->w, dims, strides, box, ones,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(stem): tensor map (weights) encode failed: CUresult %d", (int)cr);
-  }
+  // channels 24.. of the buffer lie outside the map: never read
+  const cuuint32_t box[5] = {8, (cuuint32_t)kStemHpW, (cuuint32_t)kStemHpH, (cuuint32_t)kStemHpT, 1};
+  if (int rc = encode_act5d(&mx, p->x, ActLayout(p->N, p->T, p->H, p->W, 24, p->in_ld), box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "conv3d(stem): patch"))
+    return rc;
+  // 64 output channels, 64 taps, 24 channels; boxes of one 8-channel group of one tap
+  if (int rc = encode_weights3d(&mw, p->w, 64, 64, 24, p->w_ld, 8, 64, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "conv3d(stem): weights"))
+    return rc;
   static std::atomic<unsigned long long> attr_seen{0};
-  if (first_use_on_device(attr_seen)) {
-    cudaError_t e = cudaFuncSetAttribute(conv_stem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStemSmem);
-    if (e != cudaSuccess) return fail((int)e, "conv_stem_kernel attribute: %s", cudaGetErrorString(e));
-  }
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  cfg.gridDim = dim3((unsigned)ctas); cfg.blockDim = dim3(kStemThreads); cfg.dynamicSmemBytes = kStemSmem; cfg.stream = cu(stream);
-  if (pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-  }
-  cudaError_t le = cudaLaunchKernelEx(&cfg, conv_stem_kernel, mx, mw, g, p->scale, p->shift, (__half*)p->y);
-  if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "conv_stem_kernel launch: %s", cudaGetErrorString(le)); }
-  STEP_LAUNCH_CHECK("conv_stem_kernel");
-  return 0;
+  if (int rc = allow_dynamic_smem(conv_stem_kernel, attr_seen, kStemSmem, "conv_stem_kernel")) return rc;
+  return launch_tc("conv_stem_kernel", conv_stem_kernel, dim3((unsigned)ctas), kStemThreads, kStemSmem, cu(stream), mx, mw, g,
+                   p->scale, p->shift, (__half*)p->y);
 }
 
 }  // namespace step

@@ -134,8 +134,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   const int num_kb = g.taps * g.kblocks_per_tap;
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
+    prefetch_tensormap(&map_a);
+    prefetch_tensormap(&map_b);
     for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     mbar_init(out_full, kConsumers / 32);
     mbar_init(out_empty, kCopyThreads / 32);
@@ -376,34 +376,6 @@ __global__ void __launch_bounds__(32) tma_dump_kernel(const __grid_constant__ CU
 }
 
 // ---- host side --------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                   const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn g_encode_tiled = nullptr;
-static EncodeIm2colFn g_encode_im2col = nullptr;
-
-static int load_driver_entry_points() {
-  if (g_encode_tiled && g_encode_im2col) return 0;
-  cudaDriverEntryPointQueryResult q;
-  void* f = nullptr;
-  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q);
-  if (e != cudaSuccess || !f) return fail(STEP_E_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
-  g_encode_tiled = (EncodeTiledFn)f;
-  f = nullptr;
-  e = cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &f, cudaEnableDefault, &q);
-  if (e != cudaSuccess || !f) return fail(STEP_E_DRIVER, "cuTensorMapEncodeIm2col entry point unavailable");
-  g_encode_im2col = (EncodeIm2colFn)f;
-  return 0;
-}
-
-static CUtensorMapSwizzle swizzle_for(int BK) {
-  return BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-}
-
 // Channel block width.  A tap's last block is zero-filled past Cin and its zero 16-channel steps are multiplied, not skipped
 // (a data-dependent guard around the wgmma issue makes ptxas serialise the whole sequence), so the width is the one with
 // the least padded K, the wider one on a tie: Cin = 96, 144, 160, 480, 528 -> blocks of 32 (no or less padding), 112 or
@@ -497,7 +469,6 @@ struct ConvPlan {
 };
 
 static int build_plan(const step_conv_params* p, ConvPlan* pl) {
-  if (int rc = load_driver_entry_points()) return rc;
   STEP_CHECK_ARG(p->ST == 1 && p->SH == 1 && p->SW == 1, "conv3d(f16): stride must be 1 (use the s2d stem)");
   STEP_CHECK_ARG(p->Cin % 8 == 0 && p->in_ld % 8 == 0 && p->w_ld % 8 == 0 && p->w_ld >= p->Cin,
                  "conv3d(f16): Cin=%d in_ld=%d w_ld=%d must be multiples of 8", p->Cin, p->in_ld, p->w_ld);
@@ -539,29 +510,20 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   g.OT = p->OT; g.OH = p->OH; g.OW = p->OW; g.Nimg = p->N;
   g.M = (long long)p->N * p->OT * p->OH * p->OW;
   long long m_tiles;
-  const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
-  CUresult cr;
+  int rc;
   if (mode == A_LINEAR) {
     STEP_CHECK_ARG(g.M < (1LL << 31), "conv3d(f16): M too large");
-    cuuint64_t dims[2] = {(cuuint64_t)p->Cin, (cuuint64_t)g.M};
-    cuuint64_t strides[1] = {(cuuint64_t)p->in_ld * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)kBM};
-    cr = g_encode_tiled(&pl->map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)p->x, dims, strides, box, ones,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(BK), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    rc = encode_rows2d(&pl->map_a, p->x, g.M, p->Cin, p->in_ld, BK, kBM, swizzle_for(BK), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                       "conv3d(f16): A (linear)");
     m_tiles = (g.M + kBM - 1) / kBM;
     g.a_bytes = kBM * BK * 2;
   } else {
-    cuuint64_t dims[5] = {(cuuint64_t)p->Cin, (cuuint64_t)p->W, (cuuint64_t)p->H, (cuuint64_t)p->T, (cuuint64_t)p->N};
-    cuuint64_t strides[4] = {(cuuint64_t)p->in_ld * 2, (cuuint64_t)p->W * p->in_ld * 2,
-                             (cuuint64_t)p->H * p->W * p->in_ld * 2, (cuuint64_t)p->T * p->H * p->W * p->in_ld * 2};
+    const ActLayout act(p->N, p->T, p->H, p->W, p->Cin, p->in_ld);
     if (mode == A_BOX) {
       pick_box(p->OW, p->OH, p->OT, &g.bw, &g.bh, &g.bt);
       g.tiles_w = (p->OW + g.bw - 1) / g.bw; g.tiles_h = (p->OH + g.bh - 1) / g.bh; g.tiles_t = (p->OT + g.bt - 1) / g.bt;
-      cuuint32_t box[5] = {(cuuint32_t)BK, (cuuint32_t)g.bw, (cuuint32_t)g.bh, (cuuint32_t)g.bt, 1};
-      cr = g_encode_tiled(&pl->map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, (void*)p->x, dims, strides, box, ones,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(BK), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      const cuuint32_t box[5] = {(cuuint32_t)BK, (cuuint32_t)g.bw, (cuuint32_t)g.bh, (cuuint32_t)g.bt, 1};
+      rc = encode_act5d(&pl->map_a, p->x, act, box, swizzle_for(BK), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "conv3d(f16): A (box)");
       m_tiles = (long long)p->N * g.tiles_t * g.tiles_h * g.tiles_w;
       g.a_bytes = g.bw * g.bh * g.bt * BK * 2;
     } else {
@@ -573,30 +535,23 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
       int upper[3] = {ph_w - (p->KW - 1), ph_h - (p->KH - 1), ph_t - (p->KT - 1)};
       for (int i = 0; i < 3; ++i)
         STEP_CHECK_ARG(lower[i] >= -16 && lower[i] <= 15 && upper[i] >= -16 && upper[i] <= 15, "conv3d(f16): im2col corner range");
-      cr = g_encode_im2col(&pl->map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, (void*)p->x, dims, strides, lower, upper,
-                           (cuuint32_t)BK, (cuuint32_t)kBM, ones, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(BK),
-                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      rc = encode_act5d_im2col(&pl->map_a, p->x, act, lower, upper, BK, kBM, swizzle_for(BK),
+                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "conv3d(f16): A (im2col)");
       // Same work-around CUTLASS applies (cute/atom/copy_traits_sm90_im2col.hpp): drivers <= 13.1 set a
       // descriptor bit that breaks im2col loads from tensors smaller than 128 KiB.
       int drv = 0;
       cudaDriverGetVersion(&drv);
-      if (cr == CUDA_SUCCESS && drv <= 13010 &&
+      if (rc == 0 && drv <= 13010 &&
           (size_t)p->N * p->T * p->H * p->W * p->in_ld * 2 < 131072)
         reinterpret_cast<uint64_t*>(&pl->map_a)[1] &= ~(1ULL << 21);
       m_tiles = (g.M + kBM - 1) / kBM;
       g.a_bytes = kBM * BK * 2;
     }
   }
-  if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(f16): tensor map (A, mode %d) encode failed: CUresult %d", mode, (int)cr);
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)p->Cin, (cuuint64_t)taps, (cuuint64_t)p->Cout};
-    cuuint64_t strides[2] = {(cuuint64_t)p->w_ld * 2, (cuuint64_t)taps * p->w_ld * 2};
-    cuuint32_t box[3] = {(cuuint32_t)BK, 1, (cuuint32_t)g.BN};
-    cr = g_encode_tiled(&pl->map_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)p->w, dims, strides, box, ones,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(BK), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "conv3d(f16): tensor map (B) encode failed: CUresult %d", (int)cr);
-  }
+  if (rc) return rc;
+  if ((rc = encode_weights3d(&pl->map_b, p->w, p->Cout, taps, p->Cin, p->w_ld, BK, g.BN, swizzle_for(BK),
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "conv3d(f16): B")))
+    return rc;
   STEP_CHECK_ARG(m_tiles * g.n_tiles < (1LL << 31), "conv3d(f16): grid too large");
   g.tiles = (int)(m_tiles * g.n_tiles);
   // Pipeline depth: at least three stages and the output staging tile within half of an SM's shared memory (<= 113 KB) when
@@ -633,24 +588,9 @@ int conv3d_umma_launch(const step_conv_params* p, step_stream_t stream) {
   ConvPlan pl;
   if (int rc = build_plan(p, &pl)) return rc;
   const ConvTile& t = kTiles[pl.tile];
-  if (first_use_on_device(g_attr_seen[pl.tile])) {
-    cudaError_t e = cudaFuncSetAttribute(t.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return fail((int)e, "conv3d(f16): smem attribute: %s", cudaGetErrorString(e));
-  }
-  cudaStream_t s = cu(stream);
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  cfg.gridDim = pl.grid; cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = pl.smem_bytes; cfg.stream = s;
-  if (pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-  }
-  cudaError_t le = cudaLaunchKernelEx(&cfg, t.kernel, pl.map_a, pl.map_b, pl.g, p->scale, p->shift,
-                                      (const __half*)p->residual, (__half*)p->y);
-  if (le != cudaSuccess) { cudaGetLastError(); return fail((int)le, "conv_umma_kernel launch: %s", cudaGetErrorString(le)); }
-  STEP_LAUNCH_CHECK("conv_umma_kernel");
-  return 0;
+  if (int rc = allow_dynamic_smem(t.kernel, g_attr_seen[pl.tile], 227 * 1024, "conv_umma_kernel")) return rc;
+  return launch_tc("conv_umma_kernel", t.kernel, pl.grid, kThreads, pl.smem_bytes, cu(stream), pl.map_a, pl.map_b, pl.g,
+                   p->scale, p->shift, (const __half*)p->residual, (__half*)p->y);
 }
 
 }  // namespace step

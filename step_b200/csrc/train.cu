@@ -805,17 +805,11 @@ extern "C" int step_roi_pool_bwd_slice_nhwc(const void* grad_out, int dtype, int
   const dim3 grid((K / feat_T) * roi_T, ceil_div(C, chunk));
   static std::atomic<unsigned long long> seen32{0}, seen16{0};
   if (dtype == STEP_F32) {
-    if (first_use_on_device(seen32)) {
-      cudaError_t e = cudaFuncSetAttribute(roi_pool_bwd_slice_nhwc_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPoolBwdSmem);
-      if (e != cudaSuccess) return fail((int)e, "roi_pool_bwd_slice_nhwc: shared memory attribute: %s", cudaGetErrorString(e));
-    }
+    if (int rc = allow_dynamic_smem(roi_pool_bwd_slice_nhwc_kernel<float>, seen32, kPoolBwdSmem, "roi_pool_bwd_slice_nhwc")) return rc;
     roi_pool_bwd_slice_nhwc_kernel<float><<<grid, chunk, smem, cu(stream)>>>((const float*)grad_out, out_ld, argmax, rois, R, ph * pw,
                                                                              (int)npix, C, roi_T, feat_T, t_start, grad_in, in_ld);
   } else {
-    if (first_use_on_device(seen16)) {
-      cudaError_t e = cudaFuncSetAttribute(roi_pool_bwd_slice_nhwc_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPoolBwdSmem);
-      if (e != cudaSuccess) return fail((int)e, "roi_pool_bwd_slice_nhwc: shared memory attribute: %s", cudaGetErrorString(e));
-    }
+    if (int rc = allow_dynamic_smem(roi_pool_bwd_slice_nhwc_kernel<__half>, seen16, kPoolBwdSmem, "roi_pool_bwd_slice_nhwc")) return rc;
     roi_pool_bwd_slice_nhwc_kernel<__half><<<grid, chunk, smem, cu(stream)>>>((const __half*)grad_out, out_ld, argmax, rois, R, ph * pw,
                                                                               (int)npix, C, roi_T, feat_T, t_start, grad_in, in_ld);
   }

@@ -1,14 +1,23 @@
 // umma_ptx.cuh -- thin PTX wrappers shared by the tensor-core kernels (mbarrier, TMA loads / stores, wgmma descriptors and
-// instructions).  sm_90a only.
+// instructions), and their host side: tensor maps of the project's fp16 layouts and the launch.  sm_90a only.
 #pragma once
 #include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
+
+#include <utility>
+
+#include "common.cuh"
 
 namespace step {
 
 // ---- PTX wrappers ---------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+__device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -247,5 +256,111 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// ---- host side ------------------------------------------------------------------------------
+// The driver's tensor-map encoders, looked up once per process.  Function-local statics are initialised once even when
+// several threads launch at the same time (nn.DataParallel replicas); a failed lookup stays null.
+template <typename Fn>
+inline Fn driver_entry_point(const char* symbol) {
+  void* f = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  if (cudaGetDriverEntryPointByVersion(symbol, &f, 12000, cudaEnableDefault, &q) != cudaSuccess) f = nullptr;
+  return (Fn)f;
+}
+inline PFN_cuTensorMapEncodeTiled_v12000 encode_tiled_fn() {
+  static const auto fn = driver_entry_point<PFN_cuTensorMapEncodeTiled_v12000>("cuTensorMapEncodeTiled");
+  return fn;
+}
+inline PFN_cuTensorMapEncodeIm2col_v12000 encode_im2col_fn() {
+  static const auto fn = driver_entry_point<PFN_cuTensorMapEncodeIm2col_v12000>("cuTensorMapEncodeIm2col");
+  return fn;
+}
+
+// TMA swizzle of a K-major tile with rows of BK fp16: the one desc_hi_kmajor<BK> describes to wgmma
+inline CUtensorMapSwizzle swizzle_for(int BK) {
+  return BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+}
+
+// Every map below is fp16, element strides 1, no interleave, and loads zero-fill outside the tensor (OOB_FILL_NONE).
+// Failures return STEP_E_DRIVER with `label` and the CUresult in the error text.
+constexpr cuuint32_t kTmaOnes[5] = {1, 1, 1, 1, 1};
+
+inline int encode_result(CUresult cr, const char* label) {
+  if (cr != CUDA_SUCCESS) return fail(STEP_E_DRIVER, "%s: tensor map encode failed: CUresult %d", label, (int)cr);
+  return 0;
+}
+
+inline int encode_tiled_f16(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                            const cuuint32_t* box, CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2,
+                            const char* label) {
+  const PFN_cuTensorMapEncodeTiled_v12000 enc = encode_tiled_fn();
+  if (!enc) return fail(STEP_E_DRIVER, "cuTensorMapEncodeTiled entry point unavailable");
+  return encode_result(enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides,
+                           box, kTmaOnes, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE),
+                       label);
+}
+
+// fp16 channels-last activation [N, T, H, W, ld], C live channels per pixel: the 5-D map {C, W, H, T, N}
+struct ActLayout {
+  cuuint64_t dims[5], strides[4];
+  ActLayout(int N, int T, int H, int W, int C, int ld)
+      : dims{(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)N},
+        strides{(cuuint64_t)ld * 2, (cuuint64_t)W * ld * 2, (cuuint64_t)H * W * ld * 2, (cuuint64_t)T * H * W * ld * 2} {}
+};
+
+inline int encode_act5d(CUtensorMap* map, const void* x, const ActLayout& a, const cuuint32_t (&box)[5],
+                        CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2, const char* label) {
+  return encode_tiled_f16(map, x, 5, a.dims, a.strides, box, swizzle, l2, label);
+}
+
+// The same activation in TMA im2col mode: `channels` x `pixels` boxes walking the output pixels inside the bounding box
+// [lower, upper] (w, h, t) of the padded input.
+inline int encode_act5d_im2col(CUtensorMap* map, const void* x, const ActLayout& a, const int (&lower)[3],
+                               const int (&upper)[3], int channels, int pixels, CUtensorMapSwizzle swizzle,
+                               CUtensorMapL2promotion l2, const char* label) {
+  const PFN_cuTensorMapEncodeIm2col_v12000 enc = encode_im2col_fn();
+  if (!enc) return fail(STEP_E_DRIVER, "cuTensorMapEncodeIm2col entry point unavailable");
+  return encode_result(enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(x), a.dims, a.strides, lower, upper,
+                           (cuuint32_t)channels, (cuuint32_t)pixels, kTmaOnes, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE),
+                       label);
+}
+
+// packed weights [Cout, taps, w_ld], Cin live channels per tap: the 3-D map {Cin, taps, Cout}, boxes of box_c channels
+// of one tap for box_n output channels
+inline int encode_weights3d(CUtensorMap* map, const void* w, int Cout, int taps, int Cin, int w_ld, int box_c, int box_n,
+                            CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2, const char* label) {
+  const cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)taps, (cuuint64_t)Cout};
+  const cuuint64_t strides[2] = {(cuuint64_t)w_ld * 2, (cuuint64_t)taps * w_ld * 2};
+  const cuuint32_t box[3] = {(cuuint32_t)box_c, 1, (cuuint32_t)box_n};
+  return encode_tiled_f16(map, w, 3, dims, strides, box, swizzle, l2, label);
+}
+
+// row matrix [rows, cols] with a pitch of ld elements: the 2-D map {cols, rows}, boxes of box_c columns x box_r rows
+inline int encode_rows2d(CUtensorMap* map, const void* base, long long rows, int cols, long long ld, int box_c, int box_r,
+                         CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2, const char* label) {
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  const cuuint32_t box[2] = {(cuuint32_t)box_c, (cuuint32_t)box_r};
+  return encode_tiled_f16(map, base, 2, dims, strides, box, swizzle, l2, label);
+}
+
+// Launch of a TMA + wgmma kernel: programmatic dependent launch when pdl_enabled() (the kernels order their reads of the
+// previous kernel's output behind pdl_wait()), launch errors reported naming the kernel, and the launch counted.
+template <typename... Params, typename... Args>
+inline int launch_tc(const char* name, void (*kernel)(Params...), dim3 grid, int threads, size_t smem, cudaStream_t stream,
+                     Args&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  if (pdl_enabled()) {
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+  }
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+  if (e != cudaSuccess) { cudaGetLastError(); return fail((int)e, "%s launch: %s", name, cudaGetErrorString(e)); }
+  STEP_LAUNCH_CHECK(name);
+  return 0;
+}
 
 }  // namespace step
