@@ -7,10 +7,14 @@ Convolutions go through torch.nn.grad in float64 on the zero-padded input (the S
 asymmetric, so it is applied with F.pad); pools through autograd of F.pad + F.max_pool3d(ceil_mode=True) in float64 on the
 CPU.  Never fp32 on the GPU: cuDNN convolutions default to TF32 there.
 
-The second half holds the float64 references of the inference forward's launches (conv_fwd, exit_fwd, mean_mid, linear,
+The second part holds the float64 references of the inference forward's launches (conv_fwd, exit_fwd, mean_mid, linear,
 head_regress, roi_align; pool_entry's `y` for the pools), fed what the kernel read, with the magnitude terms their error
 bounds are built from (tests/test_gpu_forward_layers.py derives the bounds), and check_fwd, the elementwise + bias check
 of one fp16 convolution output.
+
+The third part holds the references of train_step's launches outside the tape (tests/test_gpu_train_launches.py):
+roi_align_bwd (the transpose of the ROIAlign matrix roi_align uses, built once by roi_align_terms / roi_align_matrix),
+linear_bwd, head_losses and cls_loss, each with its bound derived in its docstring and a checker that applies it.
 """
 import math
 
@@ -355,29 +359,47 @@ def head_regress(feat, local_reg, neighbor_reg1, neighbor_reg2, Tc, T, wdtype=to
 
 
 ROI_MERGED = 16                  # most distinct pixels one bin of the packed ROIAlign merges (csrc/roi.cu kMaxMerged)
+ROI_CHUNK = 64                   # ROIs per batched matrix product of the ROIAlign references
 
 
-def roi_align(feat, rois, scale, ph, pw, roi_T=0, feat_T=0, t_start=0):
-    """Float64 ROIAlign (legacy sampling, sampling_ratio 0: adaptive grid ceil(roi / pooled), samples outside [-1, H]
-    dropped, 4-tap bilinear, mean over the grid) of channels-last frames feat [K, H, W, C], on the CPU.  Sample coordinates
-    and tap weights are formed in fp32 in the kernel's operation order (csrc/roi.cu roi_geometry / sample_coord /
-    make_tap, oracle/step_oracle.c), the weighted sums in float64.  rois [R, 5] (frame, x1, y1, x2, y2); with roi_T > 0 the
-    frame index f maps to (f // roi_T) * feat_T + t_start + f % roi_T.  Returns (out, out of |feat|) as [R, ph, pw, C]."""
+def roi_frames(rois, roi_T=0, feat_T=0, t_start=0):
+    """Feature frame of every ROI row: int(frame) (truncation, as the kernels' (int) cast), mapped to
+    (f // roi_T) * feat_T + t_start + f % roi_T when roi_T > 0 (ROINet.pool_into's frame map).  int64 [R]."""
+    b = rois[:, 0].to(torch.float32).trunc().to(torch.int64)
+    return (b // roi_T) * feat_T + t_start + b % roi_T if roi_T > 0 else b
+
+
+def roi_align_terms(rois, scale, ph, pw, H, W, sampling_ratio=0):
+    """Every term of the legacy ROIAlign (aligned=False; adaptive grid ceil(roi / pooled) for sampling_ratio 0; samples
+    outside [-1, extent] dropped; 4-tap bilinear; mean over the grid) of rois [R, 5] (frame, x1, y1, x2, y2) on H x W maps,
+    on the rois' device.  Sample coordinates and tap weights are formed in fp32 in the kernels' operation order
+    (csrc/roi.cu roi_geometry / sample_coord / make_tap, csrc/train.cu roi_align_bwd_frame / bilinear_taps,
+    oracle/step_oracle.c).  A clamped sample (past H-1 / W-1) keeps its duplicate taps of one pixel as separate terms, as
+    the kernels add them.  ROIs are grouped by sampling grid so that each group is one batched tensor expression.
+    Returns a list of groups dict(idx [G] int64 ROI rows, bin [S] int64, pix [G, S] int64 (-1: dropped sample),
+    w [G, S] float64 holding the fp32 tap weights, count = gh * gw), S = ph pw gh gw 4 in the kernels' (bin, iy, ix, tap)
+    order."""
     f32 = torch.float32
-    K, H, W, C = feat.shape
-    fd = feat.detach().cpu().double()
-    rois = rois.detach().cpu().to(f32)
-    R = rois.shape[0]
-    out = torch.zeros(R, ph * pw, C, dtype=torch.float64)
-    out_abs = torch.zeros_like(out)
-    sc = torch.tensor(scale, dtype=f32)
-    one = torch.tensor(1.0, dtype=f32)
+    dev = rois.device
+    r = rois.detach().to(f32)
+    sc = torch.tensor(scale, dtype=f32, device=dev)
+    sw, sh, ew, eh = (r[:, j] * sc for j in (1, 2, 3, 4))
+    one = torch.ones((), dtype=f32, device=dev)
+    rw, rh = torch.maximum(ew - sw, one), torch.maximum(eh - sh, one)
+    bin_h = rh / torch.tensor(float(ph), dtype=f32, device=dev)
+    bin_w = rw / torch.tensor(float(pw), dtype=f32, device=dev)
+    if sampling_ratio > 0:
+        gh_all = torch.full_like(bin_h, sampling_ratio, dtype=torch.int64)
+        gw_all = gh_all
+    else:
+        gh_all, gw_all = torch.ceil(bin_h).to(torch.int64), torch.ceil(bin_w).to(torch.int64)   # ceilf(roi / pooled)
 
     def taps(start, bin_, grid, n_bins, extent):
-        """per (bin, sample): low / high index and weights (lo, hi) along one axis, and validity."""
-        p = torch.arange(n_bins, dtype=f32).view(-1, 1)
-        i = torch.arange(grid, dtype=f32).view(1, -1)
-        c = (start + p * bin_) + ((i + 0.5) * bin_) / torch.tensor(float(grid), dtype=f32)
+        """[G, n_bins, grid]: low / high index, weights (hi, lo) along one axis, and validity."""
+        p = torch.arange(n_bins, dtype=f32, device=dev).view(1, -1, 1)
+        i = torch.arange(grid, dtype=f32, device=dev).view(1, 1, -1)
+        s, b = start.view(-1, 1, 1), bin_.view(-1, 1, 1)
+        c = (s + p * b) + ((i + 0.5) * b) / torch.tensor(float(grid), dtype=f32, device=dev)
         valid = (c >= -1.0) & (c <= float(extent))
         c = torch.where(c <= 0.0, torch.zeros_like(c), c)
         low = c.to(torch.int64)
@@ -386,33 +408,126 @@ def roi_align(feat, rois, scale, ph, pw, roi_T=0, feat_T=0, t_start=0):
         high = torch.where(top, low, low + 1)
         c = torch.where(top, low.to(f32), c)
         l_ = c - low.to(f32)
-        return low, high, one - l_, l_, valid
+        return low, high, 1.0 - l_, l_, valid
 
-    for r in range(R):
-        b = int(rois[r, 0])
-        frame = (b // roi_T) * feat_T + t_start + b % roi_T if roi_T > 0 else b
-        sw, sh, ew, eh = (rois[r, j] * sc for j in (1, 2, 3, 4))
-        rw, rh = torch.maximum(ew - sw, one), torch.maximum(eh - sh, one)
-        bin_h, bin_w = rh / torch.tensor(float(ph), dtype=f32), rw / torch.tensor(float(pw), dtype=f32)
-        gh, gw = int(torch.ceil(rh / float(ph))), int(torch.ceil(rw / float(pw)))
-        yl, yh, hy, ly, vy = taps(sh, bin_h, gh, ph, H)                 # [ph, gh]
-        xl, xh, hx, lx, vx = taps(sw, bin_w, gw, pw, W)                 # [pw, gw]
-        # every (p, q, iy, ix) sample: four pixels with fp32 weights hy hx, hy lx, ly hx, ly lx
-        e = lambda t: t.view(ph, 1, gh, 1)
-        f = lambda t: t.view(1, pw, 1, gw)
-        ok = (e(vy) & f(vx)).double()
-        pix = [e(yl) * W + f(xl), e(yl) * W + f(xh), e(yh) * W + f(xl), e(yh) * W + f(xh)]
-        wts = [e(hy) * f(hx), e(hy) * f(lx), e(ly) * f(hx), e(ly) * f(lx)]
-        M = torch.zeros(ph * pw, H * W, dtype=torch.float64)
-        rows = torch.arange(ph * pw).view(ph, pw, 1, 1).expand(ph, pw, gh, gw)
-        for p_, w_ in zip(pix, wts):
-            M.index_put_((rows.reshape(-1), p_.expand(ph, pw, gh, gw).reshape(-1)),
-                         (w_.double() * ok).expand(ph, pw, gh, gw).reshape(-1), accumulate=True)
-        M /= gh * gw
-        fr = fd[frame].reshape(H * W, C)
-        out[r] = M @ fr
-        out_abs[r] = M @ fr.abs()
-    return out.view(R, ph, pw, C), out_abs.view(R, ph, pw, C)
+    groups = []
+    keys = torch.stack([gh_all, gw_all], 1).cpu()
+    for gh, gw in sorted({(int(a), int(b)) for a, b in keys.tolist()}):
+        idx = ((gh_all == gh) & (gw_all == gw)).nonzero().view(-1)
+        G = idx.numel()
+        yl, yh, hy, ly, vy = taps(sh[idx], bin_h[idx], gh, ph, H)          # [G, ph, gh]
+        xl, xh, hx, lx, vx = taps(sw[idx], bin_w[idx], gw, pw, W)          # [G, pw, gw]
+        e = lambda t: t.view(G, ph, 1, gh, 1)
+        f = lambda t: t.view(G, 1, pw, 1, gw)
+        ok = e(vy) & f(vx)
+        pix = torch.stack([e(yl) * W + f(xl), e(yl) * W + f(xh), e(yh) * W + f(xl), e(yh) * W + f(xh)], -1)
+        wts = torch.stack([e(hy) * f(hx), e(hy) * f(lx), e(ly) * f(hx), e(ly) * f(lx)], -1)
+        ok = ok.unsqueeze(-1).expand_as(pix)
+        pix = torch.where(ok, pix, torch.full_like(pix, -1)).reshape(G, -1)
+        wts = torch.where(ok, wts, torch.zeros_like(wts)).double().reshape(G, -1)
+        b_ = torch.arange(ph * pw, device=dev).view(ph, pw, 1, 1, 1).expand(ph, pw, gh, gw, 4).reshape(-1)
+        groups.append(dict(idx=idx, bin=b_, pix=pix, w=wts, count=gh * gw))
+    return groups
+
+
+def roi_align_matrix(group, sel, nbins, npix):
+    """The per-ROI matrices of rows `sel` of one roi_align_terms group: M [g, nbins, npix] float64 with
+    M[bin, pix] = sum of the bin's tap weights on pix / count (the ROIAlign forward is out = M @ frame), and the number of
+    taps behind each entry, [g, nbins, npix] float64.  Shared by roi_align and roi_align_bwd."""
+    pix, w = group["pix"][sel], group["w"][sel]
+    g = pix.shape[0]
+    live = pix >= 0
+    lin = group["bin"].view(1, -1) * npix + pix.clamp(min=0)
+    M = torch.zeros((g, nbins * npix), dtype=torch.float64, device=pix.device)
+    M.scatter_add_(1, lin, torch.where(live, w, torch.zeros_like(w)) / group["count"])
+    n = torch.zeros_like(M)
+    n.scatter_add_(1, lin, live.double())
+    return M.view(g, nbins, npix), n.view(g, nbins, npix)
+
+
+def _roi_chunks(groups, frames, K):
+    """(group, row selection, ROI rows, frames) per chunk of <= ROI_CHUNK ROIs whose frame lies in [0, K)."""
+    for gr in groups:
+        fr = frames[gr["idx"]]
+        keep = ((fr >= 0) & (fr < K)).nonzero().view(-1)
+        for a in range(0, keep.numel(), ROI_CHUNK):
+            sel = keep[a:a + ROI_CHUNK]
+            yield gr, sel, gr["idx"][sel], fr[sel]
+
+
+def roi_align(feat, rois, scale, ph, pw, roi_T=0, feat_T=0, t_start=0, sampling_ratio=0):
+    """Float64 ROIAlign of channels-last frames feat [K, H, W, C] (roi_align_terms' rules; the weighted sums in float64),
+    computed on feat's device.  rois [R, 5]; with roi_T > 0 the frame index f maps to (f // roi_T) * feat_T + t_start +
+    f % roi_T.  Returns (out, out of |feat|) as [R, ph, pw, C] on the CPU."""
+    K, H, W, C = feat.shape
+    dev = feat.device
+    fd = feat.detach().double().reshape(K, H * W, C)
+    rois = rois.detach().to(dev)
+    R = rois.shape[0]
+    out = torch.zeros(R, ph * pw, C, dtype=torch.float64, device=dev)
+    out_abs = torch.zeros_like(out)
+    groups = roi_align_terms(rois, scale, ph, pw, H, W, sampling_ratio)
+    for gr, sel, rows, fr in _roi_chunks(groups, roi_frames(rois, roi_T, feat_T, t_start), K):
+        M, _ = roi_align_matrix(gr, sel, ph * pw, H * W)
+        x = fd[fr]
+        out[rows] = torch.bmm(M, x)
+        out_abs[rows] = torch.bmm(M, x.abs())
+    return out.view(R, ph, pw, C).cpu(), out_abs.view(R, ph, pw, C).cpu()
+
+
+def roi_align_bwd(grad, rois, scale, ph, pw, K, H, W, roi_T=0, feat_T=0, t_start=0, sampling_ratio=0, groups=None):
+    """Float64 ROIAlign backward, the transpose of roi_align's per-ROI matrix: grad [R, ph, pw, C] (the values the kernel
+    read, any dtype) -> grad_in [K, H, W, C] float64 with grad_in[frame(r)] += M_r^T grad[r], on grad's device.  ROIs whose
+    (mapped) frame is outside [0, K) contribute nothing, as in the kernels.  groups: roi_align_terms' output, to evaluate a
+    modified set of terms.  Returns (grad_in, mag, n): mag = sum over the terms of |g w / count| (float64), n [K, H, W, 1]
+    the number of terms per pixel (every channel of a pixel has the same terms).
+
+    Bound (roi_align_bwd_check), u32 = 2^-24: the kernels form each term as fl(fl(g w) / count) from the fp32 value of g
+    and the fp32 weight w, within (1 + u32)^2 - 1 < 2.01 u32 of g w / count (no underflow: |g| >= 2^-24 or 0, w >= 2^-48
+    or 0).  They add the n terms of an element and its initial value into one fp32 result in some order (per ROI, then
+    per frame, then into grad_in); whatever the order, that is a tree of n additions, each within u32 of its result, and
+    every partial sum is at most the sum of the absolute values: n u32 (1 + n u32) (sum |term| + |init|).  In total
+    |got - init - ref| <= (n + 3) u32 (mag + |init|) for n <= 2^11, and an element with no term keeps its initial value
+    bit for bit."""
+    dev = grad.device
+    R = grad.shape[0]
+    C = grad.shape[-1]
+    g = grad.detach().double().reshape(R, ph * pw, C)
+    gin = torch.zeros(K, H * W, C, dtype=torch.float64, device=dev)
+    mag = torch.zeros_like(gin)
+    n = torch.zeros(K, H * W, 1, dtype=torch.float64, device=dev)
+    rois = rois.detach().to(dev)
+    if groups is None:
+        groups = roi_align_terms(rois, scale, ph, pw, H, W, sampling_ratio)
+    for gr, sel, rows, fr in _roi_chunks(groups, roi_frames(rois, roi_T, feat_T, t_start), K):
+        M, cnt = roi_align_matrix(gr, sel, ph * pw, H * W)
+        Mt = M.transpose(1, 2)
+        gin.index_add_(0, fr, torch.bmm(Mt, g[rows]))
+        mag.index_add_(0, fr, torch.bmm(Mt, g[rows].abs()))
+        n.index_add_(0, fr, cnt.sum(1).unsqueeze(-1))
+    return gin.view(K, H, W, C), mag.view(K, H, W, C), n.view(K, H, W, 1)
+
+
+def roi_align_bwd_check(got, init, ref, mag, n, what="roi_align_bwd"):
+    """got (the kernel's grad_in after the launch) against init (before it) + ref within (n + 3) u32 (mag + |init|)
+    (roi_align_bwd derives it); elements with n == 0 equal init exactly.  Returns the largest |err| / bound."""
+    got, init = got.double(), init.double()
+    assert bool((n <= 2 ** 11).all()), (what, "more terms per element than the bound is derived for")
+    touched = (n > 0).expand_as(got)
+    same = (got == init) | touched
+    if not bool(same.all()):
+        i = int((~same).flatten().nonzero()[0])
+        raise AssertionError("%s: an element without a term changed at flat %d: %r -> %r" % (
+            what, i, float(init.flatten()[i]), float(got.flatten()[i])))
+    err = (got - init - ref).abs()
+    tol = (n + 3.0) * U32 * (mag + init.abs())
+    ok = (err <= tol) | ~touched
+    if not bool(ok.all()):
+        i = int((err - tol).masked_fill(~touched, -1.0).flatten().argmax())
+        raise AssertionError("%s: %d of %d elements out of bound; worst at flat %d: got %r init %r ref %r tol %r" % (
+            what, int((~ok).sum()), ok.numel(), i, float(got.flatten()[i]), float(init.flatten()[i]), float(ref.flatten()[i]),
+            float(tol.flatten()[i])))
+    return float((err / tol.clamp(min=1e-300)).masked_fill(~touched, 0.0).max()) if bool(touched.any()) else 0.0
 
 
 def roi_align_tol(out_abs, vmax):
@@ -421,3 +536,185 @@ def roi_align_tol(out_abs, vmax):
     (2^-11 of the running sum <= the abs sum, 2^-25 absolute): 17 x 2^-11 x sum |w| |v| + 16 x 2^-25 (1 + max |v|) + the
     fp32 merge (< 2^-20 relative)."""
     return (ROI_MERGED + 1) * 2.0 ** -11 * out_abs + 2.0 ** -20 * out_abs + ROI_MERGED * 2.0 ** -25 * (1.0 + vmax)
+
+
+# ---- the launches of train_step outside the tape -----------------------------------------------------------------------
+def linear_bwd(x, w, dy, init_dx=None):
+    """Float64 backward of y = x w^T + b on what step_linear_small_n_bwd read: x [M, K] (fp16 | fp32), w [Nn, K] fp32,
+    dy [M, Nn] fp32, init_dx [M, K] what dx accumulates onto (or None).  Returns dict(dx, dx_abs, dw, dw_abs, db, db_abs):
+    the values and |dy| |w| (+ |init_dx|), |dy|^T |x|, sum |dy|.
+
+    Bounds (linear_bwd_check): linear_bwd_dw_kernel forms dW[n, k] as an fmaf chain over the M rows in order and db[n] as a
+    chain of M fp32 additions; linear_bwd_dx_kernel forms dx[m, k] as an fmaf chain over the Nn columns, starting from 0 or
+    from dx when accumulating.  Each fmaf / addition rounds once, within u32 of its result, and every partial sum is at
+    most the abs sum: a chain of s roundings errs by at most s u32 (1 + s u32) abs <= (s + 1) u32 abs for s <= 2^12
+    (s = M for dW and db, Nn for dx; one more for a later fp32 addition of dx into another buffer)."""
+    xd, wd, g = x.double(), w.double(), dy.double()
+    dx = g @ wd
+    dx_abs = g.abs() @ wd.abs()
+    if init_dx is not None:
+        dx = dx + init_dx.double()
+        dx_abs = dx_abs + init_dx.double().abs()
+    return dict(dx=dx, dx_abs=dx_abs, dw=g.t() @ xd, dw_abs=g.abs().t() @ xd.abs(), db=g.sum(0), db_abs=g.abs().sum(0))
+
+
+def linear_bwd_check(got, ref, abs_, steps, what):
+    """|got - ref| <= (steps + 1) u32 abs elementwise (linear_bwd derives it).  Returns the largest |err| / bound."""
+    assert steps <= 2 ** 12, (what, steps)
+    return _check_within(got, ref, (steps + 1) * U32 * abs_, what)
+
+
+def _check_within(got, ref, tol, what):
+    got, ref, tol = got.double(), ref.double().to(got.device), tol.double().to(got.device)
+    err = (got - ref).abs()
+    ok = err <= tol
+    if not bool(ok.all()):
+        i = int((err - tol).flatten().argmax())
+        raise AssertionError("%s: %d of %d elements out of bound; worst at flat %d: got %r ref %r tol %r" % (
+            what, int((~ok).sum()), ok.numel(), i, float(got.flatten()[i]), float(ref.flatten()[i]), float(tol.flatten()[i])))
+    return float((err / tol.clamp(min=1e-300)).max()) if err.numel() else 0.0
+
+
+# The loss bounds keep the first-order terms (u32 times a magnitude); this factor covers the neglected products of two such
+# terms, each below 2^-12 of its magnitude for box coordinates below 2^10.
+SECOND_ORDER = 1.0 + 2.0 ** -10
+
+
+def _cls_terms(x, t):
+    """Classification part of the loss bounds (cls_loss_pass), float64: x the logits, t = label * mask.
+    loss l = (1 - t) x - (min(x, 0) - log1p(exp(-|x|))): expf errs by <= 2 ulp (4 u32 relative), log1pf by 1 ulp (2 u32)
+    and carries expf's error scaled by e / (1 + e) <= log1p(e) / e * e, so L = log1pf(expf(-|x|)) is within 6 u32 L; four
+    more roundings ((1 - t), * x, the two subtractions), each within u32 of A = |(1 - t) x| + |min(x, 0)| + L: 10 u32 A.
+    gradient (sigmoid(x) - t) / (N cls): sg = 1 / (1 + expf(-x)) is within 6 u32 sg (expf's 4 u32 scaled by
+    e / (1 + e) <= 1, two roundings) plus 2^-126 where expf(-x) overflows; sg - t, the fp32 1 / (N cls) and the product
+    round three times more: (6 u32 sg + 3 u32 |sg - t| + 2^-126) / (N cls)."""
+    L = torch.log1p(torch.exp(-x.abs()))
+    A = ((1.0 - t) * x).abs() + torch.clamp(x, max=0.0).abs() + L
+    sg = torch.sigmoid(x)
+    return 10.0 * U32 * A, 6.0 * U32 * sg + 3.0 * U32 * (sg - t).abs() + 2.0 ** -126
+
+
+def cls_loss(logits, targets):
+    """Float64 reference of cls_loss_kernel on its fp32 inputs (oracle.model.two_branch_losses, cls_only): returns
+    dict(loss [N cls] or the [1] zero without a classification sample, loss_tol, dlogits = d mean(loss) / d logits by
+    float64 autograd, dlogits_tol) with _cls_terms' bounds times SECOND_ORDER."""
+    from oracle.model import two_branch_losses
+    x = logits.detach().double().cpu().requires_grad_(True)
+    tg = targets.detach().double().cpu()
+    N, cls = x.shape
+    z = torch.zeros(N, 1, 4, dtype=torch.float64)
+    lc, _, _ = two_branch_losses(x, z, z, z, torch.zeros(N, 1, 5, dtype=torch.float64), tg, 1, cls_only=True)
+    t = tg[:, 1, 6:] * tg[:, 1, 4:5]
+    lt, gt = _cls_terms(x.detach(), t)
+    has = bool(tg[:, 1, 4].sum() != 0)
+    if has:
+        lc.mean().backward()
+        g = x.grad
+    else:
+        g = torch.zeros_like(x)
+    return dict(loss=lc.detach(), loss_tol=(lt.flatten() if has else torch.zeros(1, dtype=torch.float64)) * SECOND_ORDER,
+                dlogits=g.detach(), dlogits_tol=(gt / (N * cls) if has else torch.zeros_like(g)) * SECOND_ORDER)
+
+
+def _encode_terms(gt, anchor):
+    """encode4 of csrc/train.cu (tube_utils.py:143-163) in float64 and its fp32 error bound, per [N, 4] row.
+    With B = |c0| + |c2| + 1 per axis of a box (c0, c2 its two coordinates on the axis): the width fl(fl(c2 - c0) + 1) is
+    within 2 u32 B, the centre fl(c0 + 0.5 w) within 2.5 u32 B < 3 u32 B.  (gx - ax) / aw: the difference within
+    3 u32 (Bg + Ba) + u32 |num|, the division adds |enc| 2 u32 Ba / |aw| (the width) and u32 |enc|.  log(gw / aw): the ratio
+    is within delta = 2 u32 Bg / |gw| + 2 u32 Ba / |aw| + u32 relative, which moves the log by delta; logf adds 1 ulp,
+    2 u32 |enc|."""
+    enc, err = [], []
+    for lo, hi in ((0, 2), (1, 3)):
+        gw, aw = gt[:, hi] - gt[:, lo] + 1.0, anchor[:, hi] - anchor[:, lo] + 1.0
+        Bg, Ba = gt[:, lo].abs() + gt[:, hi].abs() + 1.0, anchor[:, lo].abs() + anchor[:, hi].abs() + 1.0
+        num = (gt[:, lo] + 0.5 * gw) - (anchor[:, lo] + 0.5 * aw)
+        e = num / aw
+        enc.append(e)
+        err.append((3.0 * U32 * (Bg + Ba) + U32 * num.abs()) / aw.abs() + e.abs() * 2.0 * U32 * Ba / aw.abs() + U32 * e.abs())
+    for lo, hi in ((0, 2), (1, 3)):
+        gw, aw = gt[:, hi] - gt[:, lo] + 1.0, anchor[:, hi] - anchor[:, lo] + 1.0
+        Bg, Ba = gt[:, lo].abs() + gt[:, hi].abs() + 1.0, anchor[:, lo].abs() + anchor[:, hi].abs() + 1.0
+        e = torch.log(gw / aw)
+        enc.append(e)
+        err.append(2.0 * U32 * Bg / gw.abs() + 2.0 * U32 * Ba / aw.abs() + U32 + 2.0 * U32 * e.abs())
+    return torch.stack(enc, 1), torch.stack(err, 1)
+
+
+def head_losses(logits, local_loc, first_loc, last_loc, tubes, targets, T, lambda_reg=5.0, lambda_neighbor=1.0):
+    """Float64 reference of head_losses_kernel on its fp32 inputs: oracle.model.two_branch_losses, and float64 autograd of
+    mean(loss_cls) + lambda_reg loss_loc + lambda_neighbor loss_nb.  The kernel adds d/d first_loc and d/d last_loc into
+    d/d local_loc at the frames first_loc / last_loc are slices of (two_branch.py:265-270; head_chunks), so dlocal here is
+    autograd's plus those two.  Returns dict of (value, tol) pairs: loss_cls, loss_loc, loss_nb, dlogits, dlocal, dfirst,
+    dlast, each tol times SECOND_ORDER.
+
+    Regression bounds, per coordinate of a tube (masks are 0 / 1, S their fp32 sum, exact below 2^24): d = fl(pred - enc)
+    errs by E_d = E_enc + u32 |d| (_encode_terms); smooth-L1 and its derivative clamp(d, -1, 1) are continuous at |d| = 1 with
+    slopes min(|d|, 1) and 1, so a branch flip near the boundary stays inside E_l = min(|d| + E_d, 1) E_d + u32 |l| and
+    E_g = E_d; the gradient fl(fl(g m w) / S) adds two roundings: (w / S) E_g + 2 u32 |grad|; each addition of a first / last
+    gradient into local_loc one more (u32 of the sum).  The loss sums 4N (8N for the neighbours) terms in tube order:
+    sum E_l + 4N u32 sum |l| (8N), then / S: one rounding."""
+    from oracle.model import two_branch_losses
+    d64 = lambda t: t.detach().double().cpu()
+    x = d64(logits).requires_grad_(True)
+    loc, fst, lst = (d64(t).requires_grad_(True) for t in (local_loc, first_loc, last_loc))
+    tb, tg = d64(tubes), d64(targets)
+    N, cls = x.shape
+    Tl, Tc = loc.shape[1], fst.shape[1]
+    for j in range(3):
+        assert bool(((tg[:, j, 4:6] == 0) | (tg[:, j, 4:6] == 1)).all()), "masks of 0 / 1 (the bound assumes exact products)"
+    lc, ll, ln = two_branch_losses(x, loc, fst, lst, tb, tg, T)
+    obj = lc.mean() + lambda_reg * ll.mean() + lambda_neighbor * ln.mean()
+    gx, gl, gf, gla = (torch.zeros_like(t) for t in (x, loc, fst, lst))
+    if obj.requires_grad:
+        gs = torch.autograd.grad(obj, (x, loc, fst, lst), allow_unused=True)
+        gx, gl, gf, gla = (g if g is not None else z for g, z in zip(gs, (gx, gl, gf, gla)))
+    chunks = int(Tl / T)
+    half = int(T / 2)
+    centre, first_i, last_i = (chunks // 2) * T + half, half, (chunks - 1) * T + half
+    s0, e0 = first_i - half, last_i - half
+    dlocal = gl.clone()
+    dlocal[:, s0:s0 + Tc] += gf
+    dlocal[:, e0:e0 + Tc] += gla
+    sums = gl.abs()
+    sums[:, s0:s0 + Tc] += gf.abs()
+    sums[:, e0:e0 + Tc] += gla.abs()
+    # classification
+    t = tg[:, 1, 6:] * tg[:, 1, 4:5]
+    lt, gt_ = _cls_terms(x.detach(), t)
+    has_cls = bool(tg[:, 1, 4].sum() != 0)
+    out = dict(loss_cls=(lc.detach(), (lt.flatten() if has_cls else torch.zeros(1, dtype=torch.float64)) * SECOND_ORDER),
+               dlogits=(gx, (gt_ / (N * cls) if has_cls else torch.zeros_like(gx)) * SECOND_ORDER))
+    # regression: (target row, tube frame, prediction) of the centre, first and last terms
+    terms = []
+    for j, frame, pred in ((1, centre, loc[:, centre]), (0, first_i, fst[:, half]), (2, last_i, lst[:, half])):
+        enc, e_enc = _encode_terms(tg[:, j, :4], tb[:, frame, 1:5])
+        d = pred.detach() - enc
+        E_d = e_enc + U32 * d.abs()
+        ad = d.abs()
+        l = torch.where(ad < 1.0, 0.5 * d * d, ad - 0.5)
+        E_l = torch.minimum(ad + E_d, torch.ones_like(ad)) * E_d + U32 * l
+        terms.append((tg[:, j, 5:6], l, E_l, E_d))
+    grads_tol = {}
+    for name, parts, lam in (("loss_loc", terms[:1], lambda_reg), ("loss_nb", terms[1:], lambda_neighbor)):
+        S = sum(float(m.sum()) * 4 for m, _, _, _ in parts)
+        if S == 0:
+            out[name] = ((ll if name == "loss_loc" else ln).detach(), torch.zeros(1, dtype=torch.float64))
+            grads_tol[name] = [torch.zeros_like(p[1]) for p in parts]
+            continue
+        sum_E = sum(float((E_l * m).sum()) for m, _, E_l, _ in parts)
+        sum_l = sum(float((l * m).sum()) for m, l, _, _ in parts)
+        v = (ll if name == "loss_loc" else ln).detach()
+        out[name] = (v, ((sum_E + 4 * N * len(parts) * U32 * sum_l) / S + U32 * v.abs()) * SECOND_ORDER)
+        # |grad| = (lambda / S) |clamp(d, -1, 1)| m <= (lambda / S) m
+        grads_tol[name] = [(lam / S) * m * (E_d + 2.0 * U32) for m, _, _, E_d in parts]
+    tl = torch.zeros_like(gl)
+    tl[:, centre] = grads_tol["loss_loc"][0]
+    tf, tla = torch.zeros_like(gf), torch.zeros_like(gla)
+    tf[:, half] = grads_tol["loss_nb"][0]
+    tla[:, half] = grads_tol["loss_nb"][1]
+    tlocal = tl.clone()
+    tlocal[:, s0:s0 + Tc] += tf
+    tlocal[:, e0:e0 + Tc] += tla
+    tlocal = tlocal + 2.0 * U32 * sums                               # the (up to two) additions of first / last into local
+    out.update(dlocal=(dlocal, tlocal * SECOND_ORDER), dfirst=(gf, tf * SECOND_ORDER), dlast=(gla, tla * SECOND_ORDER))
+    return out

@@ -562,3 +562,202 @@ def test_roi_align_reference_matches_the_loop_rule():
     direct[:, 0] = torch.tensor([1.0, 2.0, 4.0, 5.0])
     ref, _ = R.roi_align(feat, direct, 1.0 / 16.0, 7, 7)
     assert torch.equal(fm, ref)
+
+
+# ---- the references of train_step's launches outside the tape ---------------------------------------------------------
+EDGE_ROIS = [[0, 10.0, 20.0, 90.0, 100.0],      # inside
+             [1, -30.0, -20.0, 60.0, 40.0],     # corners in [-16, 0): samples in [-1, 0] clamped to 0
+             [2, -100.0, -90.0, 40.0, 30.0],    # corners below -16: samples dropped
+             [3, 100.0, 90.0, 200.0, 170.0],    # past the bottom and right edges: last row / column clamped
+             [4, 40.0, 40.0, 44.0, 47.0],       # grid 1x1
+             [5, 0.0, 0.0, 175.0, 143.0],       # the whole map
+             [0, 60.0, 50.0, 20.0, 30.0],       # degenerate: x2 < x1, y2 < y1 (width and height clamped to 1)
+             [1, -40.0, 5.0, 1000.0, 700.0]]    # grid 10 x 7: more than one sample table of the kernel
+
+
+def _edge_case(gen, K=6, H=9, W=11, C=8):
+    feat = half_values(K, H, W, C, gen=gen).double()
+    rois = torch.tensor(EDGE_ROIS, dtype=torch.float32)
+    return feat, rois
+
+
+@pytest.mark.parametrize("sr", [0, 2])
+def test_roi_align_bwd_is_the_adjoint_of_roi_align(sr):
+    """<roi_align(feat), g> = <feat, roi_align_bwd(g)> in float64, to 1e-12, on ROIs inside, across and past every edge,
+    degenerate and larger than one sample table; the same with the roi_T / feat_T / t_start frame map."""
+    gen = torch.Generator().manual_seed(21 + sr)
+    feat, rois = _edge_case(gen)
+    K, H, W, C = feat.shape
+    g = torch.randn(rois.shape[0], 7, 7, C, generator=gen, dtype=torch.float64)
+    out, _ = R.roi_align(feat, rois, 1.0 / 16.0, 7, 7, sampling_ratio=sr)
+    gin, mag, n = R.roi_align_bwd(g, rois, 1.0 / 16.0, 7, 7, K, H, W, sampling_ratio=sr)
+    lhs, rhs = float((out * g).sum()), float((feat * gin).sum())
+    assert abs(lhs - rhs) <= 1e-12 * float((out.abs() * g.abs()).sum()), (lhs, rhs)
+    assert bool((gin.abs() <= mag + 1e-15).all()) and bool((n >= 0).all())
+    # frame map: 2 clips of 3 frames, a 2-frame slice from t 1; ROI frames 0..3
+    fm = rois[:4].clone()
+    fm[:, 0] = torch.tensor([0.0, 1.0, 2.0, 3.0])
+    out, _ = R.roi_align(feat, fm, 1.0 / 16.0, 5, 3, roi_T=2, feat_T=3, t_start=1, sampling_ratio=sr)
+    g = g[:4, :5, :3]
+    gin, _, n = R.roi_align_bwd(g.contiguous(), fm, 1.0 / 16.0, 5, 3, K, H, W, roi_T=2, feat_T=3, t_start=1, sampling_ratio=sr)
+    assert abs(float((out * g).sum()) - float((feat * gin).sum())) <= 1e-12 * float((out.abs() * g.abs()).sum())
+    assert float(n[[0, 3]].sum()) == 0.0 and float(n[[1, 2, 4, 5]].sum()) > 0          # frames 0 and 3 are outside the slice
+
+
+def test_roi_align_bwd_matches_torchvision_autograd():
+    """On ROIs whose fp32 sample coordinates and weights are exact (corners on multiples of 1/16 of a pixel, sizes giving
+    power-of-two bins and grids), roi_align_bwd equals float64 autograd of torchvision.ops.roi_align(aligned=False),
+    including samples clamped at the far edges and dropped ones."""
+    tv = pytest.importorskip("torchvision")
+    gen = torch.Generator().manual_seed(22)
+    K, H, W, C = 3, 10, 12, 4
+    feat = torch.randn(K, C, H, W, generator=gen, dtype=torch.float64, requires_grad=True)
+    rois = torch.tensor([[0, 16.0, 32.0, 80.0, 96.0], [1, 0.0, 0.0, 256.0, 256.0], [2, 128.0, 96.0, 256.0, 224.0],
+                         [0, -32.0, -24.0, 32.0, 40.0], [2, -64.0, 40.0, 0.0, 104.0], [1, 96.0, 48.0, 112.0, 64.0]],
+                        dtype=torch.float64)
+    for ph, pw in ((4, 4), (2, 8)):
+        out = tv.ops.roi_align(feat, rois, (ph, pw), 1.0 / 16.0, 0, aligned=False)
+        g = torch.randn(out.shape, generator=gen, dtype=torch.float64)
+        (ref,) = torch.autograd.grad(out, feat, g)
+        gin, _, _ = R.roi_align_bwd(g.permute(0, 2, 3, 1).contiguous(), rois.float(), 1.0 / 16.0, ph, pw, K, H, W)
+        assert torch.allclose(gin.permute(0, 3, 1, 2), ref, rtol=0, atol=1e-13), (ph, pw)
+
+
+def _shift_clamped_tap(groups, H, W):
+    """A copy of roi_align_terms' groups with tap 0 of one sample clamped at the last row (its taps 0 and 2 on one pixel)
+    moved up by one row.  Returns (groups, True) or (groups, False) when there is no such sample."""
+    out = []
+    moved = False
+    for gr in groups:
+        gr = dict(gr, pix=gr["pix"].clone())
+        if not moved:
+            p = gr["pix"].view(gr["pix"].shape[0], -1, 4)
+            w = gr["w"].view_as(p)
+            hit = ((p[..., 0] == p[..., 2]) & (p[..., 0] >= (H - 1) * W) & (w[..., 0] > 0)).nonzero()
+            if hit.shape[0]:
+                r, s = hit[0].tolist()
+                p[r, s, 0] -= W
+                moved = True
+        out.append(gr)
+    return out, moved
+
+
+def test_roi_align_bwd_check_rejects_perturbed_references():
+    """roi_align_bwd_check accepts the float64 result rounded to fp32 on top of an initial gradient, and rejects the
+    reference with the 1/count dropped, with one tap of a clamped sample moved by a pixel, with the frame map off by one
+    frame, and scaled by 1 + 2^-12."""
+    gen = torch.Generator().manual_seed(23)
+    K, H, W, C = 6, 9, 11, 8
+    rois = torch.tensor(EDGE_ROIS, dtype=torch.float32)
+    rois[:, 0] = torch.tensor([0.0, 1.0, 2.0, 3.0, 0.0, 1.0, 2.0, 3.0])
+    args = (rois, 1.0 / 16.0, 7, 7, K, H, W)
+    fmap = dict(roi_T=2, feat_T=3, t_start=1)
+    g = half_values(rois.shape[0], 7, 7, C, gen=gen)
+    init = torch.randn(K, H, W, C, generator=gen) * 0.01
+    ref, mag, n = R.roi_align_bwd(g, *args, **fmap)
+    got = (init.double() + ref).float()
+    assert R.roi_align_bwd_check(got, init, ref, mag, n) < 1.0
+    groups = R.roi_align_terms(rois, 1.0 / 16.0, 7, 7, H, W)
+    no_count = [dict(gr, count=1) for gr in groups]
+    assert any(gr["count"] > 1 for gr in groups)
+    shifted, moved = _shift_clamped_tap(groups, H, W)
+    assert moved
+    bad = {"1/count dropped": R.roi_align_bwd(g, *args, groups=no_count, **fmap),
+           "clamped tap moved": R.roi_align_bwd(g, *args, groups=shifted, **fmap),
+           "frame map off by one": R.roi_align_bwd(g, *args, roi_T=2, feat_T=3, t_start=0),
+           "scaled": (ref * (1.0 + 2.0 ** -12), mag, n)}
+    for what, (r_, m_, n_) in bad.items():
+        with pytest.raises(AssertionError):
+            R.roi_align_bwd_check(got, init, r_, m_, n_, what)
+
+
+@pytest.mark.parametrize("xdtype", [torch.float16, torch.float32])
+def test_linear_bwd_matches_autograd_and_its_check_rejects_perturbations(xdtype):
+    """linear_bwd's dx / dW / db equal float64 autograd of x w^T + b (dx accumulated onto init_dx); linear_bwd_check
+    accepts them rounded to fp32 and rejects a 1 + 2^-12 scale and one transposed index (two columns of x swapped)."""
+    gen = torch.Generator().manual_seed(24)
+    M, K, Nn = 37, 96, 4
+    x = torch.randn(M, K, generator=gen).to(xdtype)
+    w = torch.randn(Nn, K, generator=gen)
+    dy = torch.randn(M, Nn, generator=gen)
+    init = torch.randn(M, K, generator=gen)
+    xd, wd = x.double().requires_grad_(True), w.double().requires_grad_(True)
+    bd = torch.zeros(Nn, dtype=torch.float64, requires_grad=True)
+    (xd @ wd.t() + bd).backward(dy.double())
+    r = R.linear_bwd(x, w, dy, init_dx=init)
+    assert torch.allclose(r["dx"], xd.grad + init.double(), rtol=1e-14, atol=1e-14)
+    assert torch.allclose(r["dw"], wd.grad, rtol=1e-14, atol=1e-14) and torch.allclose(r["db"], bd.grad, rtol=1e-14, atol=1e-14)
+    for key, steps in (("dx", Nn), ("dw", M), ("db", M)):
+        assert R.linear_bwd_check(r[key].float(), r[key], r[key + "_abs"], steps, key) < 1.0
+        with pytest.raises(AssertionError):
+            R.linear_bwd_check(r[key].float(), r[key] * (1.0 + 2.0 ** -12), r[key + "_abs"], steps, key)
+    xs = x.clone()
+    xs[:, [3, 4]] = xs[:, [4, 3]]
+    with pytest.raises(AssertionError):
+        rs = R.linear_bwd(xs, w, dy)
+        R.linear_bwd_check(r["dw"].float(), rs["dw"], rs["dw_abs"], M, "dw transposed")
+
+
+def _loss_case(gen, N=6, cls=5, T=3, chunks=3):
+    Tl = T * chunks
+    logits = torch.randn(N, cls, generator=gen) * 3
+    box = torch.rand(N, 1, 2, generator=gen) * 200
+    size = 20 + torch.rand(N, 1, 2, generator=gen) * 80
+    tubes = torch.cat([torch.zeros(N, Tl, 1), (box + torch.rand(N, Tl, 2, generator=gen) * 4),
+                       (box + size + torch.rand(N, Tl, 2, generator=gen) * 4)], 2)
+    tg = torch.zeros(N, 3, 6 + cls)
+    tg[:, :, :2] = box + torch.rand(N, 3, 2, generator=gen) * 10
+    tg[:, :, 2:4] = box + size + torch.rand(N, 3, 2, generator=gen) * 10
+    tg[:, :, 4:6] = (torch.rand(N, 3, 2, generator=gen) > 0.3).float()
+    tg[0, :, 4:6] = 1.0
+    tg[:, :, 6:] = (torch.rand(N, 3, cls, generator=gen) > 0.6).float()
+    # predictions near the encoded targets, some coordinates past |d| = 1 (the linear branch of smooth-L1)
+    local = torch.randn(N, Tl, 4, generator=gen) * 0.8
+    first = torch.randn(N, T, 4, generator=gen) * 0.8
+    last = torch.randn(N, T, 4, generator=gen) * 0.8
+    return logits, local, first, last, tubes, tg, T
+
+
+def test_loss_references_match_autograd_and_their_checks_reject_perturbations():
+    """head_losses: the losses of oracle.model.two_branch_losses; dlocal is autograd's through first_loc = local[s0:] + a,
+    last_loc = local[e0:] + b (the head's structure), dfirst / dlast d/da, d/db.  cls_loss: d mean(BCE) / d logits =
+    (sigmoid - t) / (N cls).  Every bound accepts the float64 values rounded to fp32 and rejects a 1 + 2^-12 scale and
+    one transposed index."""
+    from oracle.model import two_branch_losses
+    gen = torch.Generator().manual_seed(25)
+    logits, local, first, last, tubes, tg, T = _loss_case(gen)
+    ref = R.head_losses(logits, local, first, last, tubes, tg, T, 5.0, 1.0)
+    loc = local.double().requires_grad_(True)
+    s0, _, e0, _ = R.head_chunks(T, local.shape[1])
+    a = (first.double() - local.double()[:, s0:s0 + T]).requires_grad_(True)
+    b = (last.double() - local.double()[:, e0:e0 + T]).requires_grad_(True)
+    x = logits.double().requires_grad_(True)
+    lc, ll, ln = two_branch_losses(x, loc, loc[:, s0:s0 + T] + a, loc[:, e0:e0 + T] + b, tubes.double(), tg.double(), T)
+    (lc.mean() + 5.0 * ll.mean() + 1.0 * ln.mean()).backward()
+    for key, g in (("dlogits", x.grad), ("dlocal", loc.grad), ("dfirst", a.grad), ("dlast", b.grad)):
+        assert torch.allclose(ref[key][0], g, rtol=1e-12, atol=1e-15), key
+    for key, v in (("loss_cls", lc), ("loss_loc", ll), ("loss_nb", ln)):
+        assert torch.allclose(ref[key][0], v.detach(), rtol=1e-12, atol=0), key
+    t = tg[:, 1, 6:].double() * tg[:, 1, 4:5].double()
+    assert torch.allclose(ref["dlogits"][0], (torch.sigmoid(logits.double()) - t) / logits.numel(), rtol=1e-12, atol=1e-18)
+    cref = R.cls_loss(logits, tg)
+    assert torch.equal(cref["loss"], ref["loss_cls"][0]) and torch.allclose(cref["dlogits"], ref["dlogits"][0], rtol=1e-14, atol=0)
+    assert bool((ref["dlocal"][0] != 0).sum() > 0) and bool((ref["dlast"][0].abs() > 0).any())
+    assert bool((ref["dlocal"][0].abs() >= 1.0 / 6).any()), "no coordinate on smooth-L1's linear branch"
+    for key, (v, tol) in ref.items():
+        assert R._check_within(v.float(), v, tol + 0.0, key) <= 1.0
+        with pytest.raises(AssertionError):
+            R._check_within(v.float(), v * (1.0 + 2.0 ** -12), tol, key)
+    # one transposed index: two logits / two box coordinates swapped in the inputs
+    lg = logits.clone()
+    lg[:, [0, 1]] = lg[:, [1, 0]]
+    lo = local.clone()
+    lo[:, :, [0, 2]] = lo[:, :, [2, 0]]
+    fi = first.clone()
+    fi[:, :, [1, 3]] = fi[:, :, [3, 1]]
+    for args, keys in (((lg, local, first, last), ("loss_cls", "dlogits")), ((logits, lo, first, last), ("loss_loc", "dlocal")),
+                       ((logits, local, fi, last), ("loss_nb", "dfirst"))):
+        bad = R.head_losses(*args, tubes, tg, T, 5.0, 1.0)
+        for key in keys:
+            with pytest.raises(AssertionError):
+                R._check_within(ref[key][0].float(), bad[key][0], bad[key][1], (key, "transposed"))
