@@ -296,7 +296,7 @@ __global__ void __launch_bounds__(256) roi_align_fwd_nhwc_kernel(const T* __rest
 //      pixel (in fp32, with the 1/count factor) when the per-ROI table is built -> ~5.5 instead of ~10 loads;
 //  (2) the weighted sum runs in packed half2 FMAs (the result is a convex combination of the inputs: no
 //      cancellation, error <= a few fp16 ulps, far inside the fp16-path tolerance of DESIGN.md section 4).
-// Bins with more than kMaxMerged distinct pixels (sampling grids > 3x3) take the exact kernel instead.
+// ROIs whose bins can touch more than kMaxMerged distinct pixels take a direct form with fp32 FMAs instead.
 constexpr int kMaxMerged = 16;
 struct MergedBin {
   int n;
@@ -356,7 +356,8 @@ __device__ __forceinline__ void roi_gather_items(const MergedBin* bins, int nbin
 }
 
 
-__global__ void __launch_bounds__(256) roi_align_fwd_nhwc_f16_packed_kernel(const __half* __restrict__ feat, int H, int W,
+// 5 CTAs of 256 threads per SM: at most 51 registers (48 in use; without the bound the compiler takes 59).
+__global__ void __launch_bounds__(256, 5) roi_align_fwd_nhwc_f16_packed_kernel(const __half* __restrict__ feat, int H, int W,
                                                                             int C, int feat_ld, const float* __restrict__ rois,
                                                                             float scale, int ph, int pw, int sampling_ratio,
                                                                             __half* __restrict__ out, int out_ld, FrameMap fm) {
@@ -368,8 +369,12 @@ __global__ void __launch_bounds__(256) roi_align_fwd_nhwc_f16_packed_kernel(cons
   __half* obase = out + (size_t)r * nbins * out_ld;
   const int nvec = C >> 3;
   const int part = blockIdx.y, parts = gridDim.y;
-  if ((g.gh + 1) * (g.gw + 1) > kMaxMerged) {
-    // very large ROI (sampling grid > 3x3): direct form with fp32 FMAs, no table
+  // Distinct pixels one bin can touch, per axis: g + 1 when its g samples are at most one pixel apart (the bin is no wider
+  // than g pixels, always so for the adaptive grid), else two per sample.
+  const int nh = g.bin_h <= (float)g.gh ? g.gh + 1 : 2 * g.gh, nw = g.bin_w <= (float)g.gw ? g.gw + 1 : 2 * g.gw;
+  if (nh * nw > kMaxMerged) {
+    // a bin may not fit the table (sampling grid > 3x3, or a fixed sampling_ratio with bins wider than the grid):
+    // direct form with fp32 FMAs, no table
     const float ic = 1.0f / g.count;
     const int pv = nvec / parts, pv0 = part * pv;
     for (int item = threadIdx.x; item < nbins * pv; item += blockDim.x) {
@@ -412,7 +417,7 @@ __global__ void __launch_bounds__(256) roi_align_fwd_nhwc_f16_packed_kernel(cons
           int e = 0;
           while (e < n && pos[e] != tp[k]) ++e;
           if (e == n) {
-            if (n < kMaxMerged) { pos[n] = tp[k]; wt[n] = tw[k]; ++n; }
+            if (n < kMaxMerged) { pos[n] = tp[k]; wt[n] = tw[k]; ++n; }   // n <= nh * nw <= kMaxMerged (above)
           } else {
             wt[e] += tw[k];
           }

@@ -10,7 +10,8 @@ CPU.  Never fp32 on the GPU: cuDNN convolutions default to TF32 there.
 The second part holds the float64 references of the inference forward's launches (conv_fwd, exit_fwd, mean_mid, linear,
 head_regress, roi_align; pool_entry's `y` for the pools), fed what the kernel read, with the magnitude terms their error
 bounds are built from (tests/test_gpu_forward_layers.py derives the bounds), and check_fwd, the elementwise + bias check
-of one fp16 convolution output.
+of one fp16 convolution output.  roi_align_tol and roi_align_fma_tol bound the fp16 ROIAlign forward's packed-table and
+fp32-FMA paths (tests/test_gpu_roi_fwd_edges.py).
 
 The third part holds the references of train_step's launches outside the tape (tests/test_gpu_train_launches.py):
 roi_align_bwd (the transpose of the ROIAlign matrix roi_align uses, built once by roi_align_terms / roi_align_matrix),
@@ -377,8 +378,8 @@ def roi_align_terms(rois, scale, ph, pw, H, W, sampling_ratio=0):
     oracle/step_oracle.c).  A clamped sample (past H-1 / W-1) keeps its duplicate taps of one pixel as separate terms, as
     the kernels add them.  ROIs are grouped by sampling grid so that each group is one batched tensor expression.
     Returns a list of groups dict(idx [G] int64 ROI rows, bin [S] int64, pix [G, S] int64 (-1: dropped sample),
-    w [G, S] float64 holding the fp32 tap weights, count = gh * gw), S = ph pw gh gw 4 in the kernels' (bin, iy, ix, tap)
-    order."""
+    w [G, S] float64 holding the fp32 tap weights, count = gh * gw, grid = (gh, gw), bin_hw = the fp32 bin sizes [G] x 2),
+    S = ph pw gh gw 4 in the kernels' (bin, iy, ix, tap) order."""
     f32 = torch.float32
     dev = rois.device
     r = rois.detach().to(f32)
@@ -426,7 +427,7 @@ def roi_align_terms(rois, scale, ph, pw, H, W, sampling_ratio=0):
         pix = torch.where(ok, pix, torch.full_like(pix, -1)).reshape(G, -1)
         wts = torch.where(ok, wts, torch.zeros_like(wts)).double().reshape(G, -1)
         b_ = torch.arange(ph * pw, device=dev).view(ph, pw, 1, 1, 1).expand(ph, pw, gh, gw, 4).reshape(-1)
-        groups.append(dict(idx=idx, bin=b_, pix=pix, w=wts, count=gh * gw))
+        groups.append(dict(idx=idx, bin=b_, pix=pix, w=wts, count=gh * gw, grid=(gh, gw), bin_hw=(bin_h[idx], bin_w[idx])))
     return groups
 
 
@@ -455,10 +456,45 @@ def _roi_chunks(groups, frames, K):
             yield gr, sel, gr["idx"][sel], fr[sel]
 
 
-def roi_align(feat, rois, scale, ph, pw, roi_T=0, feat_T=0, t_start=0, sampling_ratio=0):
+def roi_distinct_pixels(group, nbins):
+    """Distinct pixels with a live tap per bin of every ROI of one roi_align_terms group: int64 [G, nbins].  The packed
+    ROIAlign merges a bin's taps per pixel into a table of ROI_MERGED entries."""
+    G = group["pix"].shape[0]
+    p = group["pix"].view(G, nbins, -1).sort(-1).values
+    first = torch.ones_like(p[..., :1], dtype=torch.bool)
+    new = torch.cat([first, p[..., 1:] != p[..., :-1]], -1) & (p >= 0)
+    return new.sum(-1)
+
+
+def roi_samples_per_bin(groups, R):
+    """gh * gw of every ROI row: int64 [R]."""
+    spb = torch.zeros(R, dtype=torch.int64)
+    for gr in groups:
+        spb[gr["idx"].cpu()] = gr["count"]
+    return spb
+
+
+def roi_align_fma_tol(out_abs, spb):
+    """The fp16 ROIAlign with fp32 FMAs (step_roi_align_fwd_nhwc exact=2, the table-less fallback of exact=0, and the
+    direct form of the packed kernel): per sample the four taps w_k v_k are added into an fp32 accumulator by one fmaf each,
+    with the weights w_k (1 / count) formed in fp32 (1 / count and the product each rounded once), then the sum is stored as
+    fp16.  u32 = 2^-24.  The weight of a term is w / count (1 + d1)(1 + d2); each of the n = 4 spb fmaf rounds its result
+    once, (1 + d); so every term of the sum carries at most n + 2 factors (1 + d), |d| <= u32, and the fp32 result is within
+    gamma_(n+2) sum |w| |v| / count of the float64 value, gamma_k = k u32 / (1 - k u32) (about (4 spb + 2) u32; no
+    underflow: the weights are >= 2^-61, far above fp32's normal range, and the fp32 subnormal spacing 2^-149 is below the
+    absolute term).  The fp16 store rounds once more: at most half an fp16 ulp, <= 2^-11 |x| + 2^-25.  out_abs [R, ph, pw, C]
+    the sum |w| |v| / count (roi_align's second output), spb [R] the samples per bin (roi_samples_per_bin)."""
+    k = (4.0 * spb.double() + 2.0).view(-1, *([1] * (out_abs.dim() - 1)))
+    gamma = k * U32 / (1.0 - k * U32)
+    fp32 = gamma * out_abs
+    return fp32 + 2.0 ** -11 * (out_abs + fp32) + 2.0 ** -25
+
+
+def roi_align(feat, rois, scale, ph, pw, roi_T=0, feat_T=0, t_start=0, sampling_ratio=0, groups=None):
     """Float64 ROIAlign of channels-last frames feat [K, H, W, C] (roi_align_terms' rules; the weighted sums in float64),
     computed on feat's device.  rois [R, 5]; with roi_T > 0 the frame index f maps to (f // roi_T) * feat_T + t_start +
-    f % roi_T.  Returns (out, out of |feat|) as [R, ph, pw, C] on the CPU."""
+    f % roi_T.  groups: roi_align_terms' output, to evaluate a modified set of terms.  Returns (out, out of |feat|) as
+    [R, ph, pw, C] on the CPU."""
     K, H, W, C = feat.shape
     dev = feat.device
     fd = feat.detach().double().reshape(K, H * W, C)
@@ -466,7 +502,8 @@ def roi_align(feat, rois, scale, ph, pw, roi_T=0, feat_T=0, t_start=0, sampling_
     R = rois.shape[0]
     out = torch.zeros(R, ph * pw, C, dtype=torch.float64, device=dev)
     out_abs = torch.zeros_like(out)
-    groups = roi_align_terms(rois, scale, ph, pw, H, W, sampling_ratio)
+    if groups is None:
+        groups = roi_align_terms(rois, scale, ph, pw, H, W, sampling_ratio)
     for gr, sel, rows, fr in _roi_chunks(groups, roi_frames(rois, roi_T, feat_T, t_start), K):
         M, _ = roi_align_matrix(gr, sel, ph * pw, H * W)
         x = fd[fr]

@@ -373,6 +373,40 @@ def gen_postprocess():
     np.savez_compressed(os.path.join(OUT, "postprocess_cases.npz"), **out)
 
 
+def gen_detect_edges():
+    """Detection post-processing by the reference's own loop (test.py:156-218) where the order of the rows matters: scores
+    on five levels, so that exact ties fall across classes and within a class, at and away from the top-k cut; the lowest
+    level equal to conf_thresh (not strictly greater: dropped); a degenerate box in two clips (valid_tubes replaces it by
+    the 400x400 default box); an empty clip.  Boxes of a clip lie in distinct grid cells, so that no NMS decision depends
+    on how torch.sort orders tied scores, except one near-duplicate pair with distinct scores (suppressed).  Rows carry 4
+    significant digits; the boxes differ at that precision, so the row order identifies the tubes."""
+    rs = np.random.RandomState(13)
+    out = {}
+    nums, ncls, T_ = [10, 0, 7, 1], 6, 3
+    n = sum(nums)
+    cell = np.concatenate([np.arange(nums[0]), np.arange(nums[2]), np.arange(nums[3])])
+    x1 = (cell % 5) * 44.0 + rs.uniform(0, 4, n)
+    y1 = (cell // 5) * 44.0 + rs.uniform(0, 4, n)
+    box = np.stack([x1, y1, x1 + rs.uniform(30, 38, n), y1 + rs.uniform(30, 38, n)], 1)
+    loc = (box[:, None, :] + rs.uniform(-3, 3, (n, T_, 4))).astype(np.float32)
+    loc[:, T_ // 2] = box
+    loc[4, :, 2] = loc[4, :, 0] + 1.0              # degenerate (clip 0)
+    loc[12, :, 3] = loc[12, :, 1]                  # degenerate (clip 2)
+    loc[1] = loc[0] + 1.0                          # near-duplicate of tube 0
+    levels = np.float32([0.2, 0.25, 0.5, 0.75, 0.875])
+    prob = levels[rs.randint(0, 5, (n, ncls))]
+    prob[1] = prob[0] * np.float32(0.75)          # distinct from tube 0's scores in every class
+    for name, topk in (("ties", 0), ("ties_topk", 7), ("ties_topk_all", 100)):
+        hist = [{"pred_prob": T(prob[:, None, :].repeat(T_, 1).copy()), "pred_loc": T(loc.copy()), "tubes_nums": list(nums)}]
+        dets = run_reference_eval_loop(hist, len(nums), ncls, 0.2, 0.4, topk, 224, 224)[0]
+        out[name + "_prob"], out[name + "_loc"], out[name + "_nums"] = prob, loc, np.asarray(nums)
+        out[name + "_cfg"] = np.asarray([0.2, 0.4, topk, 224, 224], np.float64)
+        rows = [(b, c, s) + tuple(bx) for b, d in enumerate(dets) for (bx, c, s) in d]
+        out[name + "_rows"] = np.asarray(rows, np.float64).reshape(-1, 7)
+        print("detect edges", name, "detections per clip:", [len(d) for d in dets])
+    np.savez_compressed(os.path.join(OUT, "detect_edge_cases.npz"), **out)
+
+
 def gen_roi_cross():
     """ROIPool forward/backward and ROIAlign backward have no CPU implementation in the reference
     (csrc/ROIPool.h:47, ROIAlign.h:66 raise on CPU tensors) -> cross-checked against torchvision 0.26's CPU ops,
@@ -402,8 +436,8 @@ def gen_roi_cross():
 
 if __name__ == "__main__":
     which = sys.argv[1:] or ["nms", "roi_align", "tubes", "pipelines", "losses", "head_grads", "trunk_grads", "c4", "c2",
-                             "postprocess", "roi_cross"]
+                             "postprocess", "detect_edges", "roi_cross"]
     for w_ in which:
         {"nms": gen_nms, "roi_align": gen_roi_align, "tubes": gen_tubes, "pipelines": gen_pipelines, "losses": gen_losses,
          "head_grads": gen_head_grads, "trunk_grads": gen_trunk_grads, "c4": gen_c4, "c2": gen_c2,
-         "postprocess": gen_postprocess, "roi_cross": gen_roi_cross}[w_]()
+         "postprocess": gen_postprocess, "detect_edges": gen_detect_edges, "roi_cross": gen_roi_cross}[w_]()

@@ -260,6 +260,140 @@ def test_detect_matches_reference_loop_rows(golden, name):
     assert rows == ref            # same detections in the same (file) order
 
 
+@pytest.mark.parametrize("name", ["ties", "ties_topk", "ties_topk_all"])
+def test_detect_row_order_with_ties_matches_reference_loop(golden, name):
+    """step_detect_f32 against the rows the reference's own loop wrote (make_golden.py::gen_detect_edges): exact score ties
+    across and within classes, at and away from the top-k cut, scores equal to conf_thresh, degenerate boxes, an empty
+    clip.  Same rows in the same order."""
+    from step_b200 import postprocess as pp
+    g = golden("detect_edge_cases")
+    conf, thr, topk, width, height = g[name + "_cfg"].tolist()
+    prob, loc, nums = g[name + "_prob"], g[name + "_loc"], g[name + "_nums"].tolist()
+    det = pp.detect(cu(prob), cu(loc), nums, conf, thr, width, height, topk=int(topk))
+    fmt = lambda v: float("{:.4}".format(float(v)))
+    rows = [(b, c) + tuple(fmt(v) for v in (s,) + tuple(bx)) for b, d in enumerate(pp.to_lists(det)) for (bx, c, s) in d]
+    ref = [(int(r[0]), int(r[1])) + tuple(fmt(v) for v in r[2:7]) for r in g[name + "_rows"]]
+    assert rows == ref
+
+
+def _oracle_rows(prob, box, nums, conf, thr, topk):
+    """The corrected oracle's detections per clip as float32 [k, 8] rows laid out as step_detect_f32's det."""
+    from oracle import postprocess as opp
+    ref = opp.detections(prob, box, nums, conf, thr, 224.0, 224.0, topk=topk, with_tube=True)
+    return [np.asarray([list(b) + [s, c, t, 0.0] for b, c, s, t in d], np.float32).reshape(-1, 8) for d in ref]
+
+
+def _device_rows(det, b):
+    return det["det"][b, :int(det["count"][b])].cpu().numpy()
+
+
+def _same_rows(got, ref, what):
+    """The same (class, tube) rows in the same order, scores and normalised boxes bit-equal as float32."""
+    assert got.shape == ref.shape, (what, got.shape, ref.shape)
+    if not np.array_equal(got.view(np.int32), ref.view(np.int32)):
+        i = int(np.nonzero((got.view(np.int32) != ref.view(np.int32)).any(1))[0][0])
+        raise AssertionError((what, "first differing row", i, got[i].tolist(), ref[i].tolist()))
+
+
+def _detect_case(nums, ncls, seed, overlap=None, levels=None):
+    """prob [R, T, ncls], loc [R, T, 4] and the centre-frame boxes [R, 4].  Boxes of the clips named in `overlap` are small
+    jitters of one box (NMS keeps few of them); the others lie in distinct cells of a 12 x 12 grid over 400 px (disjoint:
+    NMS keeps all).  Scores uniform, or drawn from `levels` (exact ties)."""
+    rs = np.random.RandomState(seed)
+    T = 3
+    boxes = []
+    for b, n in enumerate(nums):
+        if overlap and b in overlap:
+            x = rs.uniform(100, 104, (n, 2))
+            boxes.append(np.concatenate([x, x + rs.uniform(60, 64, (n, 2))], 1))
+        else:
+            cell = rs.permutation(144)[:n] if n <= 144 else np.arange(n) % 144
+            x = np.stack([cell % 12, cell // 12], 1) * 33.0 + rs.uniform(0, 3, (n, 2))
+            boxes.append(np.concatenate([x, x + rs.uniform(20, 28, (n, 2))], 1))
+    box = np.concatenate(boxes).astype(np.float32).reshape(-1, 4)
+    R_ = box.shape[0]
+    prob = rs.uniform(0, 1, (R_, ncls)).astype(np.float32) if levels is None else \
+        np.asarray(levels, np.float32)[rs.randint(0, len(levels), (R_, ncls))]
+    loc = (box[:, None, :] + rs.uniform(-2, 2, (R_, T, 4))).astype(np.float32)
+    loc[:, T // 2] = box
+    return np.ascontiguousarray(np.repeat(prob[:, None, :], T, 1)), loc, box
+
+
+@pytest.mark.parametrize("topk", [0, 50])
+def test_detect_at_scale_matches_corrected_oracle(topk):
+    """Clips of 0, 1, 129 and 1024 tubes with 60 classes and a low conf_thresh (the 129-tube clip wraps the 128 threads
+    of the rank and NMS loops; the 1024-tube clip is the per-(clip, class) limit, its boxes heavily overlapping so that NMS
+    keeps few): the kept (class, tube) rows, scores and boxes bit-equal to the corrected oracle, in its order."""
+    from step_b200 import postprocess as pp
+    nums = [0, 1, 129, 1024]
+    prob, loc, box = _detect_case(nums, 60, 61, overlap={3})
+    det = pp.detect(cu(prob), cu(loc), nums, 0.05, 0.4, 224.0, 224.0, topk=topk)
+    ref = _oracle_rows(prob[:, 1], box, nums, 0.05, 0.4, topk)
+    for b in range(len(nums)):
+        _same_rows(_device_rows(det, b), ref[b], ("clip", b, nums[b], topk))
+    kept = det["keep"].cpu().numpy()
+    assert 0 < int(kept[(129 + 1) * 60:].sum()) < 60 * 20                  # the 1024-tube clip: NMS keeps few
+
+
+@pytest.mark.parametrize("topk", [0, 3000])
+def test_detect_select_in_global_memory_matches_corrected_oracle(topk):
+    """A clip of 140 tubes with disjoint boxes and every score above conf_thresh: 8400 survivors, more than the 4096 the
+    select kernel ranks in shared memory, so it ranks against global memory.  Scores on three levels: the top-k cut falls
+    inside a run of ties, which come out in reverse file order.  A 5-tube clip before it takes the shared-memory path."""
+    from step_b200 import postprocess as pp
+    nums = [5, 140]
+    prob, loc, box = _detect_case(nums, 60, 62, levels=[0.25, 0.5, 0.75])
+    det = pp.detect(cu(prob), cu(loc), nums, 0.1, 0.4, 224.0, 224.0, topk=topk)
+    survivors = int(det["keep"][5 * 60:].sum())
+    print("\nglobal-memory select: %d survivors" % survivors)
+    assert survivors == 140 * 60 > 4096
+    ref = _oracle_rows(prob[:, 1], box, nums, 0.1, 0.4, topk)
+    for b in range(len(nums)):
+        _same_rows(_device_rows(det, b), ref[b], ("clip", b, topk))
+    if topk:
+        full = _oracle_rows(prob[:, 1], box, nums, 0.1, 0.4, 10 ** 6)[1]
+        assert full[topk - 1, 4] == full[topk, 4]                          # the cut splits a run of ties
+
+
+@pytest.mark.parametrize("topk", [0, 3000])
+def test_detect_cap_truncates_both_select_paths(topk):
+    """An output of `cap` rows per clip keeps the first cap rows of the full result and counts min(rows, cap), in the
+    shared-memory (5 tubes) and the global-memory (140 tubes) select paths."""
+    from step_b200 import postprocess as pp
+    nums = [5, 140]
+    prob, loc, box = _detect_case(nums, 60, 63, levels=[0.25, 0.5, 0.75])
+    full = pp.detect(cu(prob), cu(loc), nums, 0.1, 0.4, 224.0, 224.0, topk=topk)
+    for cap in (7, 1000):
+        d = pp.Detector(nums, 60, torch.device("cuda"), 0.1, 0.4, 224.0, 224.0, topk)
+        d.cap = cap
+        d.det = torch.full((len(nums), cap, 8), -1.0, device="cuda")
+        got = d.run(cu(prob), cu(loc))
+        for b in range(len(nums)):
+            want = _device_rows(full, b)[:cap]
+            assert int(got["count"][b]) == want.shape[0], (cap, b)
+            _same_rows(_device_rows(got, b), want, ("cap", cap, b, topk))
+    assert int(full["count"][0]) < 1000 < int(full["count"][1])
+
+
+def test_detect_rejects_a_clip_over_1024_tubes_before_any_launch():
+    """1025 tubes in one clip exceed the per-(clip, class) NMS problem: Detector raises, and so does the C entry when
+    asked directly, and nothing is launched."""
+    from step_b200 import _lib as L
+    from step_b200 import postprocess as pp
+    assert L.lib().step_nms_segmented_max_rows() == 1024
+    nums = [3, 1025]
+    prob, loc, _ = _detect_case(nums, 4, 64, overlap={1})
+    before = L.launch_count()
+    with pytest.raises(RuntimeError, match="1025 tubes"):
+        pp.detect(cu(prob), cu(loc), nums, 0.1, 0.4, 224.0, 224.0)
+    d = pp.Detector([3, 1024], 4, torch.device("cuda"), 0.1, 0.4, 224.0, 224.0)
+    d.max_n = 1025
+    with pytest.raises(RuntimeError, match="1025 tubes in one clip"):
+        d.run(cu(prob[:1027]), cu(loc[:1027]))
+    torch.cuda.synchronize()
+    assert L.launch_count() == before
+
+
 def test_roi_pool_and_align_backward_match_torchvision(golden):
     """The device ROIPool fwd/bwd and ROIAlign bwd against torchvision's CPU ops (the reference has no CPU
     implementation of them; see tests/golden/make_golden.py::gen_roi_cross)."""

@@ -231,6 +231,36 @@ def test_postprocess_oracle_matches_reference_loop(golden, name):
     assert _det_key(rows) == _det_key(ref)
 
 
+def _rows4(rows):
+    """Detection rows (clip, class, score, box) as the reference writes them, 4 significant digits ('{:.4}'), in order."""
+    fmt = lambda v: float("{:.4}".format(float(v)))
+    return [(int(r[0]), int(r[1])) + tuple(fmt(v) for v in r[2:7]) for r in rows]
+
+
+@pytest.mark.parametrize("name", ["ties", "ties_topk", "ties_topk_all"])
+def test_postprocess_oracle_row_order_matches_reference_loop(golden, name):
+    """oracle/postprocess.py writes the same rows in the same order as the reference's own loop
+    (tests/golden/make_golden.py::gen_detect_edges) on scores with exact ties across and within classes, at the top-k cut
+    and away from it, scores equal to conf_thresh and degenerate boxes: file order for topk 0, tied scores in reverse file
+    order under a top-k sort."""
+    from oracle import postprocess as opp
+    g = golden("detect_edge_cases")
+    conf, thr, topk, width, height = g[name + "_cfg"].tolist()
+    prob, loc, nums = g[name + "_prob"], g[name + "_loc"], g[name + "_nums"].tolist()
+    dets = opp.detections(prob, loc[:, loc.shape[1] // 2].copy(), nums, conf, thr, width, height, topk=int(topk))
+    rows = [(b, c, s) + tuple(bx) for b, d in enumerate(dets) for (bx, c, s) in d]
+    ref = g[name + "_rows"]
+    assert _rows4(rows) == _rows4(ref)
+    # the case exercises what it is for: tied scores next to each other in the output, and at the cut
+    s = ref[:, 2]
+    assert bool((s[1:] == s[:-1]).any())
+    assert not bool((prob == np.float32(conf)).all()) and bool((prob == np.float32(conf)).any())
+    if name == "ties_topk":
+        full = opp.detections(prob, loc[:, loc.shape[1] // 2].copy(), nums, conf, thr, width, height, topk=10 ** 6)
+        cut = [d for d in full if len(d) > int(topk)]
+        assert cut and all(d[int(topk) - 1][2] == d[int(topk)][2] for d in cut)      # the cut splits a run of ties
+
+
 def test_roi_pool_and_align_backward_match_torchvision(golden):
     """ROIPool fwd/bwd and ROIAlign bwd have no CPU implementation in the reference (ROIPool.h:47, ROIAlign.h:66), so
     the C restatement (cuda/ROIPool_cuda.cu:40-132, cuda/ROIAlign_cuda.cu:201-278) is cross-checked against

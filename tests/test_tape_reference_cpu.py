@@ -671,6 +671,96 @@ def test_roi_align_bwd_check_rejects_perturbed_references():
             R.roi_align_bwd_check(got, init, r_, m_, n_, what)
 
 
+def _roi_fma_chain(feat, rois, groups, nbins):
+    """What the fp16 ROIAlign with fp32 FMAs computes (csrc/roi.cu: roi_align_fwd_nhwc_kernel<__half, false> and the
+    direct form of the packed kernel), restated on the CPU: fp32 weights w * fp32(1 / count), one fp32 rounding per tap
+    added in (bin, iy, ix, tap) order, an fp16 store.  fp16 [R, nbins, C]."""
+    K, H, W, C = feat.shape
+    f = feat.reshape(K, H * W, C).double()
+    fr = R.roi_frames(rois)
+    out = torch.zeros(rois.shape[0], nbins, C, dtype=torch.float16)
+    for gr in groups:
+        G = gr["idx"].numel()
+        ic = torch.tensor(1.0, dtype=torch.float32) / gr["count"]
+        live = gr["pix"] >= 0
+        w = torch.where(live, gr["w"].float() * ic, torch.zeros(())).double().view(G, nbins, -1)
+        v = f[fr[gr["idx"]].view(-1, 1), gr["pix"].clamp(min=0)].view(G, nbins, -1, C)
+        acc = torch.zeros(G, nbins, C, dtype=torch.float32)
+        for k in range(w.shape[-1]):
+            acc = (acc.double() + w[..., k, None] * v[..., k, :]).float()
+        out[gr["idx"]] = acc.half()
+    return out
+
+
+@pytest.mark.parametrize("sr", [0, 3])
+def test_roi_align_fma_tol_accepts_the_fma_chain_and_rejects_perturbed_references(sr):
+    """The fp32-FMA ROIAlign restated on the CPU is within roi_align_fma_tol of the float64 reference on the edge ROIs;
+    the bound rejects the reference scaled by 1 + 2^-10, with the 1/count dropped, and with one tap of a clamped sample
+    moved by a pixel."""
+    gen = torch.Generator().manual_seed(25 + sr)
+    feat, rois = _edge_case(gen)
+    K, H, W, C = feat.shape
+    groups = R.roi_align_terms(rois, 1.0 / 16.0, 7, 7, H, W, sr)
+    ref, out_abs = R.roi_align(feat, rois, 1.0 / 16.0, 7, 7, sampling_ratio=sr)
+    tol = R.roi_align_fma_tol(out_abs, R.roi_samples_per_bin(groups, rois.shape[0]))
+    got = _roi_fma_chain(feat, rois, groups, 49).view_as(ref)
+    assert R._check_within(got, ref, tol, ("fma chain", sr)) < 1.0
+    no_count = [dict(gr, count=1) for gr in groups]
+    assert any(gr["count"] > 1 for gr in groups)
+    shifted, moved = _shift_clamped_tap(groups, H, W)
+    assert moved
+    bad = {"scaled": ref * (1.0 + 2.0 ** -10),
+           "1/count dropped": R.roi_align(feat, rois, 1.0 / 16.0, 7, 7, groups=no_count)[0],
+           "clamped tap moved": R.roi_align(feat, rois, 1.0 / 16.0, 7, 7, groups=shifted)[0]}
+    for what, r_ in bad.items():
+        with pytest.raises(AssertionError):
+            R._check_within(got, r_, tol, what)
+
+
+def _packed_table_terms(groups, nbins):
+    """roi_align_terms' groups with every tap of a bin whose pixel is not among the bin's first ROI_MERGED distinct pixels,
+    in (iy, ix, tap) order, zeroed: what a merged table that silently drops pixels past its capacity would sum."""
+    out = []
+    for gr in groups:
+        G = gr["idx"].numel()
+        pix = gr["pix"].view(G, nbins, -1)
+        w = gr["w"].clone().view_as(pix)
+        for g in range(G):
+            for b in range(nbins):
+                seen = set()
+                for k, p in enumerate(pix[g, b].tolist()):
+                    if p < 0 or p in seen:
+                        continue
+                    if len(seen) < R.ROI_MERGED:
+                        seen.add(p)
+                    else:
+                        w[g, b, k] = 0.0
+        out.append(dict(gr, w=w.view_as(gr["w"])))
+    return out
+
+
+def test_roi_align_tol_rejects_a_bin_with_pixels_past_the_table_dropped():
+    """sampling_ratio 3 with 10-pixel bins (a 70 px ROI inside an 80 x 80 map, at 7 x 7): a bin's 9 samples touch 36
+    distinct pixels.  roi_align_tol rejects the sum over the first 16 alone (the 17th..36th pixel dropped); at
+    sampling_ratio 2 no bin exceeds 16 pixels and nothing is dropped."""
+    gen = torch.Generator().manual_seed(27)
+    H = W = 80
+    feat = (0.5 + 0.5 * torch.rand(1, H, W, 8, generator=gen)).half()
+    rois = torch.tensor([[0, 80.0, 80.0, 1200.0, 1200.0]], dtype=torch.float32)
+    vmax = float(feat.abs().max())
+    for sr, most in ((3, 36), (2, 16)):
+        groups = R.roi_align_terms(rois, 1.0 / 16.0, 7, 7, H, W, sr)
+        assert max(int(R.roi_distinct_pixels(gr, 49).max()) for gr in groups) == most
+        ref, out_abs = R.roi_align(feat, rois, 1.0 / 16.0, 7, 7, sampling_ratio=sr)
+        packed, _ = R.roi_align(feat, rois, 1.0 / 16.0, 7, 7, groups=_packed_table_terms(groups, 49))
+        tol = R.roi_align_tol(out_abs, vmax)
+        if most > R.ROI_MERGED:
+            with pytest.raises(AssertionError):
+                R._check_within(packed, ref, tol, "17th..36th pixel dropped")
+        else:
+            assert torch.equal(packed, ref)
+
+
 @pytest.mark.parametrize("xdtype", [torch.float16, torch.float32])
 def test_linear_bwd_matches_autograd_and_its_check_rejects_perturbations(xdtype):
     """linear_bwd's dx / dW / db equal float64 autograd of x w^T + b (dx accumulated onto init_dx); linear_bwd_check
