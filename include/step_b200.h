@@ -422,6 +422,47 @@ int step_multi_tensor_adam_f32(const step_optim_tensor* table, int n_tensors, co
 int step_multi_tensor_sgd_f32(const step_optim_tensor* table, int n_tensors, const step_optim_block* blocks, int n_blocks,
                               step_stream_t stream);
 
+/* ---- training-sample selection (select.cu): train_select, utils/utils.py:135-423, one refinement step per call ---- */
+enum { STEP_SAMPLING_UNIFORM = 0, STEP_SAMPLING_RANDOM = 1, STEP_SAMPLING_SOFTMAX = 2 };
+typedef struct {
+  int step;                  /* 1-based refinement step; step 1 selects from the proposals, later steps from the history */
+  int B;                     /* clips */
+  int C;                     /* classes */
+  int L;                     /* frames of the candidates (the proposals at step 1, the history's pred_loc after) */
+  int T;                     /* frames per chunk */
+  int Lout;                  /* frames of the selected tubes: L, or L + 2T when ext_mode extends them */
+  int ext_mode;              /* STEP_EXT_*: how the selected tubes grow by one chunk on each side (utils.py:283-312) */
+  int max_chunks;            /* chunks of the targets */
+  int gt_mid;                /* chunk of the targets the IoU and the centre target use */
+  int predict_nb;            /* write the neighbour targets of chunks nb_first / nb_last (utils.py:319-331) */
+  int nb_first, nb_last;
+  int topk;                  /* <= 0: every tube is a candidate */
+  int max_pos, neg_ratio, sampling;
+  int max_rows;              /* output rows per clip, >= max_pos * (1 + neg_ratio) */
+  int n_max, g_max;          /* largest tube and ground-truth count of one clip */
+  int prop_f64;              /* step 1: the proposals are float64 (the IoU then rounds as numpy does for mixed types) */
+  float cls_thresh, reg_thresh, width, height;
+  long long prob_sr, prob_sl, prob_sc;  /* element strides of pred_prob [R, L, C] */
+  const int32_t* tube_off;   /* [B + 1] first tube of each clip */
+  const int32_t* gt_off;     /* [B + 1] first ground truth of each clip */
+  const float* prob;         /* step > 1 */
+  const float* loc;          /* step > 1: [R, L, 4] */
+  const float* first;        /* STEP_EXT_PREDICT: [R, T, 4] */
+  const float* last;
+  const double* props;       /* step 1: [R, L, 4] */
+  const float* targets;      /* [sum G, max_chunks, 4 + C] */
+  uint32_t* mt;              /* [2][625]: numpy's, then Python's MT19937 key with its position last; advanced in place */
+  float* out_tubes;          /* [B * max_rows, Lout, 5], rows packed clip after clip */
+  float* out_targets;        /* [B * max_rows, 3, 6 + C] */
+  int32_t* counts;           /* [B] rows of each clip */
+} step_select_params;
+/* One CTA walks the clips in order: candidates, IoU, positive assignment, the draws from the two generators, and the
+ * selected rows.  STEP_E_ARG before any launch when an argument is out of range. */
+int step_select_step_f32(const step_select_params* p, step_stream_t stream);
+/* The checks of step_select_step_f32 that need no pointer (every field, the shared memory the step needs), with no launch:
+ * a caller validates every step before it uploads or launches anything. */
+int step_select_check_f32(const step_select_params* p);
+
 #ifdef __cplusplus
 }
 #endif

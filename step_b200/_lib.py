@@ -124,6 +124,8 @@ def _declare(lib):
         "step_multi_tensor_sgd_f32": ([P, I, P, I, S], c_int),
         "step_frames_to_clip_u8": ([P, I, I, I, I, I, P, P, P, S], c_int),
         "step_frames_to_clip_aug_u8": ([P, P, P, P, I, I, I, I, I, P, P, P, S], c_int),
+        "step_select_step_f32": ([P, S], c_int),
+        "step_select_check_f32": ([P], c_int),
         "step_debug_tma_tile": ([ctypes.POINTER(ConvParams), I, I, I, I, I, P, P, P, S], c_int),
     }
     for name, (argtypes, restype) in sigs.items():

@@ -553,7 +553,7 @@ def step_frames(cfg, i):
 def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9, weight_decay=0.0, lambda_reg=5.0,
                lambda_neighbor=1.0, loss_scale=1024.0, sgd_state=None, world_size=1, optimizer=None, scaler=None):
     """One optimisation step of train.py:263-348 on the device, for already selected training samples
-    (`train_select`, utils/utils.py:135-423, is the host-side sampling of SURVEY.md section 8f rank 4 and is not built):
+    (`train_select`, utils/utils.py:135-423, is step_b200.select_samples, which returns step_tubes and step_targets):
         conv_feat = base_net(clips); context_feat = context_net(conv_feat) unless cfg.no_context      train.py:266-269
         for each refinement step i: T_start, T_length from cfg.NUM_CHUNKS / cfg.T / cfg.max_iter; ROI-pool the step's
             flat tubes from conv_feat[:, T_start:T_start+T_length]; run det_net[i-1] with targets and each tube's clip
