@@ -9,6 +9,7 @@
 // D2H copy and no host scan: ordering, the 64x64 bitmask tiles, the greedy resolve and the
 // compaction all run on the caller's stream.
 #include "common.cuh"
+#include "tube_math.cuh"
 
 namespace step {
 
@@ -120,71 +121,81 @@ __global__ void __launch_bounds__(1024) nms_resolve_kernel(const unsigned long l
   }
 }
 
-// ---- 4. compaction: kept original indices ascending (nms_cpu.cpp:88 nonzero(suppressed == 0))
-__global__ void __launch_bounds__(1024) nms_compact_kernel(const uint8_t* __restrict__ keep_flag, int n,
-                                                           int64_t* __restrict__ keep_out,
-                                                           int* __restrict__ n_keep) {
-  __shared__ int warp_tot[32];
+// Block-wide compaction in index order with a warp-ballot scan: calls emit(i, slot) for every i in [0, n) with flag(i)
+// nonzero, slot = the number of such i before it, and returns their count.  Called by the whole CTA of kWarps warps.
+template <int kWarps, class Flag, class Emit>
+__device__ __forceinline__ int ballot_compact(int n, Flag flag, Emit emit) {
+  __shared__ int warp_tot[kWarps];
   __shared__ int base_s;
   if (threadIdx.x == 0) base_s = 0;
   __syncthreads();
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   for (int start = 0; start < n; start += blockDim.x) {
-    int i = start + threadIdx.x;
-    int f = (i < n) ? keep_flag[i] : 0;
-    unsigned bal = __ballot_sync(0xffffffffu, f);
-    int within = __popc(bal & ((1u << lane) - 1));
+    const int i = start + threadIdx.x;
+    const int f = (i < n) ? flag(i) : 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, f);
     if (lane == 0) warp_tot[wid] = __popc(bal);
     __syncthreads();
     int off = base_s;
     for (int w = 0; w < wid; ++w) off += warp_tot[w];
-    if (f) keep_out[off + within] = i;
+    if (f) emit(i, off + __popc(bal & ((1u << lane) - 1)));
     __syncthreads();
     if (threadIdx.x == 0) {
       int t = 0;
-      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += warp_tot[w];
+      for (int w = 0; w < kWarps; ++w) t += warp_tot[w];
       base_s += t;
     }
     __syncthreads();
   }
-  if (threadIdx.x == 0) *n_keep = base_s;
+  return base_s;
 }
 
-// ---- segmented small-problem kernel: one CTA per (clip, class) segment, everything in smem.
+// ---- 4. compaction: kept original indices ascending (nms_cpu.cpp:88 nonzero(suppressed == 0))
+__global__ void __launch_bounds__(1024) nms_compact_kernel(const uint8_t* __restrict__ keep_flag, int n,
+                                                           int64_t* __restrict__ keep_out,
+                                                           int* __restrict__ n_keep) {
+  const int total = ballot_compact<32>(n, [&](int i) { return (int)keep_flag[i]; },
+                                       [&](int i, int slot) { keep_out[slot] = i; });
+  if (threadIdx.x == 0) *n_keep = total;
+}
+
+// ---- greedy NMS of one small problem in shared memory (nms_cpu.cpp:57-88), one CTA.  Rows i in [0, n) whose score
+//      passes the threshold are ranked (score descending, index ascending), then suppressed in rank order; the other rows
+//      are dropped.  The caller says how rows are read and where their keep flags go:
+//        score(i)    row i's score;
+//        pass(s)     whether a row of score s takes part;
+//        box(i, s)   row i's box, asked once for every row before its threshold test;
+//        keep(i, k)  stores row i's keep flag k.
 constexpr int kSegMax = 1024;
-__global__ void __launch_bounds__(256) nms_segmented_kernel(const float* __restrict__ boxes,
-                                                            const float* __restrict__ scores,
-                                                            const int* __restrict__ seg_offsets, float thr,
-                                                            int ge, float min_score,
-                                                            uint8_t* __restrict__ keep_mask) {
+template <class Score, class Pass, class Box, class Keep>
+__device__ __forceinline__ void greedy_nms_smem(int n, float thr, int ge, Score score, Pass pass, Box box, Keep keep) {
   __shared__ float4 sb[kSegMax];
   __shared__ float sa[kSegMax];
   __shared__ float ss[kSegMax];
   __shared__ short sorig[kSegMax];
   __shared__ uint8_t sup[kSegMax];
   __shared__ int m_s;
-  const int beg = seg_offsets[blockIdx.x], n = seg_offsets[blockIdx.x + 1] - beg;
   if (n <= 0) return;
-  if (n > kSegMax) __trap();   // callers check step_nms_segmented_max_rows(); never overrun shared memory
+  // the host bounds n (step_nms_segmented_max_rows(), step_detect_f32's max_per_clip); never overrun shared memory
+  if (n > kSegMax) __trap();
   if (threadIdx.x == 0) m_s = 0;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) ss[i] = scores[beg + i];
+  for (int i = threadIdx.x; i < n; i += blockDim.x) ss[i] = score(i);
   __syncthreads();
-  // rank among rows passing the confidence threshold (test.py:183); others are dropped
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    float si = ss[i];
-    if (si >= min_score) {
+    const float si = ss[i];
+    const float4 b = box(i, si);
+    if (pass(si)) {
       int rank = 0;
       for (int t = 0; t < n; ++t) {
-        float st = ss[t];
-        rank += (st >= min_score) && ((st > si) || (st == si && t < i));
+        const float st = ss[t];
+        rank += pass(st) && ((st > si) || (st == si && t < i));
       }
-      float4 b = reinterpret_cast<const float4*>(boxes)[beg + i];
       sb[rank] = b;
       sa[rank] = box_area(b);
       sorig[rank] = (short)i;
       atomicAdd(&m_s, 1);
     } else {
-      keep_mask[beg + i] = 0;
+      keep(i, 0);
     }
   }
   __syncthreads();
@@ -193,14 +204,28 @@ __global__ void __launch_bounds__(256) nms_segmented_kernel(const float* __restr
   __syncthreads();
   for (int i = 0; i < m; ++i) {
     if (!sup[i]) {  // uniform across the CTA (smem, synced)
-      float4 a = sb[i];
-      float aa = sa[i];
+      const float4 a = sb[i];
+      const float aa = sa[i];
       for (int j = i + 1 + threadIdx.x; j < m; j += blockDim.x)
         if (!sup[j] && suppresses(a, aa, sb[j], sa[j], thr, ge)) sup[j] = 1;
     }
     __syncthreads();
   }
-  for (int i = threadIdx.x; i < m; i += blockDim.x) keep_mask[beg + sorig[i]] = sup[i] ? 0 : 1;
+  for (int i = threadIdx.x; i < m; i += blockDim.x) keep(sorig[i], sup[i] ? 0 : 1);
+}
+
+// ---- segmented small-problem kernel: one CTA per (clip, class) segment.
+__global__ void __launch_bounds__(256) nms_segmented_kernel(const float* __restrict__ boxes,
+                                                            const float* __restrict__ scores,
+                                                            const int* __restrict__ seg_offsets, float thr,
+                                                            int ge, float min_score,
+                                                            uint8_t* __restrict__ keep_mask) {
+  const int beg = seg_offsets[blockIdx.x], n = seg_offsets[blockIdx.x + 1] - beg;
+  greedy_nms_smem(
+      n, thr, ge, [&](int i) { return scores[beg + i]; },
+      [&](float s) { return s >= min_score; },   // the confidence threshold of test.py:183
+      [&](int i, float) { return reinterpret_cast<const float4*>(boxes)[beg + i]; },
+      [&](int i, uint8_t k) { keep_mask[beg + i] = k; });
 }
 
 
@@ -214,68 +239,25 @@ __global__ void __launch_bounds__(256) nms_segmented_kernel(const float* __restr
 //   detect_select_kernel  one CTA per clip: orders the kept candidates as the reference does -- file order (class, tube)
 //                         when topk <= 0, else the tuple sort of test.py:205-208, (score, class, j) descending, cut at
 //                         topk -- and writes them compactly: det[clip][rank] = {x1, y1, x2, y2, score, class, tube, 0}.
-__device__ __forceinline__ float4 valid_box(float4 b, float width, float height) {
-  // tube_utils.py:72-88 (same arithmetic as tubes.cu::valid_one)
-  b.x = fmaxf(0.0f, b.x); b.y = fmaxf(0.0f, b.y);
-  b.z = fminf(width, b.z); b.w = fminf(height, b.w);
-  if (!(b.x < __fsub_rn(b.z, 2.0f) && b.y < __fsub_rn(b.w, 2.0f))) { b.x = 0.0f; b.y = 0.0f; b.z = width; b.w = height; }
-  return b;
-}
-
 __global__ void __launch_bounds__(128) detect_nms_kernel(const float* __restrict__ prob, int prob_ld,
                                                          const float* __restrict__ loc, int loc_ld,
                                                          const int* __restrict__ clip_offsets, int ncls, float conf,
                                                          float thr, int ge, float vw, float vh, float nw, float nh,
                                                          uint8_t* __restrict__ keep, float* __restrict__ score_out,
                                                          float4* __restrict__ box_out) {
-  __shared__ float4 sb[kSegMax];
-  __shared__ float sa[kSegMax];
-  __shared__ float ss[kSegMax];
-  __shared__ short sorig[kSegMax];
-  __shared__ uint8_t sup[kSegMax];
-  __shared__ int m_s;
   const int clip = blockIdx.x / ncls, c = blockIdx.x - clip * ncls;
   const int beg = clip_offsets[clip], n = clip_offsets[clip + 1] - beg;
-  if (n <= 0) return;
-  if (n > kSegMax) __trap();   // the host checks this bound (step_detect_f32: max_per_clip); never overrun shared memory
   const size_t cand0 = (size_t)beg * ncls + (size_t)c * n;
-  if (threadIdx.x == 0) m_s = 0;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) ss[i] = prob[(size_t)(beg + i) * prob_ld + c];
-  __syncthreads();
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const float si = ss[i];
-    const float* lp = loc + (size_t)(beg + i) * loc_ld;
-    const float4 b = valid_box(make_float4(lp[0], lp[1], lp[2], lp[3]), vw, vh);   // test.py:191
-    score_out[cand0 + i] = si;
-    box_out[cand0 + i] = make_float4(__fdiv_rn(b.x, nw), __fdiv_rn(b.y, nh), __fdiv_rn(b.z, nw), __fdiv_rn(b.w, nh));  // test.py:197-198
-    if (si > conf) {                                                                // test.py:183 scores.gt(conf)
-      int rank = 0;
-      for (int t = 0; t < n; ++t) {
-        const float st = ss[t];
-        rank += (st > conf) && ((st > si) || (st == si && t < i));
-      }
-      sb[rank] = b;
-      sa[rank] = box_area(b);
-      sorig[rank] = (short)i;
-      atomicAdd(&m_s, 1);
-    } else {
-      keep[cand0 + i] = 0;
-    }
-  }
-  __syncthreads();
-  const int m = m_s;
-  for (int i = threadIdx.x; i < m; i += blockDim.x) sup[i] = 0;
-  __syncthreads();
-  for (int i = 0; i < m; ++i) {
-    if (!sup[i]) {
-      const float4 a = sb[i];
-      const float aa = sa[i];
-      for (int j = i + 1 + threadIdx.x; j < m; j += blockDim.x)
-        if (!sup[j] && suppresses(a, aa, sb[j], sa[j], thr, ge)) sup[j] = 1;
-    }
-    __syncthreads();
-  }
-  for (int i = threadIdx.x; i < m; i += blockDim.x) keep[cand0 + sorig[i]] = sup[i] ? 0 : 1;
+  greedy_nms_smem(
+      n, thr, ge, [&](int i) { return prob[(size_t)(beg + i) * prob_ld + c]; },
+      [&](float s) { return s > conf; },   // test.py:183 scores.gt(conf)
+      [&](int i, float s) {
+        const float4 b = valid_one(ld4(loc + (size_t)(beg + i) * loc_ld), vw, vh);   // test.py:191
+        score_out[cand0 + i] = s;
+        box_out[cand0 + i] = make_float4(__fdiv_rn(b.x, nw), __fdiv_rn(b.y, nh), __fdiv_rn(b.z, nw), __fdiv_rn(b.w, nh));  // test.py:197-198
+        return b;
+      },
+      [&](int i, uint8_t k) { keep[cand0 + i] = k; });
 }
 
 // One CTA per clip.  Pass 1 compacts the kept candidates in candidate order (= the reference's file order: class, tube)
@@ -288,35 +270,14 @@ __global__ void __launch_bounds__(256) detect_select_kernel(const uint8_t* __res
                                                             int cap, float* __restrict__ det, int* __restrict__ det_count) {
   __shared__ float s_score[kSelMax];
   __shared__ int s_idx[kSelMax];
-  __shared__ int warp_tot[8];
-  __shared__ int base_s;
   const int clip = blockIdx.x;
   const int beg = clip_offsets[clip], n = clip_offsets[clip + 1] - beg;
   const int cands = n * ncls;
   const size_t cand0 = (size_t)beg * ncls;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (threadIdx.x == 0) base_s = 0;
-  __syncthreads();
   // ---- pass 1: kept candidates, ascending candidate index -> slot (prefix count)
-  for (int start = 0; start < cands; start += blockDim.x) {
-    const int i = start + threadIdx.x;
-    const int f = (i < cands) ? keep[cand0 + i] : 0;
-    const unsigned bal = __ballot_sync(0xffffffffu, f);
-    if (lane == 0) warp_tot[wid] = __popc(bal);
-    __syncthreads();
-    int off = base_s;
-    for (int w = 0; w < wid; ++w) off += warp_tot[w];
-    const int slot = off + __popc(bal & ((1u << lane) - 1));
-    if (f && slot < kSelMax) { s_idx[slot] = i; s_score[slot] = score[cand0 + i]; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int t = 0;
-      for (int w = 0; w < 8; ++w) t += warp_tot[w];
-      base_s += t;
-    }
-    __syncthreads();
-  }
-  const int m = base_s;
+  const int m = ballot_compact<8>(cands, [&](int i) { return (int)keep[cand0 + i]; }, [&](int i, int slot) {
+    if (slot < kSelMax) { s_idx[slot] = i; s_score[slot] = score[cand0 + i]; }
+  });
   const bool in_smem = m <= kSelMax;
   auto emit = [&](int i, float si, int rank) {
     if (rank >= cap) return;

@@ -1,4 +1,5 @@
-// tube_math.cuh -- per-box tube arithmetic shared by tubes.cu (the inference loop) and select.cu (train_select).
+// tube_math.cuh -- per-box tube arithmetic of utils/tube_utils.py shared by tubes.cu (the inference loop), select.cu
+// (train_select), train.cu (the regression targets of the losses) and nms.cu (the detection boxes).
 #pragma once
 #include "common.cuh"
 
@@ -14,6 +15,40 @@ __device__ __forceinline__ float4 valid_one(float4 b, float width, float height)
 
 __device__ __forceinline__ float4 ld4(const float* p) { return make_float4(p[0], p[1], p[2], p[3]); }
 __device__ __forceinline__ void st4(float* p, float4 v) { p[0] = v.x; p[1] = v.y; p[2] = v.z; p[3] = v.w; }
+
+struct CS { float x, y, w, h; };
+
+__device__ __forceinline__ CS center_size(float x1, float y1, float x2, float y2) {
+  // tube_utils.py:136-139
+  CS c;
+  c.w = __fadd_rn(__fsub_rn(x2, x1), 1.0f);
+  c.h = __fadd_rn(__fsub_rn(y2, y1), 1.0f);
+  c.x = __fadd_rn(x1, __fmul_rn(0.5f, c.w));
+  c.y = __fadd_rn(y1, __fmul_rn(0.5f, c.h));
+  return c;
+}
+
+__device__ __forceinline__ float4 decode_one(float4 a, float4 d) {
+  // tube_utils.py:176-187
+  CS c = center_size(a.x, a.y, a.z, a.w);
+  float px = __fadd_rn(__fmul_rn(c.w, d.x), c.x);
+  float py = __fadd_rn(__fmul_rn(c.h, d.y), c.y);
+  float pw = __fmul_rn(c.w, expf(d.z));
+  float ph = __fmul_rn(c.h, expf(d.w));
+  float4 o;
+  o.x = __fsub_rn(px, __fmul_rn(0.5f, pw));
+  o.y = __fsub_rn(py, __fmul_rn(0.5f, ph));
+  o.z = __fsub_rn(__fadd_rn(px, __fmul_rn(0.5f, pw)), 1.0f);
+  o.w = __fsub_rn(__fadd_rn(py, __fmul_rn(0.5f, ph)), 1.0f);
+  return o;
+}
+
+__device__ __forceinline__ float4 encode_one(float4 g, float4 a) {
+  // tube_utils.py:143-163 encode_coef(gt, anchor) -> (dx, dy, dw, dh)
+  CS cg = center_size(g.x, g.y, g.z, g.w), ca = center_size(a.x, a.y, a.z, a.w);
+  return make_float4(__fdiv_rn(__fsub_rn(cg.x, ca.x), ca.w), __fdiv_rn(__fsub_rn(cg.y, ca.y), ca.h),
+                     logf(__fdiv_rn(cg.w, ca.w)), logf(__fdiv_rn(cg.h, ca.h)));
+}
 
 // linear recurrence of tube_utils.py:18-20; coefficients are Python doubles multiplied into fp32
 // arrays (numpy casts the python scalar to fp32 first), so a = fl32(T/(T-1)), b = fl32(1/(T-1)).

@@ -11,33 +11,6 @@
 
 namespace step {
 
-struct CS { float x, y, w, h; };
-
-__device__ __forceinline__ CS center_size(float x1, float y1, float x2, float y2) {
-  // tube_utils.py:136-139
-  CS c;
-  c.w = __fadd_rn(__fsub_rn(x2, x1), 1.0f);
-  c.h = __fadd_rn(__fsub_rn(y2, y1), 1.0f);
-  c.x = __fadd_rn(x1, __fmul_rn(0.5f, c.w));
-  c.y = __fadd_rn(y1, __fmul_rn(0.5f, c.h));
-  return c;
-}
-
-__device__ __forceinline__ float4 decode_one(float4 a, float4 d) {
-  // tube_utils.py:176-187
-  CS c = center_size(a.x, a.y, a.z, a.w);
-  float px = __fadd_rn(__fmul_rn(c.w, d.x), c.x);
-  float py = __fadd_rn(__fmul_rn(c.h, d.y), c.y);
-  float pw = __fmul_rn(c.w, expf(d.z));
-  float ph = __fmul_rn(c.h, expf(d.w));
-  float4 o;
-  o.x = __fsub_rn(px, __fmul_rn(0.5f, pw));
-  o.y = __fsub_rn(py, __fmul_rn(0.5f, ph));
-  o.z = __fsub_rn(__fadd_rn(px, __fmul_rn(0.5f, pw)), 1.0f);
-  o.w = __fsub_rn(__fadd_rn(py, __fmul_rn(0.5f, ph)), 1.0f);
-  return o;
-}
-
 __global__ void tube_decode_kernel(const float* __restrict__ anchors, int astride, const float* __restrict__ deltas,
                                    int n, float* __restrict__ out) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -48,11 +21,7 @@ __global__ void tube_encode_kernel(const float* __restrict__ gt, const float* __
                                    float* __restrict__ out) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  float4 g = ld4(gt + 4 * (size_t)i), a = ld4(anchors + (size_t)i * astride);
-  CS cg = center_size(g.x, g.y, g.z, g.w), ca = center_size(a.x, a.y, a.z, a.w);
-  // tube_utils.py:158-161
-  st4(out + 4 * (size_t)i, make_float4(__fdiv_rn(__fsub_rn(cg.x, ca.x), ca.w), __fdiv_rn(__fsub_rn(cg.y, ca.y), ca.h),
-                                       logf(__fdiv_rn(cg.w, ca.w)), logf(__fdiv_rn(cg.h, ca.h))));
+  st4(out + 4 * (size_t)i, encode_one(ld4(gt + 4 * (size_t)i), ld4(anchors + (size_t)i * astride)));
 }
 
 __global__ void tube_valid_kernel(float* __restrict__ boxes, int n, float width, float height) {

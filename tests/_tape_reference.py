@@ -374,8 +374,8 @@ def roi_align_terms(rois, scale, ph, pw, H, W, sampling_ratio=0):
     """Every term of the legacy ROIAlign (aligned=False; adaptive grid ceil(roi / pooled) for sampling_ratio 0; samples
     outside [-1, extent] dropped; 4-tap bilinear; mean over the grid) of rois [R, 5] (frame, x1, y1, x2, y2) on H x W maps,
     on the rois' device.  Sample coordinates and tap weights are formed in fp32 in the kernels' operation order
-    (csrc/roi.cu roi_geometry / sample_coord / make_tap, csrc/train.cu roi_align_bwd_frame / bilinear_taps,
-    oracle/step_oracle.c).  A clamped sample (past H-1 / W-1) keeps its duplicate taps of one pixel as separate terms, as
+    (csrc/roi_math.cuh roi_geometry / sample_coord / make_tap, which csrc/roi.cu and csrc/train.cu roi_align_bwd_frame
+    share, oracle/step_oracle.c).  A clamped sample (past H-1 / W-1) keeps its duplicate taps of one pixel as separate terms, as
     the kernels add them.  ROIs are grouped by sampling grid so that each group is one batched tensor expression.
     Returns a list of groups dict(idx [G] int64 ROI rows, bin [S] int64, pix [G, S] int64 (-1: dropped sample),
     w [G, S] float64 holding the fp32 tap weights, count = gh * gw, grid = (gh, gw), bin_hw = the fp32 bin sizes [G] x 2),
@@ -654,7 +654,7 @@ def cls_loss(logits, targets):
 
 
 def _encode_terms(gt, anchor):
-    """encode4 of csrc/train.cu (tube_utils.py:143-163) in float64 and its fp32 error bound, per [N, 4] row.
+    """encode_one of csrc/tube_math.cuh (tube_utils.py:143-163) in float64 and its fp32 error bound, per [N, 4] row.
     With B = |c0| + |c2| + 1 per axis of a box (c0, c2 its two coordinates on the axis): the width fl(fl(c2 - c0) + 1) is
     within 2 u32 B, the centre fl(c0 + 0.5 w) within 2.5 u32 B < 3 u32 B.  (gx - ax) / aw: the difference within
     3 u32 (Bg + Ba) + u32 |num|, the division adds |enc| 2 u32 Ba / |aw| (the width) and u32 |enc|.  log(gw / aw): the ratio

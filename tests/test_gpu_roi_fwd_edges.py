@@ -43,7 +43,7 @@ from test_gpu_train_launches import EDGE_ROIS  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 SCALE = 1.0 / 16.0
-TAPS = 784                                  # the exact kernels' shared sample table (csrc/roi.cu kMaxTaps)
+TAPS = 784                                  # the exact kernels' shared sample table (csrc/roi_math.cuh kMaxTaps)
 MERGED_BIN = 8 + 8 * R.ROI_MERGED           # bytes per bin of the packed table (csrc/roi.cu MergedBin)
 PACKED_SMEM = 48 * 1024                     # largest packed table
 FMAP = (2, 4, 1)                            # roi_T, feat_T, t_start: ROI frames 0..3 read frames 1, 2, 5, 6 of 8
