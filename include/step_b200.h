@@ -463,6 +463,64 @@ int step_select_step_f32(const step_select_params* p, step_stream_t stream);
  * a caller validates every step before it uploads or launches anything. */
 int step_select_check_f32(const step_select_params* p);
 
+/* ---- frame-mAP (eval.cu): the AVA Pascal evaluator of get_ava_performance.run_evaluation, fed by step_detect_f32 ---- */
+enum {
+  STEP_EVAL_MAX_CLIPS = 64,              /* clips of one append call */
+  STEP_EVAL_MAX_IMAGES = 1 << 20,        /* image ids are < this */
+  STEP_EVAL_MAX_CLASSES = 128,           /* evaluator classes (the label map's largest id) */
+  STEP_EVAL_MAX_GT_PER_IMAGE = 1024,     /* ground-truth rows of one image */
+  STEP_EVAL_MAX_ROWS = 1 << 30           /* detection rows, and rows read (whitelisted rows, kept or not) */
+};
+/* The row store append and evaluate share: one row per kept detection, in the order the rows were read. */
+typedef struct {
+  long long capacity;        /* rows the arrays below hold */
+  int32_t* counters;         /* [2] device: rows kept, rows read */
+  int32_t* img_first;        /* [STEP_EVAL_MAX_IMAGES] first row read of each image (INT32_MAX: none yet) */
+  double* box;               /* [capacity, 4] y1, x1, y2, x2 after the CSV rounding */
+  double* score;             /* [capacity] score after the CSV rounding */
+  int32_t* scode;            /* [capacity] order-preserving integer code of the rounded score */
+  int32_t* img;              /* [capacity] image id */
+  int32_t* cls;              /* [capacity] evaluator class index (label id - 1) */
+} step_eval_rows;
+typedef struct {
+  const float* det;          /* [B, cap, 8] step_detect_f32's rows: x1, y1, x2, y2, score, class, tube, 0 */
+  const int32_t* count;      /* [B] rows of each clip */
+  int B, cap;
+  int ncls;                  /* detector classes */
+  const int32_t* class_of;   /* [ncls] evaluator class index of each detector class; -1 drops its rows (not whitelisted) */
+  int32_t img[STEP_EVAL_MAX_CLIPS];  /* image id of each clip; -1 drops the clip (an excluded key) */
+  step_eval_rows rows;
+} step_eval_append_params;
+/* Appends the clips' rows in order: every box coordinate and score rounded as '{:.4}' then float() round them, rows of
+ * other classes dropped, rows with y1 >= y2, x1 >= x2 or score <= -10 dropped after they are counted as read.  One CTA,
+ * no synchronisation.  Rows past rows.capacity are counted but not stored: the caller keeps room for B * cap more. */
+int step_eval_append(const step_eval_append_params* p, step_stream_t stream);
+/* The checks of step_eval_append, with no launch. */
+int step_eval_append_check(const step_eval_append_params* p);
+typedef struct {
+  step_eval_rows rows;
+  int n_rows;                /* rows kept (counters[0], read back by the caller) */
+  int n_classes;             /* evaluator classes */
+  int n_images;              /* image ids are < n_images */
+  int n_gt;                  /* ground-truth rows */
+  int max_gt_per_image;
+  const double* gt_box;      /* [n_gt, 4] y1, x1, y2, x2, sorted by (image, class), row order kept within */
+  const int32_t* gt_cls;     /* [n_gt] */
+  const int32_t* gt_img_off; /* [n_images + 1] first ground-truth row of each image */
+  const int32_t* num_gt;     /* [n_classes] ground-truth rows of each class */
+  void* workspace;
+  size_t workspace_bytes;    /* >= step_eval_workspace_bytes(n_rows, n_classes, n_gt) */
+  double* ap;                /* [n_classes] per-class AP: NaN without ground truth */
+} step_eval_params;
+size_t step_eval_workspace_bytes(int n_rows, int n_classes, int n_gt);
+/* Per-class AP of get_ava_performance.run_evaluation (PascalDetectionEvaluator, IoU 0.5).  Per image and class: the
+ * rows by descending score (ties: later row first), the first 10,000, greedy matching on the float64 IoU of np_box_ops.iou.
+ * Per class: the rows by descending score (ties: later image, then earlier row, first), precision and recall, the
+ * precision made non-increasing, and the AP terms summed in numpy's pairwise order. */
+int step_eval_run(const step_eval_params* p, step_stream_t stream);
+/* The checks of step_eval_run, with no launch. */
+int step_eval_check(const step_eval_params* p);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,6 +4,7 @@ Public surface mirrors the reference (SURVEY.md section 8b):
     from step_b200 import BaseNet, ROINet, TwoBranchNet, ContextNet      # models/__init__.py:6-7
     from step_b200 import inference                                       # utils/utils.py:15
     from step_b200 import select_samples                                  # utils/utils.py:135 train_select, per step
+    from step_b200 import FrameAP                                         # utils/eval_utils.py ava_evaluation
     from step_b200.roi_layers import nms, roi_align, ROIAlign, roi_pool, ROIPool
     from step_b200 import tube_utils                                      # utils/tube_utils.py
 All compute goes through libstep_b200.so (include/step_b200.h); there is no CPU/PyTorch fallback.
@@ -13,6 +14,8 @@ from .two_branch import ContextNet, TwoBranchNet  # noqa: F401
 from .inference import inference  # noqa: F401
 from .runner import StepRunner  # noqa: F401
 from .select import select_samples  # noqa: F401
+from .evaluation import FrameAP  # noqa: F401
 from . import optim, postprocess, roi_layers, tube_utils  # noqa: F401
 
-__all__ = ["BaseNet", "ROINet", "TwoBranchNet", "ContextNet", "inference", "select_samples", "StepRunner", "roi_layers", "tube_utils", "postprocess"]
+__all__ = ["BaseNet", "ROINet", "TwoBranchNet", "ContextNet", "inference", "select_samples", "FrameAP", "StepRunner", "roi_layers",
+           "tube_utils", "postprocess"]

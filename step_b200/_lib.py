@@ -126,6 +126,11 @@ def _declare(lib):
         "step_frames_to_clip_aug_u8": ([P, P, P, P, I, I, I, I, I, P, P, P, S], c_int),
         "step_select_step_f32": ([P, S], c_int),
         "step_select_check_f32": ([P], c_int),
+        "step_eval_append": ([P, S], c_int),
+        "step_eval_append_check": ([P], c_int),
+        "step_eval_workspace_bytes": ([I, I, I], c_size_t),
+        "step_eval_run": ([P, S], c_int),
+        "step_eval_check": ([P], c_int),
         "step_debug_tma_tile": ([ctypes.POINTER(ConvParams), I, I, I, I, I, P, P, P, S], c_int),
     }
     for name, (argtypes, restype) in sigs.items():

@@ -13,14 +13,15 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libstep_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-SOURCES = ["api.cu", "nms.cu", "roi.cu", "tubes.cu", "pool_layout.cu", "conv_simt.cu", "conv_umma.cu", "conv_halo.cu", "conv_stem.cu", "bottleneck_exit.cu", "train.cu", "optim.cu", "clip_prep.cu", "select.cu"]
+SOURCES = ["api.cu", "nms.cu", "roi.cu", "tubes.cu", "pool_layout.cu", "conv_simt.cu", "conv_umma.cu", "conv_halo.cu", "conv_stem.cu", "bottleneck_exit.cu", "train.cu", "optim.cu", "clip_prep.cu", "select.cu", "eval.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 # nms/roi/tubes rely on explicitly rounded intrinsics; -fmad=false additionally forbids contraction.  optim.cu rounds each
 # step of the torch optimizers' kernel sequence separately, where contraction would fuse what torch rounds twice.  clip_prep.cu
 # reproduces cv2's resize, whose products and sums (float and double) are rounded one at a time.  select.cu repeats
-# numpy's float32 and float64 operations of train_select one rounding at a time.
-NO_FMAD = {"nms.cu", "roi.cu", "tubes.cu", "train.cu", "optim.cu", "clip_prep.cu", "select.cu"}
+# numpy's float32 and float64 operations of train_select one rounding at a time.  eval.cu repeats the float64 IoU and
+# precision / recall arithmetic of the AVA evaluator, and its decimal rounding relies on unfused products.
+NO_FMAD = {"nms.cu", "roi.cu", "tubes.cu", "train.cu", "optim.cu", "clip_prep.cu", "select.cu", "eval.cu"}
 
 
 def _deps(src):
