@@ -208,6 +208,11 @@ int step_frames_to_clip_aug_u8(const step_frame_src* table, const step_clip_aug*
                                const float* std3, float* out, step_stream_t stream);
 
 /* ------------------------------------------------------------------ conv / pool / linear - */
+/* step_conv_params.a_mode, the addressing of the f16 path: auto (linear for 1x1x1, else box), linear (1x1x1 only), box
+ * tiles, TMA im2col, halo (input patch staged in shared memory: stride 1, Cin in {16,32,64}, Cout <= 256; or the s2d
+ * stem, see zero_cin_last_kt), best of im2col / halo per layer shape, SIMT (the kernel of the fp32 path). */
+enum { STEP_A_AUTO = 0, STEP_A_LINEAR = 1, STEP_A_BOX = 2, STEP_A_IM2COL = 3, STEP_A_HALO = 4, STEP_A_BEST = 5,
+       STEP_A_SIMT = 9 };
 typedef struct {
   int dtype;                 /* STEP_F32: SIMT fp32 path.  STEP_F16: wgmma implicit GEMM, fp32 accumulate */
   int N, T, H, W;            /* input extent (pixels) */
@@ -226,10 +231,7 @@ typedef struct {
   const void* residual;      /* optional tensor added before relu (two_branch.py:79-81), layout of y */
   int res_ld, res_coff;
   void* y;
-  int a_mode;                /* f16 path: 0 auto, 1 linear (1x1x1 only), 2 box tiles, 3 TMA im2col,
-                                4 input patch staged in shared memory (stride 1, Cin in {16,32,64}, Cout <= 256;
-                                  or the s2d stem, see zero_cin_last_kt),
-                                5 best of 3 / 4 per layer shape, 9 SIMT */
+  int a_mode;                /* STEP_A_* (f16 path) */
   /* Horizontally fused 1x1x1 layers that share an input (Mixed.branch_0 / branch_1[0] / branch_2[0],
    * i3dpt.py:133-147): output channels [0, split[0]) go to y, [split[0], split[1]) to y_extra[0],
    * [split[1], Cout) to y_extra[1], each with its own channel stride / offset.  n_splits = 0: plain conv.
@@ -239,14 +241,18 @@ typedef struct {
   void* y_extra[2];
   int ld_extra[2];
   int coff_extra[2];
-  /* Structured zeros of the weights (a_mode 4 only): for the filter taps of the LAST t plane (kt == KT-1) the input
+  /* Structured zeros of the weights (STEP_A_HALO only): for the filter taps of the LAST t plane (kt == KT-1) the input
    * channels [zero_cin_last_kt, Cin) carry zero weights.  0 = no such structure.  The space-to-depth stem has it: tap plane
-   * qt = 2 only holds the rt = 0 sub-position (k = 2(q+1)+r <= 6), engine.pack_stem_s2d.  The stem kernel (a_mode 4,
+   * qt = 2 only holds the rt = 0 sub-position (k = 2(q+1)+r <= 6), engine.pack_stem_s2d.  The stem kernel (STEP_A_HALO,
    * Cin = 24, Cout = 64, 4x4x4, pad 1) is chosen only when 0 < zero_cin_last_kt <= 16 and skips channels 16..23 of that
    * plane; the generic patch kernel multiplies the zeros. */
   int zero_cin_last_kt;
 } step_conv_params;
 int step_conv3d_fwd(const step_conv_params* p, step_stream_t stream);
+/* Test hook of the f16 path: the raw bytes of the A tile m_tile, tap (kt, kh, kw), channels from c0, as the TMA stages it
+ * in shared memory -> out [128 * BK * 2]; *bk_out = BK, box_out [3] = the box tile's (w, h, t) extent. */
+int step_debug_tma_tile(const step_conv_params* p, int m_tile, int kt, int kh, int kw, int c0, void* out, int* bk_out,
+                        int* box_out, step_stream_t stream);
 
 /* MaxPool3dTFPadding (i3dpt.py:114-126): zero pad (low PT/PH/PW, high implied), ceil_mode. */
 int step_maxpool3d_fwd(const void* x, int dtype, int N, int T, int H, int W, int C, int in_ld, int KT,
@@ -424,6 +430,7 @@ int step_multi_tensor_sgd_f32(const step_optim_tensor* table, int n_tensors, con
 
 /* ---- training-sample selection (select.cu): train_select, utils/utils.py:135-423, one refinement step per call ---- */
 enum { STEP_SAMPLING_UNIFORM = 0, STEP_SAMPLING_RANDOM = 1, STEP_SAMPLING_SOFTMAX = 2 };
+enum { STEP_SELECT_MT_WORDS = 625 };  /* one MT19937 state: 624 key words, then the position */
 typedef struct {
   int step;                  /* 1-based refinement step; step 1 selects from the proposals, later steps from the history */
   int B;                     /* clips */
@@ -451,7 +458,7 @@ typedef struct {
   const float* last;
   const double* props;       /* step 1: [R, L, 4] */
   const float* targets;      /* [sum G, max_chunks, 4 + C] */
-  uint32_t* mt;              /* [2][625]: numpy's, then Python's MT19937 key with its position last; advanced in place */
+  uint32_t* mt;              /* [2][STEP_SELECT_MT_WORDS]: numpy's, then Python's MT19937 state; advanced in place */
   float* out_tubes;          /* [B * max_rows, Lout, 5], rows packed clip after clip */
   float* out_targets;        /* [B * max_rows, 3, 6 + C] */
   int32_t* counts;           /* [B] rows of each clip */

@@ -1,143 +1,109 @@
-"""ctypes binding of libstep_b200.so (the C ABI declared in include/step_b200.h).
+"""ctypes binding of libstep_b200.so, read from the C ABI in include/step_b200.h.
 
 PyTorch only supplies device memory and the current CUDA stream; every compute call below goes
 through the C ABI.  There is no fallback: if the library is missing or a tensor is not on a CUDA
 device the call raises (north_star: "no CPU fallback").
+
+The header is the one declaration of the ABI.  At import, `read_header` turns it into the enum constants (exposed here
+with the STEP_ prefix dropped: STEP_F16 -> F16, STEP_E_ARG -> E_ARG), one ctypes.Structure per struct typedef (exposed
+under its C name: step_conv_params, ...) and the argtypes / restype of every entry point, which `lib()` sets.  A
+declaration the reader does not know raises at import, so a header edit it cannot follow fails on the host instead of
+shifting the arguments of a launch.
 """
 import ctypes
 import os
+import re
 
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libstep_b200.so")
-
-F32, F16 = 0, 1
-EXT_NONE, EXT_PREDICT, EXT_EXTRAPOLATE, EXT_MEAN = 0, 1, 2, 3
-A_AUTO, A_LINEAR, A_BOX, A_IM2COL, A_HALO, A_BEST, A_SIMT = 0, 1, 2, 3, 4, 5, 9
+HEADER = os.path.join(os.path.dirname(HERE), "include", "step_b200.h")
 
 _lib = None
 
-c_int, c_float, c_void_p, c_size_t = ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
+c_void_p = ctypes.c_void_p
 
 
-class ConvParams(ctypes.Structure):
-    """mirror of step_conv_params (include/step_b200.h)"""
-    _fields_ = [(n, c_int) for n in
-                ("dtype", "N", "T", "H", "W", "Cin", "in_ld", "Cout", "out_ld", "out_coff", "KT", "KH", "KW",
-                 "ST", "SH", "SW", "PT", "PH", "PW", "OT", "OH", "OW", "relu", "w_ld")] + \
-               [("x", c_void_p), ("w", c_void_p), ("scale", c_void_p), ("shift", c_void_p),
-                ("residual", c_void_p), ("res_ld", c_int), ("res_coff", c_int), ("y", c_void_p),
-                ("a_mode", c_int), ("n_splits", c_int), ("split", c_int * 2), ("y_extra", c_void_p * 2),
-                ("ld_extra", c_int * 2), ("coff_extra", c_int * 2), ("zero_cin_last_kt", c_int)]
+class Struct(ctypes.Structure):
+    """Base of the header's structs.  Every pointer parameter and step_stream_t binds as c_void_p, which takes an int
+    address, c_void_p, ctypes.byref(...), a ctypes array or None in C; an instance of one of these structs passes by
+    reference through `_as_parameter_`.  (A Python-level from_param would run on every pointer argument of every call.)"""
+
+    @property
+    def _as_parameter_(self):
+        return ctypes.byref(self)
 
 
-class OptimTensor(ctypes.Structure):
-    """mirror of step_optim_tensor (include/step_b200.h)"""
-    _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p),
-                ("numel", ctypes.c_longlong)] + \
-               [(n, c_float) for n in ("step_size", "inv_bias_correction2_sqrt", "weight_decay", "one_minus_beta1", "beta2",
-                                       "one_minus_beta2", "eps", "momentum")] + [("buf_uninit", c_int)]
+_SCALARS = {"int": ctypes.c_int, "int32_t": ctypes.c_int32, "float": ctypes.c_float, "long long": ctypes.c_longlong,
+            "size_t": ctypes.c_size_t, "uint64_t": ctypes.c_uint64}
+_STATEMENT = re.compile(r"\s*(?:enum\s*\{(?P<enum>[^{}]*)\}|typedef\s+struct\s*\{(?P<fields>[^{}]*)\}\s*(?P<struct>\w+)"
+                        r"|typedef\s+struct\s+\w+\s*\*\s*(?P<handle>\w+)"
+                        r"|(?P<ret>[\w\s*]+?)\s*\b(?P<fn>step_\w+)\s*\((?P<params>[^;{}()]*)\))\s*;")
+_DECLARATOR = re.compile(r"(?:const\s+)?(?P<type>\w+(?:\s+\w+)*?)\s*(?P<ptr>\*?)\s*(?P<name>\w+)(?:\[(?P<len>\w+)\])?")
 
 
-class OptimBlock(ctypes.Structure):
-    """mirror of step_optim_block (include/step_b200.h)"""
-    _fields_ = [("tensor", c_int), ("chunk", c_int)]
+def read_header(text):
+    """(constants, structs, functions) of a header written in the C subset of include/step_b200.h: enums of integer
+    literals and `1 << n`; `typedef struct { ... } name;` with scalar, pointer (c_void_p), fixed-array and struct fields,
+    several declarators per line allowed; opaque handles `typedef struct X* name;`; `step_*` prototypes of scalars and
+    pointers (every pointer and handle binds as c_void_p, a `const char*` result as c_char_p).  Anything else raises
+    ValueError naming the declaration."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"#ifdef __cplusplus.*?#endif|#[^\n]*", " ", text, flags=re.S)
+    consts, structs, functions, handles = {}, {}, {}, set()
+
+    def fail(declaration):
+        raise ValueError("step_b200.h: cannot bind %r" % " ".join(declaration.split()))
+
+    def bind(decl, field=False):
+        """(name, ctypes type) of one declarator `[const] type [*]name[[len]]`."""
+        d = _DECLARATOR.fullmatch(decl.strip())
+        if d is None or (d["len"] and not field):
+            fail(stmt)
+        pointer = d["ptr"] or d["type"] in handles
+        t = ctypes.c_void_p if pointer else _SCALARS.get(d["type"]) or field and structs.get(d["type"])
+        if d["len"]:
+            n = int(d["len"]) if d["len"].isdigit() else consts.get(d["len"])
+            t = t and n and t * n
+        return d["name"], t or fail(stmt)
+
+    pos = 0
+    while text[pos:].strip():
+        m = _STATEMENT.match(text, pos)
+        stmt = m.group(0) if m else text[pos:text.find(";", pos) + 1 or len(text)]
+        if m is None:
+            fail(stmt)
+        pos = m.end()
+        if m["enum"] is not None:
+            for item in filter(str.strip, m["enum"].split(",")):
+                e = re.fullmatch(r"\s*(\w+)\s*=\s*(\d+)(?:\s*<<\s*(\d+))?\s*", item) or fail(stmt)
+                consts[e[1]] = int(e[2]) << int(e[3] or 0)
+        elif m["struct"]:
+            fields = []
+            for line in filter(str.strip, m["fields"].split(";")):
+                first, *more = line.split(",")
+                base = (_DECLARATOR.fullmatch(first.strip()) or fail(stmt))["type"]
+                fields += [bind(d, field=True) for d in [first] + [base + " " + d for d in more]]
+            structs[m["struct"]] = type(m["struct"], (Struct,), {"_fields_": fields})
+        elif m["handle"]:
+            handles.add(m["handle"])
+        else:
+            ret = m["ret"].strip()
+            restype = ctypes.c_char_p if re.fullmatch(r"const char\s*\*", ret) else bind(ret + " " + m["fn"])[1]
+            params = [] if m["params"].strip() == "void" else m["params"].split(",")
+            functions[m["fn"]] = ([bind(p)[1] for p in params], restype)
+    return consts, structs, functions
 
 
-class FrameSrc(ctypes.Structure):
-    """mirror of step_frame_src (include/step_b200.h)"""
-    _fields_ = [("data", c_void_p), ("H0", c_int), ("W0", c_int)] + \
-               [(n, ctypes.c_longlong) for n in ("stride_t", "stride_c", "stride_h", "stride_w")]
-
-
-class ClipAug(ctypes.Structure):
-    """mirror of step_clip_aug (include/step_b200.h)"""
-    _fields_ = [(n, c_int) for n in ("x0", "y0", "w", "h", "flip", "photometric", "brightness", "contrast",
-                                     "contrast_first", "saturation", "hue")] + \
-               [(n, c_float) for n in ("brightness_delta", "contrast_alpha", "saturation_alpha", "hue_delta")] + \
-               [("perm", c_int * 3), ("erase_begin", c_int), ("erase_count", c_int)]
-
-
-class AugErase(ctypes.Structure):
-    """mirror of step_aug_erase (include/step_b200.h)"""
-    _fields_ = [(n, c_int) for n in ("x1", "y1", "x2", "y2")] + [("noise", ctypes.c_longlong)]
-
-
-def _declare(lib):
-    P, I, Fl, S = c_void_p, c_int, c_float, c_void_p  # S = stream
-    sigs = {
-        "step_version": ([], c_int),
-        "step_last_error": ([], ctypes.c_char_p),
-        "step_launch_count": ([], ctypes.c_uint64),
-        "step_nms_workspace_bytes": ([I], c_size_t),
-        "step_nms_f32": ([P, P, I, Fl, I, P, P, P, c_size_t, S], c_int),
-        "step_nms_segmented_f32": ([P, P, P, I, Fl, I, Fl, P, S], c_int),
-        "step_nms_segmented_max_rows": ([], c_int),
-        "step_detect_f32": ([P, I, P, I, P, I, I, I, I, Fl, Fl, I, Fl, Fl, Fl, Fl, I, I, P, P, P, P, P, S], c_int),
-        "step_roi_align_fwd_nchw_f32": ([P, I, I, I, I, P, I, Fl, I, I, I, P, S], c_int),
-        "step_roi_align_bwd_nchw_f32": ([P, P, I, Fl, I, I, I, I, I, I, I, P, S], c_int),
-        "step_roi_pool_fwd_nchw_f32": ([P, I, I, I, I, P, I, Fl, I, I, P, P, S], c_int),
-        "step_roi_pool_bwd_nchw_f32": ([P, P, P, I, I, I, I, I, I, I, P, S], c_int),
-        "step_roi_align_fwd_nhwc": ([P, I, I, I, I, I, I, P, I, Fl, I, I, I, P, I, I, I, I, I, S], c_int),
-        "step_roi_pool_fwd_nhwc": ([P, I, I, I, I, I, I, P, I, Fl, I, I, P, I, I, I, I, S], c_int),
-        "step_roi_pool_fwd_argmax_nhwc": ([P, I, I, I, I, I, I, P, I, Fl, I, I, P, I, I, I, I, P, S], c_int),
-        "step_tube_decode_f32": ([P, I, P, I, P, S], c_int),
-        "step_tube_encode_f32": ([P, P, I, I, P, S], c_int),
-        "step_tube_valid_f32": ([P, I, Fl, Fl, S], c_int),
-        "step_tube_extrapolate_f32": ([P, I, I, I, Fl, Fl, P, S], c_int),
-        "step_tube_extend_f32": ([P, I, Fl, Fl, Fl, P, S], c_int),
-        "step_tube_update_f32": ([P, P, P, P, P, I, I, I, I, I, Fl, Fl, P, P, P, P, S], c_int),
-        "step_clip_to_ndhwc": ([P, I, I, I, I, I, P, I, I, S], c_int),
-        "step_clip_to_s2d_f16": ([P, I, I, I, I, I, P, I, S], c_int),
-        "step_nhwc_to_nchw_f32": ([P, I, I, I, I, I, P, S], c_int),
-        "step_nchw_to_nhwc": ([P, I, I, I, P, I, I, S], c_int),
-        "step_conv3d_fwd": ([ctypes.POINTER(ConvParams), S], c_int),
-        "step_maxpool3d_fwd": ([P, I] + [I] * 21 + [P, I, S], c_int),
-        "step_mean_mid": ([P, I, I, I, I, I, I, P, I, S], c_int),
-        "step_mean_mid_strided": ([P, I, I, I, I, I, I, ctypes.c_longlong, P, I, S], c_int),
-        "step_linear_small_n_workspace_bytes": ([I, I, I], c_size_t),
-        "step_linear_small_n": ([P, I, I, I, I, P, P, I, P, I, I, I, P, P, c_size_t, S], c_int),
-        "step_head_regress": ([P, I, I, I, I, I, P, P, I, I, I, I, P, P, P, P, c_size_t, S], c_int),
-        "step_bottleneck_exit_f16": ([P, ctypes.c_longlong, P, P, ctypes.c_longlong, P, P, I, P, ctypes.c_longlong, P, ctypes.c_longlong,
-                                     ctypes.c_longlong, I, I, I, S], c_int),
-        "step_head_losses_f32": ([P, P, P, P, P, P, I, I, I, I, I, Fl, Fl, P, P, P, P, P, P, P, P, P, S], c_int),
-        "step_cls_loss_f32": ([P, P, I, I, P, P, P, S], c_int),
-        "step_roi_align_bwd_nhwc": ([P, I, I, P, I, Fl, I, I, I, I, I, I, I, P, I, S], c_int),
-        "step_roi_align_bwd_slice_workspace_bytes": ([I, I, I, I, I, I], c_size_t),
-        "step_roi_align_bwd_slice_nhwc": ([P, I, I, P, I, Fl, I, I, I, I, I, I, I, I, I, I, P, I, P, c_size_t, S], c_int),
-        "step_roi_pool_bwd_slice_nhwc": ([P, I, I, P, P, I, I, I, I, I, I, I, I, I, I, P, I, S], c_int),
-        "step_ctx_grad_reduce_f32": ([P, I, P, I, I, I, I, I, I, P, S], c_int),
-        "step_linear_small_n_bwd": ([P, I, I, I, I, P, P, I, P, I, P, P, S], c_int),
-        "step_conv1x1_wgrad_workspace_bytes": ([I, I, I], c_size_t),
-        "step_conv1x1_wgrad_f16": ([P, I, P, I, I, I, I, Fl, P, I, I, P, c_size_t, S], c_int),
-        "step_conv_wgrad_workspace_bytes": ([I, I, I, I], c_size_t),
-        "step_conv_wgrad_f16": ([P, I, P, I, I, I, I, I, I, I, I, I, I, I, I, I, Fl, P, I, I, P, c_size_t, S], c_int),
-        "step_act_bwd_f16": ([P, I, P, I, P, I, ctypes.c_longlong, I, P, I, P, I, S], c_int),
-        "step_colsum_f16": ([P, I, ctypes.c_longlong, I, Fl, P, P, S], c_int),
-        "step_mean_mid_bwd": ([P, I, I, I, I, Fl, P, I, S], c_int),
-        "step_f32_accum_f16": ([P, ctypes.c_longlong, I, Fl, P, I, S], c_int),
-        "step_maxpool3d_bwd_f16": ([P, I, P, I] + [I] * 20 + [P, I, P, S], c_int),
-        "step_multi_tensor_chunk": ([], c_int),
-        "step_multi_tensor_nonfinite_f32": ([P, I, P, I, P, S], c_int),
-        "step_multi_tensor_adam_f32": ([P, I, P, I, S], c_int),
-        "step_multi_tensor_sgd_f32": ([P, I, P, I, S], c_int),
-        "step_frames_to_clip_u8": ([P, I, I, I, I, I, P, P, P, S], c_int),
-        "step_frames_to_clip_aug_u8": ([P, P, P, P, I, I, I, I, I, P, P, P, S], c_int),
-        "step_select_step_f32": ([P, S], c_int),
-        "step_select_check_f32": ([P], c_int),
-        "step_eval_append": ([P, S], c_int),
-        "step_eval_append_check": ([P], c_int),
-        "step_eval_workspace_bytes": ([I, I, I], c_size_t),
-        "step_eval_run": ([P, S], c_int),
-        "step_eval_check": ([P], c_int),
-        "step_debug_tma_tile": ([ctypes.POINTER(ConvParams), I, I, I, I, I, P, P, P, S], c_int),
-    }
-    for name, (argtypes, restype) in sigs.items():
-        fn = getattr(lib, name)  # AttributeError here == header / library mismatch
-        fn.argtypes = argtypes
-        fn.restype = restype
-    return sigs
+with open(HEADER) as _f:
+    CONSTANTS, STRUCTS, FUNCTIONS = read_header(_f.read())
+globals().update({name.removeprefix("STEP_"): value for name, value in CONSTANTS.items()})
+globals().update(STRUCTS)
+# The names these structs had before they were read from the header; existing callers keep them (select.py and
+# evaluation.py keep theirs likewise).
+ConvParams, OptimTensor, OptimBlock, FrameSrc, ClipAug, AugErase = (STRUCTS[n] for n in (
+    "step_conv_params", "step_optim_tensor", "step_optim_block", "step_frame_src", "step_clip_aug", "step_aug_erase"))
 
 
 def lib():
@@ -148,13 +114,17 @@ def lib():
             raise RuntimeError("step_b200: %s not found -- run `python -m step_b200.build` (there is no "
                                "CPU / PyTorch fallback for the hot path)" % LIB_PATH)
         l = ctypes.CDLL(LIB_PATH)
-        _declare(l)
+        for name, (argtypes, restype) in FUNCTIONS.items():
+            fn = getattr(l, name)  # AttributeError here == header / library mismatch
+            fn.argtypes, fn.restype = argtypes, restype
         _lib = l
     return _lib
 
 
 def exported_symbols():
-    return sorted(_declare(lib()).keys())
+    """Every entry point the header declares; lib() has checked that the library exports each."""
+    lib()
+    return sorted(FUNCTIONS)
 
 
 def check(rc):

@@ -49,17 +49,17 @@ extern "C" int step_conv3d_fwd(const step_conv_params* p, step_stream_t stream) 
   STEP_CHECK_ARG(p->n_splits >= 0 && p->n_splits <= 2, "conv3d: bad n_splits");
   STEP_CHECK_ARG(p->n_splits > 0 || p->out_ld >= p->out_coff + p->Cout, "conv3d: output slice [%d,%d) exceeds out_ld %d",
                  p->out_coff, p->out_coff + p->Cout, p->out_ld);
-  STEP_CHECK_ARG(p->n_splits == 0 || (p->dtype == STEP_F16 && p->a_mode != 9), "conv3d: fused outputs are f16 tensor-core only");
+  STEP_CHECK_ARG(p->n_splits == 0 || (p->dtype == STEP_F16 && p->a_mode != STEP_A_SIMT), "conv3d: fused outputs are f16 tensor-core only");
   // every output position must only need taps that the declared low padding makes reachable
   STEP_CHECK_ARG((p->OT - 1) * p->ST - p->PT < p->T && (p->OH - 1) * p->SH - p->PH < p->H && (p->OW - 1) * p->SW - p->PW < p->W,
                  "conv3d: output extent inconsistent with input/stride/pad");
-  if (p->dtype == STEP_F32 || p->a_mode == 9) return conv3d_simt_launch(p, stream);
-  if (p->a_mode == 4) {   // explicit request: a patch-in-shared-memory kernel (conv_stem.cu for the s2d stem, else conv_halo.cu)
+  if (p->dtype == STEP_F32 || p->a_mode == STEP_A_SIMT) return conv3d_simt_launch(p, stream);
+  if (p->a_mode == STEP_A_HALO) {   // explicit request: a patch-in-shared-memory kernel (conv_stem.cu for the s2d stem, else conv_halo.cu)
     if (conv3d_stem_supported(p)) return conv3d_stem_launch(p, stream);
-    STEP_CHECK_ARG(p->ST == 1 && p->SH == 1 && p->SW == 1 && conv3d_halo_supported(p), "conv3d: a_mode 4 (halo) does not fit this problem");
+    STEP_CHECK_ARG(p->ST == 1 && p->SH == 1 && p->SW == 1 && conv3d_halo_supported(p), "conv3d: a_mode STEP_A_HALO does not fit this problem");
     return conv3d_halo_launch(p, stream);
   }
-  if (p->a_mode == 5) {
+  if (p->a_mode == STEP_A_BEST) {
     // "best": thin inputs on large maps go to the patch kernel, which needs far fewer bytes through TMA than one
     // im2col tile per tap; on 7x7 maps its 16 x 8 pixel tile is mostly padding.  Everything else: TMA im2col (k > 1) / linear (1x1x1).
     static const bool halo_on = !(getenv("STEP_B200_HALO") && getenv("STEP_B200_HALO")[0] == '0');
@@ -69,7 +69,7 @@ extern "C" int step_conv3d_fwd(const step_conv_params* p, step_stream_t stream) 
         p->Cin <= 32 && small >= 14)
       return conv3d_halo_launch(p, stream);
     step_conv_params q = *p;
-    q.a_mode = taps == 1 ? 0 : 3;
+    q.a_mode = taps == 1 ? STEP_A_AUTO : STEP_A_IM2COL;
     return conv3d_umma_launch(&q, stream);
   }
   return conv3d_umma_launch(p, stream);

@@ -34,8 +34,6 @@
 
 namespace step {
 
-enum { A_LINEAR = 1, A_BOX = 2, A_IM2COL = 3 };
-
 constexpr int kBM = 128;       // two m64 warpgroups
 constexpr int kMaxBN = 256;    // 128 fp32 accumulator registers per consumer thread
 constexpr int kStages = 8;     // barrier slots
@@ -78,7 +76,7 @@ struct ConvGeom {
 
 // output pixel of row `row` of M tile `m_tile`, or -1 (past the end / box overhang)
 __device__ __forceinline__ long long tile_row_pixel(const ConvGeom& g, int m_tile, int row) {
-  if (g.mode == A_BOX) {
+  if (g.mode == STEP_A_BOX) {
     int r = m_tile;
     const int bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
     const int bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
@@ -167,7 +165,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           const int m_tile = tile / g.n_tiles, n0 = (tile - m_tile * g.n_tiles) * BN;
           long long m0 = (long long)m_tile * kBM;
           int bn = 0, bt0 = 0, bh0 = 0, bw0 = 0;  // BOX origin
-          if (g.mode == A_BOX) {
+          if (g.mode == STEP_A_BOX) {
             int r = m_tile;
             bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
             bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
@@ -175,7 +173,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           }
           // IM2COL start coordinates: output pixel m0 -> (w,h,t,n) + lower corner (= -pad)
           int iw = 0, ih = 0, it = 0, in_ = 0;
-          if (g.mode == A_IM2COL) {
+          if (g.mode == STEP_A_IM2COL) {
             long long r = m0;
             iw = (int)(r % g.OW); r /= g.OW;
             ih = (int)(r % g.OH); r /= g.OH;
@@ -189,9 +187,9 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
               mbar_expect_tx(&full_bar[stage], tx_bytes);
               const int c0 = kc * BK;
               uint8_t* a_dst = sA + stage * kABytes;
-              if (g.mode == A_LINEAR) {
+              if (g.mode == STEP_A_LINEAR) {
                 tma_load_2d(&map_a, &full_bar[stage], a_dst, c0, (int)m0);
-              } else if (g.mode == A_BOX) {
+              } else if (g.mode == STEP_A_BOX) {
                 tma_load_5d(&map_a, &full_bar[stage], a_dst, c0, bw0 + kw - g.PW, bh0 + kh - g.PH, bt0 + kt - g.PT, bn);
               } else {
                 tma_load_im2col_5d(&map_a, &full_bar[stage], a_dst, c0, iw, ih, it, in_, (uint16_t)kw, (uint16_t)kh,
@@ -354,9 +352,9 @@ __global__ void __launch_bounds__(32) tma_dump_kernel(const __grid_constant__ CU
   if (threadIdx.x == 0) {
     long long m0 = (long long)m_tile * kBM;
     mbar_expect_tx(&bar, (uint32_t)g.a_bytes);
-    if (g.mode == A_LINEAR) {
+    if (g.mode == STEP_A_LINEAR) {
       tma_load_2d(&map_a, &bar, smem, c0, (int)m0);
-    } else if (g.mode == A_BOX) {
+    } else if (g.mode == STEP_A_BOX) {
       int r = m_tile;
       int bw0 = (r % g.tiles_w) * g.bw; r /= g.tiles_w;
       int bh0 = (r % g.tiles_h) * g.bh; r /= g.tiles_h;
@@ -481,9 +479,9 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   const int taps = p->KT * p->KH * p->KW;
   const bool is_1x1 = taps == 1 && p->PT == 0 && p->PH == 0 && p->PW == 0 && p->OT == p->T && p->OH == p->H && p->OW == p->W;
   int mode = p->a_mode;
-  if (mode == 0) mode = is_1x1 ? A_LINEAR : A_BOX;
-  STEP_CHECK_ARG(mode == A_LINEAR || mode == A_BOX || mode == A_IM2COL, "conv3d(f16): bad a_mode %d", p->a_mode);
-  STEP_CHECK_ARG(mode != A_LINEAR || is_1x1, "conv3d(f16): LINEAR mode needs a 1x1x1 unpadded filter");
+  if (mode == STEP_A_AUTO) mode = is_1x1 ? STEP_A_LINEAR : STEP_A_BOX;
+  STEP_CHECK_ARG(mode == STEP_A_LINEAR || mode == STEP_A_BOX || mode == STEP_A_IM2COL, "conv3d(f16): bad a_mode %d", p->a_mode);
+  STEP_CHECK_ARG(mode != STEP_A_LINEAR || is_1x1, "conv3d(f16): LINEAR mode needs a 1x1x1 unpadded filter");
   g.mode = mode;
   g.taps = taps; g.KT = p->KT; g.KH = p->KH; g.KW = p->KW; g.PT = p->PT; g.PH = p->PH; g.PW = p->PW;
   pl->BK = pick_bk(p->Cin);
@@ -511,7 +509,7 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
   g.M = (long long)p->N * p->OT * p->OH * p->OW;
   long long m_tiles;
   int rc;
-  if (mode == A_LINEAR) {
+  if (mode == STEP_A_LINEAR) {
     STEP_CHECK_ARG(g.M < (1LL << 31), "conv3d(f16): M too large");
     rc = encode_rows2d(&pl->map_a, p->x, g.M, p->Cin, p->in_ld, BK, kBM, swizzle_for(BK), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                        "conv3d(f16): A (linear)");
@@ -519,7 +517,7 @@ static int build_plan(const step_conv_params* p, ConvPlan* pl) {
     g.a_bytes = kBM * BK * 2;
   } else {
     const ActLayout act(p->N, p->T, p->H, p->W, p->Cin, p->in_ld);
-    if (mode == A_BOX) {
+    if (mode == STEP_A_BOX) {
       pick_box(p->OW, p->OH, p->OT, &g.bw, &g.bh, &g.bt);
       g.tiles_w = (p->OW + g.bw - 1) / g.bw; g.tiles_h = (p->OH + g.bh - 1) / g.bh; g.tiles_t = (p->OT + g.bt - 1) / g.bt;
       const cuuint32_t box[5] = {(cuuint32_t)BK, (cuuint32_t)g.bw, (cuuint32_t)g.bh, (cuuint32_t)g.bt, 1};

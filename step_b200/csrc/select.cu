@@ -14,7 +14,6 @@
 namespace step {
 
 constexpr int kSelThreads = 256;
-constexpr int kMtWords = 625;  // 624 key words, then the position
 constexpr int kSelMaxSmem = 200 * 1024;  // below the 227 KB opt-in limit, which includes the kernel's static shared memory
 
 // ---- MT19937, as numpy's legacy RandomState and CPython's random module run it ----
@@ -148,7 +147,7 @@ struct SelLayout {
   __host__ __device__ SelLayout(int C_, int n_, int g_, int K_, int rows_, int L_, int Lout_)
       : C(C_), n(n_), g(g_), E(C_ * K_), rows(rows_), L(L_), Lout(Lout_) {
     size_t sizes[20] = {
-        2 * kMtWords * 4,                     // 0 mt
+        2 * STEP_SELECT_MT_WORDS * 4,         // 0 mt
         (size_t)C * n * 4,                    // 1 mean scores
         (size_t)E * 4, (size_t)E * 4,         // 2 entry score, 3 entry tube
         (size_t)E * 4,                        // 4 entry position
@@ -193,7 +192,7 @@ __global__ void __launch_bounds__(kSelThreads) select_step_kernel(step_select_pa
   float* stage = (float*)(sm + lay.off[19]);
   __shared__ int s_nc, s_npos, s_rows, s_base;
 
-  for (int i = tid; i < 2 * kMtWords; i += blockDim.x) mt[i] = p.mt[i];
+  for (int i = tid; i < 2 * STEP_SELECT_MT_WORDS; i += blockDim.x) mt[i] = p.mt[i];
   if (tid == 0) s_base = 0;
   const int TC = 4 + C, OC = 6 + C;
   for (int b = 0; b < p.B; ++b) {
@@ -279,7 +278,7 @@ __global__ void __launch_bounds__(kSelThreads) select_step_kernel(step_select_pa
     __syncthreads();
     if (tid == 0) {
       uint32_t* np_mt = mt;
-      uint32_t* py_mt = mt + kMtWords;
+      uint32_t* py_mt = mt + STEP_SELECT_MT_WORDS;
       for (int j = 0; j < Nc; ++j) occ[j] = 0;
       int npos = 0;
       // :360-368, each ground truth in turn (the one with the largest remaining IoU) takes its best unoccupied candidate
@@ -419,7 +418,7 @@ __global__ void __launch_bounds__(kSelThreads) select_step_kernel(step_select_pa
     if (tid == 0) s_base = base + rows;
   }
   __syncthreads();
-  for (int i = tid; i < 2 * kMtWords; i += blockDim.x) p.mt[i] = mt[i];
+  for (int i = tid; i < 2 * STEP_SELECT_MT_WORDS; i += blockDim.x) p.mt[i] = mt[i];
 }
 
 }  // namespace step

@@ -221,7 +221,7 @@ def conv(x, w_packed, scale, shift, out, k, stride=(1, 1, 1), pad_lo=None, relu=
         pad_lo = tuple(same_pad(k[i], stride[i])[0] for i in range(3))
     if out_dims is None:
         out_dims = same_out_dims((x.T, x.H, x.W), k, stride)
-    p = L.ConvParams()
+    p = L.step_conv_params()
     p.dtype = code
     p.N, p.T, p.H, p.W = x.N, x.T, x.H, x.W
     p.Cin, p.in_ld = x.C, x.ld

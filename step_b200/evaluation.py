@@ -25,30 +25,9 @@ import torch
 
 from . import _lib as L
 
-MAX_CLIPS = 64
-MAX_IMAGES = 1 << 20
-MAX_CLASSES = 128
-MAX_ROWS = 1 << 30
 INT32_MAX = 2 ** 31 - 1
-_P, _I = ctypes.c_void_p, ctypes.c_int
-
-
-class EvalRows(ctypes.Structure):
-    """mirror of step_eval_rows (include/step_b200.h)"""
-    _fields_ = [("capacity", ctypes.c_longlong)] + [(n, _P) for n in ("counters", "img_first", "box", "score", "scode", "img", "cls")]
-
-
-class EvalAppendParams(ctypes.Structure):
-    """mirror of step_eval_append_params (include/step_b200.h)"""
-    _fields_ = [("det", _P), ("count", _P), ("B", _I), ("cap", _I), ("ncls", _I), ("class_of", _P), ("img", _I * MAX_CLIPS),
-                ("rows", EvalRows)]
-
-
-class EvalParams(ctypes.Structure):
-    """mirror of step_eval_params (include/step_b200.h)"""
-    _fields_ = [("rows", EvalRows)] + [(n, _I) for n in ("n_rows", "n_classes", "n_images", "n_gt", "max_gt_per_image")] + \
-               [(n, _P) for n in ("gt_box", "gt_cls", "gt_img_off", "num_gt", "workspace")] + \
-               [("workspace_bytes", ctypes.c_size_t), ("ap", _P)]
+# the structs' names before they were read from the header
+EvalRows, EvalAppendParams, EvalParams = L.step_eval_rows, L.step_eval_append_params, L.step_eval_params
 
 
 def image_key(key):
@@ -86,8 +65,8 @@ class FrameAP:
         if min(ids) < 1:
             raise ValueError("FrameAP: category ids must be 1-based (got %d)" % min(ids))
         self.n_classes = max(ids)
-        if self.n_classes > MAX_CLASSES:
-            raise ValueError("FrameAP: largest category id %d exceeds %d" % (self.n_classes, MAX_CLASSES))
+        if self.n_classes > L.EVAL_MAX_CLASSES:
+            raise ValueError("FrameAP: largest category id %d exceeds %d" % (self.n_classes, L.EVAL_MAX_CLASSES))
         self.whitelist = set(ids)
         if isinstance(label_dict, dict):
             table = [int(label_dict.get(c, 0)) for c in range(max(label_dict) + 1)] if label_dict else []
@@ -110,7 +89,7 @@ class FrameAP:
         self._ids = {}
         self._gt = []
         self._counters = torch.zeros(2, dtype=torch.int32, device=dev)
-        self._img_first = torch.full((MAX_IMAGES,), INT32_MAX, dtype=torch.int32, device=dev)
+        self._img_first = torch.full((L.EVAL_MAX_IMAGES,), INT32_MAX, dtype=torch.int32, device=dev)
         self._cap = 0
         self._box = self._score = self._scode = self._img = self._cls = None
         self._host_counters = torch.zeros(2, dtype=torch.int32).pin_memory()
@@ -121,8 +100,9 @@ class FrameAP:
 
     # ---- the row store ----
     def _rows(self):
-        return EvalRows(capacity=self._cap, counters=_ptr(self._counters), img_first=_ptr(self._img_first), box=_ptr(self._box),
-                        score=_ptr(self._score), scode=_ptr(self._scode), img=_ptr(self._img), cls=_ptr(self._cls))
+        return L.step_eval_rows(capacity=self._cap, counters=_ptr(self._counters), img_first=_ptr(self._img_first),
+                                box=_ptr(self._box), score=_ptr(self._score), scode=_ptr(self._scode), img=_ptr(self._img),
+                                cls=_ptr(self._cls))
 
     def _refresh(self):
         """Exact counters from the copy the last add_detections queued (waits for it only if it has not landed)."""
@@ -135,8 +115,8 @@ class FrameAP:
     def reserve(self, rows):
         """Make room for `rows` detection rows in all, so that no later add_detections has to grow the store."""
         rows = int(rows)
-        if rows > MAX_ROWS:
-            raise ValueError("FrameAP: %d rows exceed the %d the store holds" % (rows, MAX_ROWS))
+        if rows > L.EVAL_MAX_ROWS:
+            raise ValueError("FrameAP: %d rows exceed the %d the store holds" % (rows, L.EVAL_MAX_ROWS))
         if rows <= self._cap:
             return
         self._refresh()
@@ -153,14 +133,14 @@ class FrameAP:
         self._cap = rows
 
     def _make_room(self, worst):
-        if self._kept_bound + worst <= self._cap and self._read_bound + worst <= MAX_ROWS:
+        if self._kept_bound + worst <= self._cap and self._read_bound + worst <= L.EVAL_MAX_ROWS:
             return
         self._refresh()
-        if self._read_bound + worst > MAX_ROWS:
+        if self._read_bound + worst > L.EVAL_MAX_ROWS:
             raise ValueError("FrameAP: %d + %d detection rows exceed the %d rows an evaluation reads"
-                             % (self._read_bound, worst, MAX_ROWS))
+                             % (self._read_bound, worst, L.EVAL_MAX_ROWS))
         if self._kept_bound + worst > self._cap:
-            self.reserve(min(MAX_ROWS, max(2 * self._cap, self._kept_bound + worst, 1 << 20)))
+            self.reserve(min(L.EVAL_MAX_ROWS, max(2 * self._cap, self._kept_bound + worst, 1 << 20)))
 
     def _image_id(self, key):
         k = image_key(key)
@@ -214,10 +194,11 @@ class FrameAP:
         self._make_room(B * cap)
         with torch.cuda.device(self.device):
             stream = L.stream()
-            for b0 in range(0, B, MAX_CLIPS):
-                nb = min(MAX_CLIPS, B - b0)
-                p = EvalAppendParams(det=d.data_ptr() + b0 * cap * 8 * 4, count=cnt.data_ptr() + b0 * 4, B=nb, cap=cap,
-                                     ncls=len(self.class_of), class_of=self._class_of.data_ptr(), rows=self._rows())
+            for b0 in range(0, B, L.EVAL_MAX_CLIPS):
+                nb = min(L.EVAL_MAX_CLIPS, B - b0)
+                p = L.step_eval_append_params(det=d.data_ptr() + b0 * cap * 8 * 4, count=cnt.data_ptr() + b0 * 4, B=nb,
+                                              cap=cap, ncls=len(self.class_of), class_of=self._class_of.data_ptr(),
+                                              rows=self._rows())
                 p.img[:nb] = ids[b0:b0 + nb]
                 L.check(L.lib().step_eval_append(ctypes.byref(p), stream))
             self._host_counters.copy_(self._counters, non_blocking=True)
@@ -251,10 +232,10 @@ class FrameAP:
         t = {k: torch.from_numpy(v).to(dev) for k, v in
              (("box", box), ("cls", cls), ("off", off), ("num_gt", num_gt))}
         ws_bytes = L.lib().step_eval_workspace_bytes(n_kept, self.n_classes, box.shape[0])
-        p = EvalParams(rows=self._rows(), n_rows=n_kept, n_classes=self.n_classes, n_images=n_images, n_gt=box.shape[0],
-                       max_gt_per_image=max_gt, gt_box=_ptr(t["box"]) if box.shape[0] else None,
-                       gt_cls=_ptr(t["cls"]) if box.shape[0] else None, gt_img_off=_ptr(t["off"]), num_gt=_ptr(t["num_gt"]),
-                       workspace_bytes=ws_bytes)
+        p = L.step_eval_params(rows=self._rows(), n_rows=n_kept, n_classes=self.n_classes, n_images=n_images,
+                               n_gt=box.shape[0], max_gt_per_image=max_gt, gt_box=_ptr(t["box"]) if box.shape[0] else None,
+                               gt_cls=_ptr(t["cls"]) if box.shape[0] else None, gt_img_off=_ptr(t["off"]),
+                               num_gt=_ptr(t["num_gt"]), workspace_bytes=ws_bytes)
         ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
         ap = torch.empty((self.n_classes,), dtype=torch.float64, device=dev)
         p.workspace, p.ap = ws.data_ptr(), ap.data_ptr()

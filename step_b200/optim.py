@@ -11,8 +11,8 @@ import torch
 
 from . import _lib as L
 
-_ROW = np.dtype(L.OptimTensor)
-_BLOCK = np.dtype(L.OptimBlock)
+_ROW = np.dtype(L.step_optim_tensor)
+_BLOCK = np.dtype(L.step_optim_block)
 
 
 class _DeviceTables:

@@ -20,19 +20,8 @@ import torch
 
 from . import _lib as L
 
-SAMPLING = {"uniform": 0, "random": 1, "softmax": 2}
-MT_WORDS = 625
-
-
-class SelectParams(ctypes.Structure):
-    """mirror of step_select_params (include/step_b200.h)"""
-    _fields_ = [(n, ctypes.c_int) for n in
-                ("step", "B", "C", "L", "T", "Lout", "ext_mode", "max_chunks", "gt_mid", "predict_nb", "nb_first", "nb_last",
-                 "topk", "max_pos", "neg_ratio", "sampling", "max_rows", "n_max", "g_max", "prop_f64")] + \
-               [(n, ctypes.c_float) for n in ("cls_thresh", "reg_thresh", "width", "height")] + \
-               [(n, ctypes.c_longlong) for n in ("prob_sr", "prob_sl", "prob_sc")] + \
-               [(n, ctypes.c_void_p) for n in ("tube_off", "gt_off", "prob", "loc", "first", "last", "props", "targets", "mt",
-                                               "out_tubes", "out_targets", "counts")]
+SAMPLING = {"uniform": L.SAMPLING_UNIFORM, "random": L.SAMPLING_RANDOM, "softmax": L.SAMPLING_SOFTMAX}
+SelectParams = L.step_select_params   # the struct's name before it was read from the header
 
 
 def _ext_mode(cfg, i):
@@ -128,12 +117,13 @@ def select_samples(cfg, history, targets, tubes):
                 raise ValueError("select_samples: step %d's neighbour chunks %d / %d are outside the targets' %d chunks"
                                  % (i, nb_first, nb_last, max_chunks))
             nb_first, nb_last = nb_first % max_chunks, nb_last % max_chunks
-        p = SelectParams(step=i, B=B, C=C, T=T, Lout=T_length, ext_mode=ext, max_chunks=max_chunks,
-                         gt_mid=int(max_chunks / 2), predict_nb=int(predict_nb), nb_first=nb_first, nb_last=nb_last,
-                         topk=cfg.topk, max_pos=cfg.max_pos_num, neg_ratio=cfg.neg_ratio,
-                         sampling=SAMPLING[cfg.selection_sampling], max_rows=max_rows, n_max=max(nums), g_max=max(ngt),
-                         prop_f64=int(prop_f64), cls_thresh=cfg.cls_thresh[i - 1], reg_thresh=cfg.reg_thresh[i - 1],
-                         width=float(cfg.image_size[0]), height=float(cfg.image_size[1]), L=L1)
+        p = L.step_select_params(step=i, B=B, C=C, T=T, Lout=T_length, ext_mode=ext, max_chunks=max_chunks,
+                                 gt_mid=int(max_chunks / 2), predict_nb=int(predict_nb), nb_first=nb_first, nb_last=nb_last,
+                                 topk=cfg.topk, max_pos=cfg.max_pos_num, neg_ratio=cfg.neg_ratio,
+                                 sampling=SAMPLING[cfg.selection_sampling], max_rows=max_rows, n_max=max(nums),
+                                 g_max=max(ngt), prop_f64=int(prop_f64), cls_thresh=cfg.cls_thresh[i - 1],
+                                 reg_thresh=cfg.reg_thresh[i - 1], width=float(cfg.image_size[0]),
+                                 height=float(cfg.image_size[1]), L=L1)
         if i > 1:
             h = history[i - 2]
             prob, loc = h["pred_prob"], h["pred_loc"]
@@ -204,7 +194,7 @@ def select_samples(cfg, history, targets, tubes):
     words = back[:blob.offsets["counts"]].view(np.uint32)
     counts = back[blob.offsets["counts"]:head].view(np.int32).reshape(n_steps, B)
     np.random.set_state(("MT19937", words[:624].copy(), int(words[624]), np_state[3], np_state[4]))
-    random.setstate((py_state[0], tuple(int(v) for v in words[MT_WORDS:2 * MT_WORDS]), py_state[2]))
+    random.setstate((py_state[0], tuple(int(v) for v in words[L.SELECT_MT_WORDS:2 * L.SELECT_MT_WORDS]), py_state[2]))
     step_tubes = [o[0][:int(c.sum())] for o, c in zip(outs, counts)]
     step_targets = [o[1][:int(c.sum())] for o, c in zip(outs, counts)]
     return step_tubes, step_targets

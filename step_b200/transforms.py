@@ -35,14 +35,14 @@ def frame_entry(clip, W):
     if W0 > MAX_WIDTH_RATIO * W:
         raise ValueError("step_b200: source width %d exceeds %d x the output width %d" % (W0, MAX_WIDTH_RATIO, W))
     st = clip.stride()
-    return L.FrameSrc(clip.data_ptr(), H0, W0, st[0], st[1], st[2], st[3])
+    return L.step_frame_src(clip.data_ptr(), H0, W0, st[0], st[1], st[2], st[3])
 
 
 def frame_table(entries, device):
     """Uploads step_frame_src entries (one per clip) to `device` on the current stream; the returned tensor is the kernel's
     `table`.  The host copy is pinned, so the upload does not wait for the stream (torch keeps the pinned block until the
     copy has run)."""
-    return upload(bytes((L.FrameSrc * len(entries))(*entries)), device)
+    return upload(bytes((L.step_frame_src * len(entries))(*entries)), device)
 
 
 def upload(data, device):
@@ -394,7 +394,7 @@ class TubeAugmentation:
             if rec.crop[2] > MAX_WIDTH_RATIO * W:
                 raise ValueError("step_b200: crop width %d exceeds %d x the output width %d" % (rec.crop[2],
                                                                                                MAX_WIDTH_RATIO, W))
-            p = L.ClipAug(*rec.crop, int(rec.flip), int(rec.photometric))
+            p = L.step_clip_aug(*rec.crop, int(rec.flip), int(rec.photometric))
             for gate, name in (("brightness", "brightness_delta"), ("contrast", "contrast_alpha"),
                                ("saturation", "saturation_alpha"), ("hue", "hue_delta")):
                 v = getattr(rec, gate)
@@ -404,15 +404,15 @@ class TubeAugmentation:
             p.perm[:] = list(rec.perm)
             p.erase_begin, p.erase_count = len(erase), len(rec.erase)
             for x1, y1, x2, y2 in rec.erase:
-                erase.append(L.AugErase(x1, y1, x2, y2, n_noise))
+                erase.append(L.step_aug_erase(x1, y1, x2, y2, n_noise))
                 n_noise += (x2 - x1) * (y2 - y1) * 3
             if len(rec.noise) != sum((x2 - x1) * (y2 - y1) * 3 for x1, y1, x2, y2 in rec.erase):
                 raise ValueError("step_b200: recipe noise does not match its erase regions")
             noise.append(rec.noise)
             params.append(p)
         table = frame_table([frame_entry(c, W) for c in clips], device)
-        params_d = upload(bytes((L.ClipAug * len(params))(*params)), device)
-        erase_d = upload(bytes((L.AugErase * len(erase))(*erase)), device) if erase else None
+        params_d = upload(bytes((L.step_clip_aug * len(params))(*params)), device)
+        erase_d = upload(bytes((L.step_aug_erase * len(erase))(*erase)), device) if erase else None
         noise_d = None
         if n_noise:
             noise_d = torch.from_numpy(np.concatenate(noise).astype(np.float32)).pin_memory().to(device,

@@ -5,15 +5,12 @@ import ctypes
 
 import pytest
 
-STEP_E_ARG = 10001
+from step_b200 import _lib
 
 
 @pytest.fixture(scope="module")
 def lib():
-    from step_b200 import _lib
-    l = _lib.lib()
-    l.step_last_error.restype = ctypes.c_char_p
-    return l
+    return _lib.lib()
 
 
 @pytest.fixture(scope="module")
@@ -23,34 +20,30 @@ def fake():
 
 
 def rows(p, **kw):
-    from step_b200.evaluation import EvalRows
     d = dict(capacity=1000, counters=p, img_first=p, box=p, score=p, scode=p, img=p, cls=p)
     d.update(kw)
-    return EvalRows(**d)
+    return _lib.step_eval_rows(**d)
 
 
 def append_params(p, img=(0, 1), rows_kw=None, **kw):
-    from step_b200.evaluation import EvalAppendParams
     d = dict(det=p, count=p, B=len(img), cap=300, ncls=60, class_of=p, rows=rows(p, **(rows_kw or {})))
     d.update(kw)
-    prm = EvalAppendParams(**d)
+    prm = _lib.step_eval_append_params(**d)
     prm.img[:len(img)] = list(img)
     return prm
 
 
 def run_params(lib, p, rows_kw=None, **kw):
-    from step_b200.evaluation import EvalParams
     d = dict(rows=rows(p, **(rows_kw or {})), n_rows=500, n_classes=80, n_images=40, n_gt=100, max_gt_per_image=6,
              gt_box=p, gt_cls=p, gt_img_off=p, num_gt=p, workspace=p, ap=p)
     d.update(kw)
     d.setdefault("workspace_bytes", lib.step_eval_workspace_bytes(d["n_rows"], d["n_classes"], d["n_gt"]))
-    return EvalParams(**d)
+    return _lib.step_eval_params(**d)
 
 
 def expect(lib, fn, prm, *words):
-    from step_b200 import _lib
     before = _lib.launch_count()
-    assert fn(ctypes.byref(prm), None) == STEP_E_ARG
+    assert fn(ctypes.byref(prm), None) == _lib.E_ARG
     assert _lib.launch_count() == before
     msg = lib.step_last_error().decode()
     for w in words:
@@ -58,7 +51,6 @@ def expect(lib, fn, prm, *words):
 
 
 def test_checks_accept_good_arguments(lib, fake):
-    from step_b200 import _lib
     before = _lib.launch_count()
     assert lib.step_eval_append_check(ctypes.byref(append_params(fake[0]))) == 0
     assert lib.step_eval_check(ctypes.byref(run_params(lib, fake[0]))) == 0
@@ -84,7 +76,7 @@ def test_append_limits(lib, fake):
     expect(lib, lib.step_eval_append, append_params(p, img=(-2,)), "img[0] -2")
     expect(lib, lib.step_eval_append, append_params(p, rows_kw={"capacity": (1 << 30) + 1}), "rows.capacity")
     expect(lib, lib.step_eval_append, append_params(p, B=64, cap=(1 << 24) + 1), "B * cap")
-    assert lib.step_eval_append(None, None) == STEP_E_ARG
+    assert lib.step_eval_append(None, None) == _lib.E_ARG
 
 
 def test_run_limits_and_tables(lib, fake):
@@ -99,7 +91,7 @@ def test_run_limits_and_tables(lib, fake):
         expect(lib, lib.step_eval_run, run_params(lib, p, **{field: None}), "null pointer", field)
     expect(lib, lib.step_eval_run, run_params(lib, p, gt_box=None), "null pointer", "gt_box")
     assert lib.step_eval_check(ctypes.byref(run_params(lib, p, n_gt=0, gt_box=None, gt_cls=None))) == 0
-    assert lib.step_eval_run(None, None) == STEP_E_ARG
+    assert lib.step_eval_run(None, None) == _lib.E_ARG
 
 
 def test_frame_ap_rejects_bad_tables_without_cuda():

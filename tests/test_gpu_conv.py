@@ -110,7 +110,7 @@ def id_tensor(N, T, H, W, C):
 
 
 def conv_params(x, Cin, Cout, k, pad_lo, out_dims, a_mode, w):
-    p = L.ConvParams()
+    p = L.step_conv_params()
     p.dtype = L.F16
     p.N, p.T, p.H, p.W = x.shape[:4]
     p.Cin, p.in_ld = Cin, x.shape[4]

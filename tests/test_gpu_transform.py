@@ -83,7 +83,7 @@ def test_strided_sources_equal_the_contiguous_rgb_batch():
     bgr = torch.from_numpy(np.random.RandomState(5).randint(0, 256, (T, H0, W0, 3)).astype(np.uint8)).to(DEV)
     rgb = bgr.flip(-1).permute(0, 3, 1, 2).contiguous()
     want = tr.apply(rgb[None])
-    entry = L.FrameSrc(bgr.data_ptr() + 2, H0, W0, H0 * W0 * 3, -1, W0 * 3, 3)
+    entry = L.step_frame_src(bgr.data_ptr() + 2, H0, W0, H0 * W0 * 3, -1, W0 * 3, 3)
     out = torch.empty_like(want)
     tr.launch(frame_table([entry], torch.device(DEV)), 1, T, out)
     assert torch.equal(out, want)

@@ -6,16 +6,12 @@ import ctypes
 
 import pytest
 
-STEP_E_ARG = 10001
-F32, F16 = 0, 1
+from step_b200 import _lib
 
 
 @pytest.fixture(scope="module")
 def lib():
-    from step_b200 import _lib
-    l = _lib.lib()
-    l.step_last_error.restype = ctypes.c_char_p
-    return l
+    return _lib.lib()
 
 
 @pytest.fixture(scope="module")
@@ -25,14 +21,14 @@ def buf():
     return b, ctypes.c_void_p(addr)
 
 
-def fwd(lib, p, dtype=F32, K=9, H=8, W=8, C=16, feat_ld=16, R=4, out_ld=16, roi_T=3, feat_T=9, t_start=3, argmax="p",
+def fwd(lib, p, dtype=_lib.F32, K=9, H=8, W=8, C=16, feat_ld=16, R=4, out_ld=16, roi_T=3, feat_T=9, t_start=3, argmax="p",
         feat="p", rois="p", out="p"):
     pick = lambda v: p if v == "p" else v
     return lib.step_roi_pool_fwd_argmax_nhwc(pick(feat), dtype, K, H, W, C, feat_ld, pick(rois), R, 1.0 / 16.0, 7, 7, pick(out),
                                              out_ld, roi_T, feat_T, t_start, pick(argmax), None)
 
 
-def bwd(lib, p, dtype=F16, out_ld=16, R=4, K=9, H=8, W=8, C=16, roi_T=3, feat_T=9, t_start=3, in_ld=16, grad_out="p",
+def bwd(lib, p, dtype=_lib.F16, out_ld=16, R=4, K=9, H=8, W=8, C=16, roi_T=3, feat_T=9, t_start=3, in_ld=16, grad_out="p",
         argmax="p", rois="p", grad_in="p"):
     pick = lambda v: p if v == "p" else v
     return lib.step_roi_pool_bwd_slice_nhwc(pick(grad_out), dtype, out_ld, pick(argmax), pick(rois), R, 7, 7, K, H, W, C, roi_T,
@@ -40,7 +36,7 @@ def bwd(lib, p, dtype=F16, out_ld=16, R=4, K=9, H=8, W=8, C=16, roi_T=3, feat_T=
 
 
 def expect(lib, rc, *words):
-    assert rc == STEP_E_ARG
+    assert rc == _lib.E_ARG
     msg = lib.step_last_error().decode()
     for w in words:
         assert w in msg, (w, msg)
@@ -54,7 +50,7 @@ def test_forward_null_pointer(lib, buf, which):
 def test_forward_misaligned_channels_and_argmax(lib, buf):
     p = buf[1]
     expect(lib, fwd(lib, p, C=6, feat_ld=8, out_ld=8), "C=6", "multiples of 4")
-    expect(lib, fwd(lib, p, dtype=F16, C=12, feat_ld=16, out_ld=16), "C=12", "multiples of 8")
+    expect(lib, fwd(lib, p, dtype=_lib.F16, C=12, feat_ld=16, out_ld=16), "C=12", "multiples of 8")
     expect(lib, fwd(lib, p, feat_ld=18), "feat_ld=18")
     expect(lib, fwd(lib, p, argmax=ctypes.c_void_p(p.value + 4)), "argmax must be 16-byte aligned")
 

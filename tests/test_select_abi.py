@@ -5,15 +5,12 @@ import ctypes
 
 import pytest
 
-STEP_E_ARG = 10001
+from step_b200 import _lib
 
 
 @pytest.fixture(scope="module")
 def lib():
-    from step_b200 import _lib
-    l = _lib.lib()
-    l.step_last_error.restype = ctypes.c_char_p
-    return l
+    return _lib.lib()
 
 
 @pytest.fixture(scope="module")
@@ -23,18 +20,17 @@ def buf():
 
 
 def params(p, **kw):
-    from step_b200.select import SelectParams
     d = dict(step=2, B=2, C=60, L=3, T=3, Lout=9, ext_mode=1, max_chunks=3, gt_mid=1, predict_nb=0, nb_first=0, nb_last=2,
              topk=300, max_pos=5, neg_ratio=2, sampling=2, max_rows=15, n_max=34, g_max=3, prop_f64=1, cls_thresh=0.2,
              reg_thresh=0.2, width=400.0, height=400.0, prob_sr=60, prob_sl=0, prob_sc=1)
     d.update({k: p for k in ("tube_off", "gt_off", "prob", "loc", "first", "last", "props", "targets", "mt", "out_tubes",
                              "out_targets", "counts")})
     d.update(kw)
-    return SelectParams(**d)
+    return _lib.step_select_params(**d)
 
 
 def expect(lib, prm, *words):
-    assert lib.step_select_step_f32(ctypes.byref(prm), None) == STEP_E_ARG
+    assert lib.step_select_step_f32(ctypes.byref(prm), None) == _lib.E_ARG
     msg = lib.step_last_error().decode()
     for w in words:
         assert w in msg, (w, msg)
@@ -49,7 +45,7 @@ def test_null_step_inputs(lib, buf):
     expect(lib, params(buf[1], step=2, prob=None), "prob / loc")
     expect(lib, params(buf[1], step=2, first=None), "first / last")
     expect(lib, params(buf[1], step=1, ext_mode=0, Lout=3, props=None), "props")
-    assert lib.step_select_step_f32(None, None) == STEP_E_ARG
+    assert lib.step_select_step_f32(None, None) == _lib.E_ARG
 
 
 def test_rows_above_the_bound(lib, buf):
@@ -80,7 +76,7 @@ def test_check_entry_needs_no_pointer(lib, buf):
     """step_select_check_f32 runs the field and shared-memory checks alone: pointers may be null."""
     assert lib.step_select_check_f32(ctypes.byref(params(None))) == 0
     prm = params(None, n_max=5000, topk=-1)
-    assert lib.step_select_check_f32(ctypes.byref(prm)) == STEP_E_ARG
+    assert lib.step_select_check_f32(ctypes.byref(prm)) == _lib.E_ARG
     assert "shared memory" in lib.step_last_error().decode()
 
 

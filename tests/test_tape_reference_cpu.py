@@ -20,7 +20,6 @@ from step_b200 import _lib as L  # noqa: E402
 from step_b200 import engine as E  # noqa: E402
 from step_b200.engine import Act  # noqa: E402
 
-STEP_E_ARG, STEP_E_WORKSPACE = 10001, 10003
 HALF_ULP = 2.0 ** -11
 
 
@@ -254,9 +253,7 @@ def test_pool_reference_ties_and_asymmetric_padding(geom):
 # ---- argument checks of the backward entry points (no device work happens before them) --------------------------------
 @pytest.fixture(scope="module")
 def lib():
-    l = L.lib()
-    l.step_last_error.restype = ctypes.c_char_p
-    return l
+    return L.lib()
 
 
 @pytest.fixture(scope="module")
@@ -266,7 +263,7 @@ def buf():
     return b, ctypes.c_void_p(addr)
 
 
-def expect(lib, rc, *words, code=STEP_E_ARG):
+def expect(lib, rc, *words, code=L.E_ARG):
     assert rc == code
     msg = lib.step_last_error().decode()
     for w in words:
@@ -280,7 +277,7 @@ def act_bwd(lib, p, dy_ld=16, y_ld=16, relu=1, M=10, C=16, dz_ld=16, dres="p", d
 
 def test_act_bwd_rejects_partial_vectors_and_misalignment(lib, buf):
     p = buf[1]
-    assert act_bwd(lib, p, M=0) == STEP_E_ARG
+    assert act_bwd(lib, p, M=0) == L.E_ARG
     for kw in (dict(C=12), dict(dy_ld=20), dict(y_ld=12), dict(dz_ld=20), dict(dres_ld=12)):
         expect(lib, act_bwd(lib, p, **kw), "act_bwd: bad arguments")
     expect(lib, act_bwd(lib, p, y=None), "act_bwd: bad arguments")                 # the ReLU mask needs y
@@ -306,7 +303,7 @@ def test_conv_wgrad_rejects_bad_channels_alignment_padding_and_workspace(lib, bu
     expect(lib, wgrad(lib, p, k=(1, 1, 1), pad=(0, 1, 0)), "conv_wgrad: bad padding")  # a 1-tap filter has no padding
     expect(lib, wgrad(lib, p, ws=None), "conv_wgrad: bad arguments")
     need = lib.step_conv_wgrad_workspace_bytes(60, 16, 16, 27)
-    expect(lib, wgrad(lib, p, ws_bytes=need - 4), "workspace", code=STEP_E_WORKSPACE)
+    expect(lib, wgrad(lib, p, ws_bytes=need - 4), "workspace", code=L.E_WORKSPACE)
 
 
 def pool_bwd(lib, p, C=16, k=(3, 3, 3), s=(2, 2, 2), lo=(1, 1, 1), hi=(1, 1, 1), dims=(7, 9, 9), out=(4, 5, 5), x="p", ws="p"):

@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from oracle import transform as ot
+from step_b200 import _lib as L
 
 
 def golden_cases(golden):
@@ -47,7 +48,6 @@ def test_golden_covers_the_border_rows_and_the_area_switch(golden):
 
 
 def _call(table=16, B=1, T=1, H=8, W=8, scale=2, mean=True, std=True, out=16):
-    from step_b200 import _lib as L
     m = (ctypes.c_float * 3)(0, 0, 0) if mean else None
     s = (ctypes.c_float * 3)(1, 1, 1) if std else None
     rc = L.lib().step_frames_to_clip_u8(ctypes.c_void_p(table), B, T, H, W, scale, m, s, ctypes.c_void_p(out),
@@ -63,7 +63,7 @@ def _call(table=16, B=1, T=1, H=8, W=8, scale=2, mean=True, std=True, out=16):
 ])
 def test_frames_to_clip_argument_errors(kw, words):
     rc, msg = _call(**kw)
-    assert rc == 10001, (rc, msg)  # STEP_E_ARG
+    assert rc == L.E_ARG, (rc, msg)
     assert "frames_to_clip_u8" in msg and words in msg, msg
 
 
