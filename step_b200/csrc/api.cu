@@ -62,10 +62,9 @@ extern "C" int step_conv3d_fwd(const step_conv_params* p, step_stream_t stream) 
   if (p->a_mode == STEP_A_BEST) {
     // "best": thin inputs on large maps go to the patch kernel, which needs far fewer bytes through TMA than one
     // im2col tile per tap; on 7x7 maps its 16 x 8 pixel tile is mostly padding.  Everything else: TMA im2col (k > 1) / linear (1x1x1).
-    static const bool halo_on = !(getenv("STEP_B200_HALO") && getenv("STEP_B200_HALO")[0] == '0');
     const int taps = p->KT * p->KH * p->KW;
     const int small = p->OH < p->OW ? p->OH : p->OW;
-    if (halo_on && taps > 1 && p->ST == 1 && p->SH == 1 && p->SW == 1 && conv3d_halo_supported(p) &&
+    if (taps > 1 && p->ST == 1 && p->SH == 1 && p->SW == 1 && conv3d_halo_supported(p) &&
         p->Cin <= 32 && small >= 14)
       return conv3d_halo_launch(p, stream);
     step_conv_params q = *p;

@@ -83,8 +83,6 @@ bottleneck_exit_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_c
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
-  pdl_launch_dependents();
 
   if (warp < 4) {
     setmaxnreg_dec<kProducerRegs>();

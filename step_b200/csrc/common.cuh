@@ -35,15 +35,6 @@ inline cudaStream_t cu(step_stream_t s) { return reinterpret_cast<cudaStream_t>(
     }                                                                               \
   } while (0)
 
-// Programmatic dependent launch of the conv kernels is OPT-IN (STEP_B200_PDL=1).  History: with the earlier Blackwell (tcgen05)
-// kernels one bench.py run with three batches in flight stalled under it, cause not found.  It has not been measured or
-// stress-tested with the current wgmma kernels, so it stays off by default.
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("STEP_B200_PDL"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v == 1;
-}
-
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 constexpr int kNumSMs = 132;  // H100 SXM

@@ -73,8 +73,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     }
   }
   __syncthreads();
-  pdl_wait();                 // the producer of x (the previous kernel in the stream) has finished
-  pdl_launch_dependents();
 
   if (warp == 0) {
     // ===================== producer =====================

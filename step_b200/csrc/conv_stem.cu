@@ -110,8 +110,6 @@ conv_stem_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();                 // the producer of x (the previous kernel in the stream) has finished
-  pdl_launch_dependents();
 
   if (warp < 4) {
     // ===================== producer =====================

@@ -151,8 +151,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   };
   if (threadIdx.x < 128) stage_consts(blockIdx.x % g.n_tiles, 0, threadIdx.x, 128);
   __syncthreads();
-  pdl_wait();                 // the producer of x (the previous kernel in the stream) has finished
-  pdl_launch_dependents();
 
   if (warp < 4) {
     if constexpr (kRealloc) setmaxnreg_dec<kProducerRegs>();

@@ -90,62 +90,9 @@ __global__ void __launch_bounds__(256) maxpool3d_kernel(const T* __restrict__ x,
   }
 }
 
-// 3x3x3 / stride 1 / pad 1 (Mixed.branch_3, i3dpt.py:150-153) on maps whose width is a multiple of 7
-// (112/16 .. 7): one thread produces a 7-pixel output row segment for one 16-byte channel vector.  For
-// each of the 9 (kt, kh) input rows it loads the 9 columns once (consecutive lanes = consecutive channel
-// vectors: 512 contiguous bytes per warp per load), reduces them horizontally and folds the row into the
-// 7 accumulators: ~130 instead of ~460 instructions per output vector.
-template <typename T>
-__global__ void __launch_bounds__(256, 3) maxpool3d_333_kernel(const T* __restrict__ x, int N, int T_, int H, int W, int C,
-                                                            int in_ld, T* __restrict__ y, int out_ld) {
-  constexpr int VN = Vec16<T>::N, WB = 7;
-  const int nvec = C / VN, wsegs = W / WB;
-  const long long total = (long long)N * T_ * H * wsegs * nvec;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const int cv = (int)(idx % nvec);
-    long long r = idx / nvec;
-    const int ws = (int)(r % wsegs); r /= wsegs;
-    const int h = (int)(r % H); r /= H;
-    const int t = (int)(r % T_);
-    const int n = (int)(r / T_);
-    const int w0 = ws * WB;
-    uint4 acc[WB];
-#pragma unroll
-    for (int j = 0; j < WB; ++j) acc[j] = vec_lowest<T>();
-#pragma unroll
-    for (int dt = -1; dt <= 1; ++dt) {
-      const int tt = t + dt;
-      if (tt < 0 || tt >= T_) continue;
-#pragma unroll
-      for (int dh = -1; dh <= 1; ++dh) {
-        const int hh = h + dh;
-        if (hh < 0 || hh >= H) continue;
-        const T* rowp = x + ((((size_t)n * T_ + tt) * H + hh) * W + w0) * in_ld + cv * VN;
-        uint4 v[WB + 2];
-        v[0] = (w0 > 0) ? *reinterpret_cast<const uint4*>(rowp - in_ld) : vec_lowest<T>();
-#pragma unroll
-        for (int j = 0; j < WB; ++j) v[j + 1] = *reinterpret_cast<const uint4*>(rowp + (size_t)j * in_ld);
-        v[WB + 1] = (w0 + WB < W) ? *reinterpret_cast<const uint4*>(rowp + (size_t)WB * in_ld) : vec_lowest<T>();
-#pragma unroll
-        for (int j = 0; j < WB; ++j) acc[j] = vec_max<T>(acc[j], vec_max<T>(vec_max<T>(v[j], v[j + 1]), v[j + 2]));
-      }
-    }
-    // windows that overlap the zero padding see a 0 (ConstantPad3d, i3dpt.py:120)
-    const bool edge_th = (t == 0) || (t == T_ - 1) || (h == 0) || (h == H - 1);
-    T* orow = y + ((((size_t)n * T_ + t) * H + h) * W + w0) * out_ld + cv * VN;
-#pragma unroll
-    for (int j = 0; j < WB; ++j) {
-      uint4 m = acc[j];
-      if (edge_th || (w0 + j == 0) || (w0 + j == W - 1)) m = vec_max<T>(m, make_uint4(0, 0, 0, 0));
-      *reinterpret_cast<uint4*>(orow + (size_t)j * out_ld) = m;
-    }
-  }
-}
-
-
-// Same pooling, separable and marching along t: a thread owns a 7-pixel row segment x one 16-byte channel vector and
-// walks TS output planes.  For every input plane it loads the 3 x 9 neighbourhood once, reduces it over (h, w) into a
+// 3x3x3 / stride 1 / pad 1 (Mixed.branch_3, i3dpt.py:150-153) on maps whose width is a multiple of 7 (112/16 .. 7),
+// separable and marching along t: a thread owns a 7-pixel row segment x one 16-byte channel vector and walks TS output
+// planes.  For every input plane it loads the 3 x 9 neighbourhood once, reduces it over (h, w) into a
 // 7-vector P[tt], and emits out[t] = max(P[t-1], P[t], P[t+1]) from two carried 7-vectors: 27 loads and 70 vector
 // maxima per plane instead of 81 and 182 per output row.  The kernel is latency bound on the small maps, so the host
 // picks TS to keep ~50k threads in flight.
@@ -657,22 +604,9 @@ extern "C" int step_maxpool3d_fwd(const void* x, int dtype, int N, int T, int H,
   STEP_CHECK_ARG((((uintptr_t)x | (uintptr_t)y) & 15) == 0, "maxpool3d: pointers must be 16-byte aligned");
   if (KT == 3 && KH == 3 && KW == 3 && ST == 1 && SH == 1 && SW == 1 && PT == 1 && PH == 1 && PW == 1 && pad_hi_t == 1 &&
       pad_hi_h == 1 && pad_hi_w == 1 && OT == T && OH == H && OW == W && W % 7 == 0) {
-    const char* pv = getenv("STEP_B200_POOL333");
-    if (pv && pv[0] == '0') {   // previous kernel, kept for A/B timing
-      long long total = (long long)N * T * H * (W / 7) * (C / vn);
-      if (dtype == STEP_F16)
-        maxpool3d_333_kernel<__half><<<grid_for(total, 256), 256, 0, cu(stream)>>>((const __half*)x, N, T, H, W, C, in_ld,
-                                                                                   (__half*)y, out_ld);
-      else
-        maxpool3d_333_kernel<float><<<grid_for(total, 256), 256, 0, cu(stream)>>>((const float*)x, N, T, H, W, C, in_ld,
-                                                                                  (float*)y, out_ld);
-      STEP_LAUNCH_CHECK("maxpool3d_333_kernel");
-      return 0;
-    }
     const long long per_seg = (long long)N * H * (W / 7) * (C / vn);
     int TS = T;
     while (TS > 2 && per_seg * ceil_div(T, TS) < 50000) TS = (TS + 1) / 2;
-    if (pv && atoi(pv) >= 2) TS = atoi(pv) < T ? atoi(pv) : T;
     const long long total = per_seg * ceil_div(T, TS);
     STEP_CHECK_ARG(ceil_div(total, 128) < (1LL << 31), "maxpool3d: too many blocks");
     if (dtype == STEP_F16)
@@ -685,11 +619,9 @@ extern "C" int step_maxpool3d_fwd(const void* x, int dtype, int N, int T, int H,
     return 0;
   }
   {
-    const char* pm = getenv("STEP_B200_POOLMARCH");
-    const bool on = !(pm && pm[0] == '0');
     const bool k133 = KT == 1 && KH == 3 && KW == 3 && ST == 1 && SH == 2 && SW == 2;
     const bool k333 = KT == 3 && KH == 3 && KW == 3 && ST == 2 && SH == 2 && SW == 2;
-    if (on && (k133 || k333)) {
+    if (k133 || k333) {
       const int WB = k133 ? 7 : 4;
       const long long per_seg = (long long)N * OH * ceil_div(OW, WB) * (C / vn);
       int TS = k133 ? 1 : OT;
@@ -787,7 +719,7 @@ extern "C" int step_clip_to_s2d_f16(const float* clip, int N, int T, int Cc, int
   STEP_CHECK_ARG(T % 2 == 0 && H % 2 == 0 && W % 2 == 0 && ld >= 8 * Cc, "clip_to_s2d: T,H,W must be even, ld >= 8*Cc");
   STEP_CHECK_ARG(ld % 8 == 0 && ld <= 64 && 256 % (ld / 8) == 0 && (size_t)4 * Cc * W * sizeof(float) <= 48 * 1024, "clip_to_s2d: ld must divide 2048, row tile must fit 48 KB smem");
   STEP_CHECK_ARG(((uintptr_t)out & 15) == 0, "clip_to_s2d: out must be 16-byte aligned");
-  if (Cc == 3 && ld == 32 && ((uintptr_t)clip & 7) == 0 && ((uintptr_t)out & 31) == 0 && !(getenv("STEP_B200_S2D") && getenv("STEP_B200_S2D")[0] == '0')) {
+  if (Cc == 3 && ld == 32 && ((uintptr_t)clip & 7) == 0 && ((uintptr_t)out & 31) == 0) {
     const long long total = (long long)N * (T / 2) * (H / 2) * (W / 2);
     STEP_CHECK_ARG(ceil_div(total, 256) < (1LL << 31), "clip_to_s2d: too many pixels");
     clip_to_s2d_rgb_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, cu(stream)>>>(clip, N, T, H, W, (__half*)out);

@@ -250,20 +250,17 @@ __device__ __forceinline__ void hfma2x4(__half2* a, __half2 w, const uint4& v) {
 
 template <int V>
 __device__ __forceinline__ void roi_gather_items(const MergedBin* bins, int nbins, int nvec, const __half* fbase, __half* obase,
-                                                 int out_ld, int part, int parts) {
-  // this CTA handles channel vectors [cv0, cv0 + cnt) of every V-th of the row (blockIdx.y = part): small batches of
-  // ROIs (704 rows in the pipeline) are split over `parts` CTAs per row so that the gather is not one short wave
+                                                 int out_ld) {
   const int hv = nvec / V;
-  const int cnt = hv / parts, cv0 = part * cnt;
-  int bin = threadIdx.x / cnt, cv = threadIdx.x - bin * cnt;   // incremental (bin, cv): no per-item division
-  const int dbin = blockDim.x / cnt, dcv = blockDim.x - dbin * cnt;
+  int bin = threadIdx.x / hv, cv = threadIdx.x - bin * hv;   // incremental (bin, cv): no per-item division
+  const int dbin = blockDim.x / hv, dcv = blockDim.x - dbin * hv;
   const __half2 z2 = __float2half2_rn(0.0f);
   while (bin < nbins) {
     const MergedBin& b = bins[bin];
     __half2 acc[V][4];
 #pragma unroll
     for (int u = 0; u < V; ++u) acc[u][0] = acc[u][1] = acc[u][2] = acc[u][3] = z2;
-    const __half* fp = fbase + (cv0 + cv) * 8;
+    const __half* fp = fbase + cv * 8;
     const int n = b.n;
     int e = 0;
     for (; e + 1 < n; e += 2) {
@@ -284,11 +281,11 @@ __device__ __forceinline__ void roi_gather_items(const MergedBin* bins, int nbin
 #pragma unroll
       for (int u = 0; u < V; ++u) hfma2x4(acc[u], w0, *reinterpret_cast<const uint4*>(fp + e0.x + u * hv * 8));
     }
-    __half* op = obase + (size_t)bin * out_ld + (cv0 + cv) * 8;
+    __half* op = obase + (size_t)bin * out_ld + cv * 8;
 #pragma unroll
     for (int u = 0; u < V; ++u) *reinterpret_cast<uint4*>(op + u * hv * 8) = *reinterpret_cast<const uint4*>(acc[u]);
     bin += dbin; cv += dcv;
-    if (cv >= cnt) { cv -= cnt; ++bin; }
+    if (cv >= hv) { cv -= hv; ++bin; }
   }
 }
 
@@ -303,9 +300,7 @@ __global__ void __launch_bounds__(256, 5) roi_align_fwd_nhwc_f16_packed_kernel(c
   const RoiGeom g = roi_geometry(rois + 5 * (size_t)r, scale, ph, pw, sampling_ratio);
   const int nbins = ph * pw;
   const __half* fbase = feat + (size_t)fm.map(g.batch) * H * W * feat_ld;
-  __half* obase = out + (size_t)r * nbins * out_ld;
   const int nvec = C >> 3;
-  const int part = blockIdx.y, parts = gridDim.y;
   // Distinct pixels one bin can touch, per axis: g + 1 when its g samples are at most one pixel apart (the bin is no wider
   // than g pixels, always so for the adaptive grid), else two per sample.
   const int nh = g.bin_h <= (float)g.gh ? g.gh + 1 : 2 * g.gh, nw = g.bin_w <= (float)g.gw ? g.gw + 1 : 2 * g.gw;
@@ -313,9 +308,9 @@ __global__ void __launch_bounds__(256, 5) roi_align_fwd_nhwc_f16_packed_kernel(c
     // a bin may not fit the table (sampling grid > 3x3, or a fixed sampling_ratio with bins wider than the grid):
     // direct form with fp32 FMAs, no table
     const float ic = 1.0f / g.count;
-    const int pv = nvec / parts, pv0 = part * pv;
-    for (int item = threadIdx.x; item < nbins * pv; item += blockDim.x) {
-      const int bin = item / pv, cv = pv0 + item - bin * pv;
+    __half* obase = out + (size_t)r * nbins * out_ld;
+    for (int item = threadIdx.x; item < nbins * nvec; item += blockDim.x) {
+      const int bin = item / nvec, cv = item - bin * nvec;
       const int p = bin / pw, q = bin - p * pw;
       float acc[8];
 #pragma unroll
@@ -370,8 +365,10 @@ __global__ void __launch_bounds__(256, 5) roi_align_fwd_nhwc_f16_packed_kernel(c
   __syncthreads();
   // Gather: an item is (bin, V channel vectors a V-th of a row apart): the 8-byte table entry (pixel offset, merged
   // weight) is read once for V 16-byte vectors, and two entries are in flight per iteration (2V independent loads).
-  if ((nvec & 1) == 0) roi_gather_items<2>(bins, nbins, nvec, fbase, obase, out_ld, part, parts);
-  else roi_gather_items<1>(bins, nbins, nvec, fbase, obase, out_ld, part, parts);
+  // formed here, not before the table build: held across it, obase spills under the 51-register bound
+  __half* obase = out + (size_t)r * nbins * out_ld;
+  if ((nvec & 1) == 0) roi_gather_items<2>(bins, nbins, nvec, fbase, obase, out_ld);
+  else roi_gather_items<1>(bins, nbins, nvec, fbase, obase, out_ld);
 }
 
 // kArgmax (training): also record, per output element, the frame-local pixel h*W + w of the maximum in `argmax`
@@ -509,14 +506,8 @@ extern "C" int step_roi_align_fwd_nhwc(const void* feat, int dtype, int K, int H
   FrameMap fm{roi_T, feat_T, t_start};
   if (dtype == STEP_F16 && exact == 0 && (size_t)ph * pw * sizeof(MergedBin) <= 48 * 1024 &&
       (long long)H * W * feat_ld < (1LL << 31)) {   // table entries hold 32-bit element offsets inside one frame
-    // One CTA per ROI row by default.  Splitting a row's channels over several CTAs (STEP_B200_ROI_PARTS=2|4, kept for A/B)
-    // makes every part rebuild the row's tap table.
-    int parts = 1;
-    if (const char* e = getenv("STEP_B200_ROI_PARTS")) {
-      const int nvec = C / 8, hv = (nvec & 1) == 0 ? nvec / 2 : nvec, v = atoi(e);
-      if (v >= 1 && hv % v == 0 && nvec % v == 0) parts = v;
-    }
-    roi_align_fwd_nhwc_f16_packed_kernel<<<dim3(R, parts), 128 * (parts > 1 ? 1 : 2), (size_t)ph * pw * sizeof(MergedBin), cu(stream)>>>(
+    // one CTA per ROI row: the row's tap table is built once, in shared memory
+    roi_align_fwd_nhwc_f16_packed_kernel<<<R, 256, (size_t)ph * pw * sizeof(MergedBin), cu(stream)>>>(
         (const __half*)feat, H, W, C, feat_ld, rois, scale, ph, pw, sampling_ratio, (__half*)out, out_ld, fm);
     STEP_LAUNCH_CHECK("roi_align_fwd_nhwc_f16_packed_kernel");
     return 0;

@@ -239,13 +239,6 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// Programmatic dependent launch (cudaLaunchAttributeProgrammaticStreamSerialization): a kernel launched with the attribute
-// may start while its predecessor in the stream is still running; everything up to pdl_wait() (barrier init, descriptor
-// prefetch, constant loads) overlaps the predecessor's tail.  pdl_wait() returns once the predecessor grid has completed
-// and its writes are visible; pdl_launch_dependents() lets the NEXT kernel start early.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -344,19 +337,12 @@ inline int encode_rows2d(CUtensorMap* map, const void* base, long long rows, int
   return encode_tiled_f16(map, base, 2, dims, strides, box, swizzle, l2, label);
 }
 
-// Launch of a TMA + wgmma kernel: programmatic dependent launch when pdl_enabled() (the kernels order their reads of the
-// previous kernel's output behind pdl_wait()), launch errors reported naming the kernel, and the launch counted.
+// Launch of a TMA + wgmma kernel: launch errors reported naming the kernel, and the launch counted.
 template <typename... Params, typename... Args>
 inline int launch_tc(const char* name, void (*kernel)(Params...), dim3 grid, int threads, size_t smem, cudaStream_t stream,
                      Args&&... args) {
   cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
   cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  if (pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-  }
   const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
   if (e != cudaSuccess) { cudaGetLastError(); return fail((int)e, "%s launch: %s", name, cudaGetErrorString(e)); }
   STEP_LAUNCH_CHECK(name);

@@ -1,6 +1,6 @@
-"""CPU: the C-ABI library loads and exports every symbol include/step_b200.h declares; the ctypes binding read from the
-header has the C compiler's struct layouts and constants, and its reader refuses what it cannot read; the product never
-imports the oracle; no compute calls are made here (no GPU in this tier)."""
+"""CPU: the C-ABI library loads, exports every symbol include/step_b200.h declares and reads no environment variable; the
+ctypes binding read from the header has the C compiler's struct layouts and constants, and its reader refuses what it
+cannot read; the product never imports the oracle; no compute calls are made here (no GPU in this tier)."""
 import ctypes
 import os
 import re
@@ -33,6 +33,19 @@ def test_library_is_sm90a_native():
     out = subprocess.run(["cuobjdump", "-lelf", os.path.join(ROOT, "step_b200", "libstep_b200.so")],
                          capture_output=True, text=True).stdout
     assert "sm_90a" in out
+
+
+def test_library_reads_no_environment():
+    """A call's result and speed follow from its arguments alone: no object of the library calls getenv.  The objects are
+    checked, not the .so, because the .so links cudart statically and cudart reads its own variables."""
+    from step_b200 import build
+    build.build()
+    readers = []
+    for src in build.SOURCES:
+        obj = os.path.join(build.OBJ, src.replace(".cu", ".o"))
+        out = subprocess.run(["nm", "--undefined-only", obj], capture_output=True, text=True, check=True).stdout
+        readers += ["%s: %s" % (src, s) for s in out.split() if s in ("getenv", "secure_getenv")]
+    assert not readers, readers
 
 
 def test_product_never_touches_the_oracle():

@@ -22,7 +22,6 @@ sampling_ratio 0..4; the ROIs of the ROIAlign backward's edge test (the whole im
 edges), 40 overlapping ROIs on one frame and 200 random ones.  The strided layout reads a channel slice at an offset of a
 wider feature row, writes rows of pitch C + 8 into a canary-filled buffer (the columns past C and the rows of other ROIs
 stay bit-identical) and maps ROI frames through (roi_T, feat_T, t_start), with NaN in the frames it must never read.
-Every exact=0 launch is repeated with STEP_B200_ROI_PARTS=2 and 4 (a row split over 2 or 4 CTAs): bit-identical.
 """
 import json
 import os
@@ -147,12 +146,11 @@ class Layout:
         return R.roi_frames(rois, *self.fmap) if self.strided else R.roi_frames(rois)
 
 
-def _check(feat32, rois_cpu, ph, pw, sr, strided, monkeypatch, what):
+def _check(feat32, rois_cpu, ph, pw, sr, strided, what):
     K, H, W, C = feat32.shape
     n = rois_cpu.shape[0]
     rois = rois_cpu.cuda()
     lay = Layout(strided, feat32, n, ph, pw)
-    monkeypatch.delenv("STEP_B200_ROI_PARTS", raising=False)
 
     # exact=1: the C oracle on the mapped frames, fp32 bit for bit, fp16 = fp16(exact fp32) on the fp16 inputs
     direct_rois = rois_cpu.clone()
@@ -188,13 +186,6 @@ def _check(feat32, rois_cpu, ph, pw, sr, strided, monkeypatch, what):
     if bool(table.any()):
         tol = R.roi_align_tol(out_abs[table], float(feat32.abs().max()))
         _note("packed table", R._check_within(packed[table], ref[table], tol, what + ("exact=0 table",)))
-    nvec = C // 8
-    hv = nvec // 2 if nvec % 2 == 0 else nvec
-    for parts in (2, 4):
-        monkeypatch.setenv("STEP_B200_ROI_PARTS", str(parts))
-        split = lay.run(torch.float16, rois, sr, 0).cpu()
-        monkeypatch.delenv("STEP_B200_ROI_PARTS")
-        assert torch.equal(split, packed), (what, "STEP_B200_ROI_PARTS=%d" % parts, hv % parts == 0)
     return dict(spb=spb, big_grid=big_grid, wide=wide, overflow=overflow, table=table)
 
 
@@ -210,12 +201,12 @@ BINS = [(7, 7), (5, 3), (1, 1), (19, 19), (20, 20)]
 @pytest.mark.parametrize("C,strided", [(8, False), (24, True), (64, False), (64, True)])
 @pytest.mark.parametrize("bins", BINS, ids=["%dx%d" % b for b in BINS])
 @pytest.mark.parametrize("sr", [0, 1, 2, 3, 4])
-def test_roi_align_fwd_edges(C, strided, bins, sr, monkeypatch):
+def test_roi_align_fwd_edges(C, strided, bins, sr):
     ph, pw = bins
     H = W = 28
     rois = _rois()
     feat = _feat(8 if strided else 4, H, W, C, 52 + C + sr)
-    p = _check(feat, rois, ph, pw, sr, strided, monkeypatch, ("edges", C, strided, bins, sr))
+    p = _check(feat, rois, ph, pw, sr, strided, ("edges", C, strided, bins, sr))
     # the dispatch this sweep relies on, so that a change to a threshold is noticed
     if bins == (7, 7) and sr == 0:
         assert int(p["spb"][0]) * 49 == TAPS and int(p["spb"][2]) == 25   # a full cached table and an uncached one
@@ -232,11 +223,11 @@ def test_roi_align_fwd_edges(C, strided, bins, sr, monkeypatch):
 
 
 @pytest.mark.parametrize("sr", [0, 1, 2, 3, 4])
-def test_roi_align_fwd_shipped_map(sr, monkeypatch):
+def test_roi_align_fwd_shipped_map(sr):
     """The shipped map, 25 x 25 x 832 (C / 8 = 104: roi_gather_items<2>), 7 x 7 bins, with the strided layout."""
     rois = _rois(100, seed=53)
     feat = _feat(8, 25, 25, 832, 54 + sr)
-    _check(feat, rois, 7, 7, sr, True, monkeypatch, ("shipped", sr))
+    _check(feat, rois, 7, 7, sr, True, ("shipped", sr))
 
 
 REACH = [r"roi_align_fwd_nhwc_f16_packed_kernel", r"roi_align_fwd_nhwc_kernel<__half, ?false>",
