@@ -78,6 +78,19 @@ int step_detect_f32(const float* prob, int prob_ld, const float* loc, int loc_ld
                     int n_clips, int n_rows, int max_per_clip, int ncls, float conf_thresh, float nms_thresh,
                     int ge, float valid_w, float valid_h, float norm_w, float norm_h, int topk, int cap,
                     uint8_t* keep, float* score, float* box, float* det, int* det_count, step_stream_t stream);
+/* Class-only detections of the classification pre-training stage's validation (train_cls.py:505-543) in one launch: for
+ * every clip, class and row of the clip, in that order (the reference's file order), the row's class score when it is
+ * > conf_thresh (scores.gt), with the row's box divided by (norm_w, norm_h) in float32.  No valid_tubes clamp, no NMS, no
+ * top-k.  prob [n_rows, prob_ld >= ncls]; the box of row r at box + r*box_ld (the centre frame of a flat tube, e.g.
+ * flat_tubes[:, T/2, 1:5]); clip_offsets as for step_detect_f32, at most max_per_clip rows per clip.  det [n_clips, cap, 8]
+ * = {x1, y1, x2, y2, score, class, row in clip, 0}, det_count [n_clips]; cap >= max_per_clip * ncls, so no row is cut. */
+int step_detect_scores_f32(const float* prob, int prob_ld, const float* box, int box_ld, const int* clip_offsets,
+                           int n_clips, int n_rows, int max_per_clip, int ncls, float conf_thresh, float norm_w,
+                           float norm_h, int cap, float* det, int* det_count, step_stream_t stream);
+/* The checks of step_detect_scores_f32, with no launch. */
+int step_detect_scores_check(const float* prob, int prob_ld, const float* box, int box_ld, const int* clip_offsets,
+                             int n_clips, int n_rows, int max_per_clip, int ncls, int cap, const float* det,
+                             const int* det_count);
 
 /* ------------------------------------------------------------------ ROI ops -------------- */
 /* Reference layout (NCHW fp32 in, [R,C,ph,pw] fp32 out), arithmetic order of the reference. */
@@ -462,7 +475,13 @@ typedef struct {
   float* out_tubes;          /* [B * max_rows, Lout, 5], rows packed clip after clip */
   float* out_targets;        /* [B * max_rows, 3, 6 + C] */
   int32_t* counts;           /* [B] rows of each clip */
+  int target_mode;           /* STEP_TARGETS_*: the rows of train_select (0, the zero-initialised default) or train_cls.py */
 } step_select_params;
+/* step_select_params.target_mode.  STEP_TARGETS_CLS writes the rows of the classification pre-training stage
+ * (train_cls.py:271-291): a positive carries its ground truth's box, classification flag 1 and labels, a negative only
+ * classification flag 1; the regression flag stays 0 and the three rows of a sample are the same.  It needs step 1,
+ * STEP_EXT_NONE and predict_nb 0. */
+enum { STEP_TARGETS_SELECT = 0, STEP_TARGETS_CLS = 1 };
 /* One CTA walks the clips in order: candidates, IoU, positive assignment, the draws from the two generators, and the
  * selected rows.  STEP_E_ARG before any launch when an argument is out of range. */
 int step_select_step_f32(const step_select_params* p, step_stream_t stream);

@@ -328,6 +328,34 @@ __global__ void __launch_bounds__(256) detect_select_kernel(const uint8_t* __res
   }
 }
 
+// ---- class-only detections (train_cls.py:505-543): no valid_tubes clamp, no NMS, no top-k --------------------------
+// One CTA per clip.  Candidate i = class * n_clip + proposal is the reference's file order (clip, class, proposal
+// ascending); the ballot scan thresholds each candidate (scores.gt), counts the passing ones and writes them compactly:
+// det[clip][slot] = {x1/nw, y1/nh, x2/nw, y2/nh, score, class, proposal, 0}, box = the proposal's centre frame.
+__global__ void __launch_bounds__(256) detect_scores_kernel(const float* __restrict__ prob, int prob_ld,
+                                                            const float* __restrict__ box, int box_ld,
+                                                            const int* __restrict__ clip_offsets, int ncls, float conf,
+                                                            float nw, float nh, int cap, float* __restrict__ det,
+                                                            int* __restrict__ det_count) {
+  const int clip = blockIdx.x;
+  const int beg = clip_offsets[clip], n = clip_offsets[clip + 1] - beg;
+  const int cands = n > 0 ? n * ncls : 0;
+  auto score = [&](int i) {
+    const int c = i / n;
+    return prob[(size_t)(beg + i - c * n) * prob_ld + c];
+  };
+  const int m = ballot_compact<8>(cands, [&](int i) { return (int)(score(i) > conf); }, [&](int i, int slot) {
+    if (slot >= cap) return;   // the host sizes cap for every candidate; never write past it
+    const int c = i / n, j = i - c * n;
+    const float* b = box + (size_t)(beg + j) * box_ld;
+    float* o = det + ((size_t)clip * cap + slot) * 8;
+    // train_cls.py:533-534, numpy float32 division by the image size
+    o[0] = __fdiv_rn(b[0], nw); o[1] = __fdiv_rn(b[1], nh); o[2] = __fdiv_rn(b[2], nw); o[3] = __fdiv_rn(b[3], nh);
+    o[4] = score(i); o[5] = (float)c; o[6] = (float)j; o[7] = 0.0f;
+  });
+  if (threadIdx.x == 0) det_count[clip] = m < cap ? m : cap;
+}
+
 static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 }  // namespace step
@@ -410,5 +438,31 @@ extern "C" int step_detect_f32(const float* prob, int prob_ld, const float* loc,
   STEP_LAUNCH_CHECK("detect_nms_kernel");
   detect_select_kernel<<<n_clips, 256, 0, s>>>(keep, score, (const float4*)box, clip_offsets, ncls, topk, cap, det, det_count);
   STEP_LAUNCH_CHECK("detect_select_kernel");
+  return 0;
+}
+
+extern "C" int step_detect_scores_check(const float* prob, int prob_ld, const float* box, int box_ld, const int* clip_offsets,
+                                        int n_clips, int n_rows, int max_per_clip, int ncls, int cap, const float* det,
+                                        const int* det_count) {
+  STEP_CHECK_ARG(n_clips >= 0 && n_rows >= 0 && ncls > 0 && max_per_clip >= 0 && max_per_clip <= n_rows,
+                 "step_detect_scores_f32: bad sizes (n_clips %d, n_rows %d, max_per_clip %d, ncls %d)", n_clips, n_rows,
+                 max_per_clip, ncls);
+  if (n_clips == 0) return 0;
+  STEP_CHECK_ARG(prob && box && clip_offsets && det && det_count, "step_detect_scores_f32: null pointer");
+  STEP_CHECK_ARG(prob_ld >= ncls && box_ld >= 4, "step_detect_scores_f32: bad strides (prob_ld %d, box_ld %d)", prob_ld, box_ld);
+  STEP_CHECK_ARG(cap > 0 && (long long)max_per_clip * ncls <= cap,
+                 "step_detect_scores_f32: cap %d below max_per_clip %d * ncls %d", cap, max_per_clip, ncls);
+  return 0;
+}
+
+extern "C" int step_detect_scores_f32(const float* prob, int prob_ld, const float* box, int box_ld, const int* clip_offsets,
+                                      int n_clips, int n_rows, int max_per_clip, int ncls, float conf_thresh, float norm_w,
+                                      float norm_h, int cap, float* det, int* det_count, step_stream_t stream) {
+  const int rc = step_detect_scores_check(prob, prob_ld, box, box_ld, clip_offsets, n_clips, n_rows, max_per_clip, ncls, cap,
+                                          det, det_count);
+  if (rc || n_clips == 0) return rc;
+  detect_scores_kernel<<<n_clips, 256, 0, cu(stream)>>>(prob, prob_ld, box, box_ld, clip_offsets, ncls, conf_thresh, norm_w,
+                                                        norm_h, cap, det, det_count);
+  STEP_LAUNCH_CHECK("detect_scores_kernel");
   return 0;
 }

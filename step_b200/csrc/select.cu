@@ -6,6 +6,7 @@
 // Arithmetic follows numpy's types: float32 operations are rounded one at a time (the file is built with -fmad=false),
 // the choice weights and their cdf are float64.  Two parity contracts (README.md): every argsort(x)[::-1] is a
 // stable ascending argsort reversed, and the softmax weights use the correctly rounded float32(exp(float64(x))).
+// target_mode STEP_TARGETS_CLS writes the rows of train_cls.py:271-291 instead (step 1 only): same IoU, assignment and draws.
 #include <limits.h>
 
 #include "common.cuh"
@@ -401,7 +402,10 @@ __global__ void __launch_bounds__(kSelThreads) select_step_kernel(step_select_pa
       const int g = pairs[r].x, j = pairs[r].y;
       const bool pos = r < npos;
       float v = 0.0f;
-      if (k == 1) {
+      if (p.target_mode == STEP_TARGETS_CLS) {   // train_cls.py:274-288: one centre row, copied to all three
+        const float* src = tg + ((size_t)g * p.max_chunks + p.gt_mid) * TC;
+        v = col == 4 ? 1.0f : col == 5 || !pos ? 0.0f : col < 4 ? src[col] : src[col - 2];
+      } else if (k == 1) {
         if (pos || iou[g * Nc + j] >= p.reg_thresh) {
           const float* src = tg + ((size_t)g * p.max_chunks + p.gt_mid) * TC;
           v = col < 4 ? src[col] : col == 4 ? (pos ? 1.0f : 0.0f) : col == 5 ? 1.0f : src[col - 2];
@@ -435,6 +439,11 @@ static int select_check_fields(const step_select_params* p, int* K_out, int* pai
   STEP_CHECK_ARG(p->Lout == p->L + (p->ext_mode != STEP_EXT_NONE ? 2 * p->T : 0),
                  "select_step: T_length %d does not match L=%d, T=%d and ext_mode %d", p->Lout, p->L, p->T, p->ext_mode);
   STEP_CHECK_ARG(p->ext_mode != STEP_EXT_EXTRAPOLATE || (p->T >= 2 && p->L >= p->T), "select_step: EXTRAPOLATE needs L >= T >= 2");
+  STEP_CHECK_ARG(p->target_mode == STEP_TARGETS_SELECT || p->target_mode == STEP_TARGETS_CLS, "select_step: bad target_mode %d",
+                 p->target_mode);
+  STEP_CHECK_ARG(p->target_mode != STEP_TARGETS_CLS || (p->step == 1 && p->ext_mode == STEP_EXT_NONE && !p->predict_nb),
+                 "select_step: target_mode %d needs step 1, no extension and no neighbour rows (step %d, ext_mode %d, "
+                 "predict_nb %d)", p->target_mode, p->step, p->ext_mode, p->predict_nb);
   STEP_CHECK_ARG(p->max_chunks >= 1 && p->gt_mid >= 0 && p->gt_mid < p->max_chunks, "select_step: gt_mid %d outside %d chunks",
                  p->gt_mid, p->max_chunks);
   STEP_CHECK_ARG(!p->predict_nb || (p->nb_first >= 0 && p->nb_first < p->max_chunks && p->nb_last >= 0 && p->nb_last < p->max_chunks),

@@ -71,6 +71,46 @@ class Detector:
                 "tubes_nums": self.nums}
 
 
+class ClsDetector:
+    """The class-only detections of the classification pre-training stage's validation (train_cls.py:505-543) in one
+    launch of `step_detect_scores_f32`: for every clip, class and proposal (the reference's file order), the proposal's
+    score when it is > conf_thresh, with its centre-frame box divided by (width, height) in float32.  No valid_tubes clamp,
+    no NMS, no top-k.  The result has Detector.run's layout, so FrameAP.add_detections takes it; `run` only launches
+    (no allocation for float32 inputs, no synchronisation), so it can be captured in a CUDA graph."""
+
+    def __init__(self, tubes_nums, num_classes, device, conf_thresh, width, height):
+        self.nums = [int(n) for n in tubes_nums]
+        self.B, self.R, self.ncls = len(self.nums), int(sum(self.nums)), int(num_classes)
+        self.max_n = max(self.nums) if self.nums else 0
+        self.conf, self.w, self.h = float(conf_thresh), float(width), float(height)
+        self.cap = max(1, self.max_n * self.ncls)       # every row of a clip fits: nothing is cut
+        self.offs = _plan(self.nums, device)
+        self.det = torch.zeros((max(self.B, 1), self.cap, 8), dtype=torch.float32, device=device)
+        self.count = torch.zeros((max(self.B, 1),), dtype=torch.int32, device=device)
+
+    def run(self, global_prob, flat_tubes):
+        """global_prob [R, cls] (the class-only head's output; any row stride), flat_tubes [R, T, 5] (frame index first)."""
+        L.need_cuda(global_prob, flat_tubes)
+        prob = global_prob
+        if prob.dtype != torch.float32 or prob.dim() != 2 or prob.stride(1) != 1:
+            prob = prob.float().reshape(prob.shape[0], -1).contiguous()
+        if flat_tubes.dtype != torch.float32 or not flat_tubes.is_contiguous():
+            flat_tubes = flat_tubes.float().contiguous()
+        if prob.shape[0] != self.R or prob.shape[1] != self.ncls:
+            raise RuntimeError("detect_scores: expected %d x %d scores, got %s" % (self.R, self.ncls, tuple(global_prob.shape)))
+        if flat_tubes.dim() != 3 or flat_tubes.shape[0] != self.R or flat_tubes.shape[2] != 5:
+            raise RuntimeError("detect_scores: expected [%d, T, 5] tubes, got %s" % (self.R, tuple(flat_tubes.shape)))
+        T = flat_tubes.shape[1]
+        box = flat_tubes.data_ptr() + ((T // 2) * 5 + 1) * 4                        # flat_tubes[:, T // 2, 1:5]
+        if self.R and self.B:
+            with torch.cuda.device(prob.device):
+                L.check(L.lib().step_detect_scores_f32(L.ptr(prob), prob.stride(0), L.c_void_p(box), flat_tubes.stride(0),
+                                                       L.ptr(self.offs), self.B, self.R, self.max_n, self.ncls, self.conf,
+                                                       self.w, self.h, self.cap, L.ptr(self.det), L.ptr(self.count),
+                                                       L.stream(prob.device)))
+        return {"det": self.det, "count": self.count, "tubes_nums": self.nums}
+
+
 def detect(pred_prob, pred_loc, tubes_nums, conf_thresh, nms_thresh, width, height, topk=0, valid_size=(400, 400)):
     """pred_prob [R,T,cls] | [R,cls], pred_loc [R,T,4] (history[i] of `inference`), all on the device.
     Returns device tensors, no synchronisation:

@@ -1,5 +1,7 @@
 """`select_samples()` -- the training-sample selection of train.py:291-310 on the device: for every refinement step
 `train_select` (utils/utils.py:135-340, `select_proposals` at :342-423) and the two `flatten_tubes` calls after it.
+`select_cls_samples()` -- the same for the classification pre-training stage (train_cls.py:260-297): `select_proposals`
+with that stage's rows, one launch of the same kernel in its train_cls row mode.
 
 The reference copies the history to the host at every step, ranks the candidates with numpy and Python sorts, draws
 with `random.shuffle` and `np.random.choice`, and uploads the result.  Here one host-to-device copy carries the targets,
@@ -67,6 +69,21 @@ class _Blob:
         for o, a in self.parts:
             buf[o:o + a.nbytes] = a.reshape(-1).view(np.uint8)
         return buf
+
+
+def _add_states(blob):
+    """numpy's global RandomState, then Python's `random`, as the kernel's two MT19937 words ("mt"); returns the states
+    for _restore_states."""
+    np_state, py_state = np.random.get_state(), random.getstate()
+    blob.add("mt", np.concatenate([np.asarray(np_state[1], np.uint32), [np.uint32(np_state[2])],
+                                   np.asarray(py_state[1], np.uint32)]))
+    return np_state, py_state
+
+
+def _restore_states(words, np_state, py_state):
+    """Leaves both generators where the kernel left its copies (words: the read-back "mt" section)."""
+    np.random.set_state(("MT19937", words[:624].copy(), int(words[624]), np_state[3], np_state[4]))
+    random.setstate((py_state[0], tuple(int(v) for v in words[L.SELECT_MT_WORDS:2 * L.SELECT_MT_WORDS]), py_state[2]))
 
 
 def select_samples(cfg, history, targets, tubes):
@@ -147,10 +164,8 @@ def select_samples(cfg, history, targets, tubes):
     L.need_cuda(*tensors)
     dev = history[0]["pred_loc"].device if n_steps > 1 else torch.device("cuda", torch.cuda.current_device())
 
-    np_state, py_state = np.random.get_state(), random.getstate()
     blob = _Blob()
-    blob.add("mt", np.concatenate([np.asarray(np_state[1], np.uint32), [np.uint32(np_state[2])],
-                                   np.asarray(py_state[1], np.uint32)]))
+    np_state, py_state = _add_states(blob)
     blob.add("counts", np.zeros(n_steps * B, np.int32))
     blob.add("tube_off", np.concatenate([[0], np.cumsum(nums)]).astype(np.int32))
     blob.add("gt_off", np.concatenate([[0], np.cumsum(ngt)]).astype(np.int32))
@@ -193,8 +208,73 @@ def select_samples(cfg, history, targets, tubes):
         back = dbuf[:head].cpu().numpy()                 # the one synchronisation
     words = back[:blob.offsets["counts"]].view(np.uint32)
     counts = back[blob.offsets["counts"]:head].view(np.int32).reshape(n_steps, B)
-    np.random.set_state(("MT19937", words[:624].copy(), int(words[624]), np_state[3], np_state[4]))
-    random.setstate((py_state[0], tuple(int(v) for v in words[L.SELECT_MT_WORDS:2 * L.SELECT_MT_WORDS]), py_state[2]))
+    _restore_states(words, np_state, py_state)
     step_tubes = [o[0][:int(c.sum())] for o, c in zip(outs, counts)]
     step_targets = [o[1][:int(c.sum())] for o, c in zip(outs, counts)]
     return step_tubes, step_targets
+
+
+def select_cls_samples(targets, tubes, num_classes, cls_thresh=0.75, max_pos_num=5, sampling="uniform", neg_ratio=3):
+    """Same result as train_cls.py:260-297: per clip select_proposals(targets[b][:, 0], tubes[b][:, T // 2], None,
+    cls_thresh, max_pos_num, sampling, neg_ratio) with the stage's rows, then flatten_tubes of the targets and (with the
+    frame index first) of the selected tubes.  The defaults are train_cls.py's literals.
+
+    targets / tubes: the loader's numpy lists, [n_gt_b, chunks, 4 + C] (chunk 0 is read: the stage's max_chunks is 1) and
+    [n_b, T, 4] per clip (float64, as its sample_anchors makes them, or float32).
+    Rows: a positive carries its ground truth's box, classification flag 1 and labels; a negative classification flag 1
+    only; the regression flag is 0, and the three target rows of a sample are the same.
+    Consumes numpy's global RandomState and Python's `random` as the reference does, and leaves them where it leaves them.
+    Returns (flat_tubes [R, T, 5], flat_targets [R, 3, 6 + C]), fp32 on the current CUDA device -- what
+    training.train_step takes for the class-only heads."""
+    if len(targets) != len(tubes) or len(targets) == 0:
+        raise ValueError("select_cls_samples: %d target lists for %d proposal lists" % (len(targets), len(tubes)))
+    for b, (g, t) in enumerate(zip(targets, tubes)):
+        if np.asarray(g).shape[0] == 0:
+            raise ValueError("select_cls_samples: clip %d has no ground truth" % b)
+        if np.asarray(t).shape[0] == 0:
+            raise ValueError("select_cls_samples: clip %d has no proposals" % b)
+    if sampling not in SAMPLING:
+        raise ValueError("select_cls_samples: sampling %r is not one of %s" % (sampling, tuple(SAMPLING)))
+    if max_pos_num < 0 or neg_ratio < 0:
+        raise ValueError("select_cls_samples: max_pos_num and neg_ratio must be >= 0")
+    B, C = len(targets), int(num_classes)
+    tg = [np.asarray(g, dtype=np.float32) for g in targets]
+    chunks = tg[0].shape[1] if tg[0].ndim == 3 else 0
+    for b, g in enumerate(tg):
+        if g.ndim != 3 or g.shape[1] < 1 or g.shape[1:] != (chunks, 4 + C):
+            raise ValueError("select_cls_samples: targets[%d] has shape %s, expected [n_gt, %d, %d]"
+                             % (b, g.shape, max(chunks, 1), 4 + C))
+    props = [np.asarray(t) for t in tubes]
+    T = props[0].shape[1] if props[0].ndim == 3 else 0
+    for b, p in enumerate(props):
+        if p.ndim != 3 or T < 1 or p.shape[1:] != (T, 4):
+            raise ValueError("select_cls_samples: tubes[%d] has shape %s, expected [n, %d, 4]" % (b, p.shape, max(T, 1)))
+    nums, ngt = [p.shape[0] for p in props], [g.shape[0] for g in tg]
+    max_rows = max_pos_num * (1 + neg_ratio)
+    p = L.step_select_params(step=1, B=B, C=C, L=T, T=T, Lout=T, ext_mode=L.EXT_NONE, max_chunks=chunks, gt_mid=0,
+                             max_pos=max_pos_num, neg_ratio=neg_ratio, sampling=SAMPLING[sampling], max_rows=max_rows,
+                             n_max=max(nums), g_max=max(ngt), prop_f64=int(any(q.dtype == np.float64 for q in props)),
+                             cls_thresh=float(cls_thresh), target_mode=L.TARGETS_CLS)
+    L.check(L.lib().step_select_check_f32(ctypes.byref(p)))
+    dev = torch.device("cuda", torch.cuda.current_device())
+
+    blob = _Blob()
+    np_state, py_state = _add_states(blob)
+    blob.add("counts", np.zeros(B, np.int32))
+    blob.add("tube_off", np.concatenate([[0], np.cumsum(nums)]).astype(np.int32))
+    blob.add("gt_off", np.concatenate([[0], np.cumsum(ngt)]).astype(np.int32))
+    blob.add("targets", np.concatenate(tg))
+    blob.add("props", np.concatenate([q.astype(np.float64) for q in props]))
+    dbuf = torch.from_numpy(blob.pack()).to(dev)
+    at = lambda name: dbuf.data_ptr() + blob.offsets[name]
+    head = blob.offsets["counts"] + 4 * B                    # the states and the counts: what comes back
+    rows = max(B * max_rows, 1)
+    out_t = torch.empty((rows, T, 5), dtype=torch.float32, device=dev)
+    out_g = torch.empty((rows, 3, 6 + C), dtype=torch.float32, device=dev)
+    p.tube_off, p.gt_off, p.targets, p.props, p.mt = at("tube_off"), at("gt_off"), at("targets"), at("props"), at("mt")
+    p.out_tubes, p.out_targets, p.counts = out_t.data_ptr(), out_g.data_ptr(), at("counts")
+    L.check(L.lib().step_select_step_f32(ctypes.byref(p), L.stream()))
+    back = dbuf[:head].cpu().numpy()                         # the one synchronisation
+    _restore_states(back[:blob.offsets["counts"]].view(np.uint32), np_state, py_state)
+    R = int(back[blob.offsets["counts"]:head].view(np.int32).sum())
+    return out_t[:R], out_g[:R]
