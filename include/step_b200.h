@@ -395,6 +395,28 @@ int step_maxpool3d_bwd_f16(const void* x, int x_ld, const void* dy, int dy_ld, i
                            int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
                            int pad_hi_w, int OT, int OH, int OW, void* dx, int dx_ld, uint8_t* argmax_ws, step_stream_t stream);
 
+/* The fp32 training path (cfg.fp16 = False: fp32 activations and activation gradients).
+ * Weight gradient of a convolution with any filter, stride and low padding on the CUDA cores (fp32 FFMA, no TF32):
+ * dw[Cout, taps, dw_ld >= Cin] (+)= scale * sum_m dz[m, co] x[src(m, tap), ci] over the N*OT*OH*OW output pixels m, where
+ * tap (kt, kh, kw) of output pixel (n, ot, oh, ow) reads input pixel (n, ot*ST + kt - PT, oh*SH + kh - PH, ow*SW + kw - PW)
+ * of x [N, T, H, W] (zero outside).  dz [M, dz_ld], x [N*T*H*W, x_ld]; Cout, Cin and the strides multiples of 4; 16-byte
+ * aligned operands.  The pixel chunks' partial sums are added in a fixed order: bit-identical from run to run. */
+size_t step_conv_wgrad_f32_workspace_bytes(long long M, int Cout, int Cin, int taps);
+int step_conv_wgrad_f32(const float* dz, int dz_ld, const float* x, int x_ld, int N, int T, int H, int W, int OT, int OH,
+                        int OW, int Cout, int Cin, int KT, int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW,
+                        float scale, float* dw, int dw_ld, int accumulate, void* workspace, size_t ws_bytes,
+                        step_stream_t stream);
+/* fp32 storage siblings of step_act_bwd_f16 (C and the ld arguments multiples of 4), step_colsum_f16, step_mean_mid_bwd,
+ * step_f32_accum_f16 and step_maxpool3d_bwd_f16, with the same arithmetic in fp32 and no rounding to fp16. */
+int step_act_bwd_f32(const float* dy, int dy_ld, const float* y, int y_ld, const float* scale, int relu, long long M, int C,
+                     float* dz, int dz_ld, float* dres, int dres_ld, step_stream_t stream);
+int step_colsum_f32(const float* x, int ld, long long M, int C, float scale, float* out, float* workspace, step_stream_t stream);
+int step_mean_mid_bwd_f32(const float* g, int A, int B, int P, int C, float gscale, float* dx, int ld, step_stream_t stream);
+int step_f32_accum_f32(const float* src, long long M, int C, float gscale, float* dst, int ld, step_stream_t stream);
+int step_maxpool3d_bwd_f32(const float* x, int x_ld, const float* dy, int dy_ld, int N, int T, int H, int W, int C, int KT,
+                           int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
+                           int pad_hi_w, int OT, int OH, int OW, float* dx, int dx_ld, uint8_t* argmax_ws, step_stream_t stream);
+
 /* ------------------------------------------------------------------ optimizer ------------ */
 /* Multi-tensor parameter update (train.py:123-128, 345-348): one launch over every tensor of a parameter set, described by a
  * device table of step_optim_tensor rows and a device block map.  Row r describes one fp32 tensor of `numel` contiguous

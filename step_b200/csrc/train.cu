@@ -426,46 +426,50 @@ __global__ void __launch_bounds__(256) linear_bwd_dx_kernel(const float* __restr
 // y = relu(scale * conv + shift (+ residual))  (Unit3Dpy, i3dpt.py:103-111; Bottleneck, two_branch.py:60-111):
 //   dz = dy * [y > 0] * scale      gradient w.r.t. the raw convolution output (operand of dgrad / wgrad)
 //   dres += dy * [y > 0]           gradient flowing into the residual input, accumulated in place
-// dy / y / dres are channel slices of wider fp16 buffers (ld, coff); dz is dense [M, C] at dz_ld / dz_coff.
-__global__ void __launch_bounds__(256) act_bwd_kernel(const __half* __restrict__ dy, int dy_ld, const __half* __restrict__ y,
+// dy / y / dres are channel slices of wider buffers of T (fp16 or fp32; ld, coff); dz is dense [M, C] at dz_ld / dz_coff.
+// One thread per 16-byte vector (8 fp16 or 4 fp32 channels).
+template <typename T>
+__global__ void __launch_bounds__(256) act_bwd_kernel(const T* __restrict__ dy, int dy_ld, const T* __restrict__ y,
                                                       int y_ld, const float* __restrict__ scale, int relu, long long M, int C,
-                                                      __half* __restrict__ dz, int dz_ld, __half* __restrict__ dres,
+                                                      T* __restrict__ dz, int dz_ld, T* __restrict__ dres,
                                                       int dres_ld) {
-  const int cv = C >> 3;
+  constexpr int V = Vec16<T>::N, LOG_V = V == 8 ? 3 : 2;
+  const int cv = C >> LOG_V;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= M * cv) return;
   const long long m = i / cv;
-  const int c = (int)(i - m * cv) * 8;
-  float g[8], v[8];
+  const int c = (int)(i - m * cv) * V;
+  float g[V], v[V];
   load16(dy + (size_t)m * dy_ld + c, g);
   if (relu) {
     load16(y + (size_t)m * y_ld + c, v);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) g[k] = v[k] > 0.0f ? g[k] : 0.0f;
+    for (int k = 0; k < V; ++k) g[k] = v[k] > 0.0f ? g[k] : 0.0f;
   }
   if (dres) {
-    float r[8];
+    float r[V];
     load16(dres + (size_t)m * dres_ld + c, r);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) r[k] += g[k];
+    for (int k = 0; k < V; ++k) r[k] += g[k];
     store16(dres + (size_t)m * dres_ld + c, r);
   }
   if (scale) {
 #pragma unroll
-    for (int k = 0; k < 8; ++k) g[k] *= scale[c + k];
+    for (int k = 0; k < V; ++k) g[k] *= scale[c + k];
   }
   store16(dz + (size_t)m * dz_ld + c, g);
 }
 
-// column sums of a [M, C] fp16 matrix in fp32 (bias gradients), fixed order: thread per column block, rows ascending in
-// chunks that a second pass adds in chunk order
-__global__ void __launch_bounds__(256) colsum_partial_kernel(const __half* __restrict__ x, int ld, long long M, int C, int rows_per,
+// column sums of a [M, C] fp16 / fp32 matrix in fp32 (bias gradients), fixed order: thread per column block, rows ascending
+// in chunks that a second pass adds in chunk order
+template <typename T>
+__global__ void __launch_bounds__(256) colsum_partial_kernel(const T* __restrict__ x, int ld, long long M, int C, int rows_per,
                                                              float* __restrict__ partial) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const long long m0 = (long long)blockIdx.y * rows_per, m1 = m0 + rows_per < M ? m0 + rows_per : M;
   float acc = 0.0f;
-  for (long long m = m0; m < m1; ++m) acc += __half2float(x[(size_t)m * ld + c]);
+  for (long long m = m0; m < m1; ++m) acc += to_f32<T>(x[(size_t)m * ld + c]);
   partial[(size_t)blockIdx.y * C + c] = acc;
 }
 __global__ void __launch_bounds__(256) colsum_reduce_kernel(const float* __restrict__ partial, int chunks, int C, float scale,
@@ -478,8 +482,9 @@ __global__ void __launch_bounds__(256) colsum_reduce_kernel(const float* __restr
 }
 
 // temporal-mean backward (two_branch.py:249: the class scores are averaged over T'):  dx[a][b][p][c] += g[a][p*C + c] / B
+template <typename T>
 __global__ void __launch_bounds__(256) mean_mid_bwd_kernel(const float* __restrict__ g, int A, int B, int P, int C, float gscale,
-                                                           __half* __restrict__ dx, int ld) {
+                                                           T* __restrict__ dx, int ld) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)A * B * P * C) return;
   const int c = (int)(i % C);
@@ -487,8 +492,8 @@ __global__ void __launch_bounds__(256) mean_mid_bwd_kernel(const float* __restri
   const int p = (int)(r % P); r /= P;
   const int b = (int)(r % B);
   const int a = (int)(r / B);
-  __half* d = dx + ((((size_t)a * B + b) * P + p) * ld + c);
-  *d = __float2half_rn(__half2float(*d) + g[(size_t)a * P * C + (size_t)p * C + c] * gscale / (float)B);
+  T* d = dx + ((((size_t)a * B + b) * P + p) * ld + c);
+  *d = from_f32<T>(to_f32<T>(*d) + g[(size_t)a * P * C + (size_t)p * C + c] * gscale / (float)B);
 }
 
 // fp32 [M, C] (scaled) accumulated into an fp16 channel slice
@@ -502,13 +507,25 @@ __global__ void __launch_bounds__(256) f32_accum_f16_kernel(const float* __restr
   *d = __float2half_rn(__half2float(*d) + src[i] * gscale);
 }
 
+// the same into an fp32 channel slice (the fp32 training path)
+__global__ void __launch_bounds__(256) f32_accum_f32_kernel(const float* __restrict__ src, long long M, int C, float gscale,
+                                                            float* __restrict__ dst, int ld) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M * C) return;
+  const long long m = i / C;
+  const int c = (int)(i - m * C);
+  float* d = dst + (size_t)m * ld + c;
+  *d = *d + src[i] * gscale;
+}
+
 // ---- max-pool backward (MaxPool3dTFPadding, i3dpt.py:114-126: zero ConstantPad3d, then MaxPool3d) ---------------------------
 // Pass 1 (per output): which tap of the window holds the maximum -- first maximum in (kt, kh, kw) scan order with '>' like
 // ATen's max_pool3d_with_indices; a padded position holds the value 0 and takes part (its gradient is dropped).
 // Pass 2 (per input): gather dy from the windows whose recorded tap points at this input.  No atomics.
 struct PoolGeom { int N, T, H, W, C, KT, KH, KW, ST, SH, SW, PT, PH, PW, OT, OH, OW, QT, QH, QW; };   // Q*: high-side zero padding
 
-__global__ void __launch_bounds__(256) maxpool_argmax_kernel(PoolGeom g, const __half* __restrict__ x, int x_ld,
+template <typename T>
+__global__ void __launch_bounds__(256) maxpool_argmax_kernel(PoolGeom g, const T* __restrict__ x, int x_ld,
                                                              uint8_t* __restrict__ arg) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)g.N * g.OT * g.OH * g.OW * g.C;
@@ -531,14 +548,15 @@ __global__ void __launch_bounds__(256) maxpool_argmax_kernel(PoolGeom g, const _
                    pad_w = w < 0 || (w >= g.W && w < g.W + g.QW);
         if (!((in_t || pad_t) && (in_h || pad_h) && (in_w || pad_w))) continue;
         const bool real = in_t && in_h && in_w;
-        const float v = real ? __half2float(x[((((size_t)n * g.T + t) * g.H + h) * g.W + w) * x_ld + c]) : 0.0f;
+        const float v = real ? to_f32<T>(x[((((size_t)n * g.T + t) * g.H + h) * g.W + w) * x_ld + c]) : 0.0f;
         if (bi < 0 || v > best) { best = v; bi = real ? tap : 254; }
       }
   arg[i] = (uint8_t)(bi < 0 ? 255 : bi);
 }
 
-__global__ void __launch_bounds__(256) maxpool_bwd_kernel(PoolGeom g, const __half* __restrict__ dy, int dy_ld,
-                                                          const uint8_t* __restrict__ arg, __half* __restrict__ dx, int dx_ld) {
+template <typename T>
+__global__ void __launch_bounds__(256) maxpool_bwd_kernel(PoolGeom g, const T* __restrict__ dy, int dy_ld,
+                                                          const uint8_t* __restrict__ arg, T* __restrict__ dx, int dx_ld) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)g.N * g.T * g.H * g.W * g.C;
   if (i >= total) return;
@@ -566,12 +584,12 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(PoolGeom g, const __ha
         const int ow = wn / g.SW;
         if (ow >= g.OW) continue;
         const size_t o = (((size_t)n * g.OT + ot) * g.OH + oh) * g.OW + ow;
-        if (arg[o * g.C + c] == (uint8_t)((kt * g.KH + kh) * g.KW + kw)) acc += __half2float(dy[o * dy_ld + c]);
+        if (arg[o * g.C + c] == (uint8_t)((kt * g.KH + kh) * g.KW + kw)) acc += to_f32<T>(dy[o * dy_ld + c]);
       }
     }
   }
-  __half* d = dx + ((((size_t)n * g.T + t) * g.H + h) * g.W + w) * dx_ld + c;
-  *d = __float2half_rn(__half2float(*d) + acc);
+  T* d = dx + ((((size_t)n * g.T + t) * g.H + h) * g.W + w) * dx_ld + c;
+  *d = from_f32<T>(to_f32<T>(*d) + acc);
 }
 
 // ---- 1x1 convolution weight gradient on the tensor cores ------------------------------------------------------------
@@ -657,6 +675,127 @@ __global__ void __launch_bounds__(256) conv1x1_wgrad_reduce_kernel(const float* 
   for (int c = 0; c < chunks; ++c) acc += partial[off + (size_t)c * stride];   // chunk order: deterministic
   float* d = dw + ((size_t)co * taps + tap) * dw_ld + ci;
   *d = accumulate ? *d + acc * scale : acc * scale;
+}
+
+
+// ---- fp32 weight gradient of a 3-D convolution on the CUDA cores (the fp32 training path) ---------------------------
+// dW[co][tap][ci] = sum_m dz[m][co] * x[src(m, tap)][ci] over the output pixels m = (n, ot, oh, ow), where tap (kt, kh, kw)
+// reads input pixel (n, ot * ST + kt - PT, oh * SH + kh - PH, ow * SW + kw - PW) of the [N, T, H, W] input, zero outside
+// it (the TF-"SAME" padding, i3dpt.py:14-31, with its high side implied by the output extent).  As a GEMM: rows co,
+// columns j = tap * Cin + ci (Cin % 4 == 0, so the 4 columns of a vector share a tap), reduction over m.  Folding the taps
+// into the columns keeps thin inputs such as the fp32 stem (Cin = 4, 343 taps) as dense as wide ones.
+// A CTA owns a 64 (co) x 64 (j) tile for one chunk of pixels: 16 pixels of both operands are staged per step in shared
+// memory (double-buffered, the next step's 16-byte loads in flight during the current FFMAs), and each of the 256 threads
+// accumulates a 4 x 4 register tile with fmaf -- fp32 FFMA throughout, no TF32.  Partial tiles land in the workspace and a
+// second kernel adds them in chunk order, so the result is bit-identical from run to run.
+constexpr int kWfTile = 64, kWfStep = 16;
+constexpr int kWfTargetCtas = 2048;   // chunks per tile are chosen for about this many CTAs (a shape-only rule: deterministic)
+constexpr int kWfMinChunk = 256;      // pixels
+
+struct WfGeom {
+  int T, H, W, OT, OH, OW, KH, KW, ST, SH, SW, PT, PH, PW;
+  int Cin, cols;                      // cols = taps * Cin
+  int M, chunk;                       // output pixels, pixels per chunk (a multiple of kWfStep)
+};
+
+__global__ void __launch_bounds__(256) conv_wgrad_f32_partial_kernel(const float* __restrict__ dz, int dz_ld,
+                                                                     const float* __restrict__ x, int x_ld, int Cout, WfGeom g,
+                                                                     float* __restrict__ partial) {
+  __shared__ __align__(16) float sA[2][kWfStep][kWfTile + 4];   // sA[k][co]
+  __shared__ __align__(16) float sB[2][kWfStep][kWfTile + 4];   // sB[k][j]
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;    // compute: co ty*4.., j tx*4..
+  const int lr = tid >> 4, lv = tid & 15;                       // staging: pixel row lr, 4-channel vector lv
+  const int co0 = blockIdx.x * kWfTile, j0 = blockIdx.y * kWfTile;
+  const int m_beg = blockIdx.z * g.chunk, m_end = min(g.M, m_beg + g.chunk);
+  const int co_l = co0 + lv * 4, j_l = j0 + lv * 4;
+  const bool a_ok = co_l < Cout, b_ok = j_l < g.cols;
+  int dkt = 0, dkh = 0, dkw = 0, ci = 0;
+  if (b_ok) {
+    const int tap = j_l / g.Cin;
+    ci = j_l - tap * g.Cin;
+    dkw = tap % g.KW - g.PW;
+    dkh = (tap / g.KW) % g.KH - g.PH;
+    dkt = tap / (g.KW * g.KH) - g.PT;
+  }
+  float4 ra, rb;
+  auto load = [&](int m0) {
+    const int m = m0 + lr;
+    ra = make_float4(0.f, 0.f, 0.f, 0.f);
+    rb = ra;
+    if (m >= m_end) return;
+    if (a_ok) ra = *reinterpret_cast<const float4*>(dz + (size_t)m * dz_ld + co_l);
+    if (b_ok) {
+      const int ow = m % g.OW, r1 = m / g.OW, oh = r1 % g.OH, r2 = r1 / g.OH, ot = r2 % g.OT, n = r2 / g.OT;
+      const int it = ot * g.ST + dkt, ih = oh * g.SH + dkh, iw = ow * g.SW + dkw;
+      if (it >= 0 && it < g.T && ih >= 0 && ih < g.H && iw >= 0 && iw < g.W)
+        rb = *reinterpret_cast<const float4*>(x + ((((size_t)n * g.T + it) * g.H + ih) * g.W + iw) * x_ld + ci);
+    }
+  };
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+  load(m_beg);
+  int buf = 0;
+  for (int m0 = m_beg; m0 < m_end; m0 += kWfStep) {
+    // one barrier per step: the buffer written here was last read two steps ago, before the previous barrier
+    *reinterpret_cast<float4*>(&sA[buf][lr][lv * 4]) = ra;
+    *reinterpret_cast<float4*>(&sB[buf][lr][lv * 4]) = rb;
+    __syncthreads();
+    if (m0 + kWfStep < m_end) load(m0 + kWfStep);
+#pragma unroll
+    for (int k = 0; k < kWfStep; ++k) {
+      const float4 a = *reinterpret_cast<const float4*>(&sA[buf][k][ty * 4]);
+      const float4 b = *reinterpret_cast<const float4*>(&sB[buf][k][tx * 4]);
+      const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+    }
+    buf ^= 1;
+  }
+  // partial tiles [chunk][j tile][co tile][64 x 64]
+  float* out = partial + (((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * (kWfTile * kWfTile);
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    *reinterpret_cast<float4*>(out + (ty * 4 + i) * kWfTile + tx * 4) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+}
+
+// dw[co][tap][ci] (dw_ld >= Cin) = scale * (sum of the chunks' partial tiles in chunk order) (+ dw when accumulate)
+__global__ void __launch_bounds__(256) conv_wgrad_f32_reduce_kernel(const float* __restrict__ partial, int chunks, int tiles_co,
+                                                                    int tiles_j, int Cout, int Cin, int cols, float scale,
+                                                                    float* __restrict__ dw, int dw_ld, int accumulate) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)Cout * cols) return;
+  const int co = (int)(i / cols), j = (int)(i - (long long)co * cols);
+  const int tco = co / kWfTile, tj = j / kWfTile;
+  const size_t off = ((size_t)tj * tiles_co + tco) * (kWfTile * kWfTile) + (size_t)(co - tco * kWfTile) * kWfTile + (j - tj * kWfTile);
+  const size_t stride = (size_t)tiles_co * tiles_j * (kWfTile * kWfTile);
+  float acc = 0.0f;
+  for (int c = 0; c < chunks; ++c) acc += partial[off + (size_t)c * stride];
+  const int tap = j / Cin, ci = j - tap * Cin;
+  const int taps = cols / Cin;
+  float* d = dw + ((size_t)co * taps + tap) * dw_ld + ci;
+  *d = accumulate ? *d + acc * scale : acc * scale;
+}
+
+// The chunk plan of step_conv_wgrad_f32: a function of the shape alone, so that the summation order does not depend on
+// the device.
+struct WfPlan { int tiles_co, tiles_j, chunks, chunk; };
+inline WfPlan wgrad_f32_plan(long long M, int Cout, long long cols) {
+  WfPlan p;
+  p.tiles_co = ceil_div(Cout, kWfTile);
+  p.tiles_j = ceil_div(cols, kWfTile);
+  const long long tiles = (long long)p.tiles_co * p.tiles_j;
+  long long want = (kWfTargetCtas + tiles - 1) / tiles;
+  const long long most = (M + kWfMinChunk - 1) / kWfMinChunk;
+  want = want < 1 ? 1 : (want > most ? most : want);
+  const long long per = (M + want - 1) / want;
+  p.chunk = (int)((per + kWfStep - 1) / kWfStep * kWfStep);
+  p.chunks = ceil_div(M, p.chunk);
+  return p;
 }
 
 }  // namespace step
@@ -858,34 +997,65 @@ extern "C" int step_conv_wgrad_f16(const void* dz, int dz_ld, const void* x, int
   return 0;
 }
 
-extern "C" int step_act_bwd_f16(const void* dy, int dy_ld, const void* y, int y_ld, const float* scale, int relu, long long M, int C,
-                                void* dz, int dz_ld, void* dres, int dres_ld, step_stream_t stream) {
-  STEP_CHECK_ARG(M > 0 && C > 0 && C % 8 == 0 && dy_ld % 8 == 0 && dz_ld % 8 == 0 && dy && dz && (!relu || (y && y_ld % 8 == 0)) &&
-                 (!dres || dres_ld % 8 == 0), "act_bwd: bad arguments");
+template <typename T>
+static int act_bwd_launch(const void* dy, int dy_ld, const void* y, int y_ld, const float* scale, int relu, long long M, int C,
+                          void* dz, int dz_ld, void* dres, int dres_ld, step_stream_t stream) {
+  constexpr int V = Vec16<T>::N;
+  STEP_CHECK_ARG(M > 0 && C > 0 && C % V == 0 && dy_ld % V == 0 && dz_ld % V == 0 && dy && dz && (!relu || (y && y_ld % V == 0)) &&
+                 (!dres || dres_ld % V == 0), "act_bwd: bad arguments");
   STEP_CHECK_ARG((((uintptr_t)dy | (uintptr_t)y | (uintptr_t)dz | (uintptr_t)dres) & 15) == 0, "act_bwd: pointers must be 16-byte aligned");
-  act_bwd_kernel<<<ceil_div(M * (C / 8), 256), 256, 0, cu(stream)>>>((const __half*)dy, dy_ld, (const __half*)y, y_ld, scale, relu, M, C,
-                                                                    (__half*)dz, dz_ld, (__half*)dres, dres_ld);
+  act_bwd_kernel<T><<<ceil_div(M * (C / V), 256), 256, 0, cu(stream)>>>((const T*)dy, dy_ld, (const T*)y, y_ld, scale, relu, M, C,
+                                                                        (T*)dz, dz_ld, (T*)dres, dres_ld);
   STEP_LAUNCH_CHECK("act_bwd_kernel");
   return 0;
 }
 
-extern "C" int step_colsum_f16(const void* x, int ld, long long M, int C, float scale, float* out, float* workspace /* >= 64*C floats */,
-                               step_stream_t stream) {
+extern "C" int step_act_bwd_f16(const void* dy, int dy_ld, const void* y, int y_ld, const float* scale, int relu, long long M, int C,
+                                void* dz, int dz_ld, void* dres, int dres_ld, step_stream_t stream) {
+  return act_bwd_launch<__half>(dy, dy_ld, y, y_ld, scale, relu, M, C, dz, dz_ld, dres, dres_ld, stream);
+}
+
+extern "C" int step_act_bwd_f32(const float* dy, int dy_ld, const float* y, int y_ld, const float* scale, int relu, long long M, int C,
+                                float* dz, int dz_ld, float* dres, int dres_ld, step_stream_t stream) {
+  return act_bwd_launch<float>(dy, dy_ld, y, y_ld, scale, relu, M, C, dz, dz_ld, dres, dres_ld, stream);
+}
+
+template <typename T>
+static int colsum_launch(const void* x, int ld, long long M, int C, float scale, float* out, float* workspace, step_stream_t stream) {
   STEP_CHECK_ARG(x && out && workspace && M > 0 && C > 0, "colsum: bad arguments");
   const int chunks = (int)(M < 64 ? M : 64);
   const int rows_per = ceil_div(M, chunks);
-  colsum_partial_kernel<<<dim3(ceil_div(C, 256), chunks), 256, 0, cu(stream)>>>((const __half*)x, ld, M, C, rows_per, workspace);
+  colsum_partial_kernel<T><<<dim3(ceil_div(C, 256), chunks), 256, 0, cu(stream)>>>((const T*)x, ld, M, C, rows_per, workspace);
   STEP_LAUNCH_CHECK("colsum_partial_kernel");
   colsum_reduce_kernel<<<ceil_div(C, 256), 256, 0, cu(stream)>>>(workspace, chunks, C, scale, out);
   STEP_LAUNCH_CHECK("colsum_reduce_kernel");
   return 0;
 }
 
-extern "C" int step_mean_mid_bwd(const float* g, int A, int B, int P, int C, float gscale, void* dx, int ld, step_stream_t stream) {
+extern "C" int step_colsum_f16(const void* x, int ld, long long M, int C, float scale, float* out, float* workspace /* >= 64*C floats */,
+                               step_stream_t stream) {
+  return colsum_launch<__half>(x, ld, M, C, scale, out, workspace, stream);
+}
+
+extern "C" int step_colsum_f32(const float* x, int ld, long long M, int C, float scale, float* out, float* workspace /* >= 64*C floats */,
+                               step_stream_t stream) {
+  return colsum_launch<float>(x, ld, M, C, scale, out, workspace, stream);
+}
+
+template <typename T>
+static int mean_mid_bwd_launch(const float* g, int A, int B, int P, int C, float gscale, void* dx, int ld, step_stream_t stream) {
   STEP_CHECK_ARG(g && dx && A > 0 && B > 0 && P > 0 && C > 0 && ld >= C, "mean_mid_bwd: bad arguments");
-  mean_mid_bwd_kernel<<<ceil_div((long long)A * B * P * C, 256), 256, 0, cu(stream)>>>(g, A, B, P, C, gscale, (__half*)dx, ld);
+  mean_mid_bwd_kernel<T><<<ceil_div((long long)A * B * P * C, 256), 256, 0, cu(stream)>>>(g, A, B, P, C, gscale, (T*)dx, ld);
   STEP_LAUNCH_CHECK("mean_mid_bwd_kernel");
   return 0;
+}
+
+extern "C" int step_mean_mid_bwd(const float* g, int A, int B, int P, int C, float gscale, void* dx, int ld, step_stream_t stream) {
+  return mean_mid_bwd_launch<__half>(g, A, B, P, C, gscale, dx, ld, stream);
+}
+
+extern "C" int step_mean_mid_bwd_f32(const float* g, int A, int B, int P, int C, float gscale, float* dx, int ld, step_stream_t stream) {
+  return mean_mid_bwd_launch<float>(g, A, B, P, C, gscale, dx, ld, stream);
 }
 
 extern "C" int step_f32_accum_f16(const float* src, long long M, int C, float gscale, void* dst, int ld, step_stream_t stream) {
@@ -895,21 +1065,82 @@ extern "C" int step_f32_accum_f16(const float* src, long long M, int C, float gs
   return 0;
 }
 
-extern "C" int step_maxpool3d_bwd_f16(const void* x, int x_ld, const void* dy, int dy_ld, int N, int T, int H, int W, int C, int KT,
-                                      int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
-                                      int pad_hi_w, int OT, int OH, int OW, void* dx /* accumulated in place */, int dx_ld, uint8_t* argmax_ws /* N*OT*OH*OW*C bytes */,
-                                      step_stream_t stream) {
-  STEP_CHECK_ARG(x && dy && dx && argmax_ws && N > 0 && T > 0 && H > 0 && W > 0 && C > 0 && KT * KH * KW < 254, "maxpool3d_bwd: bad arguments");
+extern "C" int step_f32_accum_f32(const float* src, long long M, int C, float gscale, float* dst, int ld, step_stream_t stream) {
+  STEP_CHECK_ARG(src && dst && M > 0 && C > 0 && ld >= C, "f32_accum_f32: bad arguments");
+  f32_accum_f32_kernel<<<ceil_div(M * C, 256), 256, 0, cu(stream)>>>(src, M, C, gscale, dst, ld);
+  STEP_LAUNCH_CHECK("f32_accum_f32_kernel");
+  return 0;
+}
+
+template <typename T>
+static int maxpool3d_bwd_launch(const void* x, int x_ld, const void* dy, int dy_ld, int N, int T_, int H, int W, int C, int KT,
+                                int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
+                                int pad_hi_w, int OT, int OH, int OW, void* dx, int dx_ld, uint8_t* argmax_ws, step_stream_t stream) {
+  STEP_CHECK_ARG(x && dy && dx && argmax_ws && N > 0 && T_ > 0 && H > 0 && W > 0 && C > 0 && KT * KH * KW < 254, "maxpool3d_bwd: bad arguments");
   // the argmax pass divides by the strides, and a window must start inside its padding for every tap index to fit a byte
   STEP_CHECK_ARG(KT > 0 && KH > 0 && KW > 0 && ST > 0 && SH > 0 && SW > 0 && OT > 0 && OH > 0 && OW > 0,
                  "maxpool3d_bwd: kernel %dx%dx%d, stride %dx%dx%d, output %dx%dx%d must be positive", KT, KH, KW, ST, SH, SW, OT, OH, OW);
   STEP_CHECK_ARG(PT >= 0 && PT < KT && PH >= 0 && PH < KH && PW >= 0 && PW < KW && pad_hi_t >= 0 && pad_hi_h >= 0 && pad_hi_w >= 0,
                  "maxpool3d_bwd: bad padding (%d,%d,%d) / (%d,%d,%d) for kernel %dx%dx%d", PT, PH, PW, pad_hi_t, pad_hi_h, pad_hi_w, KT, KH, KW);
-  PoolGeom g = {N, T, H, W, C, KT, KH, KW, ST, SH, SW, PT, PH, PW, OT, OH, OW, pad_hi_t, pad_hi_h, pad_hi_w};
-  const long long n_out = (long long)N * OT * OH * OW * C, n_in = (long long)N * T * H * W * C;
-  maxpool_argmax_kernel<<<ceil_div(n_out, 256), 256, 0, cu(stream)>>>(g, (const __half*)x, x_ld, argmax_ws);
+  PoolGeom g = {N, T_, H, W, C, KT, KH, KW, ST, SH, SW, PT, PH, PW, OT, OH, OW, pad_hi_t, pad_hi_h, pad_hi_w};
+  const long long n_out = (long long)N * OT * OH * OW * C, n_in = (long long)N * T_ * H * W * C;
+  maxpool_argmax_kernel<T><<<ceil_div(n_out, 256), 256, 0, cu(stream)>>>(g, (const T*)x, x_ld, argmax_ws);
   STEP_LAUNCH_CHECK("maxpool_argmax_kernel");
-  maxpool_bwd_kernel<<<ceil_div(n_in, 256), 256, 0, cu(stream)>>>(g, (const __half*)dy, dy_ld, argmax_ws, (__half*)dx, dx_ld);
+  maxpool_bwd_kernel<T><<<ceil_div(n_in, 256), 256, 0, cu(stream)>>>(g, (const T*)dy, dy_ld, argmax_ws, (T*)dx, dx_ld);
   STEP_LAUNCH_CHECK("maxpool_bwd_kernel");
+  return 0;
+}
+
+extern "C" int step_maxpool3d_bwd_f16(const void* x, int x_ld, const void* dy, int dy_ld, int N, int T, int H, int W, int C, int KT,
+                                      int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
+                                      int pad_hi_w, int OT, int OH, int OW, void* dx /* accumulated in place */, int dx_ld, uint8_t* argmax_ws /* N*OT*OH*OW*C bytes */,
+                                      step_stream_t stream) {
+  return maxpool3d_bwd_launch<__half>(x, x_ld, dy, dy_ld, N, T, H, W, C, KT, KH, KW, ST, SH, SW, PT, PH, PW, pad_hi_t, pad_hi_h, pad_hi_w,
+                                      OT, OH, OW, dx, dx_ld, argmax_ws, stream);
+}
+
+extern "C" int step_maxpool3d_bwd_f32(const float* x, int x_ld, const float* dy, int dy_ld, int N, int T, int H, int W, int C, int KT,
+                                      int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
+                                      int pad_hi_w, int OT, int OH, int OW, float* dx /* accumulated in place */, int dx_ld, uint8_t* argmax_ws,
+                                      step_stream_t stream) {
+  return maxpool3d_bwd_launch<float>(x, x_ld, dy, dy_ld, N, T, H, W, C, KT, KH, KW, ST, SH, SW, PT, PH, PW, pad_hi_t, pad_hi_h, pad_hi_w,
+                                     OT, OH, OW, dx, dx_ld, argmax_ws, stream);
+}
+
+extern "C" size_t step_conv_wgrad_f32_workspace_bytes(long long M, int Cout, int Cin, int taps) {
+  if (M <= 0 || Cout <= 0 || Cin <= 0 || taps <= 0) return 0;
+  const WfPlan p = wgrad_f32_plan(M, Cout, (long long)taps * Cin);
+  return (size_t)p.chunks * p.tiles_co * p.tiles_j * kWfTile * kWfTile * sizeof(float);
+}
+
+extern "C" int step_conv_wgrad_f32(const float* dz, int dz_ld, const float* x, int x_ld, int N, int T, int H, int W, int OT, int OH,
+                                   int OW, int Cout, int Cin, int KT, int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW,
+                                   float scale, float* dw, int dw_ld, int accumulate, void* workspace, size_t ws_bytes,
+                                   step_stream_t stream) {
+  STEP_CHECK_ARG(N > 0 && T > 0 && H > 0 && W > 0 && OT > 0 && OH > 0 && OW > 0 && Cout > 0 && Cin > 0 && KT > 0 && KH > 0 && KW > 0 &&
+                 ST > 0 && SH > 0 && SW > 0 && dz && x && dw && workspace, "conv_wgrad_f32: bad arguments");
+  const long long M = (long long)N * OT * OH * OW, cols = (long long)KT * KH * KW * Cin;
+  STEP_CHECK_ARG(M < (1LL << 31) && (long long)N * T * H * W < (1LL << 31) && cols < (1LL << 31),
+                 "conv_wgrad_f32: %lld output pixels / %lld weight columns exceed 2^31", M, cols);
+  STEP_CHECK_ARG(Cout % 4 == 0 && Cin % 4 == 0 && dz_ld % 4 == 0 && x_ld % 4 == 0 && dz_ld >= Cout && x_ld >= Cin && dw_ld >= Cin,
+                 "conv_wgrad_f32: channel counts / strides must be multiples of 4 (Cout=%d Cin=%d dz_ld=%d x_ld=%d dw_ld=%d)",
+                 Cout, Cin, dz_ld, x_ld, dw_ld);
+  STEP_CHECK_ARG((((uintptr_t)dz | (uintptr_t)x) & 15) == 0, "conv_wgrad_f32: pointers must be 16-byte aligned");
+  STEP_CHECK_ARG(PT >= 0 && PT < KT && PH >= 0 && PH < KH && PW >= 0 && PW < KW, "conv_wgrad_f32: bad padding");
+  // every output pixel's first tap lies inside the padded input (as step_conv3d_fwd requires)
+  STEP_CHECK_ARG((OT - 1) * ST - PT < T && (OH - 1) * SH - PH < H && (OW - 1) * SW - PW < W,
+                 "conv_wgrad_f32: output extent %dx%dx%d inconsistent with input %dx%dx%d / stride / pad", OT, OH, OW, T, H, W);
+  const size_t need = step_conv_wgrad_f32_workspace_bytes(M, Cout, Cin, KT * KH * KW);
+  if (ws_bytes < need) return fail(STEP_E_WORKSPACE, "conv_wgrad_f32: workspace %zu < %zu", ws_bytes, need);
+  const WfPlan p = wgrad_f32_plan(M, Cout, cols);
+  STEP_CHECK_ARG(p.tiles_j <= 65535 && p.chunks <= 65535, "conv_wgrad_f32: grid too large");
+  const WfGeom g = {T, H, W, OT, OH, OW, KH, KW, ST, SH, SW, PT, PH, PW, Cin, (int)cols, (int)M, p.chunk};
+  conv_wgrad_f32_partial_kernel<<<dim3(p.tiles_co, p.tiles_j, p.chunks), 256, 0, cu(stream)>>>(dz, dz_ld, x, x_ld, Cout, g,
+                                                                                               (float*)workspace);
+  STEP_LAUNCH_CHECK("conv_wgrad_f32_partial_kernel");
+  conv_wgrad_f32_reduce_kernel<<<ceil_div((long long)Cout * cols, 256), 256, 0, cu(stream)>>>((const float*)workspace, p.chunks, p.tiles_co,
+                                                                                              p.tiles_j, Cout, Cin, (int)cols, scale, dw,
+                                                                                              dw_ld, accumulate);
+  STEP_LAUNCH_CHECK("conv_wgrad_f32_reduce_kernel");
   return 0;
 }

@@ -10,6 +10,9 @@ trunk (`trunk_forward_backward`), the SGD update with the gradient all-reduce (`
 and temporal mode with or without the context branch (`train_step`), which can also update through the optimizers of
 `optim` with dynamic loss scaling.  `BaseNet` / `ContextNet` / `TwoBranchNet` still run
 without autograd (their outputs carry no grad_fn): the backward walks the tape their forward records.
+Every piece runs on both precision paths of the modules (cfg.fp16): fp16 activations and activation gradients with the
+tensor-core weight gradient, or fp32 storage throughout (the reference's default precision) with the fp32 SIMT kernels and
+`conv_wgrad_f32`.  Weight gradients are fp32 on both.
 """
 import contextlib
 
@@ -181,9 +184,30 @@ def conv1x1_wgrad(dz, x, scale=1.0, out=None, accumulate=False):
     return dw
 
 
-# ---- backward of the wgmma / pool tape ---------------------------------------------------------------------------------
+def conv_wgrad_f32(dz, x, k, stride=(1, 1, 1), pad_lo=(0, 0, 0), scale=1.0, out=None, accumulate=False):
+    """Weight gradient of a convolution on the fp32 path: dz Act [N, OT, OH, OW, Cout] (the gradient of the raw convolution
+    output), x Act [N, T, H, W, Cin] (its input; channel slices allowed) -> dW [Cout, taps, Cin] fp32 (+)= scale * dz^T x
+    over every tap, for any filter k, stride and low padding pad_lo (step_conv_wgrad_f32: fp32 FFMA, deterministic)."""
+    dev = L.same_device(dz.buf, x.buf)
+    if dz.code != L.F32 or x.code != L.F32:
+        raise RuntimeError("conv_wgrad_f32: fp32 operands")
+    taps = k[0] * k[1] * k[2]
+    M = dz.N * dz.T * dz.H * dz.W
+    with torch.cuda.device(dev):
+        dw = out if out is not None else torch.empty((dz.C, taps, x.C), dtype=torch.float32, device=dev)
+        nbytes = L.lib().step_conv_wgrad_f32_workspace_bytes(M, dz.C, x.C, taps)
+        ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
+        L.check(L.lib().step_conv_wgrad_f32(L.c_void_p(dz.data_ptr()), dz.ld, L.c_void_p(x.data_ptr()), x.ld, x.N, x.T, x.H, x.W,
+                                            dz.T, dz.H, dz.W, dz.C, x.C, k[0], k[1], k[2], stride[0], stride[1], stride[2],
+                                            pad_lo[0], pad_lo[1], pad_lo[2], float(scale), L.ptr(dw), dw.shape[2],
+                                            1 if accumulate else 0, L.ptr(ws), nbytes, L.stream()))
+    return dw
+
+
+# ---- backward of the conv / pool tape ----------------------------------------------------------------------------------
 class GradStore:
-    """fp16 gradient buffers, one per activation buffer of the forward (same shape, zero-initialised on first use).
+    """Gradient buffers, one per activation buffer of the forward (same shape and storage type -- fp16 or fp32 --,
+    zero-initialised on first use).
     Every consumer ACCUMULATES into the slice it read, so fan-out (Inception branches, residuals, the shared concat
     buffer of two_branch.py:256) needs no special casing."""
 
@@ -245,11 +269,14 @@ def timing_summary():
 
 
 def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
-    """Reverse pass over the conv / max-pool tape recorded by engine.TAPE (fp16 path).  `grads` (GradStore) must already
-    hold d(loss * loss_scale)/d(output) of the last layers.  Returns {parameter tensor: fp32 gradient in the parameter's
-    own layout} (BatchNorm is frozen, i3dpt / networks.py:136-142: only conv weights and biases train).
-    The input gradient of every layer is produced by the SAME wgmma convolution kernels run on the transposed, flipped
-    filter (stride-1 convolutions: dx = conv(dz, flip(w)^T)), accumulated through their residual input."""
+    """Reverse pass over the conv / max-pool tape recorded by engine.TAPE, in the storage type of each entry's activations
+    (fp16: tensor-core weight gradient; fp32: step_conv_wgrad_f32).  `grads` (GradStore) must already hold
+    d(loss * loss_scale)/d(output) of the last layers.  Returns {parameter tensor: fp32 gradient in the parameter's own
+    layout} (BatchNorm is frozen, i3dpt / networks.py:136-142: only conv weights and biases train).
+    The input gradient of every layer is produced by the SAME convolution kernels as its forward (wgmma on fp16, SIMT on
+    fp32), run on the transposed, flipped filter (stride-1 convolutions: dx = conv(dz, flip(w)^T)), accumulated through
+    their residual input.  need_input_grad(entry) -> bool limits which entries form it (default: all).  A strided
+    convolution (the fp32 trunk's 7x7x7 stem) gets its weight gradient only; asking for its input gradient raises."""
     from . import engine as E
     from .engine import Act
     out = {}
@@ -260,23 +287,30 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
         out[param] = out[param] + g if param in out else g
 
     for e in reversed(tape):
+        f16 = e["x"].code == L.F16
         if e["kind"] == "pool":
             x, y = e["x"], e["out"]
             gy, gx = grads.of(y), grads.of(x)
             k, s, pl, ph = e["k"], e["stride"], e["pad_lo"], e["pad_hi"]
             ws = torch.empty((y.N * y.T * y.H * y.W * y.C,), dtype=torch.uint8, device=x.device)
+            pool_bwd = lib.step_maxpool3d_bwd_f16 if f16 else lib.step_maxpool3d_bwd_f32
             with _phase("pool_bwd"):
-                L.check(lib.step_maxpool3d_bwd_f16(L.c_void_p(x.data_ptr()), x.ld, L.c_void_p(gy.data_ptr()), gy.ld, x.N, x.T, x.H,
+                L.check(pool_bwd(L.c_void_p(x.data_ptr()), x.ld, L.c_void_p(gy.data_ptr()), gy.ld, x.N, x.T, x.H,
                                                    x.W, x.C, k[0], k[1], k[2], s[0], s[1], s[2], pl[0], pl[1], pl[2], ph[0], ph[1],
                                                    ph[2], y.T, y.H, y.W, L.c_void_p(gx.data_ptr()), gx.ld, L.ptr(ws), L.stream()))
             continue
         x, w, k = e["x"], e["w"], e["k"]
-        if e["stride"] != (1, 1, 1):
-            raise NotImplementedError("tape_backward: strided convolution (the trunk's stem) is not built")
+        strided = e["stride"] != (1, 1, 1)
+        if strided and (f16 or need_input_grad is None or need_input_grad(e)):
+            raise NotImplementedError("tape_backward: a strided convolution has a weight gradient on the fp32 path only, and no "
+                                      "input gradient (the trunk's stem needs none)")
         outs = [e["out"]] + e["extra_outs"]
-        M = x.N * x.T * x.H * x.W
+        y0 = e["out"]
+        M = y0.N * y0.T * y0.H * y0.W
         n_total = sum(o.C for o in outs)
-        dz = torch.empty((x.N, x.T, x.H, x.W, n_total), dtype=torch.float16, device=x.device)
+        dz = torch.empty((y0.N, y0.T, y0.H, y0.W, n_total), dtype=x.buf.dtype, device=x.device)
+        esz = dz.element_size()
+        act_bwd = lib.step_act_bwd_f16 if f16 else lib.step_act_bwd_f32
         col = 0
         with _phase("act_bwd"):
             for o in outs:
@@ -284,21 +318,24 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
                 sc = e["scale"][col:col + o.C] if e["scale"] is not None else None
                 res = e["residual"]
                 gres = grads.of(res) if res is not None else None
-                L.check(lib.step_act_bwd_f16(L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, L.ptr(sc),
-                                             1 if e["relu"] else 0, M, o.C, L.c_void_p(dz.data_ptr() + 2 * col), n_total,
-                                             L.c_void_p(gres.data_ptr()) if gres is not None else None,
-                                             gres.ld if gres is not None else 0, L.stream()))
+                L.check(act_bwd(L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, L.ptr(sc),
+                                1 if e["relu"] else 0, M, o.C, L.c_void_p(dz.data_ptr() + esz * col), n_total,
+                                L.c_void_p(gres.data_ptr()) if gres is not None else None,
+                                gres.ld if gres is not None else 0, L.stream()))
                 col += o.C
         # ---- weight (and bias) gradients
         taps = k[0] * k[1] * k[2]
-        dw = torch.empty((n_total, taps, x.C), dtype=torch.float32, device=x.device)
-        nbytes = lib.step_conv_wgrad_workspace_bytes(M, n_total, x.C, taps)
-        ws = torch.empty((nbytes // 4,), dtype=torch.float32, device=x.device)
         pl = e["pad_lo"]
         with _phase("wgrad_k%d" % taps):
-            L.check(lib.step_conv_wgrad_f16(L.ptr(dz), n_total, L.c_void_p(x.data_ptr()), x.ld, x.N, x.T, x.H, x.W, n_total, x.C,
-                                            k[0], k[1], k[2], pl[0], pl[1], pl[2], inv, L.ptr(dw), x.C, 0, L.ptr(ws), nbytes,
-                                            L.stream()))
+            if f16:
+                dw = torch.empty((n_total, taps, x.C), dtype=torch.float32, device=x.device)
+                nbytes = lib.step_conv_wgrad_workspace_bytes(M, n_total, x.C, taps)
+                ws = torch.empty((nbytes // 4,), dtype=torch.float32, device=x.device)
+                L.check(lib.step_conv_wgrad_f16(L.ptr(dz), n_total, L.c_void_p(x.data_ptr()), x.ld, x.N, x.T, x.H, x.W, n_total, x.C,
+                                                k[0], k[1], k[2], pl[0], pl[1], pl[2], inv, L.ptr(dw), x.C, 0, L.ptr(ws), nbytes,
+                                                L.stream()))
+            else:
+                dw = conv_wgrad_f32(Act(dz), x, k, e["stride"], pl, inv)
         if isinstance(e["tag"], tuple) and e["tag"][0] == "s2d":
             unit = e["tag"][1]
             if unit.conv3d.weight.requires_grad:
@@ -311,14 +348,16 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
                 row += o.C
                 continue
             conv = getattr(tg, "conv3d", tg)          # Unit3Dpy holds its nn.Conv3d; nn.Conv2d / nn.Conv3d containers are themselves
-            g = dw[row:row + o.C].view((o.C,) + tuple(conv.weight.shape[2:]) + (x.C,))
+            cin = conv.weight.shape[1]                # x.C, or fewer on the fp32 stem (the clip's padding channel)
+            g = dw[row:row + o.C, :, :cin].reshape((o.C,) + tuple(conv.weight.shape[2:]) + (cin,))
             g = g.permute(0, g.dim() - 1, *range(1, g.dim() - 1)).contiguous()        # [Cout, Cin, *k]
             if conv.weight.requires_grad:
                 add(conv.weight, g)
             if conv.bias is not None and conv.bias.requires_grad:
                 db = torch.empty((o.C,), dtype=torch.float32, device=x.device)
                 wsb = torch.empty((64 * o.C,), dtype=torch.float32, device=x.device)
-                L.check(lib.step_colsum_f16(L.c_void_p(dz.data_ptr() + 2 * row), n_total, M, o.C, inv, L.ptr(db), L.ptr(wsb), L.stream()))
+                colsum = lib.step_colsum_f16 if f16 else lib.step_colsum_f32
+                L.check(colsum(L.c_void_p(dz.data_ptr() + esz * row), n_total, M, o.C, inv, L.ptr(db), L.ptr(wsb), L.stream()))
                 add(conv.bias, db)
             row += o.C
         # ---- input gradient: the forward kernel on the transposed, flipped filter, accumulated into grad(x)
@@ -335,9 +374,10 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
                           loss_scale=1024.0, cat=None, objective_scale=1.0):
     """One training-time evaluation of a TwoBranchNet on the device (train.py:323-347 for one refinement step): forward
     with targets, the three losses, and the gradient of  mean(loss_cls) + lambda_reg * loss_loc + lambda_neighbor * loss_nb
-    with respect to every trainable parameter of the head and to the pooled ROI features.  fp16 activations / activation
-    gradients with a static loss scale (apex-style), fp32 weight gradients.  Dropout is the identity (eval mode), like the
-    reference's gradient goldens.
+    with respect to every trainable parameter of the head and to the pooled ROI features, on the head's precision path
+    (net.fp16): fp16 or fp32 activations / activation gradients, fp32 weight gradients, with the static loss scale
+    `loss_scale` applied to the activation gradients on both (apex-style; on fp32 a power of two is exact, and 1.0 is the
+    reference's fp32 arithmetic).  Dropout is the identity (eval mode), like the reference's gradient goldens.
     Class-only heads (TwoBranchNet(cls_only=True), the first training stage of train_cls.py) have no local branch: the
     objective is mean(loss_cls) alone (`cls_loss`), the regression losses are the reference's [1] zeros and grads holds the
     16 tensors of Mixed_5b / Mixed_5c, `downsample` and `global_cls`.
@@ -352,8 +392,7 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
     from . import engine as E
     from .engine import Act
     from .networks import to_act
-    if E.dtype_code(net.fp16) != L.F16:
-        raise RuntimeError("head_forward_backward runs on the fp16 path (cfg.fp16=True)")
+    code = E.dtype_code(net.fp16)
     fc, ps = net.fc_dim, net.pool_size
     D = fc * ps * ps
     if cat is None:
@@ -362,14 +401,17 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
     else:   # ROI features already pooled into the [ROI | downsample] concat buffer (ROINet.pool_into)
         dev = L.same_device(cat.buf, tubes, targets)
         N, Tl, Wd, Hd, C = cat.N, cat.T, cat.H, cat.W, cat.ld - fc
+        if cat.code != code:
+            raise RuntimeError("head_forward_backward: the concat buffer is %s but the head runs on the %s path"
+                               % (cat.buf.dtype, E.torch_dtype(code)))
     hw = net._head_weights()
     if (context_feat is None) != (hw["ctx_w"] is None):
         raise RuntimeError("head_forward_backward: global_cls has %d context columns but context_feat is %s"
                            % (0 if hw["ctx_w"] is None else hw["ctx_w"].shape[1], "None" if context_feat is None else "given"))
     with torch.cuda.device(dev), torch.no_grad():
         if cat is None:
-            cat = Act.empty(N, Tl, Wd, Hd, C + fc, L.F16, dev)
-            src = to_act(global_feat, L.F16)
+            cat = Act.empty(N, Tl, Wd, Hd, C + fc, code, dev)
+            src = to_act(global_feat, code)
             cat.buf[..., :C].copy_(src.buf[..., src.coff:src.coff + C])
         ctx_mean, row_map, ctx_module_form = None, None, False
         if isinstance(context_feat, (tuple, list)):
@@ -413,8 +455,9 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
         out[net.global_cls.weight] = dw.reshape(net.global_cls.weight.shape)
         out[net.global_cls.bias] = db
         gcat = grads.of(cat)
-        L.check(L.lib().step_mean_mid_bwd(L.ptr(dxbar), N, Tl, ps * ps, fc, float(loss_scale),
-                                          L.c_void_p(gcat.data_ptr() + 2 * C), gcat.ld, L.stream()))
+        mean_mid_bwd = L.lib().step_mean_mid_bwd if code == L.F16 else L.lib().step_mean_mid_bwd_f32
+        L.check(mean_mid_bwd(L.ptr(dxbar), N, Tl, ps * ps, fc, float(loss_scale),
+                             L.c_void_p(gcat.data_ptr() + gcat.buf.element_size() * C), gcat.ld, L.stream()))
         # ---- regressors (two_branch.py:261-270): local_reg on every frame, neighbor_reg1 / 2 on the first / last chunk.
         # Class-only heads have no local branch: their tape ends at `downsample`.
         if not net.cls_only:
@@ -430,8 +473,8 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
                 dlf2[:, a:b] += dx.view(N, b - a, D)                      # disjoint frame ranges of one buffer (host-side glue)
                 out[mod.weight], out[mod.bias] = unperm(dw), db
             glf2 = grads.of(lf2)
-            L.check(L.lib().step_f32_accum_f16(L.ptr(dlf2), N * Tl * ps * ps, fc, float(loss_scale), L.c_void_p(glf2.data_ptr()), glf2.ld,
-                                               L.stream()))
+            f32_accum = L.lib().step_f32_accum_f16 if code == L.F16 else L.lib().step_f32_accum_f32
+            L.check(f32_accum(L.ptr(dlf2), N * Tl * ps * ps, fc, float(loss_scale), L.c_void_p(glf2.data_ptr()), glf2.ld, L.stream()))
         # ---- every convolution and pool of the head, in reverse
         out.update(tape_backward(tape, grads, loss_scale))
         gcat = grads.of(cat)
@@ -442,11 +485,14 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
 
 
 def context_forward(context_net, feat):
-    """ContextNet.forward_act (two_branch.py:132-138) on the fp16 path with the tape on.  feat: the trunk's output Act
-    [B,T',H',W',832].  Returns (ctx [B,T',1024] fp32, state for context_backward)."""
+    """ContextNet.forward_act (two_branch.py:132-138) with the tape on, in the storage type of feat, the trunk's output Act
+    [B,T',H',W',832] (fp16 or fp32, which must be the ContextNet's cfg.fp16 path).  Returns (ctx [B,T',1024] fp32, state
+    for context_backward)."""
     from . import engine as E
-    if E.dtype_code(context_net.fp16) != L.F16:
-        raise RuntimeError("context_forward runs on the fp16 path (cfg.fp16=True)")
+    code = E.dtype_code(context_net.fp16)
+    if feat.code != code:
+        raise RuntimeError("context_forward: conv_feat is %s but the ContextNet runs on the %s path"
+                           % (feat.buf.dtype, E.torch_dtype(code)))
     with torch.cuda.device(feat.device), torch.no_grad():
         tape, keep = [], {}
         with E.recording(tape):
@@ -457,15 +503,15 @@ def context_forward(context_net, feat):
 def context_backward(state, d_ctx, loss_scale=1024.0):
     """Backward of context_forward from d_ctx = d(loss)/d(ctx), fp32 [B,T',1024]: the spatial mean's backward into the
     gradient of Mixed_5c's output, then the tape (Mixed_5c, Mixed_5b, the (1,3,3)/(1,2,2) max-pool).  Returns
-    ({conv weight: fp32 gradient} for the 12 Unit3D convolutions -- BatchNorm stays frozen --, fp16 [B,T',H',W',832] (a
-    channel-slice view) holding loss_scale * d(loss)/d(conv_feat) through the context branch)."""
+    ({conv weight: fp32 gradient} for the 12 Unit3D convolutions -- BatchNorm stays frozen --, [B,T',H',W',832] in the
+    forward's storage type (a channel-slice view) holding loss_scale * d(loss)/d(conv_feat) through the context branch)."""
     x = state["x"]
     with torch.cuda.device(x.device), torch.no_grad():
         grads = GradStore()
         gx = grads.of(x)
         d = d_ctx.float().contiguous()
-        L.check(L.lib().step_mean_mid_bwd(L.ptr(d), x.N * x.T, x.H * x.W, 1, x.C, float(loss_scale), L.c_void_p(gx.data_ptr()), gx.ld,
-                                          L.stream()))
+        mean_mid_bwd = L.lib().step_mean_mid_bwd if gx.code == L.F16 else L.lib().step_mean_mid_bwd_f32
+        L.check(mean_mid_bwd(L.ptr(d), x.N * x.T, x.H * x.W, 1, x.C, float(loss_scale), L.c_void_p(gx.data_ptr()), gx.ld, L.stream()))
         out = tape_backward(state["tape"], grads, loss_scale)
         gfeat = grads.of(state["feat"])
     return out, gfeat.buf[..., gfeat.coff:gfeat.coff + gfeat.C]
@@ -486,7 +532,9 @@ def context_grad_reduce(dctx, tubes, acc, t_start):
 
 
 def trunk_forward_backward(base_net, clips, d_feat_fn, loss_scale=1024.0):
-    """I3D trunk forward on the fp16 path with the tape on, then backward from d(loss)/d(conv_feat).
+    """I3D trunk forward on base_net's precision path (cfg.fp16) with the tape on, then backward from d(loss)/d(conv_feat).
+    On fp32 the stem is the stride-2 7x7x7 convolution over the clip padded to 4 channels; its weight gradient comes from
+    step_conv_wgrad_f32 (on fp16 the stem runs as the space-to-depth 4x4x4 filter, stem_s2d_wgrad).
     d_feat_fn(feat_act) -> fp32 tensor [N,T',H',W',832] (channels-last) with the gradient of the loss w.r.t. the trunk
     output (e.g. the sum of the ROIAlign backward results of the refinement steps).
     Returns (feat Act, {conv weight: fp32 gradient}).  BatchNorm stays frozen (networks.py:85-99,136-142)."""
@@ -500,8 +548,10 @@ def trunk_forward_backward(base_net, clips, d_feat_fn, loss_scale=1024.0):
         gfeat = grads.of(feat)
         d = d_feat_fn(feat).to(torch.float32).contiguous()
         M = feat.N * feat.T * feat.H * feat.W
-        L.check(L.lib().step_f32_accum_f16(L.ptr(d), M, feat.C, float(loss_scale), L.c_void_p(gfeat.data_ptr()), gfeat.ld, L.stream()))
-        out = tape_backward(tape, grads, loss_scale)
+        f32_accum = L.lib().step_f32_accum_f16 if feat.code == L.F16 else L.lib().step_f32_accum_f32
+        L.check(f32_accum(L.ptr(d), M, feat.C, float(loss_scale), L.c_void_p(gfeat.data_ptr()), gfeat.ld, L.stream()))
+        stem = tape[0]                                # the clip needs no gradient
+        out = tape_backward(tape, grads, loss_scale, need_input_grad=lambda e: e is not stem)
     return feat, out
 
 
@@ -572,7 +622,10 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     Parameter update: with lr, `sgd_step` (one global rate); with optimizer (a step_b200.optim.Adam / SGD over the nets'
     parameters, e.g. built from the reference's get_params, and lr None), the gradients, averaged over the ranks, become
     p.grad and optimizer.step() runs -- it skips the update when a gradient is inf or NaN (skipped=True).  scaler (a
-    step_b200.optim.LossScaler; needs optimizer) replaces loss_scale by its dynamic scale and is updated from the step."""
+    step_b200.optim.LossScaler; needs optimizer) replaces loss_scale by its dynamic scale and is updated from the step.
+    Precision: that of the nets (cfg.fp16, one value for all of them).  fp16 stores activations and their gradients in
+    fp16 (apex O1-like); fp32 stores everything in fp32, the reference's default (config.py:26-27), and with
+    loss_scale=1.0 and no scaler it is the reference's fp32 arithmetic.  Weight gradients and updates are fp32 on both."""
     from .engine import Act
     if optimizer is not None and lr is not None:
         raise ValueError("train_step: give either lr (sgd_step) or optimizer, not both")
@@ -610,7 +663,7 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
             if flat.shape[1] != t_len or t_start + t_len > T_all:
                 raise RuntimeError("train_step: step %d pools frames [%d, %d) of T'=%d (cfg.T=%d, NUM_CHUNKS=%s) but its tubes have %d frames"
                                    % (i + 1, t_start, t_start + t_len, T_all, cfg.T, cfg.NUM_CHUNKS, flat.shape[1]))
-            cat = Act.empty(R, t_len, head.pool_size, head.pool_size, 832 + head.fc_dim, L.F16, dev)
+            cat = Act.empty(R, t_len, head.pool_size, head.pool_size, 832 + head.fc_dim, feat.code, dev)
             argmax = None
             if pool_mode == "pool":   # the pixel of every maximum, for this step's ROIPool backward
                 argmax = torch.empty((R * t_len * head.pool_size * head.pool_size * feat.C,), dtype=torch.int32, device=dev)
