@@ -417,6 +417,60 @@ int step_maxpool3d_bwd_f32(const float* x, int x_ld, const float* dy, int dy_ld,
                            int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
                            int pad_hi_w, int OT, int OH, int OW, float* dx, int dx_ld, uint8_t* argmax_ws, step_stream_t stream);
 
+/* ------------------------------------------------------------------ the heads' dropout ---- */
+/* One draw of torch.nn.functional.dropout(x, p, training=True) on a CUDA fp32 tensor of n elements (n % 4 == 0, n < 2^31,
+ * 16-byte aligned and contiguous, as every dropout input of the heads is): seed and offset are the device generator's
+ * initial_seed() and get_offset() before the draw, sm_count and threads_per_sm the device's multi_processor_count and
+ * max_threads_per_multi_processor, which set torch's launch geometry and with it which random number every element takes.
+ * The entries below reproduce that draw's keep mask bit for bit and regenerate it in the backward (nothing is stored); an
+ * element is kept with factor (float)(1.0 / (double)(float)(1 - p)), dropped with factor 0.  The geometry is
+ * step_b200/csrc/dropout.cuh's.  Every entry returns STEP_E_ARG for keep outside (0, 1) (torch draws nothing at p = 0 or 1),
+ * non-positive sm_count or threads_per_sm < 256, and null pointers, and STEP_E_UNSUPPORTED for other n, before any launch.
+ * The two draws of a head (two_branch.py:244, 261), each over the reference's tensor and element order:
+ *   global  [R, C' = C*P + ctx_cols, T], element (r*C' + c')*T + t: c' = c*P + p is the downsample output's channel c at pixel
+ *           p of frame t; c' = C*P + k is context column k (ctx_cols = 1024 with context, 0 without);
+ *   local   [F = R*T, C, P], element (f*C + c)*P + p: downsample2's output, channel c at pixel p of frame row f.
+ * Inputs and outputs stay in this library's channels-last layouts; the map to the reference's order is the entries' own. */
+typedef struct {
+  uint64_t seed, offset;
+  float keep;                      /* (float)(1 - p), 1 - p formed in double from the drop probability p as torch does */
+  int sm_count, threads_per_sm;
+} step_dropout_draw;
+/* The argument checks of a draw of n elements; *offset_step (may be NULL) receives what the draw advances the generator's
+ * offset by, ((n - 1) / (4 * n_threads) + 1) * 4. */
+int step_dropout_check(const step_dropout_draw* draw, long long n, uint64_t* offset_step);
+/* mask[e] = 1 if element e of the draw is kept, else 0 (uint8 [n], the dropped tensor's element order). */
+int step_dropout_mask_u8(const step_dropout_draw* draw, long long n, uint8_t* mask, step_stream_t stream);
+/* The global draw's downsample part: y[r, t, p, c] = x[r, t, p, c] * factor (fp32 product rounded once to dtype) for the
+ * channels-last slice x [R, T, P, C] (pixel stride x_ld; the downsample channels of the ROI concat buffer), y likewise. */
+int step_dropout_global_fwd(const step_dropout_draw* draw, const void* x, int dtype, int x_ld, int R, int T, int P, int C,
+                            int ctx_cols, void* y, int y_ld, step_stream_t stream);
+/* The global draw's context part, reduced: out[r, k] = (sum over t ascending of ctx(r, t, k) * factor) / T, fp32 [R, K], for
+ * ctx(r, t, k) = ctx[row * row_stride + t * t_stride + k * k_stride], row = row_map[r] (int32, may be NULL: row = r).
+ * ContextNet's output [B, T', 1024] from frame t_start: ctx += t_start * 1024, row_stride = T' * 1024, t_stride = 1024,
+ * k_stride = 1, row_map = each tube's clip; the per-tube [R, 1024, T]: row_stride = 1024 * T, t_stride = 1, k_stride = T.
+ * P and C are the downsample part's pixels and channels (the draw is [R, C*P + K, T]). */
+int step_dropout_ctx_mean_f32(const step_dropout_draw* draw, int P, int C, const float* ctx, const int32_t* row_map,
+                              long long row_stride, int t_stride, int k_stride, int R, int T, int K, float* out,
+                              step_stream_t stream);
+/* The local draw: y[f, p, c] = x[f, p, c] * factor for x [F, P, C] channels-last (pixel stride x_ld), y likewise. */
+int step_dropout_local_fwd(const step_dropout_draw* draw, const void* x, int dtype, int x_ld, int F, int P, int C, void* y,
+                           int y_ld, step_stream_t stream);
+/* step_mean_mid_bwd / step_mean_mid_bwd_f32 through the global draw (A = R tubes, B = T frames): dx[a, b, p, c] += gscale *
+ * factor * g[a, p*C + c] / B; dx in dtype (STEP_F16 / STEP_F32), channel stride ld. */
+int step_mean_mid_bwd_dropout(const step_dropout_draw* draw, int ctx_cols, const float* g, int A, int B, int P, int C,
+                              float gscale, void* dx, int dtype, int ld, step_stream_t stream);
+/* step_f32_accum_f16 / step_f32_accum_f32 through the local draw: dst[f, p, c] += gscale * factor * src[f, p, c], src fp32
+ * [F*P, C] dense, dst in dtype with channel stride ld. */
+int step_f32_accum_dropout(const step_dropout_draw* draw, const float* src, int F, int P, int C, float gscale, void* dst,
+                           int dtype, int ld, step_stream_t stream);
+/* step_ctx_grad_reduce_f32 through the global draw's context part, for the [R, 1024] gradient dctx of
+ * step_dropout_ctx_mean_f32's output: acc[b, t_start + t, k] += (sum over the tubes r of clip b, ascending, of
+ * factor(r, t, k) * dctx[r, k]) / T_len.  P, Cg: the downsample part's pixels and channels.  Deterministic, no atomics. */
+int step_ctx_grad_reduce_dropout_f32(const step_dropout_draw* draw, int P, int Cg, const float* dctx, int dctx_ld,
+                                     const float* tubes, int R, int T_len, int B, int feat_T, int t_start, int C, float* acc,
+                                     step_stream_t stream);
+
 /* ------------------------------------------------------------------ optimizer ------------ */
 /* Multi-tensor parameter update (train.py:123-128, 345-348): one launch over every tensor of a parameter set, described by a
  * device table of step_optim_tensor rows and a device block map.  Row r describes one fp32 tensor of `numel` contiguous

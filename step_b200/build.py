@@ -26,7 +26,7 @@ NO_FMAD = {"nms.cu", "roi.cu", "tubes.cu", "train.cu", "optim.cu", "clip_prep.cu
 
 def _deps(src):
     return [os.path.join(CSRC, src), os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "umma_ptx.cuh"), os.path.join(CSRC, "tube_math.cuh"),
-            os.path.join(CSRC, "roi_math.cuh"), os.path.join(os.path.dirname(HERE), "include", "step_b200.h")]
+            os.path.join(CSRC, "roi_math.cuh"), os.path.join(CSRC, "dropout.cuh"), os.path.join(os.path.dirname(HERE), "include", "step_b200.h")]
 
 
 def _stale(target, deps):

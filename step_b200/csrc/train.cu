@@ -22,9 +22,12 @@
 // operations that are not bit-exact (tolerance stated in tests/test_gpu_train.py).
 #include <math.h>
 
+#include <algorithm>
+
 #include <mma.h>
 
 #include "common.cuh"
+#include "dropout.cuh"
 #include "roi_math.cuh"
 #include "tube_math.cuh"
 
@@ -376,18 +379,69 @@ __global__ void __launch_bounds__(kPoolBwdMaxChunk) roi_pool_bwd_slice_nhwc_kern
 // dctx[r, c] is the gradient of tube r's context input of the classifier (the slice mean the forward feeds to global_cls).
 // acc[b, t, c] += (sum over the tubes r of clip b, ascending r, of dctx[r, c]) / T_len for t in [t_start, t_start + T_len);
 // clip(r) = floor(frame(r) / T_len) with frame(r) = tubes[r, 0, 0].  One thread per (clip, channel): no atomics.
+// DROP: the classifier read the dropped context (two_branch.py:244), so tube r's term on frame t is multiplied by the factor of
+// its element (r, t, c) of the draw (map: DropMap at(r, t, 0, c)), and every frame has its own sum.
+template <bool DROP>
 __global__ void __launch_bounds__(256) ctx_grad_reduce_kernel(const float* __restrict__ dctx, int dctx_ld, const float* __restrict__ tubes,
                                                               int R, int T_len, int B, int feat_T, int t_start, int C,
-                                                              float* __restrict__ acc) {
+                                                              float* __restrict__ acc, DropDraw dd, DropMap mp) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)B * C) return;
   const int b = (int)(i / C), c = (int)(i - (long long)b * C);
-  float s = 0.0f;
-  for (int r = 0; r < R; ++r)
-    if ((int)__fdiv_rn(tubes[(size_t)r * T_len * 5], (float)T_len) == b) s = __fadd_rn(s, dctx[(size_t)r * dctx_ld + c]);
-  const float v = __fdiv_rn(s, (float)T_len);
   float* d = acc + ((size_t)b * feat_T + t_start) * C + c;
-  for (int t = 0; t < T_len; ++t) d[(size_t)t * C] = __fadd_rn(d[(size_t)t * C], v);
+  if constexpr (DROP) {
+    for (int t = 0; t < T_len; ++t) {
+      float s = 0.0f;
+      for (int r = 0; r < R; ++r)
+        if ((int)__fdiv_rn(tubes[(size_t)r * T_len * 5], (float)T_len) == b)
+          s = __fadd_rn(s, __fmul_rn(dctx[(size_t)r * dctx_ld + c], drop_factor(dd, mp.at(r, t, 0, c))));
+      d[(size_t)t * C] = __fadd_rn(d[(size_t)t * C], __fdiv_rn(s, (float)T_len));
+    }
+  } else {
+    float s = 0.0f;
+    for (int r = 0; r < R; ++r)
+      if ((int)__fdiv_rn(tubes[(size_t)r * T_len * 5], (float)T_len) == b) s = __fadd_rn(s, dctx[(size_t)r * dctx_ld + c]);
+    const float v = __fdiv_rn(s, (float)T_len);
+    for (int t = 0; t < T_len; ++t) d[(size_t)t * C] = __fadd_rn(d[(size_t)t * C], v);
+  }
+}
+
+// ---- dropout (two_branch.py:244, 261; the draw itself is dropout.cuh) -------------------------------------------------------
+// the keep mask of a whole draw, in the order of the dropped tensor's elements
+__global__ void __launch_bounds__(256) dropout_mask_kernel(DropDraw dd, long long n, uint8_t* __restrict__ mask) {
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x)
+    mask[e] = drop_keep(dd, e) ? 1 : 0;
+}
+
+// y[m, c] = x[m, c] * factor (fp32 product, rounded once to T) over pixels m = (r * T_len + t) * P + p of a channels-last
+// [R, T_len, P, C] slice; element (r, t, p, c) of the draw is mp.at(r, t, p, c).
+template <typename T>
+__global__ void __launch_bounds__(256) dropout_copy_kernel(const T* __restrict__ x, int x_ld, long long M, int T_len, int P, int C,
+                                                           T* __restrict__ y, int y_ld, DropDraw dd, DropMap mp) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M * C) return;
+  const long long m = i / C;
+  const int c = (int)(i - m * C);
+  const long long f = m / P;
+  const int p = (int)(m - f * P);
+  const long long r = f / T_len;
+  const int t = (int)(f - r * T_len);
+  y[(size_t)m * y_ld + c] = from_f32<T>(__fmul_rn(to_f32<T>(x[(size_t)m * x_ld + c]), drop_factor(dd, mp.at(r, t, p, c))));
+}
+
+// out[r, k] = (sum over t ascending of ctx[row(r) * row_stride + t * t_stride + k * k_stride] * factor) / T_len: the temporal
+// mean of tube r's dropped context columns (the classifier is linear, so it takes the mean instead of the frames);
+// row(r) = row_map[r], or r without a map.  Element (r, t, k) of the draw is mp.at(r, t, 0, k).
+__global__ void __launch_bounds__(256) ctx_mean_dropout_kernel(const float* __restrict__ ctx, const int32_t* __restrict__ row_map,
+                                                               long long row_stride, int t_stride, int k_stride, int R, int T_len,
+                                                               int K, float* __restrict__ out, DropDraw dd, DropMap mp) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)R * K) return;
+  const int r = (int)(i / K), k = (int)(i - (long long)r * K);
+  const float* src = ctx + (size_t)(row_map ? row_map[r] : r) * row_stride + (size_t)k * k_stride;
+  float s = 0.0f;
+  for (int t = 0; t < T_len; ++t) s = __fadd_rn(s, __fmul_rn(src[(size_t)t * t_stride], drop_factor(dd, mp.at(r, t, 0, k))));
+  out[i] = __fdiv_rn(s, (float)T_len);
 }
 
 // ---- small-N linear backward -----------------------------------------------------------------------------------------
@@ -482,9 +536,11 @@ __global__ void __launch_bounds__(256) colsum_reduce_kernel(const float* __restr
 }
 
 // temporal-mean backward (two_branch.py:249: the class scores are averaged over T'):  dx[a][b][p][c] += g[a][p*C + c] / B
-template <typename T>
+// DROP: the mean was taken over the dropped frames, so each term is also multiplied by the factor of element mp.at(a, b, p, c)
+// of the draw.
+template <typename T, bool DROP>
 __global__ void __launch_bounds__(256) mean_mid_bwd_kernel(const float* __restrict__ g, int A, int B, int P, int C, float gscale,
-                                                           T* __restrict__ dx, int ld) {
+                                                           T* __restrict__ dx, int ld, DropDraw dd, DropMap mp) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)A * B * P * C) return;
   const int c = (int)(i % C);
@@ -493,29 +549,38 @@ __global__ void __launch_bounds__(256) mean_mid_bwd_kernel(const float* __restri
   const int b = (int)(r % B);
   const int a = (int)(r / B);
   T* d = dx + ((((size_t)a * B + b) * P + p) * ld + c);
-  *d = from_f32<T>(to_f32<T>(*d) + g[(size_t)a * P * C + (size_t)p * C + c] * gscale / (float)B);
+  float v = g[(size_t)a * P * C + (size_t)p * C + c] * gscale / (float)B;
+  if constexpr (DROP) v = v * drop_factor(dd, mp.at(a, b, p, c));
+  *d = from_f32<T>(to_f32<T>(*d) + v);
 }
 
-// fp32 [M, C] (scaled) accumulated into an fp16 channel slice
+// fp32 [M, C] (scaled) accumulated into an fp16 channel slice.  DROP: src is the gradient of the dropped copy of the slice,
+// whose pixel m = f * P + p, channel c is element mp.at(f, 0, p, c) of the draw.
+template <bool DROP>
 __global__ void __launch_bounds__(256) f32_accum_f16_kernel(const float* __restrict__ src, long long M, int C, float gscale,
-                                                            __half* __restrict__ dst, int ld) {
+                                                            __half* __restrict__ dst, int ld, int P, DropDraw dd, DropMap mp) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= M * C) return;
   const long long m = i / C;
   const int c = (int)(i - m * C);
   __half* d = dst + (size_t)m * ld + c;
-  *d = __float2half_rn(__half2float(*d) + src[i] * gscale);
+  float v = src[i];
+  if constexpr (DROP) v = v * drop_factor(dd, mp.at(m / P, 0, (int)(m % P), c));
+  *d = __float2half_rn(__half2float(*d) + v * gscale);
 }
 
 // the same into an fp32 channel slice (the fp32 training path)
+template <bool DROP>
 __global__ void __launch_bounds__(256) f32_accum_f32_kernel(const float* __restrict__ src, long long M, int C, float gscale,
-                                                            float* __restrict__ dst, int ld) {
+                                                            float* __restrict__ dst, int ld, int P, DropDraw dd, DropMap mp) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= M * C) return;
   const long long m = i / C;
   const int c = (int)(i - m * C);
   float* d = dst + (size_t)m * ld + c;
-  *d = *d + src[i] * gscale;
+  float v = src[i];
+  if constexpr (DROP) v = v * drop_factor(dd, mp.at(m / P, 0, (int)(m % P), c));
+  *d = *d + v * gscale;
 }
 
 // ---- max-pool backward (MaxPool3dTFPadding, i3dpt.py:114-126: zero ConstantPad3d, then MaxPool3d) ---------------------------
@@ -922,7 +987,8 @@ extern "C" int step_ctx_grad_reduce_f32(const float* dctx, int dctx_ld, const fl
   STEP_CHECK_ARG(B > 0 && C > 0 && R >= 0 && T_len > 0 && dctx_ld >= C && t_start >= 0 && t_start + T_len <= feat_T,
                  "ctx_grad_reduce: bad shape B=%d C=%d R=%d T_len=%d feat_T=%d t_start=%d", B, C, R, T_len, feat_T, t_start);
   STEP_CHECK_ARG(acc && (R == 0 || (dctx && tubes)), "ctx_grad_reduce: null pointer");
-  ctx_grad_reduce_kernel<<<ceil_div((long long)B * C, 256), 256, 0, cu(stream)>>>(dctx, dctx_ld, tubes, R, T_len, B, feat_T, t_start, C, acc);
+  ctx_grad_reduce_kernel<false><<<ceil_div((long long)B * C, 256), 256, 0, cu(stream)>>>(dctx, dctx_ld, tubes, R, T_len, B, feat_T,
+                                                                                         t_start, C, acc, DropDraw{}, DropMap{});
   STEP_LAUNCH_CHECK("ctx_grad_reduce_kernel");
   return 0;
 }
@@ -1045,7 +1111,8 @@ extern "C" int step_colsum_f32(const float* x, int ld, long long M, int C, float
 template <typename T>
 static int mean_mid_bwd_launch(const float* g, int A, int B, int P, int C, float gscale, void* dx, int ld, step_stream_t stream) {
   STEP_CHECK_ARG(g && dx && A > 0 && B > 0 && P > 0 && C > 0 && ld >= C, "mean_mid_bwd: bad arguments");
-  mean_mid_bwd_kernel<T><<<ceil_div((long long)A * B * P * C, 256), 256, 0, cu(stream)>>>(g, A, B, P, C, gscale, (T*)dx, ld);
+  mean_mid_bwd_kernel<T, false><<<ceil_div((long long)A * B * P * C, 256), 256, 0, cu(stream)>>>(g, A, B, P, C, gscale, (T*)dx, ld,
+                                                                                                  DropDraw{}, DropMap{});
   STEP_LAUNCH_CHECK("mean_mid_bwd_kernel");
   return 0;
 }
@@ -1060,14 +1127,14 @@ extern "C" int step_mean_mid_bwd_f32(const float* g, int A, int B, int P, int C,
 
 extern "C" int step_f32_accum_f16(const float* src, long long M, int C, float gscale, void* dst, int ld, step_stream_t stream) {
   STEP_CHECK_ARG(src && dst && M > 0 && C > 0 && ld >= C, "f32_accum_f16: bad arguments");
-  f32_accum_f16_kernel<<<ceil_div(M * C, 256), 256, 0, cu(stream)>>>(src, M, C, gscale, (__half*)dst, ld);
+  f32_accum_f16_kernel<false><<<ceil_div(M * C, 256), 256, 0, cu(stream)>>>(src, M, C, gscale, (__half*)dst, ld, 1, DropDraw{}, DropMap{});
   STEP_LAUNCH_CHECK("f32_accum_f16_kernel");
   return 0;
 }
 
 extern "C" int step_f32_accum_f32(const float* src, long long M, int C, float gscale, float* dst, int ld, step_stream_t stream) {
   STEP_CHECK_ARG(src && dst && M > 0 && C > 0 && ld >= C, "f32_accum_f32: bad arguments");
-  f32_accum_f32_kernel<<<ceil_div(M * C, 256), 256, 0, cu(stream)>>>(src, M, C, gscale, dst, ld);
+  f32_accum_f32_kernel<false><<<ceil_div(M * C, 256), 256, 0, cu(stream)>>>(src, M, C, gscale, dst, ld, 1, DropDraw{}, DropMap{});
   STEP_LAUNCH_CHECK("f32_accum_f32_kernel");
   return 0;
 }
@@ -1144,3 +1211,147 @@ extern "C" int step_conv_wgrad_f32(const float* dz, int dz_ld, const float* x, i
   STEP_LAUNCH_CHECK("conv_wgrad_f32_reduce_kernel");
   return 0;
 }
+
+// ---- dropout entries -------------------------------------------------------------------------------------------------------
+// torch's launch geometry for a draw of n elements (dropout.cuh); the argument checks every dropout entry makes first
+static int make_draw(const step_dropout_draw* d, long long n, const char* who, DropDraw* out, unsigned long long* offset_step) {
+  STEP_CHECK_ARG(d, "%s: null draw", who);
+  STEP_CHECK_ARG(d->keep > 0.0f && d->keep < 1.0f, "%s: keep probability %g outside (0, 1) (torch draws nothing at p = 0 or 1)", who,
+                 (double)d->keep);
+  STEP_CHECK_ARG(d->sm_count > 0 && d->threads_per_sm >= 256, "%s: sm_count %d / threads_per_sm %d must be positive and >= 256", who,
+                 d->sm_count, d->threads_per_sm);
+  if (n <= 0 || n % 4 != 0 || n > 0x7fffffffLL)
+    return fail(STEP_E_UNSUPPORTED, "%s: a draw of %lld elements (only 0 < n < 2^31 with n %% 4 == 0 is reproduced)", who, n);
+  const long long grid = std::min((n + 255) / 256, (long long)d->sm_count * (d->threads_per_sm / 256));
+  if (out) *out = DropDraw{(unsigned long long)d->seed, (unsigned long long)d->offset, d->keep, (float)(1.0 / (double)d->keep),
+                           (unsigned int)(grid * 256)};
+  if (offset_step) *offset_step = (unsigned long long)(((n - 1) / (grid * 256 * 4) + 1) * 4);
+  return 0;
+}
+
+// the global draw's tensor [R, C' = C*P + ctx_cols, T_len] (two_branch.py:239-244): element (r, t, p, c) of the downsample
+// output is (r * C' + c * P + p) * T_len + t; with base C*P*T_len and channel stride T_len, (r, t, 0, k) is context column k
+static DropMap global_map(int T_len, int P, int C, int ctx_cols, bool context) {
+  const long long Cp = (long long)C * P + ctx_cols;
+  if (context) return DropMap{(long long)C * P * T_len, Cp * T_len, 1, 0, T_len};
+  return DropMap{0, Cp * T_len, 1, T_len, P * T_len};
+}
+// the local draw's tensor [F, C, P] (two_branch.py:259-261): element (f, 0, p, c) is (f * C + c) * P + p
+static DropMap local_map(int P, int C) { return DropMap{0, (long long)C * P, 0, 1, P}; }
+
+extern "C" int step_dropout_check(const step_dropout_draw* draw, long long n, uint64_t* offset_step) {
+  unsigned long long s = 0;
+  if (int rc = make_draw(draw, n, "dropout", nullptr, &s)) return rc;
+  if (offset_step) *offset_step = s;
+  return 0;
+}
+
+extern "C" int step_dropout_mask_u8(const step_dropout_draw* draw, long long n, uint8_t* mask, step_stream_t stream) {
+  DropDraw dd;
+  if (int rc = make_draw(draw, n, "dropout_mask_u8", &dd, nullptr)) return rc;
+  STEP_CHECK_ARG(mask, "dropout_mask_u8: null pointer");
+  dropout_mask_kernel<<<(unsigned)std::min((n + 255) / 256, 8LL * kNumSMs * 8), 256, 0, cu(stream)>>>(dd, n, mask);
+  STEP_LAUNCH_CHECK("dropout_mask_kernel");
+  return 0;
+}
+
+template <typename T>
+static int dropout_copy_launch(const DropDraw& dd, const DropMap& mp, const void* x, int x_ld, long long M, int T_len, int P, int C,
+                               void* y, int y_ld, step_stream_t stream) {
+  dropout_copy_kernel<T><<<ceil_div(M * C, 256), 256, 0, cu(stream)>>>((const T*)x, x_ld, M, T_len, P, C, (T*)y, y_ld, dd, mp);
+  STEP_LAUNCH_CHECK("dropout_copy_kernel");
+  return 0;
+}
+
+extern "C" int step_dropout_global_fwd(const step_dropout_draw* draw, const void* x, int dtype, int x_ld, int R, int T_len, int P,
+                                       int C, int ctx_cols, void* y, int y_ld, step_stream_t stream) {
+  STEP_CHECK_ARG(R > 0 && T_len > 0 && P > 0 && C > 0 && ctx_cols >= 0 && x_ld >= C && y_ld >= C,
+                 "dropout_global_fwd: bad shape R=%d T=%d P=%d C=%d ctx_cols=%d x_ld=%d y_ld=%d", R, T_len, P, C, ctx_cols, x_ld, y_ld);
+  DropDraw dd;
+  if (int rc = make_draw(draw, (long long)R * ((long long)C * P + ctx_cols) * T_len, "dropout_global_fwd", &dd, nullptr)) return rc;
+  STEP_CHECK_ARG(x && y, "dropout_global_fwd: null pointer");
+  const DropMap mp = global_map(T_len, P, C, ctx_cols, false);
+  const long long M = (long long)R * T_len * P;
+  if (dtype == STEP_F32) return dropout_copy_launch<float>(dd, mp, x, x_ld, M, T_len, P, C, y, y_ld, stream);
+  if (dtype == STEP_F16) return dropout_copy_launch<__half>(dd, mp, x, x_ld, M, T_len, P, C, y, y_ld, stream);
+  return fail(STEP_E_ARG, "dropout_global_fwd: dtype %d", dtype);
+}
+
+extern "C" int step_dropout_local_fwd(const step_dropout_draw* draw, const void* x, int dtype, int x_ld, int F, int P, int C, void* y,
+                                      int y_ld, step_stream_t stream) {
+  STEP_CHECK_ARG(F > 0 && P > 0 && C > 0 && x_ld >= C && y_ld >= C, "dropout_local_fwd: bad shape F=%d P=%d C=%d x_ld=%d y_ld=%d", F, P,
+                 C, x_ld, y_ld);
+  DropDraw dd;
+  if (int rc = make_draw(draw, (long long)F * C * P, "dropout_local_fwd", &dd, nullptr)) return rc;
+  STEP_CHECK_ARG(x && y, "dropout_local_fwd: null pointer");
+  const DropMap mp = local_map(P, C);
+  const long long M = (long long)F * P;
+  if (dtype == STEP_F32) return dropout_copy_launch<float>(dd, mp, x, x_ld, M, 1, P, C, y, y_ld, stream);
+  if (dtype == STEP_F16) return dropout_copy_launch<__half>(dd, mp, x, x_ld, M, 1, P, C, y, y_ld, stream);
+  return fail(STEP_E_ARG, "dropout_local_fwd: dtype %d", dtype);
+}
+
+extern "C" int step_dropout_ctx_mean_f32(const step_dropout_draw* draw, int P, int C, const float* ctx, const int32_t* row_map,
+                                         long long row_stride, int t_stride, int k_stride, int R, int T_len, int K, float* out,
+                                         step_stream_t stream) {
+  STEP_CHECK_ARG(R > 0 && T_len > 0 && K > 0 && P > 0 && C > 0 && row_stride >= 0 && t_stride >= 0 && k_stride >= 0,
+                 "dropout_ctx_mean_f32: bad shape R=%d T=%d K=%d P=%d C=%d", R, T_len, K, P, C);
+  DropDraw dd;
+  if (int rc = make_draw(draw, (long long)R * ((long long)C * P + K) * T_len, "dropout_ctx_mean_f32", &dd, nullptr)) return rc;
+  STEP_CHECK_ARG(ctx && out, "dropout_ctx_mean_f32: null pointer");
+  ctx_mean_dropout_kernel<<<ceil_div((long long)R * K, 256), 256, 0, cu(stream)>>>(ctx, row_map, row_stride, t_stride, k_stride, R, T_len,
+                                                                                   K, out, dd, global_map(T_len, P, C, K, true));
+  STEP_LAUNCH_CHECK("ctx_mean_dropout_kernel");
+  return 0;
+}
+
+extern "C" int step_mean_mid_bwd_dropout(const step_dropout_draw* draw, int ctx_cols, const float* g, int A, int B, int P, int C,
+                                         float gscale, void* dx, int dtype, int ld, step_stream_t stream) {
+  STEP_CHECK_ARG(A > 0 && B > 0 && P > 0 && C > 0 && ctx_cols >= 0 && ld >= C, "mean_mid_bwd_dropout: bad arguments");
+  DropDraw dd;
+  if (int rc = make_draw(draw, (long long)A * ((long long)C * P + ctx_cols) * B, "mean_mid_bwd_dropout", &dd, nullptr)) return rc;
+  STEP_CHECK_ARG(g && dx, "mean_mid_bwd_dropout: null pointer");
+  const DropMap mp = global_map(B, P, C, ctx_cols, false);
+  const int grid = ceil_div((long long)A * B * P * C, 256);
+  if (dtype == STEP_F32)
+    mean_mid_bwd_kernel<float, true><<<grid, 256, 0, cu(stream)>>>(g, A, B, P, C, gscale, (float*)dx, ld, dd, mp);
+  else if (dtype == STEP_F16)
+    mean_mid_bwd_kernel<__half, true><<<grid, 256, 0, cu(stream)>>>(g, A, B, P, C, gscale, (__half*)dx, ld, dd, mp);
+  else
+    return fail(STEP_E_ARG, "mean_mid_bwd_dropout: dtype %d", dtype);
+  STEP_LAUNCH_CHECK("mean_mid_bwd_kernel");
+  return 0;
+}
+
+extern "C" int step_f32_accum_dropout(const step_dropout_draw* draw, const float* src, int F, int P, int C, float gscale, void* dst,
+                                      int dtype, int ld, step_stream_t stream) {
+  STEP_CHECK_ARG(F > 0 && P > 0 && C > 0 && ld >= C, "f32_accum_dropout: bad arguments");
+  DropDraw dd;
+  if (int rc = make_draw(draw, (long long)F * C * P, "f32_accum_dropout", &dd, nullptr)) return rc;
+  STEP_CHECK_ARG(src && dst, "f32_accum_dropout: null pointer");
+  const long long M = (long long)F * P;
+  const DropMap mp = local_map(P, C);
+  if (dtype == STEP_F32)
+    f32_accum_f32_kernel<true><<<ceil_div(M * C, 256), 256, 0, cu(stream)>>>(src, M, C, gscale, (float*)dst, ld, P, dd, mp);
+  else if (dtype == STEP_F16)
+    f32_accum_f16_kernel<true><<<ceil_div(M * C, 256), 256, 0, cu(stream)>>>(src, M, C, gscale, (__half*)dst, ld, P, dd, mp);
+  else
+    return fail(STEP_E_ARG, "f32_accum_dropout: dtype %d", dtype);
+  STEP_LAUNCH_CHECK("f32_accum_dropout_kernel");
+  return 0;
+}
+
+extern "C" int step_ctx_grad_reduce_dropout_f32(const step_dropout_draw* draw, int P, int Cg, const float* dctx, int dctx_ld,
+                                                const float* tubes, int R, int T_len, int B, int feat_T, int t_start, int C, float* acc,
+                                                step_stream_t stream) {
+  STEP_CHECK_ARG(B > 0 && C > 0 && R > 0 && T_len > 0 && P > 0 && Cg > 0 && dctx_ld >= C && t_start >= 0 && t_start + T_len <= feat_T,
+                 "ctx_grad_reduce_dropout: bad shape B=%d C=%d R=%d T_len=%d feat_T=%d t_start=%d", B, C, R, T_len, feat_T, t_start);
+  DropDraw dd;
+  if (int rc = make_draw(draw, (long long)R * ((long long)Cg * P + C) * T_len, "ctx_grad_reduce_dropout", &dd, nullptr)) return rc;
+  STEP_CHECK_ARG(acc && dctx && tubes, "ctx_grad_reduce_dropout: null pointer");
+  ctx_grad_reduce_kernel<true><<<ceil_div((long long)B * C, 256), 256, 0, cu(stream)>>>(dctx, dctx_ld, tubes, R, T_len, B, feat_T, t_start,
+                                                                                        C, acc, dd, global_map(T_len, P, Cg, C, true));
+  STEP_LAUNCH_CHECK("ctx_grad_reduce_kernel");
+  return 0;
+}
+

@@ -15,6 +15,7 @@ tensor-core weight gradient, or fp32 storage throughout (the reference's default
 `conv_wgrad_f32`.  Weight gradients are fp32 on both.
 """
 import contextlib
+import ctypes
 
 import torch
 
@@ -370,25 +371,84 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
     return out
 
 
+# ---- the heads' dropout (two_branch.py:244, 261) -------------------------------------------------------------------------
+_DEVICE_GEOMETRY = {}
+
+
+def dropout_draw(device, p, n):
+    """Take the draw that torch.nn.functional.dropout(x, p, training=True) makes for an n-element fp32 tensor x on `device`
+    from torch.cuda.default_generators[device]: returns the step_dropout_draw of the generator's state before it (seed,
+    offset, p, and the device's launch geometry), and advances the generator's offset as that call does.  The library
+    reproduces the call's keep mask from the draw (step_b200.h, step_dropout_*).  0 < p < 1 and n % 4 == 0, or it raises
+    before touching the generator; inside CUDA stream capture it raises (the offset moves on the host)."""
+    torch.cuda.init()                     # default_generators is empty until CUDA is initialised
+    device = torch.device(device)
+    index = device.index if device.index is not None else torch.cuda.current_device()
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("dropout_draw: the draw advances the generator's offset on the host and cannot be captured in a CUDA graph")
+    geom = _DEVICE_GEOMETRY.get(index)
+    if geom is None:
+        prop = torch.cuda.get_device_properties(index)
+        geom = _DEVICE_GEOMETRY[index] = (prop.multi_processor_count, prop.max_threads_per_multi_processor)
+    gen = torch.cuda.default_generators[index]
+    # keep = (float)(1 - p) with 1 - p in double, as ATen's dropout_cuda forms it (ctypes rounds the double to float)
+    draw = L.step_dropout_draw(seed=gen.initial_seed(), offset=gen.get_offset(), keep=1.0 - float(p), sm_count=geom[0],
+                               threads_per_sm=geom[1])
+    step = ctypes.c_uint64()
+    L.check(L.lib().step_dropout_check(draw, int(n), ctypes.byref(step)))
+    gen.set_offset(draw.offset + step.value)
+    return draw
+
+
+def dropout_mask(draw, n, device):
+    """The keep mask of a draw of n elements (uint8 [n], 1 = kept), in the dropped tensor's element order."""
+    with torch.cuda.device(device):
+        mask = torch.empty((n,), dtype=torch.uint8, device=device)
+        L.check(L.lib().step_dropout_mask_u8(draw, int(n), L.ptr(mask), L.stream()))
+    return mask
+
+
+def head_dropout_draws(net, R, T, context=True):
+    """The draws head `net` makes in a training forward over R tubes of T frames (two_branch.py:244, then 261), taken from
+    the default generator of the head's device: (global, local) -- local None for class-only heads -- or None when the head
+    draws nothing (net.dropout in eval mode, or p == 0).  context: whether the classifier reads the context columns."""
+    p = float(net.dropout.p)
+    if not net.dropout.training or p == 0.0:
+        return None
+    if p >= 1.0:
+        raise ValueError("head_dropout_draws: dropout p = %g zeroes the head's inputs; only p < 1 is supported" % p)
+    dev = net.global_cls.weight.device
+    D = net.fc_dim * net.pool_size ** 2
+    ctx_cols = net.global_cls.weight.shape[1] - D if context else 0
+    g = dropout_draw(dev, p, R * (D + ctx_cols) * T)
+    return g, None if net.cls_only else dropout_draw(dev, p, R * T * D)
+
+
 def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, lambda_reg=5.0, lambda_neighbor=1.0,
-                          loss_scale=1024.0, cat=None, objective_scale=1.0):
+                          loss_scale=1024.0, cat=None, objective_scale=1.0, dropout=False):
     """One training-time evaluation of a TwoBranchNet on the device (train.py:323-347 for one refinement step): forward
     with targets, the three losses, and the gradient of  mean(loss_cls) + lambda_reg * loss_loc + lambda_neighbor * loss_nb
     with respect to every trainable parameter of the head and to the pooled ROI features, on the head's precision path
     (net.fp16): fp16 or fp32 activations / activation gradients, fp32 weight gradients, with the static loss scale
     `loss_scale` applied to the activation gradients on both (apex-style; on fp32 a power of two is exact, and 1.0 is the
-    reference's fp32 arithmetic).  Dropout is the identity (eval mode), like the reference's gradient goldens.
+    reference's fp32 arithmetic).  Dropout is the identity (eval mode), like the reference's gradient goldens, unless
+    dropout=True and the head's nn.Dropout is in training mode with 0 < p < 1: then the head makes the reference's two draws
+    (`head_dropout_draws`) from the CUDA generator of its device, exactly the masks F.dropout would draw there, and the
+    forward and backward go through them (two_branch.py:244, 261; see step_b200.h, step_dropout_*).
     Class-only heads (TwoBranchNet(cls_only=True), the first training stage of train_cls.py) have no local branch: the
     objective is mean(loss_cls) alone (`cls_loss`), the regression losses are the reference's [1] zeros and grads holds the
     16 tensors of Mixed_5b / Mixed_5c, `downsample` and `global_cls`.
     context_feat (heads built with the context columns, cfg.no_context=False), in one of two forms:
       * [N,1024,T',1,1], the per-tube context feature the reference passes (train.py:317-321, two_branch.py:242-249);
       * (ctx_mean, row_map): ctx_mean fp32 [rows, 1024] is the mean of the context feature over the step's frames and
-        row_map int32 [N] (or None = identity) the row of each tube (ContextNet output per clip, as train_step feeds it).
+        row_map int32 [N] (or None = identity) the row of each tube (ContextNet output per clip, as train_step feeds it);
+        with dropout the frames themselves are needed: (ctx_mean, row_map, ctx, t_start), ctx the ContextNet output
+        [clips, T'', 1024] fp32 and t_start the step's first frame in it (row_map then gives each tube's clip).
     Returns dict(prob, loc, first, last, losses=(cls, loc, nb), loss, grads={param: grad}, feat_grad=[N,T',832,7,7] fp32,
     ctx_grad): grads holds the whole global_cls.weight (context columns included); ctx_grad is the gradient with respect to
     the context input, [N,1024,T',1,1] for the first form and the per-tube [N,1024] gradient of the row each tube reads for
-    the second (None without context)."""
+    the second (None without context).  With dropout the second form's ctx_grad is the gradient of each tube's dropped
+    context mean, and ctx_dropout holds what `context_grad_reduce` needs to take it through the draw."""
     from . import engine as E
     from .engine import Act
     from .networks import to_act
@@ -413,20 +473,37 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
             cat = Act.empty(N, Tl, Wd, Hd, C + fc, code, dev)
             src = to_act(global_feat, code)
             cat.buf[..., :C].copy_(src.buf[..., src.coff:src.coff + C])
+        drop = head_dropout_draws(net, N, Tl, context=context_feat is not None) if dropout else None
         ctx_mean, row_map, ctx_module_form = None, None, False
         if isinstance(context_feat, (tuple, list)):
-            ctx_mean, row_map = context_feat
+            ctx_mean, row_map = context_feat[:2]
             L.same_device(ctx_mean, row_map, cat.buf)
             ctx_mean = ctx_mean.float().contiguous()
+            if drop is not None:
+                if len(context_feat) != 4:
+                    raise RuntimeError("head_forward_backward: dropout needs the context frames: (ctx_mean, row_map, ctx, t_start)")
+                ctx, t0 = context_feat[2].detach().float().contiguous(), int(context_feat[3])
+                L.same_device(ctx, cat.buf)
+                K = ctx.shape[2]
+                rm = row_map.to(torch.int32).contiguous() if row_map is not None else None
+                ctx_mean = torch.empty((N, K), dtype=torch.float32, device=dev)
+                L.check(L.lib().step_dropout_ctx_mean_f32(drop[0], ps * ps, fc, L.c_void_p(ctx.data_ptr() + 4 * t0 * K), L.ptr(rm),
+                                                          ctx.shape[1] * K, K, 1, N, Tl, K, L.ptr(ctx_mean), L.stream()))
+                row_map = None
         elif context_feat is not None:
             ctx_module_form = True
             if tuple(context_feat.shape) != (N, 1024, Tl, 1, 1):
                 raise RuntimeError("head_forward_backward: context_feat %s, expected [%d,1024,%d,1,1]" % (tuple(context_feat.shape), N, Tl))
             cf = context_feat.detach().to(dev).float().contiguous().view(N * 1024, Tl)
-            ctx_mean = E.mean_mid(cf.data_ptr(), L.F32, N * 1024, Tl, 1, 1, 1, dev).view(N, 1024)   # as TwoBranchNet.forward
+            if drop is None:
+                ctx_mean = E.mean_mid(cf.data_ptr(), L.F32, N * 1024, Tl, 1, 1, 1, dev).view(N, 1024)   # as TwoBranchNet.forward
+            else:
+                ctx_mean = torch.empty((N, 1024), dtype=torch.float32, device=dev)
+                L.check(L.lib().step_dropout_ctx_mean_f32(drop[0], ps * ps, fc, L.ptr(cf), None, 1024 * Tl, 1, Tl, N, Tl, 1024,
+                                                          L.ptr(ctx_mean), L.stream()))
         tape, keep = [], {}
         with E.recording(tape):
-            prob, loc, first, last, logits = net.forward_act(cat, ctx_mean, row_map, want_logits=True, keep=keep)
+            prob, loc, first, last, logits = net.forward_act(cat, ctx_mean, row_map, want_logits=True, keep=keep, dropout=drop)
         if net.cls_only:
             # class-only heads: the regression losses are the reference's zeros (two_branch.py:252,276-280)
             lc, dlogits = cls_loss(logits, targets, want_grads=True)
@@ -448,21 +525,32 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
             xc = ctx_mean if row_map is None else ctx_mean.index_select(0, row_map.long())
             ctx_grad, dw_ctx, _ = linear_backward(xc, hw["ctx_w"], g["logits"])
             dw = torch.cat([unperm(dw), dw_ctx], 1)
-            if ctx_module_form:   # the classifier averages its per-frame logits over T' (two_branch.py:249)
+            if ctx_module_form and drop is not None:
+                # every tube is its own clip of T' frames: the reduce through the draw gives [N, T', 1024]
+                own = torch.zeros((N, Tl, 5), dtype=torch.float32, device=dev)
+                own[:, 0, 0] = torch.arange(N, dtype=torch.float32, device=dev) * Tl
+                acc = torch.zeros((N, Tl, 1024), dtype=torch.float32, device=dev)
+                context_grad_reduce(ctx_grad, own, acc, 0, dropout=(drop[0], ps * ps, fc))
+                ctx_grad = acc.permute(0, 2, 1).contiguous().view(N, 1024, Tl, 1, 1)
+            elif ctx_module_form:   # the classifier averages its per-frame logits over T' (two_branch.py:249)
                 ctx_grad = (ctx_grad * (1.0 / Tl)).view(N, 1024, 1, 1, 1).expand(N, 1024, Tl, 1, 1).contiguous()
         else:
             dw = unperm(dw)
         out[net.global_cls.weight] = dw.reshape(net.global_cls.weight.shape)
         out[net.global_cls.bias] = db
         gcat = grads.of(cat)
-        mean_mid_bwd = L.lib().step_mean_mid_bwd if code == L.F16 else L.lib().step_mean_mid_bwd_f32
-        L.check(mean_mid_bwd(L.ptr(dxbar), N, Tl, ps * ps, fc, float(loss_scale),
-                             L.c_void_p(gcat.data_ptr() + gcat.buf.element_size() * C), gcat.ld, L.stream()))
+        gconv_grad = L.c_void_p(gcat.data_ptr() + gcat.buf.element_size() * C)
+        if drop is not None:
+            L.check(L.lib().step_mean_mid_bwd_dropout(drop[0], 0 if ctx_mean is None else ctx_mean.shape[1], L.ptr(dxbar), N, Tl,
+                                                      ps * ps, fc, float(loss_scale), gconv_grad, code, gcat.ld, L.stream()))
+        else:
+            mean_mid_bwd = L.lib().step_mean_mid_bwd if code == L.F16 else L.lib().step_mean_mid_bwd_f32
+            L.check(mean_mid_bwd(L.ptr(dxbar), N, Tl, ps * ps, fc, float(loss_scale), gconv_grad, gcat.ld, L.stream()))
         # ---- regressors (two_branch.py:261-270): local_reg on every frame, neighbor_reg1 / 2 on the first / last chunk.
         # Class-only heads have no local branch: their tape ends at `downsample`.
         if not net.cls_only:
             lf2 = keep["local_feat2"]
-            lf2v = lf2.buf.view(N, Tl, D)
+            lf2v = keep["local_feat2_dropped"].buf.view(N, Tl, D)      # the regressors' input (lf2 itself without dropout)
             s0, s1, e0, e1 = keep["slices"]
             dlf2 = torch.zeros((N, Tl, D), dtype=torch.float32, device=dev)
             dx, dw, db = linear_backward(lf2v.reshape(N * Tl, D), hw["local_reg_w32"], g["local_loc"].reshape(N * Tl, 4), dx_out=dlf2.view(N * Tl, D))
@@ -473,15 +561,20 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
                 dlf2[:, a:b] += dx.view(N, b - a, D)                      # disjoint frame ranges of one buffer (host-side glue)
                 out[mod.weight], out[mod.bias] = unperm(dw), db
             glf2 = grads.of(lf2)
-            f32_accum = L.lib().step_f32_accum_f16 if code == L.F16 else L.lib().step_f32_accum_f32
-            L.check(f32_accum(L.ptr(dlf2), N * Tl * ps * ps, fc, float(loss_scale), L.c_void_p(glf2.data_ptr()), glf2.ld, L.stream()))
+            if drop is not None:
+                L.check(L.lib().step_f32_accum_dropout(drop[1], L.ptr(dlf2), N * Tl, ps * ps, fc, float(loss_scale),
+                                                       L.c_void_p(glf2.data_ptr()), code, glf2.ld, L.stream()))
+            else:
+                f32_accum = L.lib().step_f32_accum_f16 if code == L.F16 else L.lib().step_f32_accum_f32
+                L.check(f32_accum(L.ptr(dlf2), N * Tl * ps * ps, fc, float(loss_scale), L.c_void_p(glf2.data_ptr()), glf2.ld, L.stream()))
         # ---- every convolution and pool of the head, in reverse
         out.update(tape_backward(tape, grads, loss_scale))
         gcat = grads.of(cat)
         fg = gcat.buf[..., :C].float().mul_(1.0 / loss_scale).permute(0, 1, 4, 2, 3).contiguous() if global_feat is not None else None
     loss = lc.mean() + lambda_reg * ll.mean() + lambda_neighbor * ln.mean()
+    ctx_dropout = (drop[0], ps * ps, fc) if drop is not None and ctx_mean is not None and not ctx_module_form else None
     return dict(prob=prob, loc=loc, first=first, last=last, losses=(lc, ll, ln), loss=loss, grads=out, feat_grad=fg,
-                roi_grad=Act(gcat.buf, C, 0), ctx_grad=ctx_grad)
+                roi_grad=Act(gcat.buf, C, 0), ctx_grad=ctx_grad, ctx_dropout=ctx_dropout)
 
 
 def context_forward(context_net, feat):
@@ -517,17 +610,24 @@ def context_backward(state, d_ctx, loss_scale=1024.0):
     return out, gfeat.buf[..., gfeat.coff:gfeat.coff + gfeat.C]
 
 
-def context_grad_reduce(dctx, tubes, acc, t_start):
+def context_grad_reduce(dctx, tubes, acc, t_start, dropout=None):
     """acc [B, T', 1024] fp32 += the gradient of ContextNet's output from one refinement step: dctx [R, 1024] is each
     tube's gradient of the context row it read, tubes [R, T_len, 5] the step's flat tubes (train.py:317-321: clip =
-    floor(frame / T_len), frames [t_start, t_start + T_len) of the clip, weight 1 / T_len).  Deterministic."""
+    floor(frame / T_len), frames [t_start, t_start + T_len) of the clip, weight 1 / T_len).  Deterministic.
+    dropout: head_forward_backward's ctx_dropout when the classifier read the dropped context (dctx is then the gradient of
+    each tube's dropped context mean, and every frame's term goes through its element of the head's global draw)."""
     dev = L.same_device(dctx, tubes, acc)
     R, T_len = tubes.shape[0], tubes.shape[1]
     B, T_all, C = acc.shape
     d = dctx.float().contiguous()
     tb = tubes.float().contiguous()
     with torch.cuda.device(dev):
-        L.check(L.lib().step_ctx_grad_reduce_f32(L.ptr(d), C, L.ptr(tb), R, T_len, B, T_all, int(t_start), C, L.ptr(acc), L.stream()))
+        if dropout is not None:
+            draw, P, Cg = dropout
+            L.check(L.lib().step_ctx_grad_reduce_dropout_f32(draw, P, Cg, L.ptr(d), C, L.ptr(tb), R, T_len, B, T_all, int(t_start), C,
+                                                             L.ptr(acc), L.stream()))
+        else:
+            L.check(L.lib().step_ctx_grad_reduce_f32(L.ptr(d), C, L.ptr(tb), R, T_len, B, T_all, int(t_start), C, L.ptr(acc), L.stream()))
     return acc
 
 
@@ -601,7 +701,7 @@ def step_frames(cfg, i):
 
 
 def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9, weight_decay=0.0, lambda_reg=5.0,
-               lambda_neighbor=1.0, loss_scale=1024.0, sgd_state=None, world_size=1, optimizer=None, scaler=None):
+               lambda_neighbor=1.0, loss_scale=1024.0, sgd_state=None, world_size=1, optimizer=None, scaler=None, dropout=False):
     """One optimisation step of train.py:263-348 on the device, for already selected training samples
     (`train_select`, utils/utils.py:135-423, is step_b200.select_samples, which returns step_tubes and step_targets):
         conv_feat = base_net(clips); context_feat = context_net(conv_feat) unless cfg.no_context      train.py:266-269
@@ -625,7 +725,12 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     step_b200.optim.LossScaler; needs optimizer) replaces loss_scale by its dynamic scale and is updated from the step.
     Precision: that of the nets (cfg.fp16, one value for all of them).  fp16 stores activations and their gradients in
     fp16 (apex O1-like); fp32 stores everything in fp32, the reference's default (config.py:26-27), and with
-    loss_scale=1.0 and no scaler it is the reference's fp32 arithmetic.  Weight gradients and updates are fp32 on both."""
+    loss_scale=1.0 and no scaler it is the reference's fp32 arithmetic.  Weight gradients and updates are fp32 on both.
+    dropout=True: every head whose nn.Dropout is in training mode with 0 < p < 1 (the reference trains with --dropout 0.3,
+    scripts/train_step.sh and train_cls.sh) draws its masks as the reference's training forward does, step by step, global
+    then local, from the default CUDA generator of clips' device, and leaves that generator where those F.dropout calls
+    leave it (head_forward_backward); nothing else here draws from it.  With one GPU this is the reference's draw sequence
+    exactly.  Not in a CUDA graph: the draws move the generator's offset on the host."""
     from .engine import Act
     if optimizer is not None and lr is not None:
         raise ValueError("train_step: give either lr (sgd_step) or optimizer, not both")
@@ -676,12 +781,14 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
                 L.check(L.lib().step_mean_mid_strided(L.c_void_p(sl.data_ptr()), L.F32, B, t_len, 1, ctx.shape[2], ctx.shape[2],
                                                       T_all * ctx.shape[2], L.ptr(ctx_mean), L.F32, L.stream()))
                 row_map = torch.div(flat[:, 0, 0], float(t_len), rounding_mode="floor").to(torch.int32)
-                context = (ctx_mean, row_map)
+                context = (ctx_mean, row_map, ctx, t_start)
             r = head_forward_backward(head, None, flat, step_targets[i].to(dev), context_feat=context, lambda_reg=lambda_reg,
-                                      lambda_neighbor=lambda_neighbor, loss_scale=loss_scale, cat=cat)
+                                      lambda_neighbor=lambda_neighbor, loss_scale=loss_scale, cat=cat, dropout=dropout)
             results.append(r)
             all_grads.update(r["grads"])
-            if use_ctx:
+            if use_ctx and r["ctx_dropout"] is not None:
+                context_grad_reduce(r["ctx_grad"], flat, d_ctx, t_start, dropout=r["ctx_dropout"])
+            elif use_ctx:
                 context_grad_reduce(r["ctx_grad"], flat, d_ctx, t_start)
             with _phase("roi_bwd"):
                 if pool_mode == "pool":

@@ -268,10 +268,15 @@ class TwoBranchNet(nn.Module):
         lc, ll, ln = training.head_losses(logits, loc, first, last, tb, tg, self.T)
         return prob, loc, first, last, lc, ll, ln
 
-    def forward_act(self, cat, ctx_mean=None, ctx_row_map=None, want_logits=False, keep=None):
+    def forward_act(self, cat, ctx_mean=None, ctx_row_map=None, want_logits=False, keep=None, dropout=None):
         """cat: Act [R, T', 7, 7, ld >= 832 + fc] whose first 832 channels hold the ROI features.
         ctx_mean: fp32 [rows, 1024] temporal mean of the context feature; ctx_row_map: int32 [R]
-        row of ctx_mean for each tube (None = identity).  Returns fp32 tensors."""
+        row of ctx_mean for each tube (None = identity).  Returns fp32 tensors.
+        dropout: None (eval-mode dropout, the identity), or the head's two training-mode draws (global, local) of
+        step_b200.training.dropout_draw (local None for class-only heads): the classifier then reads the dropped copy of the
+        downsample output (two_branch.py:244; the concat into the local branch stays undropped, :256) and the regressors the
+        dropped downsample2 output (:261).  The context columns' draw is the caller's: ctx_mean is then already the mean of
+        the dropped context (training.head_forward_backward)."""
         R, T, ps = cat.N, cat.T, self.pool_size
         code = cat.code
         roi = cat.slice(0, 832)
@@ -283,8 +288,14 @@ class TwoBranchNet(nn.Module):
         E.conv(g, w, None, bias, gconv, (1, 1, 1), relu=False, tag=self.downsample)
         hw = self._head_weights()
         D = self.fc_dim * ps * ps
+        gsrc = gconv
+        if dropout is not None:
+            gsrc = Act.empty(R, T, ps, ps, self.fc_dim, code, cat.device)
+            ctx_cols = 0 if hw["ctx_w"] is None else hw["ctx_w"].shape[1]
+            L.check(L.lib().step_dropout_global_fwd(dropout[0], L.c_void_p(gconv.data_ptr()), code, cat.ld, R, T, ps * ps, self.fc_dim,
+                                                    ctx_cols, L.c_void_p(gsrc.data_ptr()), gsrc.ld, L.stream()))
         # temporal mean then classifier (+ context columns) then sigmoid (two_branch.py:246-249,337)
-        xbar = E.mean_mid(gconv.data_ptr(), code, R, T, ps * ps, self.fc_dim, cat.ld, cat.device)
+        xbar = E.mean_mid(gsrc.data_ptr(), code, R, T, ps * ps, self.fc_dim, gsrc.ld, cat.device)
         has_ctx = ctx_mean is not None and hw["ctx_w"] is not None
         logits = E.linear_small_n(xbar, R, D, D, hw["cls_w"], hw["cls_b"], self.num_classes,
                                   act=0 if has_ctx else 1)
@@ -305,6 +316,11 @@ class TwoBranchNet(nn.Module):
             return (prob, z, z, z, raw) if want_logits else (prob, z, z, z)
         # local branch on frames (two_branch.py:253-262)
         lf, lf2 = self._local_branch(cat.frames(), want_lf=keep is not None)
+        lf2d = lf2
+        if dropout is not None:
+            lf2d = Act.empty(R * T, 1, ps, ps, self.fc_dim, code, cat.device)
+            L.check(L.lib().step_dropout_local_fwd(dropout[1], L.c_void_p(lf2.data_ptr()), code, lf2.ld, R * T, ps * ps, self.fc_dim,
+                                                   L.c_void_p(lf2d.data_ptr()), lf2d.ld, L.stream()))
         # the three regressors share their input: one pass with the twelve weight rows (two_branch.py:261-270)
         Tc = self.T
         chunks = int(T / Tc)
@@ -318,10 +334,10 @@ class TwoBranchNet(nn.Module):
         last = torch.empty((R, e1 - e0, 4), dtype=torch.float32, device=cat.device)
         nbytes = L.lib().step_linear_small_n_workspace_bytes(R * T, D, 12)
         ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=cat.device)
-        L.check(L.lib().step_head_regress(L.ptr(lf2.buf), code, R, T, D, D, L.ptr(w12), L.ptr(b12), s0, s1, e0, e1,
+        L.check(L.lib().step_head_regress(L.ptr(lf2d.buf), code, R, T, D, D, L.ptr(w12), L.ptr(b12), s0, s1, e0, e1,
                                           L.ptr(local_loc), L.ptr(first), L.ptr(last), L.ptr(ws), nbytes, L.stream()))
         if keep is not None:   # activations the training pieces need (step_b200/training.py): channels-last layouts
-            keep.update(xbar=xbar, local_feat=lf, local_feat2=lf2, slices=(s0, s1, e0, e1))
+            keep.update(xbar=xbar, local_feat=lf, local_feat2=lf2, local_feat2_dropped=lf2d, slices=(s0, s1, e0, e1))
         return (prob, local_loc, first, last, raw) if want_logits else (prob, local_loc, first, last)
 
     def _local_branch(self, frames, want_lf=False):
