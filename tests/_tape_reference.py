@@ -258,6 +258,17 @@ def check_fwd(got, ref, xw, epi, steps, what, extra=None):
     return n, d, thr
 
 
+def check_fwd32(got, ref, xw, epi, n, what):
+    """One fp32 SIMT convolution output (csrc/conv_simt.cu, fp32 storage) against its reference, elementwise:
+        |got - ref| <= gamma_n |scale| (|x| |w|) + 3 u32 (|acc scale| + |shift| + |res|),   gamma_n = n u32 / (1 - n u32),
+    n = taps x Cin: the accumulation is one fmaf chain of n terms (each rounding within u32 of a partial sum <= the abs
+    sum), the epilogue's multiply and two additions round once each, ReLU is 1-Lipschitz and the store is exact.  xw / epi
+    are conv_fwd's.  Returns the largest |err| / bound."""
+    assert n * U32 < 0.5, (what, n)
+    tol = n * U32 / (1.0 - n * U32) * xw.double() + 3.0 * U32 * epi.double()
+    return _check_within(got, ref, tol, what)
+
+
 def exit_fwd(h, w3, x, w1, shift2, relu2):
     """Float64 reference of step_bottleneck_exit_f16 on rows: h fp16 [M, planes], w3 [inplanes, 1, planes], x fp16
     [M, inplanes], w1 [outplanes, 1, inplanes], shift2 fp32 [outplanes] | None.

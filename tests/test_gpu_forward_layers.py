@@ -101,9 +101,10 @@ def _clone(t):
     return t.detach().clone() if t is not None else None
 
 
-def install(mp, rec):
+def install(mp, rec, fused_exit=True):
     """The wrappers.  Each clones what its launch reads before calling the original and what it wrote right after, on the
-    current (issuing) stream."""
+    current (issuing) stream.  fused_exit: the full head runs the fused bottleneck exit (the fp16 inference path; the
+    fp32 path runs it as separate convolutions and its regressors read downsample2's conv output)."""
     from step_b200 import _lib as L
     from step_b200 import engine as E
     from step_b200 import networks, two_branch
@@ -170,8 +171,12 @@ def install(mp, rec):
         res = orig["forward_act"](self, cat, ctx_mean, ctx_row_map, want_logits, keep)
         if not self.cls_only:
             exits = [r for r in rec.recs[start:] if r["kind"] == "exit"]
-            assert exits, "the inference head runs the fused exit"
-            lf2 = exits[-1]["outs"][0][1]
+            if fused_exit:
+                assert exits, "the inference head runs the fused exit"
+                lf2 = exits[-1]["outs"][0][1]
+            else:
+                assert not exits, "this head was expected to run its exits unfused"
+                lf2 = [r for r in rec.recs[start:] if r["kind"] == "conv"][-1]["outs"][0][1]    # downsample2
             rec.recs.append(dict(kind="regress", x=lf2.reshape(-1, *lf2.shape[2:]), mods=(self.local_reg, self.neighbor_reg1,
                                  self.neighbor_reg2), Tc=self.T, T=cat.T, outs=[(t, t.clone()) for t in res[1:4]]))
         return res
@@ -291,6 +296,12 @@ def test_kernels_reached(geom):
 
 
 def test_instrumented_run_is_bit_identical_and_writes_persist(geom):
+    check_instrumented_run(geom)
+
+
+def check_instrumented_run(geom):
+    """The instrumented run's outputs equal the plain run's bit for bit, every region a launch wrote still holds what it
+    wrote when the forward ends, and an accumulating linear launch read what the launch before it wrote."""
     assert len(geom["plain"]) == len(geom["inst"])
     for a, b in zip(geom["plain"], geom["inst"]):
         assert torch.equal(a, b)
