@@ -417,6 +417,25 @@ int step_maxpool3d_bwd_f32(const float* x, int x_ld, const float* dy, int dy_ld,
                            int KH, int KW, int ST, int SH, int SW, int PT, int PH, int PW, int pad_hi_t, int pad_hi_h,
                            int pad_hi_w, int OT, int OH, int OW, float* dx, int dx_ld, uint8_t* argmax_ws, step_stream_t stream);
 
+/* BatchNorm affine gradients of y = relu(BN_eval(z)) = relu(scale * z + shift), scale = gamma / sqrt(running_var + eps), for a
+ * Unit3Dpy whose gamma / beta train (freeze_affine=False).  Writes dz and dres exactly as step_act_bwd_f16 / _f32 (the same
+ * arguments, bit for bit) and, from the same read of dy and y, with g = dy * [y > 0] (g = dy without relu):
+ *   dbeta[c]  = gscale * sum_m g[m, c]
+ *   dgamma[c] = gscale * (sum_m g[m, c] * (y[m, c] - beta[c])) / gamma[c]
+ * because wherever g != 0, y = gamma * xhat + beta.  beta, gamma: fp32 [C], the BatchNorm's own parameters for the C channels
+ * of the slice; gscale: 1 / loss_scale.  dgamma or dbeta may be NULL (not both).  gamma[c] == 0 gives dgamma[c] = 0, which
+ * is exact when the channel's g is all zero (relu and beta[c] <= 0); with beta[c] > 0, xhat cannot be recovered from y and
+ * the caller must refuse the channel.  Per-chunk partials go to the workspace (step_act_bn_bwd_workspace_bytes) and are added
+ * in chunk order by a second kernel: no atomics, bit-identical from run to run.  C and the ld arguments multiples of the
+ * 16-byte vector (8 fp16, 4 fp32), 16-byte aligned dy / y / dz / dres. */
+size_t step_act_bn_bwd_workspace_bytes(long long M, int C);
+int step_act_bn_bwd_f16(const void* dy, int dy_ld, const void* y, int y_ld, const float* scale, int relu, long long M, int C,
+                        void* dz, int dz_ld, void* dres, int dres_ld, const float* beta, const float* gamma, float gscale,
+                        float* dgamma, float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream);
+int step_act_bn_bwd_f32(const float* dy, int dy_ld, const float* y, int y_ld, const float* scale, int relu, long long M, int C,
+                        float* dz, int dz_ld, float* dres, int dres_ld, const float* beta, const float* gamma, float gscale,
+                        float* dgamma, float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream);
+
 /* ------------------------------------------------------------------ the heads' dropout ---- */
 /* One draw of torch.nn.functional.dropout(x, p, training=True) on a CUDA fp32 tensor of n elements (n % 4 == 0, n < 2^31,
  * 16-byte aligned and contiguous, as every dropout input of the heads is): seed and offset are the device generator's

@@ -514,6 +514,98 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const T* __restrict__ dy, 
   store16(dz + (size_t)m * dz_ld + c, g);
 }
 
+// act_bwd_kernel for a Unit3Dpy whose BatchNorm affine trains (freeze_affine=False): the same dz / dres, and in the same
+// pass the per-chunk, per-channel partials of  sum g  and  sum g * (y - beta)  (g = dy * [y > 0]), the numerators of
+// dbeta and gamma * dgamma: wherever g != 0 the stored y is gamma * xhat + beta.  The block holds `cols` channel vectors
+// of `rows` pixels at a time (cols * rows <= 256 threads) and walks its chunk's pixels; its rows are added in ascending
+// order through shared memory.  partial: [chunks, 2, C] fp32 (sum g, then sum g (y - beta)).
+constexpr int kBnRowsPerChunk = 256, kBnMaxChunks = 512;
+template <typename T>
+__global__ void __launch_bounds__(256) act_bn_bwd_partial_kernel(const T* __restrict__ dy, int dy_ld, const T* __restrict__ y,
+                                                                 int y_ld, const float* __restrict__ scale, int relu, long long M,
+                                                                 int C, T* __restrict__ dz, int dz_ld, T* __restrict__ dres,
+                                                                 int dres_ld, const float* __restrict__ beta, int cols, int rows,
+                                                                 long long rows_per_chunk, float* __restrict__ partial) {
+  constexpr int V = Vec16<T>::N;
+  __shared__ float red[2][256 * V];
+  const int cv = C / V;
+  const int t = threadIdx.x, col = t % cols, r = t / cols;
+  const int cvec = blockIdx.y * cols + col;
+  const bool live = r < rows && cvec < cv;
+  const int c = cvec * V;
+  float sg[V], sgy[V];
+#pragma unroll
+  for (int k = 0; k < V; ++k) sg[k] = sgy[k] = 0.0f;
+  if (live) {
+    float b[V];
+#pragma unroll
+    for (int k = 0; k < V; ++k) b[k] = beta[c + k];
+    const long long m0 = (long long)blockIdx.x * rows_per_chunk, m1 = m0 + rows_per_chunk < M ? m0 + rows_per_chunk : M;
+    for (long long m = m0 + r; m < m1; m += rows) {
+      float g[V], v[V];
+      load16(dy + (size_t)m * dy_ld + c, g);
+      load16(y + (size_t)m * y_ld + c, v);
+      if (relu) {
+#pragma unroll
+        for (int k = 0; k < V; ++k) g[k] = v[k] > 0.0f ? g[k] : 0.0f;
+      }
+#pragma unroll
+      for (int k = 0; k < V; ++k) {
+        sg[k] += g[k];
+        sgy[k] += g[k] * (v[k] - b[k]);
+      }
+      if (dres) {
+        float rr[V];
+        load16(dres + (size_t)m * dres_ld + c, rr);
+#pragma unroll
+        for (int k = 0; k < V; ++k) rr[k] += g[k];
+        store16(dres + (size_t)m * dres_ld + c, rr);
+      }
+      if (scale) {
+#pragma unroll
+        for (int k = 0; k < V; ++k) g[k] *= scale[c + k];
+      }
+      store16(dz + (size_t)m * dz_ld + c, g);
+    }
+  }
+  if (r < rows) {
+#pragma unroll
+    for (int k = 0; k < V; ++k) {
+      red[0][r * cols * V + col * V + k] = sg[k];
+      red[1][r * cols * V + col * V + k] = sgy[k];
+    }
+  }
+  __syncthreads();
+  const int width = cols * V;
+  for (int j = t; j < 2 * width; j += blockDim.x) {
+    const int which = j / width, ch = j - which * width;
+    if (blockIdx.y * width + ch >= C) continue;
+    float acc = 0.0f;
+    for (int q = 0; q < rows; ++q) acc += red[which][q * width + ch];
+    partial[((size_t)blockIdx.x * 2 + which) * C + blockIdx.y * width + ch] = acc;
+  }
+}
+
+// dbeta[c] = gscale * sum_chunks sum g;  dgamma[c] = gscale * (sum_chunks sum g (y - beta)) / gamma[c], chunks in order.
+// gamma[c] == 0 gives dgamma[c] = 0: exact when g is 0 on the whole channel (ReLU and beta <= 0); the caller refuses the
+// other case (beta > 0), where xhat cannot be recovered from y.
+__global__ void __launch_bounds__(256) act_bn_bwd_reduce_kernel(const float* __restrict__ partial, int chunks, int C,
+                                                                const float* __restrict__ gamma, float gscale,
+                                                                float* __restrict__ dgamma, float* __restrict__ dbeta) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float sg = 0.0f, sgy = 0.0f;
+  for (int k = 0; k < chunks; ++k) {
+    sg += partial[(size_t)k * 2 * C + c];
+    sgy += partial[((size_t)k * 2 + 1) * C + c];
+  }
+  if (dbeta) dbeta[c] = sg * gscale;
+  if (dgamma) {
+    const float gm = gamma[c];
+    dgamma[c] = gm == 0.0f ? 0.0f : (sgy * gscale) / gm;
+  }
+}
+
 // column sums of a [M, C] fp16 / fp32 matrix in fp32 (bias gradients), fixed order: thread per column block, rows ascending
 // in chunks that a second pass adds in chunk order
 template <typename T>
@@ -1084,6 +1176,57 @@ extern "C" int step_act_bwd_f16(const void* dy, int dy_ld, const void* y, int y_
 extern "C" int step_act_bwd_f32(const float* dy, int dy_ld, const float* y, int y_ld, const float* scale, int relu, long long M, int C,
                                 float* dz, int dz_ld, float* dres, int dres_ld, step_stream_t stream) {
   return act_bwd_launch<float>(dy, dy_ld, y, y_ld, scale, relu, M, C, dz, dz_ld, dres, dres_ld, stream);
+}
+
+static int act_bn_bwd_chunks(long long M) {
+  const long long c = (M + kBnRowsPerChunk - 1) / kBnRowsPerChunk;
+  return (int)(c < kBnMaxChunks ? c : kBnMaxChunks);
+}
+
+extern "C" size_t step_act_bn_bwd_workspace_bytes(long long M, int C) {
+  if (M <= 0 || C <= 0) return 0;
+  return (size_t)act_bn_bwd_chunks(M) * 2 * C * sizeof(float);
+}
+
+template <typename T>
+static int act_bn_bwd_launch(const void* dy, int dy_ld, const void* y, int y_ld, const float* scale, int relu, long long M, int C,
+                             void* dz, int dz_ld, void* dres, int dres_ld, const float* beta, const float* gamma, float gscale,
+                             float* dgamma, float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream) {
+  constexpr int V = Vec16<T>::N;
+  STEP_CHECK_ARG(M > 0 && C > 0 && dy && y && dz && beta && gamma && workspace && (dgamma || dbeta), "act_bn_bwd: bad arguments");
+  STEP_CHECK_ARG(C % V == 0 && dy_ld % V == 0 && y_ld % V == 0 && dz_ld % V == 0 && (!dres || dres_ld % V == 0) && dy_ld >= C &&
+                 y_ld >= C && dz_ld >= C && (!dres || dres_ld >= C),
+                 "act_bn_bwd: C and the ld arguments must be multiples of %d (C=%d dy_ld=%d y_ld=%d dz_ld=%d dres_ld=%d)", V, C, dy_ld,
+                 y_ld, dz_ld, dres_ld);
+  STEP_CHECK_ARG((((uintptr_t)dy | (uintptr_t)y | (uintptr_t)dz | (uintptr_t)dres) & 15) == 0, "act_bn_bwd: pointers must be 16-byte aligned");
+  const size_t need = step_act_bn_bwd_workspace_bytes(M, C);
+  if (ws_bytes < need) return fail(STEP_E_WORKSPACE, "act_bn_bwd: workspace %zu < %zu", ws_bytes, need);
+  const int cv = C / V, cols = cv < 256 ? cv : 256, rows = 256 / cols;
+  const int chunks = act_bn_bwd_chunks(M);
+  const long long rows_per_chunk = (M + chunks - 1) / chunks;
+  act_bn_bwd_partial_kernel<T><<<dim3(chunks, ceil_div(cv, cols)), 256, 0, cu(stream)>>>(
+      (const T*)dy, dy_ld, (const T*)y, y_ld, scale, relu, M, C, (T*)dz, dz_ld, (T*)dres, dres_ld, beta, cols, rows, rows_per_chunk,
+      (float*)workspace);
+  STEP_LAUNCH_CHECK("act_bn_bwd_partial_kernel");
+  act_bn_bwd_reduce_kernel<<<ceil_div(C, 256), 256, 0, cu(stream)>>>((const float*)workspace, chunks, C, gamma, gscale, dgamma, dbeta);
+  STEP_LAUNCH_CHECK("act_bn_bwd_reduce_kernel");
+  return 0;
+}
+
+extern "C" int step_act_bn_bwd_f16(const void* dy, int dy_ld, const void* y, int y_ld, const float* scale, int relu, long long M,
+                                   int C, void* dz, int dz_ld, void* dres, int dres_ld, const float* beta, const float* gamma,
+                                   float gscale, float* dgamma, float* dbeta, void* workspace, size_t ws_bytes,
+                                   step_stream_t stream) {
+  return act_bn_bwd_launch<__half>(dy, dy_ld, y, y_ld, scale, relu, M, C, dz, dz_ld, dres, dres_ld, beta, gamma, gscale, dgamma,
+                                   dbeta, workspace, ws_bytes, stream);
+}
+
+extern "C" int step_act_bn_bwd_f32(const float* dy, int dy_ld, const float* y, int y_ld, const float* scale, int relu, long long M,
+                                   int C, float* dz, int dz_ld, float* dres, int dres_ld, const float* beta, const float* gamma,
+                                   float gscale, float* dgamma, float* dbeta, void* workspace, size_t ws_bytes,
+                                   step_stream_t stream) {
+  return act_bn_bwd_launch<float>(dy, dy_ld, y, y_ld, scale, relu, M, C, dz, dz_ld, dres, dres_ld, beta, gamma, gscale, dgamma,
+                                  dbeta, workspace, ws_bytes, stream);
 }
 
 template <typename T>

@@ -269,11 +269,42 @@ def timing_summary():
     return {k: round(sum(a.elapsed_time(b) for a, b in v), 2) for k, v in (TIMING or {}).items()}
 
 
+def trainable_bn(tag):
+    """The BatchNorm3d of a tape tag (a Unit3Dpy) whose weight (gamma) or bias (beta) requires grad -- freeze_affine=False,
+    networks.py:136-142 / two_branch.py:46-50 -- else None."""
+    bn = getattr(tag, "batch3d", None) if getattr(tag, "use_bn", False) else None
+    if bn is None or not (bn.weight.requires_grad or bn.bias.requires_grad):
+        return None
+    return bn
+
+
+def check_bn_affine(nets):
+    """Raise ValueError naming the first BatchNorm of nets ({key: module}) whose affine parameters train and that has a
+    channel with gamma == 0 and beta > 0: that channel's output is relu(beta), constant, and its normalised input, which the
+    gamma gradient needs, cannot be recovered from it.  One device-to-host read for all layers, none when no BatchNorm
+    trains."""
+    bns = [("%s.%s" % (key, name), m) for key, mod in nets.items() if mod is not None for name, m in mod.named_modules()
+           if isinstance(m, torch.nn.BatchNorm3d) and (m.weight.requires_grad or m.bias.requires_grad)]
+    if not bns:
+        return
+    with torch.no_grad():
+        bad = torch.stack([((m.weight == 0) & (m.bias > 0)).any() for _, m in bns]).cpu()
+    if bool(bad.any()):
+        name = bns[int(bad.nonzero()[0, 0])][0]
+        raise ValueError("BatchNorm %s has a channel with gamma == 0 and beta > 0: its output is constant and gamma's gradient "
+                         "cannot be recovered from it; freeze that layer's affine parameters or give gamma a non-zero value"
+                         % name)
+
+
 def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
     """Reverse pass over the conv / max-pool tape recorded by engine.TAPE, in the storage type of each entry's activations
     (fp16: tensor-core weight gradient; fp32: step_conv_wgrad_f32).  `grads` (GradStore) must already hold
     d(loss * loss_scale)/d(output) of the last layers.  Returns {parameter tensor: fp32 gradient in the parameter's own
-    layout} (BatchNorm is frozen, i3dpt / networks.py:136-142: only conv weights and biases train).
+    layout}: conv weights and biases, and the weight (gamma) and bias (beta) of every Unit3Dpy BatchNorm whose affine
+    parameters require grad (freeze_affine=False; step_act_bn_bwd_*, from the stored output: wherever its gradient is
+    non-zero, y = gamma * xhat + beta).  Each BatchNorm tensor is returned only if it requires grad.  BatchNorm always
+    normalises with its running statistics (freeze_stats=True).  A channel with gamma == 0 gives dgamma = 0, exact unless
+    beta > 0, which `check_bn_affine` refuses.
     The input gradient of every layer is produced by the SAME convolution kernels as its forward (wgmma on fp16, SIMT on
     fp32), run on the transposed, flipped filter (stride-1 convolutions: dx = conv(dz, flip(w)^T)), accumulated through
     their residual input.  need_input_grad(entry) -> bool limits which entries form it (default: all).  A strided
@@ -312,17 +343,35 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
         dz = torch.empty((y0.N, y0.T, y0.H, y0.W, n_total), dtype=x.buf.dtype, device=x.device)
         esz = dz.element_size()
         act_bwd = lib.step_act_bwd_f16 if f16 else lib.step_act_bwd_f32
+        s2d = isinstance(e["tag"], tuple) and e["tag"][0] == "s2d"
+        out_tags = [e["tag"][1]] if s2d else list(e["tag"]) if isinstance(e["tag"], (list, tuple)) else [e["tag"]]
+        out_tags += [None] * (len(outs) - len(out_tags))        # every output gets its activation backward
         col = 0
         with _phase("act_bwd"):
-            for o in outs:
+            for o, tg in zip(outs, out_tags):
                 gy = grads.of(o)
                 sc = e["scale"][col:col + o.C] if e["scale"] is not None else None
                 res = e["residual"]
                 gres = grads.of(res) if res is not None else None
-                L.check(act_bwd(L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, L.ptr(sc),
-                                1 if e["relu"] else 0, M, o.C, L.c_void_p(dz.data_ptr() + esz * col), n_total,
-                                L.c_void_p(gres.data_ptr()) if gres is not None else None,
-                                gres.ld if gres is not None else 0, L.stream()))
+                args = (L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, L.ptr(sc), 1 if e["relu"] else 0, M,
+                        o.C, L.c_void_p(dz.data_ptr() + esz * col), n_total,
+                        L.c_void_p(gres.data_ptr()) if gres is not None else None, gres.ld if gres is not None else 0)
+                bn = trainable_bn(tg)
+                if bn is None:
+                    L.check(act_bwd(*args, L.stream()))
+                else:   # the same dz / dres, and the BatchNorm's gamma / beta gradients from the same pass
+                    gam, bet = bn.weight, bn.bias
+                    dgam = torch.empty((o.C,), dtype=torch.float32, device=x.device) if gam.requires_grad else None
+                    dbet = torch.empty((o.C,), dtype=torch.float32, device=x.device) if bet.requires_grad else None
+                    nbytes = lib.step_act_bn_bwd_workspace_bytes(M, o.C)
+                    ws = torch.empty((nbytes // 4,), dtype=torch.float32, device=x.device)
+                    act_bn_bwd = lib.step_act_bn_bwd_f16 if f16 else lib.step_act_bn_bwd_f32
+                    L.check(act_bn_bwd(*args, L.ptr(bet.detach()), L.ptr(gam.detach()), inv, L.ptr(dgam), L.ptr(dbet), L.ptr(ws),
+                                       nbytes, L.stream()))
+                    if dgam is not None:
+                        add(gam, dgam)
+                    if dbet is not None:
+                        add(bet, dbet)
                 col += o.C
         # ---- weight (and bias) gradients
         taps = k[0] * k[1] * k[2]
@@ -337,7 +386,7 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
                                                 L.stream()))
             else:
                 dw = conv_wgrad_f32(Act(dz), x, k, e["stride"], pl, inv)
-        if isinstance(e["tag"], tuple) and e["tag"][0] == "s2d":
+        if s2d:
             unit = e["tag"][1]
             if unit.conv3d.weight.requires_grad:
                 add(unit.conv3d.weight, stem_s2d_wgrad(dw, unit.conv3d.in_channels))
@@ -437,7 +486,8 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
     forward and backward go through them (two_branch.py:244, 261; see step_b200.h, step_dropout_*).
     Class-only heads (TwoBranchNet(cls_only=True), the first training stage of train_cls.py) have no local branch: the
     objective is mean(loss_cls) alone (`cls_loss`), the regression losses are the reference's [1] zeros and grads holds the
-    16 tensors of Mixed_5b / Mixed_5c, `downsample` and `global_cls`.
+    16 tensors of Mixed_5b / Mixed_5c, `downsample` and `global_cls`.  With freeze_affine=False grads also holds the gamma
+    and beta of the head's Unit3D BatchNorms that require grad (tape_backward).
     context_feat (heads built with the context columns, cfg.no_context=False), in one of two forms:
       * [N,1024,T',1,1], the per-tube context feature the reference passes (train.py:317-321, two_branch.py:242-249);
       * (ctx_mean, row_map): ctx_mean fp32 [rows, 1024] is the mean of the context feature over the step's frames and
@@ -596,7 +646,8 @@ def context_forward(context_net, feat):
 def context_backward(state, d_ctx, loss_scale=1024.0):
     """Backward of context_forward from d_ctx = d(loss)/d(ctx), fp32 [B,T',1024]: the spatial mean's backward into the
     gradient of Mixed_5c's output, then the tape (Mixed_5c, Mixed_5b, the (1,3,3)/(1,2,2) max-pool).  Returns
-    ({conv weight: fp32 gradient} for the 12 Unit3D convolutions -- BatchNorm stays frozen --, [B,T',H',W',832] in the
+    ({parameter: fp32 gradient} for the 12 Unit3D convolutions, and their BatchNorms' gamma / beta when those require grad
+    (freeze_affine=False, tape_backward), [B,T',H',W',832] in the
     forward's storage type (a channel-slice view) holding loss_scale * d(loss)/d(conv_feat) through the context branch)."""
     x = state["x"]
     with torch.cuda.device(x.device), torch.no_grad():
@@ -637,7 +688,8 @@ def trunk_forward_backward(base_net, clips, d_feat_fn, loss_scale=1024.0):
     step_conv_wgrad_f32 (on fp16 the stem runs as the space-to-depth 4x4x4 filter, stem_s2d_wgrad).
     d_feat_fn(feat_act) -> fp32 tensor [N,T',H',W',832] (channels-last) with the gradient of the loss w.r.t. the trunk
     output (e.g. the sum of the ROIAlign backward results of the refinement steps).
-    Returns (feat Act, {conv weight: fp32 gradient}).  BatchNorm stays frozen (networks.py:85-99,136-142)."""
+    Returns (feat Act, {parameter: fp32 gradient}): the conv weights, and the BatchNorms' gamma / beta where they require
+    grad (freeze_affine=False, networks.py:136-142; the statistics stay the running ones, networks.py:85-99)."""
     from . import engine as E
     dev = clips.device
     with torch.cuda.device(dev), torch.no_grad():
@@ -718,7 +770,9 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     the context branch's; the pooling is nets['roi_net'].pool_mode's: ROIAlign ('align') or ROIPool ('pool', the
     reference's default, config.py:67), whose backward routes each gradient to the pixel of the maximum recorded by the
     step's forward.  Returns dict(loss, losses=[(cls, loc, nb)], grads={param: fp32 grad} (trunk, heads and, with
-    the context branch, ContextNet's convolutions), skipped, loss_scale).
+    the context branch, ContextNet's convolutions; with freeze_affine=False also every BatchNorm gamma / beta that requires
+    grad), skipped, loss_scale).  When some BatchNorm's affine parameters train, a layer with a channel of gamma == 0 and
+    beta > 0 raises ValueError before anything runs (check_bn_affine: one device-to-host read).
     Parameter update: with lr, `sgd_step` (one global rate); with optimizer (a step_b200.optim.Adam / SGD over the nets'
     parameters, e.g. built from the reference's get_params, and lr None), the gradients, averaged over the ranks, become
     p.grad and optimizer.step() runs -- it skips the update when a gradient is inf or NaN (skipped=True).  scaler (a
@@ -739,6 +793,7 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
             raise ValueError("train_step: scaler needs an optimizer (it is updated from optimizer.found_inf)")
         loss_scale = scaler.scale
     base, roi_net = nets["base_net"], nets["roi_net"]
+    check_bn_affine(nets)
     pool_mode = roi_net.pool_mode
     if pool_mode not in ("align", "pool"):
         raise RuntimeError("train_step: ROINet pool_mode %r is neither 'align' nor 'pool'" % pool_mode)
