@@ -7,13 +7,19 @@ There is no dataset or checkpoint offline, so parity tests and the benchmark use
   * clips ~ clamp(randn, -1, 1)  (the reference's scale_norm=2 input range, augmentations.py:80-82);
   * N grid proposals per clip built like data/data_utils.py:19-45 plus a centre and a full box.
 
-Everything here is host-side numpy/torch-CPU generation; no compute on the hot path.
+The data is host-side numpy/torch-CPU generation; device_nets and make_workload load it into the nets and move them and
+the step's inputs to a device, so that the benchmark tools and the training tests run the same workloads.
 """
 import math
+from collections import namedtuple
 from types import SimpleNamespace
 
 import numpy as np
 import torch
+
+from .networks import BaseNet, ROINet
+from .tube_utils import flatten_tubes
+from .two_branch import ContextNet, TwoBranchNet
 
 # (in_channels, [b0, b1a, b1b, b2a, b2b, b3]) -- i3dpt.py:213-231
 MIXED_PLAN = {
@@ -272,6 +278,81 @@ def make_cls_case(cfg, B, N, W, H, seed=3):
         tg[:, 0, 4] = 1.0
         targets.append(tg.repeat(1, 3, 1))
     return torch.cat(tubes).contiguous(), torch.cat(targets).contiguous()
+
+
+def _on(net, device):
+    net = net.to(device).eval()
+    if hasattr(net, "set_device"):
+        net.set_device(device)
+    return net
+
+
+def device_head(cfg, sd, cls_only=False, device="cuda:0"):
+    """TwoBranchNet(cfg, cls_only) loaded with sd, on device in eval mode."""
+    h = TwoBranchNet(cfg, cls_only=cls_only)
+    h.load_state_dict(sd, strict=True)
+    return _on(h, device)
+
+
+def device_nets(cfg, heads_sd, pool_mode="align", context=False, cls_only=False, device="cuda:0"):
+    """The nets dict of train_step and inference on device in eval mode: the synthetic trunk, ROINet(pool_mode, 7), with
+    context the synthetic ContextNet, and one head det_net<i> per state dict of heads_sd."""
+    nets = {"base_net": BaseNet(cfg), "roi_net": ROINet(pool_mode, 7)}
+    nets["base_net"].load_state_dict(base_net_state_dict(), strict=True)
+    if context:
+        nets["context_net"] = ContextNet(cfg)
+        nets["context_net"].load_state_dict(context_net_state_dict(), strict=True)
+    nets = {k: _on(net, device) for k, net in nets.items()}
+    for i, sd in enumerate(heads_sd):
+        nets["det_net%d" % i] = device_head(cfg, sd, cls_only, device)
+    return nets
+
+
+# The named training workloads: make_cfg keywords, B clips of T_in x HW x HW and N tubes per clip.  The tools time them
+# by name, so that numbers taken by different tools are numbers of the same step.
+#   c4       BASELINE.json config 4 (bench.py's batch) trained: 3 spatial steps of T'=8, no context
+#   shipped  scripts/train_step.sh: T=3, temporal mode (NUM_CHUNKS {1:1, 2:1, 3:3}: steps of 3, 3 and 9 frames),
+#            context on
+#   cls      scripts/train_cls.sh, the classification pre-training stage: one class-only head over T=9 frames,
+#            context on
+Workload = namedtuple("Workload", "cfg B N T_in HW")
+WORKLOADS = {
+    "c4": Workload(dict(T=8, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 1}), B=8, N=11, T_in=32, HW=224),
+    "shipped": Workload(dict(T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False),
+                        B=2, N=34, T_in=36, HW=400),
+    "cls": Workload(dict(T=9, max_iter=1, NUM_CHUNKS={1: 1}, no_context=False), B=4, N=20, T_in=36, HW=400),
+}
+
+
+def make_workload(name, fp16=True, pool_mode="align", B=None, device="cuda:0", **cfg_kw):
+    """One training step of WORKLOADS[name] on device: (cfg, nets, clips, step_tubes, step_targets).  cfg takes the
+    workload's keywords, fp16, pool_mode and cfg_kw (e.g. dropout=0.3, freeze_affine=False); nets are device_nets with
+    ContextNet where the workload has context and heads seeded 100 + i (cls: one class-only head); B defaults to the
+    workload's.  The samples are make_cls_case's (cls), make_train_case's (shipped), or for c4 the grid proposals of
+    every clip with seeded targets, the same rows at every step."""
+    w = WORKLOADS[name]
+    B = w.B if B is None else B
+    cfg = make_cfg(fp16=fp16, pool_mode=pool_mode, image_size=(w.HW, w.HW), **w.cfg, **cfg_kw)
+    cls = name == "cls"
+    heads = [cls_head_state_dict(100, cfg)] if cls else [head_state_dict(100 + i, cfg) for i in range(cfg.max_iter)]
+    nets = device_nets(cfg, heads, pool_mode, context=not cfg.no_context, cls_only=cls, device=device)
+    clips = make_clips(B, w.T_in, w.HW, w.HW).to(device)
+    if cls:
+        tubes, targets = make_cls_case(cfg, B, w.N, w.HW, w.HW)
+        step_tubes, step_targets = [tubes], [targets]
+    elif name == "shipped":
+        step_tubes, step_targets = make_train_case(cfg, B, w.N, w.HW, w.HW)
+    else:
+        R = B * w.N
+        tubes = torch.from_numpy(flatten_tubes(make_proposals(B, w.N, cfg.T, w.HW, w.HW), batch_idx=True)[0])
+        g = torch.Generator().manual_seed(0)
+        tg = torch.zeros(R, 3, 6 + cfg.num_classes)
+        tg[:, :, :4] = tubes[:, 4:5, 1:] + torch.rand(R, 3, 4, generator=g) * 6
+        tg[:, :, 4:6] = (torch.rand(R, 3, 2, generator=g) > 0.3).float()
+        tg[0, :, 4:6] = 1
+        tg[:, :, 6:] = (torch.rand(R, 3, cfg.num_classes, generator=g) > 0.9).float()
+        step_tubes, step_targets = [tubes] * cfg.max_iter, [tg] * cfg.max_iter
+    return cfg, nets, clips, [t.to(device) for t in step_tubes], [t.to(device) for t in step_targets]
 
 
 def make_conv_feat(B, T, H, W, seed=2468):

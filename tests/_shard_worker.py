@@ -15,17 +15,8 @@ from step_b200 import synth  # noqa: E402
 
 
 def build(cfg, dev):
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet(cfg.pool_mode, cfg.pool_size)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict())
-    for i in range(cfg.max_iter):
-        h = step_b200.TwoBranchNet(cfg)
-        h.load_state_dict(synth.head_state_dict(100 + i, cfg))
-        nets["det_net%d" % i] = h
-    for k in nets:
-        nets[k] = nets[k].to(dev).eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device(dev)
-    return nets
+    heads = [synth.head_state_dict(100 + i, cfg) for i in range(cfg.max_iter)]
+    return synth.device_nets(cfg, heads, cfg.pool_mode, device=dev)
 
 
 def run_shard(dev, clips, B, T_in, HW, N, detect):

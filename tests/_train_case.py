@@ -1,10 +1,10 @@
-"""Set-up shared by the train_step tests: the synthetic nets on the device, the seeded two-step spatial case, which
-state-dict entries the oracle trains, and the comparison of train_step's gradients with the oracle's autograd.
-step_b200 is imported inside the functions, so that the CPU-only oracle tests can import this module too."""
+"""Set-up shared by the train_step tests: the seeded two-step spatial case, which state-dict entries the oracle trains,
+and the comparison of train_step's gradients with the oracle's autograd."""
 import torch
 
-# scripts/train_step.sh: T=3, temporal mode (NUM_CHUNKS {1:1, 2:1, 3:3}: steps of 3, 3 and 9 frames), context on
-SHIPPED = dict(T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False)
+from step_b200 import synth
+
+SHIPPED = synth.WORKLOADS["shipped"].cfg
 
 
 def rel_l2(got, ref):
@@ -16,41 +16,9 @@ def trainable(sd):
     return {k: v.clone().requires_grad_(v.is_floating_point() and "running_" not in k and "batch3d" not in k) for k, v in sd.items()}
 
 
-def _to_device(net):
-    net = net.cuda().eval()
-    if hasattr(net, "set_device"):
-        net.set_device("cuda:0")
-    return net
-
-
-def device_head(cfg, sd, cls_only=False):
-    """TwoBranchNet(cfg, cls_only) loaded with sd, on cuda:0 in eval mode."""
-    import step_b200
-    h = step_b200.TwoBranchNet(cfg, cls_only=cls_only)
-    h.load_state_dict(sd, strict=True)
-    return _to_device(h)
-
-
-def device_nets(cfg, heads_sd, pool_mode="align", context=False, cls_only=False):
-    """The nets dict of train_step on cuda:0 in eval mode: the synthetic trunk, ROINet(pool_mode, 7), with context the
-    synthetic ContextNet, and one head det_net<i> per state dict of heads_sd."""
-    import step_b200
-    from step_b200 import synth
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet(pool_mode, 7)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict(), strict=True)
-    if context:
-        nets["context_net"] = step_b200.ContextNet(cfg)
-        nets["context_net"].load_state_dict(synth.context_net_state_dict(), strict=True)
-    nets = {k: _to_device(net) for k, net in nets.items()}
-    for i, sd in enumerate(heads_sd):
-        nets["det_net%d" % i] = device_head(cfg, sd, cls_only)
-    return nets
-
-
 def spatial_case():
     """Two spatial refinement steps (T=2, NUM_CHUNKS {1:1, 2:1}) over 2 clips of 8x64x64 with 3 seeded tubes per clip and
     targets with mixed flags: (cfg, clips, step_tubes, step_targets) on the CPU."""
-    from step_b200 import synth
     B, N = 2, 3
     cfg = synth.make_cfg(fp16=True, T=2, max_iter=2, NUM_CHUNKS={1: 1, 2: 1}, image_size=(64, 64))
     x = synth.make_clips(B, 8, 64, 64, seed=11)

@@ -12,7 +12,8 @@ import torch
 from oracle import augment as oa
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from _train_case import SHIPPED, device_nets  # noqa: E402
+from _train_case import SHIPPED  # noqa: E402
+from step_b200.synth import device_nets  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 

@@ -29,7 +29,8 @@ from step_b200 import synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import _tape_reference as R  # noqa: E402
-from _train_case import SHIPPED, device_nets  # noqa: E402
+from _train_case import SHIPPED  # noqa: E402
+from step_b200.synth import device_head, device_nets  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -54,20 +55,10 @@ def record(fn):
 
 
 def nets(cfg):
-    import step_b200
-    base = step_b200.BaseNet(cfg)
-    base.load_state_dict(synth.base_net_state_dict())
-    ctx = step_b200.ContextNet(cfg)
-    ctx.load_state_dict(synth.context_net_state_dict())
-    head = step_b200.TwoBranchNet(cfg)
-    head.load_state_dict(synth.head_state_dict(100, cfg))
+    n = device_nets(cfg, [synth.head_state_dict(100, cfg)], context=True)
     ccfg = synth.make_cfg(fp16=True, T=cfg.T, no_context=True)
-    cls = step_b200.TwoBranchNet(ccfg, cls_only=True)
-    cls.load_state_dict(synth.cls_head_state_dict(101, ccfg))
-    out = [m.cuda().eval() for m in (base, ctx, head, cls)]
-    for m in out[2:]:
-        m.set_device("cuda:0")
-    return out
+    cls = device_head(ccfg, synth.cls_head_state_dict(101, ccfg), cls_only=True)
+    return n["base_net"], n["context_net"], n["det_net0"], cls
 
 
 def head_tape(net, R_, T_, seed, ctx=True):

@@ -30,7 +30,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import test_oracle_cls  # noqa: E402
 import test_oracle_context  # noqa: E402
-from _train_case import SHIPPED, device_head, device_nets, rel_l2  # noqa: E402
+from _train_case import SHIPPED, rel_l2  # noqa: E402
+from step_b200.synth import device_head, device_nets  # noqa: E402
 from test_bn_affine_cpu import affine_groups, bn_trainable  # noqa: E402
 from test_gpu_train_fp32 import (CHAIN_L2_TOL, L2_TOL, TRAIN_TRUNK_L2_TOL, Recorder, downstream_flags,  # noqa: E402
                                  near_decisions)

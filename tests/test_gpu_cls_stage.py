@@ -79,14 +79,13 @@ def test_train_step_on_device_rows_equals_host_rows():
     head with ContextNet on the device rows and on oracle/select_cls.py's host rows under the same generator states."""
     import step_b200
     from step_b200 import synth, training
-    from _train_case import device_nets
     from test_oracle_cls import CLS_CFG
     targets, props, before, _, _ = selection_inputs("shuffle_cut")
     s = 64.0 / 400.0
     targets = [np.concatenate([t[:, :, :4] * F(s), t[:, :, 4:]], 2) for t in targets]
     props = [p * s for p in props]
     cfg = synth.make_cfg(fp16=True, **CLS_CFG, image_size=(64, 64))
-    nets = device_nets(cfg, [synth.cls_head_state_dict(100, cfg)], context=True, cls_only=True)
+    nets = synth.device_nets(cfg, [synth.cls_head_state_dict(100, cfg)], context=True, cls_only=True)
     x = synth.make_clips(2, 36, 64, 64, seed=11).cuda()
     set_states(before)
     dt, dg = step_b200.select_cls_samples(targets, props, cfg.num_classes)

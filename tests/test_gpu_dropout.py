@@ -29,7 +29,8 @@ import _dropout_oracle as DO  # noqa: E402
 import test_gpu_train_fp32 as F32  # noqa: E402
 import test_oracle_cls  # noqa: E402
 import test_oracle_context  # noqa: E402
-from _train_case import SHIPPED, device_head, device_nets, rel_l2, trainable  # noqa: E402
+from _train_case import SHIPPED, rel_l2, trainable  # noqa: E402
+from step_b200.synth import device_head, device_nets  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 P = 0.3

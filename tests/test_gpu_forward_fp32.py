@@ -172,15 +172,11 @@ CENSUS = {
 
 
 def setup(name):
-    import step_b200
     kw, B, T_in, H, W, n, head = GEOMS[name]
     cfg = synth.make_cfg(fp16=False, **kw)
     if head == "cls":
         nets = build(synth.make_cfg(fp16=False, **dict(kw, max_iter=0)), True)
-        h = step_b200.TwoBranchNet(cfg, cls_only=True)
-        h.load_state_dict(synth.cls_head_state_dict(100, cfg), strict=True)
-        nets["det_net0"] = h.cuda().eval()
-        nets["det_net0"].set_device("cuda:0")
+        nets["det_net0"] = synth.device_head(cfg, synth.cls_head_state_dict(100, cfg), cls_only=True)
     else:
         nets = build(cfg, True)
     x = synth.make_clips(B, T_in, H, W).cuda()

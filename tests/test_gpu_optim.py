@@ -12,7 +12,8 @@ import torch
 from step_b200 import optim, synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from _train_case import SHIPPED, device_nets  # noqa: E402
+from _train_case import SHIPPED  # noqa: E402
+from step_b200.synth import device_head, device_nets  # noqa: E402
 from test_optim_cpu import fixture_groups  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -229,10 +230,7 @@ def test_update_invalidates_the_modules_weight_caches():
         p = grp["params"][0]
         p.grad = torch.randn(p.shape, generator=g).cuda()
     opt.step()
-    fresh_head = step_b200.TwoBranchNet(cfg)
-    fresh_head.load_state_dict(head.state_dict())
-    fresh_head = fresh_head.cuda().eval()
-    fresh_head.set_device("cuda:0")
+    fresh_head = device_head(cfg, head.state_dict())
     fresh_base = step_b200.BaseNet(cfg)
     fresh_base.load_state_dict(base.state_dict())
     fresh_base = fresh_base.cuda().eval()

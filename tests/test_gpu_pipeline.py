@@ -25,22 +25,8 @@ PIPES = {
 
 
 def build(cfg, context=False):
-    import step_b200
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet(cfg.pool_mode, cfg.pool_size)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict(), strict=True)
-    for i in range(cfg.max_iter):
-        h = step_b200.TwoBranchNet(cfg)
-        h.load_state_dict(synth.head_state_dict(100 + i, cfg), strict=True)
-        nets["det_net%d" % i] = h
-    if context:
-        c = step_b200.ContextNet(cfg)
-        c.load_state_dict(synth.context_net_state_dict(), strict=True)
-        nets["context_net"] = c
-    for k in nets:
-        nets[k] = nets[k].cuda().eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device("cuda:0")
-    return nets
+    heads = [synth.head_state_dict(100 + i, cfg) for i in range(cfg.max_iter)]
+    return synth.device_nets(cfg, heads, cfg.pool_mode, context=context)
 
 
 def run(name, g, fp16, context=False, **cfg_kw):

@@ -22,7 +22,8 @@ from oracle import select as osel
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import test_oracle_select as tos  # noqa: E402
-from _train_case import SHIPPED, device_nets  # noqa: E402
+from _train_case import SHIPPED  # noqa: E402
+from step_b200.synth import device_nets  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 

@@ -15,7 +15,8 @@ from oracle import model as om
 from step_b200 import synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from _train_case import compare_grads, device_head, device_nets, spatial_case, trainable  # noqa: E402
+from _train_case import compare_grads, spatial_case, trainable  # noqa: E402
+from step_b200.synth import device_head, device_nets  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 

@@ -16,7 +16,8 @@ from oracle import model as om
 from step_b200 import optim, synth
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from _train_case import SHIPPED, compare_grads, device_head, device_nets, rel_l2, trainable  # noqa: E402
+from _train_case import SHIPPED, compare_grads, rel_l2, trainable  # noqa: E402
+from step_b200.synth import device_head, device_nets  # noqa: E402
 from test_oracle_cls import CLS_CFG, cls_objective, golden_case, transfer_pretrained  # noqa: E402
 
 pytestmark = pytest.mark.gpu

@@ -31,7 +31,8 @@ sys.path.insert(0, HERE)
 import _tape_reference as R  # noqa: E402
 import test_oracle_cls  # noqa: E402
 import test_oracle_context  # noqa: E402
-from _train_case import SHIPPED, device_head, device_nets, rel_l2, trainable  # noqa: E402
+from _train_case import SHIPPED, rel_l2, trainable  # noqa: E402
+from step_b200.synth import device_head, device_nets  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 U32 = 2.0 ** -24
@@ -177,21 +178,11 @@ def test_fp32_backward_siblings_against_float64():
 
 # ---- every tape entry of the fp32 forward in isolation --------------------------------------------------------------------
 def _nets32():
-    import step_b200
     cfg = fp32_cfg(**SHIPPED, image_size=(400, 400))
-    base = step_b200.BaseNet(cfg)
-    base.load_state_dict(synth.base_net_state_dict())
-    ctx = step_b200.ContextNet(cfg)
-    ctx.load_state_dict(synth.context_net_state_dict())
-    head = step_b200.TwoBranchNet(cfg)
-    head.load_state_dict(synth.head_state_dict(100, cfg))
+    n = device_nets(cfg, [synth.head_state_dict(100, cfg)], context=True)
     ccfg = fp32_cfg(T=cfg.T, no_context=True)
-    cls = step_b200.TwoBranchNet(ccfg, cls_only=True)
-    cls.load_state_dict(synth.cls_head_state_dict(101, ccfg))
-    out = [m.cuda().eval() for m in (base, ctx, head, cls)]
-    for m in out[2:]:
-        m.set_device("cuda:0")
-    return out
+    cls = device_head(ccfg, synth.cls_head_state_dict(101, ccfg), cls_only=True)
+    return n["base_net"], n["context_net"], n["det_net0"], cls
 
 
 def _record(fn):

@@ -41,7 +41,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path[:0] = [HERE, ROOT]
 import _tape_reference as R  # noqa: E402
-from _train_case import SHIPPED, device_nets  # noqa: E402
+from _train_case import SHIPPED  # noqa: E402
+from step_b200.synth import device_nets  # noqa: E402
 from step_b200 import synth  # noqa: E402
 
 pytestmark = pytest.mark.gpu

@@ -23,7 +23,8 @@ from step_b200 import synth
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import test_oracle_cls  # noqa: E402
 import test_oracle_context  # noqa: E402
-from _train_case import SHIPPED, compare_grads, device_nets, spatial_case, trainable  # noqa: E402
+from _train_case import SHIPPED, compare_grads, spatial_case, trainable  # noqa: E402
+from step_b200.synth import device_nets  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 

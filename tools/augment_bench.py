@@ -7,8 +7,8 @@
    (step_frames_to_clip_aug_u8, every flag on, one fixed seeded recipe per clip) and the BaseTransform kernel
    (step_frames_to_clip_u8) in alternating rounds of N event-timed launches each; medians over all launches.  Bytes are
    counted from shapes: the source bytes the kernel taps read once (the crop rect's, for the augmenting kernel), the erase
-   noise once, the fp32 clip written once; the floor is those bytes at the data sheet's 3.35 TB/s.  Prints the card's name
-   and power limit with the results.
+   noise once, the fp32 clip written once; the floor is those bytes at the data sheet's 3.35 TB/s.  Prints the card's name,
+   power limit and maximum SM clock with the results.
 2. Host (--host, CPU time of one core, not device time): the host stage's time per 36-frame 360x640 clip, and, where the
    reference checkout exists (oracle/refload.py), the reference's TubeAugmentation on the same clips, tubes and seeds
    with cv2 on one thread.
@@ -25,18 +25,12 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from _bench import card  # noqa: E402
 from step_b200.transforms import BaseTransform, TubeAugmentation, frame_entry, frame_table  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
 B, T, H0, W0, HW = 2, 36, 360, 640, 400
 ALL = dict(do_flip=True, do_crop=True, do_photometric=True, do_erase=True)
-
-
-def card():
-    import subprocess
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable"}
 
 
 def clip_bgr(seed):
@@ -167,7 +161,7 @@ def main():
         lines = host(a.clips)
     else:
         assert torch.cuda.is_available(), "augment_bench needs a GPU (or --host)"
-        lines = [card()] + device(a.rounds, a.launches)
+        lines = [card(0)] + device(a.rounds, a.launches)
     for ln in lines:
         print(json.dumps(ln))
     if a.out:

@@ -8,65 +8,26 @@ steps, ContextNet on) and of `--cls 4 --pool` (the first training stage: 4 clips
 process, after one warm-up step of each, K rounds alternate the two: per round one timed train_step (wall time around a
 device synchronise, no parameter update) and one with training.TIMING on, from which the device time of the `act_bwd`
 phase (step_act_bwd_*, or step_act_bn_bwd_* where gamma / beta train) is read.  Prints one JSON line per configuration
-and precision, with the card's name and power limit.  Correctness is covered by tests/test_gpu_bn_affine.py."""
+and precision, with the card's name, power limit and maximum SM clock.
+Correctness is covered by tests/test_gpu_bn_affine.py."""
 import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
-import step_b200  # noqa: E402
+from _bench import card  # noqa: E402
 from step_b200 import synth, training  # noqa: E402
-
-T_IN, HW = 36, 400
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                       text=True)
-    name, limit = [s.strip() for s in q.stdout.strip().split(",")] if q.returncode == 0 else (torch.cuda.get_device_name(0), "unknown")
-    return name, limit
 
 
 def build(stage, fp16, freeze_affine):
-    cls = stage == "cls"
-    if cls:
-        B, N = 4, 20
-        cfg = synth.make_cfg(fp16=fp16, T=9, max_iter=1, NUM_CHUNKS={1: 1}, no_context=False, image_size=(HW, HW),
-                             freeze_affine=freeze_affine)
-    else:
-        B, N = 2, 34
-        cfg = synth.make_cfg(fp16=fp16, T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False, image_size=(HW, HW),
-                             freeze_affine=freeze_affine)
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet("pool", 7), "context_net": step_b200.ContextNet(cfg)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict())
-    nets["context_net"].load_state_dict(synth.context_net_state_dict())
-    if cls:
-        h = step_b200.TwoBranchNet(cfg, cls_only=True)
-        h.load_state_dict(synth.cls_head_state_dict(100, cfg))
-        nets["det_net0"] = h
-    else:
-        for i in range(3):
-            h = step_b200.TwoBranchNet(cfg)
-            h.load_state_dict(synth.head_state_dict(100 + i, cfg))
-            nets["det_net%d" % i] = h
-    for k in nets:
-        nets[k] = nets[k].cuda().eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device("cuda:0")
-    x = synth.make_clips(B, T_IN, HW, HW).cuda()
-    if cls:
-        ft, fg = synth.make_cls_case(cfg, B, N, HW, HW)
-        st, sg = [ft], [fg]
-    else:
-        st, sg = synth.make_train_case(cfg, B, N, HW, HW)
+    cfg, nets, x, st, sg = synth.make_workload(stage, fp16, "pool", freeze_affine=freeze_affine)
     n_bn = sum(p.requires_grad for n in nets.values() for k, p in n.named_parameters() if "batch3d" in k)
-    return dict(cfg=cfg, nets=nets, x=x, st=[t.cuda() for t in st], sg=[t.cuda() for t in sg], B=B, N=N, n_bn=n_bn)
+    return dict(cfg=cfg, nets=nets, x=x, st=st, sg=sg, n_bn=n_bn)
 
 
 def measure(stage, fp16, rounds):
@@ -93,7 +54,8 @@ def measure(stage, fp16, rounds):
             act[fa].append(step(fa, phases=True)[1])
     med = {fa: statistics.median(times[fa]) for fa in (True, False)}
     amed = {fa: statistics.median(act[fa]) for fa in (True, False)}
-    return {"config": stage, "B": runs[True]["B"], "tubes_per_clip": runs[True]["N"], "precision": "fp16" if fp16 else "fp32",
+    w = synth.WORKLOADS[stage]
+    return {"config": stage, "B": w.B, "tubes_per_clip": w.N, "precision": "fp16" if fp16 else "fp32",
             "pool_mode": "pool", "rounds": rounds, "bn_tensors_trained": runs[False]["n_bn"],
             "grads_frozen_affine": n_grads[True], "grads_trained_affine": n_grads[False],
             "step_ms_frozen_affine": round(med[True], 1), "step_ms_trained_affine": round(med[False], 1),
@@ -111,12 +73,12 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bn_affine_bench: needs a CUDA device")
-    name, limit = card()
+    gpu = card(0)
     lines = []
     for stage in ("shipped", "cls"):
         for fp16 in (True, False):
             rec = measure(stage, fp16, a.rounds)
-            rec.update(gpu=name, power_limit=limit, torch=torch.__version__)
+            rec.update(gpu, torch=torch.__version__)
             print(json.dumps(rec), flush=True)
             lines.append(json.dumps(rec))
             torch.cuda.empty_cache()

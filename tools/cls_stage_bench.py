@@ -12,7 +12,8 @@
    events), then FrameAP.evaluate() (host wall time, it ends in a read-back).  Against the host restatement of
    train_cls.py:505-554 on the first H frames: the scores and boxes copied to the host, the CSV text of :537-543 and
    oracle/evaluation.py's numpy restatement of ava_evaluation on that text (the reference's evaluator has the same loops).
-Prints the card's name and power limit with the results.  Correctness is covered by tests/test_gpu_cls_stage.py."""
+Prints the card's name, power limit and maximum SM clock with the results.
+Correctness is covered by tests/test_gpu_cls_stage.py."""
 import argparse
 import io
 import json
@@ -28,6 +29,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from _bench import card  # noqa: E402
 import step_b200  # noqa: E402
 from make_cls_stage_golden import away, cls_detection_lines, make_clip  # noqa: E402
 from oracle import evaluation as oev  # noqa: E402
@@ -35,13 +37,6 @@ from oracle import select_cls as osel  # noqa: E402
 from step_b200.postprocess import ClsDetector  # noqa: E402
 
 C, T, W, BATCH = 60, 9, 400, 8
-
-
-def card():
-    import subprocess
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable"}
 
 
 def med(v, nd=4):
@@ -178,7 +173,7 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     assert torch.cuda.is_available(), "cls_stage_bench needs a GPU"
-    lines = [card(), selection(a.reps), validation(a.frames, a.host_frames)]
+    lines = [card(0), selection(a.reps), validation(a.frames, a.host_frames)]
     for ln in lines:
         print(json.dumps(ln))
     if a.out:

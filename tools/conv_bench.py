@@ -11,6 +11,7 @@ the instantiated tiles from its STEP_CONV_TILES list.  A tool, not the benchmark
 
 --ksweep times a 1x1x1 conv at the head shape (M = 34,496, Cout = 256: BK 64 / BN 256, 270 tiles) for Cin = 256 ... 2048
 and fits the time of one wave of tiles against K: the intercept is the part of a tile's time outside the K loop."""
+import json
 import os
 import re
 import sys
@@ -18,6 +19,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch  # noqa: E402
+from _bench import card  # noqa: E402
 from step_b200 import _lib as L, engine as E  # noqa: E402
 from step_b200.engine import Act  # noqa: E402
 
@@ -137,6 +139,7 @@ def ksweep():
 
 
 def main():
+    print(json.dumps(card(0)), flush=True)
     if "--ksweep" in sys.argv:
         ksweep()
         return

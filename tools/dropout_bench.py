@@ -7,50 +7,27 @@ ContextNet on) for three configurations -- fp32 with ROIAlign, fp32 with ROIPool
 .train() (nn.Dropout(0.3)) and times train_step(..., dropout=True) against dropout=False, alternated in one process, K
 rounds each after one warm-up of each (wall time around a device synchronise).  One more dropout=True step runs under
 torch.profiler, and the device time of the dropout kernels (the draws' forward copies and context means, and the masked
-backward siblings) is summed from its trace.  Prints one JSON line per configuration, with the card's name and power limit.
-Correctness is covered by tests/test_gpu_dropout.py."""
+backward siblings) is summed from its trace.  Prints one JSON line per configuration, with the card's name, power
+limit and maximum SM clock.  Correctness is covered by tests/test_gpu_dropout.py."""
 import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
-import step_b200  # noqa: E402
+from _bench import card  # noqa: E402
 from step_b200 import synth, training  # noqa: E402
-
-B, N, T_IN, HW = 2, 34, 36, 400
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                       text=True)
-    name, limit = [s.strip() for s in q.stdout.strip().split(",")] if q.returncode == 0 else (torch.cuda.get_device_name(0), "unknown")
-    return name, limit
 
 
 def build(fp16, pool_mode):
-    cfg = synth.make_cfg(fp16=fp16, T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False, image_size=(HW, HW), dropout=0.3)
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet(pool_mode, 7), "context_net": step_b200.ContextNet(cfg)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict())
-    nets["context_net"].load_state_dict(synth.context_net_state_dict())
-    for i in range(3):
-        h = step_b200.TwoBranchNet(cfg)
-        h.load_state_dict(synth.head_state_dict(100 + i, cfg))
-        nets["det_net%d" % i] = h
-    for k in nets:
-        nets[k] = nets[k].cuda().eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device("cuda:0")
-    for i in range(3):
+    cfg, nets, x, st, sg = synth.make_workload("shipped", fp16, pool_mode, dropout=0.3)
+    for i in range(cfg.max_iter):
         nets["det_net%d" % i].train()
-    x = synth.make_clips(B, T_IN, HW, HW).cuda()
-    st, sg = synth.make_train_case(cfg, B, N, HW, HW)
-    return cfg, nets, x, [t.cuda() for t in st], [t.cuda() for t in sg]
+    return cfg, nets, x, st, sg
 
 
 def is_dropout_kernel(name):
@@ -82,7 +59,8 @@ def measure(fp16, pool_mode, rounds):
         if is_dropout_kernel(e.key):
             kern[e.key.split("(")[0]] = round(e.device_time_total / 1e3, 3)
     on, off = statistics.median(times[True]), statistics.median(times[False])
-    return {"config": "shipped", "B": B, "tubes_per_clip": N, "precision": "fp16" if fp16 else "fp32", "pool_mode": pool_mode,
+    w = synth.WORKLOADS["shipped"]
+    return {"config": "shipped", "B": w.B, "tubes_per_clip": w.N, "precision": "fp16" if fp16 else "fp32", "pool_mode": pool_mode,
             "rounds": rounds, "step_ms_dropout": round(on, 1), "step_ms_no_dropout": round(off, 1),
             "step_ms_dropout_all": [round(t, 1) for t in times[True]], "step_ms_no_dropout_all": [round(t, 1) for t in times[False]],
             "dropout_kernels_device_ms": round(sum(kern.values()), 3), "dropout_kernels": kern}
@@ -93,11 +71,11 @@ def main():
     ap.add_argument("--rounds", type=int, default=4)
     ap.add_argument("--out")
     a = ap.parse_args()
-    name, limit = card()
+    gpu = card(0)
     lines = []
     for fp16, pool_mode in ((False, "align"), (False, "pool"), (True, "align")):
         rec = measure(fp16, pool_mode, a.rounds)
-        rec.update(gpu=name, power_limit=limit, torch=torch.__version__)
+        rec.update(gpu, torch=torch.__version__)
         print(json.dumps(rec), flush=True)
         lines.append(json.dumps(rec))
     if a.out:

@@ -11,7 +11,8 @@ Rows are drawn on the device in the layout of step_detect_f32's output (det [8, 
 3. Peak device memory of the run (torch.cuda.max_memory_allocated).
 4. oracle/evaluation.py on the first M = 2,000 frames: single-threaded host wall time of one call, the CSV text parsing
    included (a stand-in for the reference's run_evaluation, which has the same loops).
-Prints the card's name and power limit with the results.  Correctness is covered by tests/test_gpu_eval.py."""
+Prints the card's name, power limit and maximum SM clock with the results.
+Correctness is covered by tests/test_gpu_eval.py."""
 import argparse
 import json
 import os
@@ -24,19 +25,13 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from _bench import card  # noqa: E402
 import step_b200  # noqa: E402
 from oracle import evaluation as oev  # noqa: E402
 
 # the AVA v2.1 label map's ids (ava_action_list_v2.1_for_activitynet_2018), names replaced by their ids
 AVA_IDS = [1, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 17, 20, 22, 24, 26, 27, 28, 29, 30, 34, 36, 37, 38, 41, 43, 45,
            46, 47, 48, 49, 51, 52, 54, 56, 57, 58, 59, 60, 61, 62, 63, 64, 65, 66, 67, 68, 69, 70, 72, 73, 74, 76, 77, 78, 79, 80]
-
-
-def card():
-    import subprocess
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable"}
 
 
 def make_batch(g, B, R, C, gt_boxes):
@@ -125,7 +120,7 @@ def main():
     om = oev.run(cats, gt_lines, det_lines)
     om.per_class_ap()
     oracle_s = time.perf_counter() - t0
-    lines = [card(),
+    lines = [card(0),
              {"what": "add_detections", "frames": a.frames, "rows_per_frame": R, "clips_per_batch": B,
               "batches": len(add_ms), "device_ms_median": round(statistics.median(add_ms), 4),
               "device_ms_p10_p90": [round(float(np.percentile(add_ms, 10)), 4), round(float(np.percentile(add_ms, 90)), 4)]},

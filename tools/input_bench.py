@@ -10,12 +10,12 @@ changes for the captured step.
 2. StepRunner at C4 (graph on, bench.py's detection post-processing) fed pinned uint8 360x640 frames (transform=...) against
    the same runner fed pinned fp32 224x224 clips, in alternating runs of S steps each (each run ends in a synchronise);
    clips/s per run, medians reported, and the host-to-device bytes per batch of both.
-Prints the card's name and power limit with the results.  Correctness is covered by tests/test_gpu_transform.py."""
+Prints the card's name, power limit and maximum SM clock with the results.
+Correctness is covered by tests/test_gpu_transform.py."""
 import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
@@ -23,6 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
+from _bench import card  # noqa: E402
 import bench  # noqa: E402
 import step_b200  # noqa: E402
 from step_b200 import synth  # noqa: E402
@@ -30,12 +31,6 @@ from step_b200.transforms import BaseTransform, frame_entry, frame_table  # noqa
 
 HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
 SHAPES = {"c4": dict(B=8, T=32, H0=360, W0=640, HW=224), "shipped": dict(B=2, T=36, H0=360, W0=640, HW=400)}
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable"}
 
 
 def frames(B, T, H0, W0, seed=0):
@@ -106,7 +101,7 @@ def main():
     assert torch.cuda.is_available(), "input_bench needs a GPU"
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    lines = [card()]
+    lines = [card(0)]
     lines += [kernel_time(k, s, a.launches, dev) for k, s in SHAPES.items()]
     lines.append(runner_rates(a.rounds, a.steps, dev))
     for ln in lines:

@@ -9,6 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 import step_b200
+from _bench import card
 from step_b200 import _lib as L, engine as E, synth
 from step_b200.engine import Act
 from step_b200.roi_layers import nms
@@ -34,7 +35,7 @@ def timeit(fn, reps=20, warm=5, flush_l2=False):
     return tot / reps
 
 
-out = {"peaks": {"hbm_gbs": PEAKS["hbm_gbs"], "bf16_tflops_burst": PEAKS["bf16_tflops"], "bf16_tflops_sustained": PEAKS["bf16_tflops_sustained"]}}
+out = {"card": card(0), "peaks": {"hbm_gbs": PEAKS["hbm_gbs"], "bf16_tflops_burst": PEAKS["bf16_tflops"], "bf16_tflops_sustained": PEAKS["bf16_tflops_sustained"]}}
 
 # ---- C2: trunk only ---------------------------------------------------------------------------
 cfg = synth.make_cfg(fp16=True)

@@ -11,7 +11,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
@@ -20,38 +19,13 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-import step_b200  # noqa: E402
+from _bench import card  # noqa: E402
 from step_b200 import _lib as L, optim, synth, training  # noqa: E402
 
 GROUPS = os.path.join(ROOT, "tests", "golden", "shipped_param_groups.npz")
 HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
 UPDATE_BYTES_PER_PARAM = 28        # Adam reads p, g, m, v and writes p, m, v (fp32)
 CHECK_BYTES_PER_PARAM = 4          # the check reads g
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable"}
-
-
-def shipped_cfg(hw):
-    return synth.make_cfg(fp16=True, T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False, image_size=(hw, hw))
-
-
-def shipped_nets(cfg):
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet("align", 7), "context_net": step_b200.ContextNet(cfg)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict())
-    nets["context_net"].load_state_dict(synth.context_net_state_dict())
-    for i in range(3):
-        h = step_b200.TwoBranchNet(cfg)
-        h.load_state_dict(synth.head_state_dict(100 + i, cfg))
-        nets["det_net%d" % i] = h
-    for k in nets:
-        nets[k] = nets[k].cuda().eval()
-        if hasattr(nets[k], "set_device"):
-            nets[k].set_device("cuda:0")
-    return nets
 
 
 def groups_of(nets):
@@ -63,7 +37,7 @@ def groups_of(nets):
 
 
 def bench_update(iters):
-    nets = shipped_nets(shipped_cfg(64))
+    nets = synth.make_workload("shipped")[1]
     ref_groups = groups_of(nets)
     n_params = sum(g["params"][0].numel() for g in ref_groups)
     gen = torch.Generator(device="cuda").manual_seed(0)
@@ -122,11 +96,7 @@ def bench_update(iters):
 
 
 def bench_train_step(reps=3):
-    cfg = shipped_cfg(400)
-    B, N = 2, 34
-    st, sg = synth.make_train_case(cfg, B, N, 400, 400)
-    batch = (synth.make_clips(B, 36, 400, 400).cuda(), [t.cuda() for t in st], [t.cuda() for t in sg])
-    nets = shipped_nets(cfg)
+    cfg, nets, *batch = synth.make_workload("shipped")
     opt = optim.Adam(groups_of(nets))
     times = {"optimizer_adam": [], "lr_none": []}
     for it in range(1 + reps):
@@ -137,8 +107,9 @@ def bench_train_step(reps=3):
             torch.cuda.synchronize()
             if it > 0:
                 times[name].append((time.perf_counter() - t0) * 1e3)
+    w = synth.WORKLOADS["shipped"]
     return {"train_step_ms": {k: [round(v, 1) for v in vs] for k, vs in times.items()},
-            "B": B, "tubes_per_clip": N, "clip": "36x400x400"}
+            "B": w.B, "tubes_per_clip": w.N, "clip": "%dx%dx%d" % (w.T_in, w.HW, w.HW)}
 
 
 if __name__ == "__main__":
@@ -146,7 +117,7 @@ if __name__ == "__main__":
     ap.add_argument("--iters", type=int, default=100)
     ap.add_argument("--train-step", action="store_true")
     a = ap.parse_args()
-    print(json.dumps(card()), flush=True)
+    print(json.dumps(card(0)), flush=True)
     print(json.dumps(bench_update(a.iters)), flush=True)
     if a.train_step:
         print(json.dumps(bench_train_step()), flush=True)

@@ -1,9 +1,10 @@
 """3x3x3 stride-1 max pools of the step (branch_3 of every Mixed block, i3dpt.py:149-152) one by one: us and DRAM GB/s on
 the compulsory bytes (input once + output once).  Inputs rotate over enough buffers to exceed the 50 MB L2; the result is
 compared bit for bit with torch's max_pool3d on the zero-padded input."""
-import os, sys
+import json, os, sys
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from _bench import card
 from step_b200 import engine as E
 from step_b200.engine import Act
 
@@ -25,7 +26,7 @@ def timed(fn, reps=20):
     return e0.elapsed_time(e1) * 1e3 / reps
 
 
-print(torch.cuda.get_device_name(), flush=True)
+print(json.dumps(card(0)), flush=True)
 for name, N, T, H, W, C in SHAPES:
     nbytes = N * T * H * W * C * 2
     nbuf = max(2, int(400e6 // (2 * nbytes)) + 1)

@@ -11,7 +11,8 @@ softmax sampling), on one GPU:
 3. The shipped ROIPool training iteration at B=2 (inference pre-pass + selection + train_step without an update), with
    the host selection (history copied to the host, oracle/select.py, upload) and with the device selection, run
    alternately K times each; medians of the wall time per iteration.
-Prints the card's name and power limit with the results.  Correctness is covered by tests/test_gpu_select.py."""
+Prints the card's name, power limit and maximum SM clock with the results.
+Correctness is covered by tests/test_gpu_select.py."""
 import argparse
 import json
 import os
@@ -26,25 +27,11 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import step_b200  # noqa: E402
+from _bench import card  # noqa: E402
 from oracle import select as osel  # noqa: E402
 from step_b200 import synth, training  # noqa: E402
 
-W = 400
-
-
-def card():
-    import subprocess
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else "unavailable"}
-
-
-def shipped_cfg():
-    cfg = synth.make_cfg(fp16=True, T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False, image_size=(W, W),
-                         pool_mode="pool")
-    cfg.__dict__.update(cls_thresh=[0.2, 0.35, 0.5], reg_thresh=[0.2, 0.35, 0.5], topk=300, max_pos_num=5,
-                        selection_sampling="softmax", neg_ratio=2)
-    return cfg
+W = synth.WORKLOADS["shipped"].HW
 
 
 def inputs(cfg, B, n=34, G=3, seed=4):
@@ -62,21 +49,6 @@ def inputs(cfg, B, n=34, G=3, seed=4):
         src[:, 2:] = np.maximum(src[:, 2:], src[:, :2] + 8)
         tubes.append(np.tile(src[:, None], (1, cfg.T, 1)))
     return targets, tubes
-
-
-def nets_for(cfg):
-    nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet("pool", 7), "context_net": step_b200.ContextNet(cfg)}
-    nets["base_net"].load_state_dict(synth.base_net_state_dict(), strict=True)
-    nets["context_net"].load_state_dict(synth.context_net_state_dict(), strict=True)
-    for i in range(cfg.max_iter):
-        h = step_b200.TwoBranchNet(cfg)
-        h.load_state_dict(synth.head_state_dict(100 + i, cfg), strict=True)
-        nets["det_net%d" % i] = h
-    for k, net in nets.items():
-        nets[k] = net.cuda().eval()
-        if hasattr(net, "set_device"):
-            net.set_device("cuda:0")
-    return nets
 
 
 def prepass(cfg, nets, x, tubes):
@@ -156,9 +128,10 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     assert torch.cuda.is_available(), "select_bench needs a GPU"
-    cfg = shipped_cfg()
-    nets = nets_for(cfg)
-    lines = [card()] + [selection(cfg, nets, B, a.reps) for B in (2, 8)] + [iteration(cfg, nets, a.iters)]
+    cfg, nets = synth.make_workload("shipped", pool_mode="pool")[:2]
+    cfg.__dict__.update(cls_thresh=[0.2, 0.35, 0.5], reg_thresh=[0.2, 0.35, 0.5], topk=300, max_pos_num=5,
+                        selection_sampling="softmax", neg_ratio=2)
+    lines = [card(0)] + [selection(cfg, nets, B, a.reps) for B in (2, 8)] + [iteration(cfg, nets, a.iters)]
     for ln in lines:
         print(json.dumps(ln))
     if a.out:

@@ -19,56 +19,16 @@ reports where the (not yet optimised) step stands."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
-import step_b200
+from _bench import card
 from step_b200 import optim, synth, training
-shipped = "--shipped" in sys.argv
-cls = "--cls" in sys.argv
+config = "cls" if "--cls" in sys.argv else "shipped" if "--shipped" in sys.argv else "c4"
+cls = config == "cls"
 pool_mode = "pool" if "--pool" in sys.argv else "align"
 fp16 = "--fp32" not in sys.argv
 pos = [a for a in sys.argv[1:] if not a.startswith("--")]
-if cls:
-    B = int(pos[0]) if pos else 4
-    N, T_in, HW = 20, 36, 400
-    cfg = synth.make_cfg(fp16=fp16, T=9, max_iter=1, NUM_CHUNKS={1: 1}, no_context=False, image_size=(HW, HW))
-elif shipped:
-    B = int(pos[0]) if pos else 2
-    N, T_in, HW = 34, 36, 400
-    cfg = synth.make_cfg(fp16=fp16, T=3, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 3}, no_context=False, image_size=(HW, HW))
-else:
-    B = int(pos[0]) if pos else 8
-    N, T_in, HW = 11, 32, 224
-    cfg = synth.make_cfg(fp16=fp16, T=8, max_iter=3, NUM_CHUNKS={1: 1, 2: 1, 3: 1}, image_size=(HW, HW))
-nets = {"base_net": step_b200.BaseNet(cfg), "roi_net": step_b200.ROINet(pool_mode, 7)}
-nets["base_net"].load_state_dict(synth.base_net_state_dict())
-if shipped or cls:
-    nets["context_net"] = step_b200.ContextNet(cfg)
-    nets["context_net"].load_state_dict(synth.context_net_state_dict())
-if cls:
-    h = step_b200.TwoBranchNet(cfg, cls_only=True); h.load_state_dict(synth.cls_head_state_dict(100, cfg)); nets["det_net0"] = h
-else:
-    for i in range(3):
-        h = step_b200.TwoBranchNet(cfg); h.load_state_dict(synth.head_state_dict(100 + i, cfg)); nets["det_net%d" % i] = h
-for k in nets:
-    nets[k] = nets[k].cuda().eval()
-    if hasattr(nets[k], "set_device"):
-        nets[k].set_device("cuda:0")
-x = synth.make_clips(B, T_in, HW, HW).cuda()
-if cls:
-    ft, fg = synth.make_cls_case(cfg, B, N, HW, HW)
-    step_tubes, step_targets = [ft.cuda()], [fg.cuda()]
-elif shipped:
-    st, sg = synth.make_train_case(cfg, B, N, HW, HW)
-    step_tubes, step_targets = [t.cuda() for t in st], [t.cuda() for t in sg]
-else:
-    props = synth.make_proposals(B, N, cfg.T, 224, 224)
-    flat, _ = step_b200.tube_utils.flatten_tubes(props, batch_idx=True)
-    tubes = torch.from_numpy(flat).cuda()
-    gen = torch.Generator().manual_seed(0)
-    tg = torch.zeros(B * N, 3, 66)
-    tg[:, :, :4] = tubes[:, 4:5, 1:].cpu() + torch.rand(B * N, 3, 4, generator=gen) * 6
-    tg[:, :, 4:6] = (torch.rand(B * N, 3, 2, generator=gen) > 0.3).float(); tg[0, :, 4:6] = 1
-    tg[:, :, 6:] = (torch.rand(B * N, 3, 60, generator=gen) > 0.9).float()
-    step_tubes, step_targets = [tubes] * 3, [tg.cuda()] * 3
+cfg, nets, x, step_tubes, step_targets = synth.make_workload(config, fp16, pool_mode, B=int(pos[0]) if pos else None)
+B = x.shape[0]
+print(json.dumps(card(0)), flush=True)
 # --cls: the step with train_cls.py's optimizer, Adam with dynamic loss scaling (one rate for all tensors: it does not change
 # the time of the single multi-tensor launch)
 opt = optim.Adam([p for n in nets.values() for p in n.parameters() if p.requires_grad], lr=5e-8) if cls else None
@@ -88,7 +48,7 @@ for it in range(4):
             if pn > 0 and gn > 0:
                 training.sgd_step({p: g}, lr=3e-4 * pn / gn, momentum=0.0)
     torch.cuda.synchronize(); dt = time.perf_counter() - t0
-    print(json.dumps({"iter": it, "config": "cls" if cls else "shipped" if shipped else "c4", "pool_mode": pool_mode, "precision": "fp16" if fp16 else "fp32", "B": B, "train_step_ms": round(dt * 1e3, 1), "loss": round(float(r["loss"]), 5),
+    print(json.dumps({"iter": it, "config": config, "pool_mode": pool_mode, "precision": "fp16" if fp16 else "fp32", "B": B, "train_step_ms": round(dt * 1e3, 1), "loss": round(float(r["loss"]), 5),
                       "clips_per_s": round(B / dt, 1), "peak_mem_gb": round(torch.cuda.max_memory_allocated() / 2**30, 2)}), flush=True)
 phases = training.timing_summary()
 wgrad = round(sum(v for k, v in phases.items() if k.startswith("wgrad_")), 2)
