@@ -436,6 +436,43 @@ int step_act_bn_bwd_f32(const float* dy, int dy_ld, const float* y, int y_ld, co
                         float* dz, int dz_ld, float* dres, int dres_ld, const float* beta, const float* gamma, float gscale,
                         float* dgamma, float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream);
 
+/* BatchNorm with batch statistics (freeze_stats=False: BatchNorm3d in training mode, models/networks.py:85-99).  The
+ * convolution writes z with the identity epilogue (no scale, shift or ReLU); these entries normalise it.  z, y, dy, dz are
+ * channel slices of fp16 (_f16) or fp32 (_f32) buffers: C, every split and every ld a multiple of the 16-byte vector (8 fp16,
+ * 4 fp32) and the pointers 16-byte aligned.  Statistics, parameters and sums are fp32.  Each reduction forms per-chunk
+ * partials in the workspace that a second kernel combines in a fixed order: no atomics, bit-identical from run to run.
+ *
+ * step_bn_stats: per channel of z [M, C], mean and biased variance var (per-chunk Welford, chunks merged by Chan's formula) ->
+ *   mean, rstd = 1 / sqrt(var + eps), scale = gamma * rstd, shift = beta - mean * scale.  With running_mean and running_var
+ *   (both or neither): running = (1 - momentum) * running + momentum * batch, the unbiased variance M / (M - 1) * var for
+ *   running_var (torch.nn.functional.batch_norm, training=True).  M < 2 is STEP_E_ARG, as torch refuses it. */
+size_t step_bn_stats_workspace_bytes(long long M, int C);
+int step_bn_stats_f16(const void* z, int z_ld, long long M, int C, const float* gamma, const float* beta, float eps, float momentum,
+                      float* running_mean, float* running_var, float* mean, float* rstd, float* scale, float* shift,
+                      void* workspace, size_t ws_bytes, step_stream_t stream);
+int step_bn_stats_f32(const float* z, int z_ld, long long M, int C, const float* gamma, const float* beta, float eps, float momentum,
+                      float* running_mean, float* running_var, float* mean, float* rstd, float* scale, float* shift,
+                      void* workspace, size_t ws_bytes, step_stream_t stream);
+/* y = relu(scale * z + shift) (relu = 0: no ReLU) for z [M, C]: columns [0, split1) go to y, [split1, split2) to y1 and
+ * [split2, C) to y2, each range from its destination's column 0 (the three outputs of Mixed's fused 1x1 branches).  One
+ * destination: split1 = split2 = C, y1 = y2 = NULL. */
+int step_bn_apply_f16(const void* z, int z_ld, long long M, int C, const float* scale, const float* shift, int relu, void* y,
+                      int y_ld, int split1, void* y1, int y1_ld, int split2, void* y2, int y2_ld, step_stream_t stream);
+int step_bn_apply_f32(const float* z, int z_ld, long long M, int C, const float* scale, const float* shift, int relu, float* y,
+                      int y_ld, int split1, float* y1, int y1_ld, int split2, float* y2, int y2_ld, step_stream_t stream);
+/* Backward of y = relu(BN_train(z)) with g = dy * [y > 0] (g = dy without relu; y may then be NULL) and
+ * xhat = (z - mean) * rstd, from step_bn_stats' mean and rstd:
+ *   dz = gamma * rstd * (g - sum(g) / M - xhat * sum(g xhat) / M)     (in the storage type, at dz_ld; keeps dy's loss scale)
+ *   dbeta = gscale * sum g,  dgamma = gscale * sum g xhat              (either may be NULL)
+ * gscale: 1 / loss_scale.  Three launches: per-chunk partials, their sums in chunk order, the dz pass. */
+size_t step_bn_bwd_workspace_bytes(long long M, int C);
+int step_bn_bwd_f16(const void* dy, int dy_ld, const void* y, int y_ld, const void* z, int z_ld, long long M, int C,
+                    const float* mean, const float* rstd, const float* gamma, int relu, float gscale, void* dz, int dz_ld,
+                    float* dgamma, float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream);
+int step_bn_bwd_f32(const float* dy, int dy_ld, const float* y, int y_ld, const float* z, int z_ld, long long M, int C,
+                    const float* mean, const float* rstd, const float* gamma, int relu, float gscale, float* dz, int dz_ld,
+                    float* dgamma, float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream);
+
 /* ------------------------------------------------------------------ the heads' dropout ---- */
 /* One draw of torch.nn.functional.dropout(x, p, training=True) on a CUDA fp32 tensor of n elements (n % 4 == 0, n < 2^31,
  * 16-byte aligned and contiguous, as every dropout input of the heads is): seed and offset are the device generator's

@@ -211,12 +211,92 @@ def params_key(*tensors):
     return tuple((t.data_ptr(), t._version, t.device, t.dtype) for t in tensors if t is not None)
 
 
+# Whether a batch-statistics forward updates the BatchNorms' running statistics.  training.train_step turns it off to repeat
+# a forward whose statistics the caller's own training-mode forward has already counted (train.py:266-269).
+UPDATE_RUNNING_STATS = True
+
+
+@contextlib.contextmanager
+def running_stats_update(on):
+    global UPDATE_RUNNING_STATS
+    saved = UPDATE_RUNNING_STATS
+    UPDATE_RUNNING_STATS = bool(on)
+    try:
+        yield
+    finally:
+        UPDATE_RUNNING_STATS = saved
+
+
+def check_batch_stats_bn(bn):
+    """The BatchNorm settings the batch-statistics kernels implement: an exponential running average (momentum) that is
+    tracked, as the reference's BatchNorm3d defaults are."""
+    if bn.momentum is None or not bn.track_running_stats:
+        raise ValueError("BatchNorm with batch statistics needs track_running_stats=True and a momentum (got momentum=%r, "
+                         "track_running_stats=%r): the cumulative average and untracked statistics are not implemented"
+                         % (bn.momentum, bn.track_running_stats))
+
+
+def _conv_batch_stats(x, w_packed, shift, outs, bns, k, stride, pad_lo, relu, a_mode, out_dims, zero_cin_last_kt, tag):
+    """conv() for Unit3Dpy outputs whose BatchNorms normalise with batch statistics (bns: one BatchNorm3d per output of outs):
+    the convolution writes z [M, sum C] with the identity epilogue (+ the conv bias `shift`), step_bn_stats forms each
+    BatchNorm's statistics over z's column range (and, when UPDATE_RUNNING_STATS, updates its running statistics once), and
+    one step_bn_apply writes y = relu(scale z + shift) to every output.  The tape entry also keeps z, mean, rstd and bns."""
+    code, dev = x.code, x.device
+    o0 = outs[0]
+    n_total = sum(o.C for o in outs)
+    z = Act.empty(o0.N, o0.T, o0.H, o0.W, n_total, code, dev)
+    with recording(None):
+        conv(x, w_packed, None, shift, z, k, stride, pad_lo, relu=False, a_mode=a_mode, out_dims=out_dims,
+             zero_cin_last_kt=zero_cin_last_kt)
+    M = o0.N * o0.T * o0.H * o0.W
+    stats = torch.empty((4, n_total), dtype=torch.float32, device=dev)          # mean, rstd, scale, shift
+    nbytes = L.lib().step_bn_stats_workspace_bytes(M, max(o.C for o in outs))
+    ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
+    bn_stats = L.lib().step_bn_stats_f16 if code == L.F16 else L.lib().step_bn_stats_f32
+    esz = z.buf.element_size()
+    col = 0
+    for o, bn in zip(outs, bns):
+        check_batch_stats_bn(bn)
+        upd = UPDATE_RUNNING_STATS
+        at = lambda r, col=col: L.c_void_p(stats[r].data_ptr() + 4 * col)
+        L.check(bn_stats(L.c_void_p(z.buf.data_ptr() + esz * col), n_total, M, o.C, L.ptr(bn.weight.detach()),
+                         L.ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum), L.ptr(bn.running_mean) if upd else None,
+                         L.ptr(bn.running_var) if upd else None, at(0), at(1), at(2), at(3), L.ptr(ws), nbytes, L.stream()))
+        if upd:
+            # written in place by the kernel: the version bump re-keys the folded weights of a later eval-mode forward
+            torch.autograd.graph.increment_version(bn.running_mean)
+            torch.autograd.graph.increment_version(bn.running_var)
+            bn.num_batches_tracked.add_(1)
+        col += o.C
+    ys = list(outs) + [None] * (3 - len(outs))
+    splits = [o0.C, o0.C + (outs[1].C if len(outs) > 1 else 0)]
+    bn_apply = L.lib().step_bn_apply_f16 if code == L.F16 else L.lib().step_bn_apply_f32
+    L.check(bn_apply(L.c_void_p(z.buf.data_ptr()), n_total, M, n_total, L.ptr(stats[2]), L.ptr(stats[3]), 1 if relu else 0,
+                     L.c_void_p(o0.data_ptr()), o0.ld, splits[0],
+                     L.c_void_p(ys[1].data_ptr()) if ys[1] is not None else None, ys[1].ld if ys[1] is not None else 0, splits[1],
+                     L.c_void_p(ys[2].data_ptr()) if ys[2] is not None else None, ys[2].ld if ys[2] is not None else 0, L.stream()))
+    if TAPE is not None:
+        TAPE.append(dict(kind="conv", x=x, w=w_packed, scale=None, out=o0, extra_outs=list(outs[1:]), k=tuple(k),
+                         stride=tuple(stride), pad_lo=tuple(pad_lo), relu=bool(relu), residual=None, tag=tag, z=z,
+                         mean=stats[0], rstd=stats[1], bn=list(bns)))
+    return o0
+
+
 def conv(x, w_packed, scale, shift, out, k, stride=(1, 1, 1), pad_lo=None, relu=True, residual=None,
-         a_mode=None, out_dims=None, extra_outs=None, zero_cin_last_kt=0, tag=None):
+         a_mode=None, out_dims=None, extra_outs=None, zero_cin_last_kt=0, tag=None, bn=None):
     """Launch step_conv3d_fwd: x (Act) * w_packed [Cout, taps, w_ld] -> out (Act slice).
     extra_outs: up to two more Act slices; output channels are then split [out.C | extra[0].C | extra[1].C]
-    (horizontally fused 1x1x1 layers sharing the input)."""
+    (horizontally fused 1x1x1 layers sharing the input).
+    bn: None, or one BatchNorm3d per output that normalises with batch statistics (freeze_stats=False in training mode):
+    scale must then be None, shift is the conv bias (or None), and there is no residual (_conv_batch_stats)."""
     code = x.code
+    if bn is not None:
+        if scale is not None or residual is not None or len(bn) != 1 + len(extra_outs or []):
+            raise RuntimeError("conv: batch statistics take one BatchNorm per output, no folded scale and no residual")
+        if pad_lo is None:
+            pad_lo = tuple(same_pad(k[i], stride[i])[0] for i in range(3))
+        return _conv_batch_stats(x, w_packed, shift, [out] + list(extra_outs or []), bn, k, stride, pad_lo, relu, a_mode,
+                                 out_dims, zero_cin_last_kt, tag)
     if pad_lo is None:
         pad_lo = tuple(same_pad(k[i], stride[i])[0] for i in range(3))
     if out_dims is None:

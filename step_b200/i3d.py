@@ -20,7 +20,12 @@ def get_padding_shape(filter_shape, stride):
 
 
 class Unit3Dpy(torch.nn.Module):
-    """i3dpt.py:43-111: [zero pad] -> Conv3d -> BatchNorm3d(eval) -> ReLU, one fused kernel."""
+    """i3dpt.py:43-111: [zero pad] -> Conv3d -> BatchNorm3d -> ReLU.  With the running statistics (eval mode, or a net built
+    with cfg.freeze_stats, the default) one fused kernel; with batch statistics (`batch_stats`) the convolution, then
+    step_bn_stats and step_bn_apply (engine.conv's `bn`)."""
+
+    # cfg.freeze_stats of the net that owns the unit (set_freeze_stats); a unit outside such a net keeps its statistics
+    freeze_stats = True
 
     def __init__(self, in_channels, out_channels, kernel_size=(1, 1, 1), stride=(1, 1, 1), activation='relu',
                  padding='SAME', use_bias=False, use_bn=True):
@@ -37,17 +42,31 @@ class Unit3Dpy(torch.nn.Module):
             self.batch3d = torch.nn.BatchNorm3d(out_channels)
         self._cache = {}
 
+    def batch_stats(self):
+        """Whether the BatchNorm normalises with the batch's statistics: the owning net was built with cfg.freeze_stats =
+        False and batch3d is in training mode (models/networks.py:85-99).  With freeze_stats the mode is never read."""
+        return not self.freeze_stats and self.use_bn and self.batch3d.training
+
     # -- weight preparation (cached per parameter version / device / dtype) --------------------
     def packed(self, code, s2d=False):
+        """(packed weight, scale, shift): the BatchNorm folded with its running statistics, or with batch statistics
+        (scale None, shift the conv bias) the weight alone, whose cache then does not follow the running statistics."""
         bn = self.batch3d if self.use_bn else None
-        tens = [self.conv3d.weight, self.conv3d.bias] + ([bn.weight, bn.bias, bn.running_mean, bn.running_var] if bn else [])
-        key = (code, s2d) + E.params_key(*tens)
+        stats = self.batch_stats()
+        tens = [self.conv3d.weight, self.conv3d.bias]
+        if bn is not None and not stats:
+            tens += [bn.weight, bn.bias, bn.running_mean, bn.running_var]
+        key = (code, s2d, stats) + E.params_key(*tens)
         hit = self._cache.get("k")
         if hit != key:
             w = E.pack_stem_s2d(self.conv3d.weight) if s2d else E.pack_conv_weight(self.conv3d.weight, code)
-            scale, shift = E.fold_bn(bn, self.conv3d.bias, self.conv3d.out_channels, w.device)
+            scale, shift = E.fold_bn(None if stats else bn, self.conv3d.bias, self.conv3d.out_channels, w.device)
             self._cache = {"k": key, "v": (w, scale, shift)}
         return self._cache["v"]
+
+    def _bn_kw(self):
+        """engine.conv's `bn` keyword with batch statistics; none otherwise, so the frozen-statistics call is unchanged."""
+        return {"bn": [self.batch3d]} if self.batch_stats() else {}
 
     def out_channels(self):
         return self.conv3d.out_channels
@@ -65,7 +84,8 @@ class Unit3Dpy(torch.nn.Module):
         if out is None:
             od = dims or E.same_out_dims((x.T, x.H, x.W), self.kernel_size, self.stride)
             out = Act.empty(x.N, od[0], od[1], od[2], self.conv3d.out_channels, x.code, x.device)
-        return E.conv(x, w, scale, shift, out, self.kernel_size, self.stride, pad_lo, relu, residual, out_dims=dims, tag=self)
+        return E.conv(x, w, scale, shift, out, self.kernel_size, self.stride, pad_lo, relu, residual, out_dims=dims, tag=self,
+                      **self._bn_kw())
 
     def forward_s2d(self, x_s2d):
         """fp16 stem: x_s2d is the space-to-depth clip [N, T/2, H/2, W/2, 32]; 4x4x4 filter, pad 1."""
@@ -78,7 +98,23 @@ class Unit3Dpy(torch.nn.Module):
         # rt = 1 half is structurally zero (engine.pack_stem_s2d) -> the stem kernel skips its channel group 16..23
         return E.conv(x, w, scale, shift, out, (4, 4, 4), (1, 1, 1), (1, 1, 1), self.activation is not None,
                       a_mode=L.A_HALO if E.STEM_HALO else None, out_dims=(x_s2d.T, x_s2d.H, x_s2d.W),
-                      zero_cin_last_kt=4 * self.conv3d.in_channels, tag=("s2d", self))
+                      zero_cin_last_kt=4 * self.conv3d.in_channels, tag=("s2d", self), **self._bn_kw())
+
+
+def set_freeze_stats(module, freeze_stats):
+    """Give every Unit3Dpy under module its net's cfg.freeze_stats (Unit3Dpy.batch_stats)."""
+    for m in module.modules():
+        if isinstance(m, Unit3Dpy):
+            m.freeze_stats = bool(freeze_stats)
+
+
+def set_bn_eval(module):
+    """The reference's train() overrides with freeze_stats (networks.py:85-99, two_branch.py:146-161, 358-373): every
+    BatchNorm under module back in eval mode.  (Their fp16 `.half()` of the BatchNorm does not apply here: the folded
+    scale and shift are fp32 on both precision paths.)"""
+    for m in module.modules():
+        if m.__class__.__name__.find('BatchNorm') != -1:
+            m.eval()
 
 
 class MaxPool3dTFPadding(torch.nn.Module):
@@ -139,8 +175,9 @@ class Mixed(torch.nn.Module):
         c = self.__dict__.get("_fused")
         if c is None or c[0] != key:
             w = torch.cat([p[0] for p in parts], 0).contiguous()
-            scale = torch.cat([p[1] for p in parts]).contiguous()
-            shift = torch.cat([p[2] for p in parts]).contiguous()
+            # batch statistics: no folded scale, and no shift (I3D's Unit3D convolutions have no bias)
+            scale = torch.cat([p[1] for p in parts]).contiguous() if parts[0][1] is not None else None
+            shift = torch.cat([p[2] for p in parts]).contiguous() if parts[0][2] is not None else None
             self.__dict__["_fused"] = (key, (w, scale, shift))
             c = self.__dict__["_fused"]
         return c[1]
@@ -153,9 +190,11 @@ class Mixed(torch.nn.Module):
         t1 = Act.empty(x.N, x.T, x.H, x.W, m1, x.code, x.device)
         t2 = Act.empty(x.N, x.T, x.H, x.W, m2, x.code, x.device)
 
+        units = [self.branch_0, self.branch_1[0], self.branch_2[0]]
+        bn = {"bn": [u.batch3d for u in units]} if self.branch_0.batch_stats() else {}
+
         def trunk():
-            E.conv(x, w, scale, shift, out.slice(0, c0), (1, 1, 1), extra_outs=[t1, t2],
-                   tag=[self.branch_0, self.branch_1[0], self.branch_2[0]])
+            E.conv(x, w, scale, shift, out.slice(0, c0), (1, 1, 1), extra_outs=[t1, t2], tag=units, **bn)
 
         def tail():
             E.run_parallel(x.device,

@@ -15,7 +15,7 @@ import torch.nn.init as init
 from . import _lib as L
 from . import engine as E
 from .engine import Act
-from .i3d import build_trunk_stages
+from .i3d import build_trunk_stages, set_bn_eval, set_freeze_stats
 from .roi_layers import ROIAlign, ROIPool
 
 
@@ -133,6 +133,7 @@ class BaseNet(nn.Module):
             self.base_model = build_base_i3d(self.kinetics_pretrain, self.freeze_affine)
         else:
             raise NotImplementedError
+        set_freeze_stats(self.base_model, self.freeze_stats)
 
     def forward(self, x):
         """x [N,T,C,H,W] fp32 CUDA -> conv_feat [N,T/4,832,H/16,W/16] (logical view)."""
@@ -165,9 +166,11 @@ class BaseNet(nn.Module):
         return a
 
     def train(self, mode=True):
-        """networks.py:85-99: BatchNorm statistics stay frozen when cfg.freeze_stats (the kernels
-        always use running statistics; training through them is not implemented, DESIGN.md)."""
+        """networks.py:85-99: with cfg.freeze_stats every BatchNorm goes back to eval mode (running statistics); without,
+        BatchNorm in training mode normalises with batch statistics and updates the running ones (Unit3Dpy.batch_stats)."""
         nn.Module.train(self, mode)
+        if mode and self.freeze_stats:
+            set_bn_eval(self.base_model)
         return self
 
 

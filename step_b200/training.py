@@ -302,9 +302,10 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
     d(loss * loss_scale)/d(output) of the last layers.  Returns {parameter tensor: fp32 gradient in the parameter's own
     layout}: conv weights and biases, and the weight (gamma) and bias (beta) of every Unit3Dpy BatchNorm whose affine
     parameters require grad (freeze_affine=False; step_act_bn_bwd_*, from the stored output: wherever its gradient is
-    non-zero, y = gamma * xhat + beta).  Each BatchNorm tensor is returned only if it requires grad.  BatchNorm always
-    normalises with its running statistics (freeze_stats=True).  A channel with gamma == 0 gives dgamma = 0, exact unless
-    beta > 0, which `check_bn_affine` refuses.
+    non-zero, y = gamma * xhat + beta).  Each BatchNorm tensor is returned only if it requires grad.  An entry recorded with
+    batch statistics (freeze_stats=False, engine.conv's `bn`) goes through step_bn_bwd_* instead: dz through the batch mean
+    and variance from the kept z, and gamma / beta gradients when they require grad.  With the running statistics a channel
+    with gamma == 0 gives dgamma = 0, exact unless beta > 0, which `check_bn_affine` refuses.
     The input gradient of every layer is produced by the SAME convolution kernels as its forward (wgmma on fp16, SIMT on
     fp32), run on the transposed, flipped filter (stride-1 convolutions: dx = conv(dz, flip(w)^T)), accumulated through
     their residual input.  need_input_grad(entry) -> bool limits which entries form it (default: all).  A strided
@@ -347,32 +348,54 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
         out_tags = [e["tag"][1]] if s2d else list(e["tag"]) if isinstance(e["tag"], (list, tuple)) else [e["tag"]]
         out_tags += [None] * (len(outs) - len(out_tags))        # every output gets its activation backward
         col = 0
-        with _phase("act_bwd"):
-            for o, tg in zip(outs, out_tags):
-                gy = grads.of(o)
-                sc = e["scale"][col:col + o.C] if e["scale"] is not None else None
-                res = e["residual"]
-                gres = grads.of(res) if res is not None else None
-                args = (L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, L.ptr(sc), 1 if e["relu"] else 0, M,
-                        o.C, L.c_void_p(dz.data_ptr() + esz * col), n_total,
-                        L.c_void_p(gres.data_ptr()) if gres is not None else None, gres.ld if gres is not None else 0)
-                bn = trainable_bn(tg)
-                if bn is None:
-                    L.check(act_bwd(*args, L.stream()))
-                else:   # the same dz / dres, and the BatchNorm's gamma / beta gradients from the same pass
+        if e.get("bn") is not None:   # batch statistics (engine._conv_batch_stats): dz through mean and variance
+            with _phase("bn_bwd"):
+                bn_bwd = lib.step_bn_bwd_f16 if f16 else lib.step_bn_bwd_f32
+                nbytes = lib.step_bn_bwd_workspace_bytes(M, max(o.C for o in outs))
+                ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=x.device)
+                z = e["z"]
+                for o, bn in zip(outs, e["bn"]):
+                    gy = grads.of(o)
                     gam, bet = bn.weight, bn.bias
                     dgam = torch.empty((o.C,), dtype=torch.float32, device=x.device) if gam.requires_grad else None
                     dbet = torch.empty((o.C,), dtype=torch.float32, device=x.device) if bet.requires_grad else None
-                    nbytes = lib.step_act_bn_bwd_workspace_bytes(M, o.C)
-                    ws = torch.empty((nbytes // 4,), dtype=torch.float32, device=x.device)
-                    act_bn_bwd = lib.step_act_bn_bwd_f16 if f16 else lib.step_act_bn_bwd_f32
-                    L.check(act_bn_bwd(*args, L.ptr(bet.detach()), L.ptr(gam.detach()), inv, L.ptr(dgam), L.ptr(dbet), L.ptr(ws),
-                                       nbytes, L.stream()))
+                    L.check(bn_bwd(L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld,
+                                   L.c_void_p(z.buf.data_ptr() + esz * col), n_total, M, o.C,
+                                   L.c_void_p(e["mean"].data_ptr() + 4 * col), L.c_void_p(e["rstd"].data_ptr() + 4 * col),
+                                   L.ptr(gam.detach()), 1 if e["relu"] else 0, inv, L.c_void_p(dz.data_ptr() + esz * col), n_total,
+                                   L.ptr(dgam), L.ptr(dbet), L.ptr(ws), nbytes, L.stream()))
                     if dgam is not None:
                         add(gam, dgam)
                     if dbet is not None:
                         add(bet, dbet)
-                col += o.C
+                    col += o.C
+        else:
+            with _phase("act_bwd"):
+                for o, tg in zip(outs, out_tags):
+                    gy = grads.of(o)
+                    sc = e["scale"][col:col + o.C] if e["scale"] is not None else None
+                    res = e["residual"]
+                    gres = grads.of(res) if res is not None else None
+                    args = (L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, L.ptr(sc), 1 if e["relu"] else 0, M,
+                            o.C, L.c_void_p(dz.data_ptr() + esz * col), n_total,
+                            L.c_void_p(gres.data_ptr()) if gres is not None else None, gres.ld if gres is not None else 0)
+                    bn = trainable_bn(tg)
+                    if bn is None:
+                        L.check(act_bwd(*args, L.stream()))
+                    else:   # the same dz / dres, and the BatchNorm's gamma / beta gradients from the same pass
+                        gam, bet = bn.weight, bn.bias
+                        dgam = torch.empty((o.C,), dtype=torch.float32, device=x.device) if gam.requires_grad else None
+                        dbet = torch.empty((o.C,), dtype=torch.float32, device=x.device) if bet.requires_grad else None
+                        nbytes = lib.step_act_bn_bwd_workspace_bytes(M, o.C)
+                        ws = torch.empty((nbytes // 4,), dtype=torch.float32, device=x.device)
+                        act_bn_bwd = lib.step_act_bn_bwd_f16 if f16 else lib.step_act_bn_bwd_f32
+                        L.check(act_bn_bwd(*args, L.ptr(bet.detach()), L.ptr(gam.detach()), inv, L.ptr(dgam), L.ptr(dbet), L.ptr(ws),
+                                           nbytes, L.stream()))
+                        if dgam is not None:
+                            add(gam, dgam)
+                        if dbet is not None:
+                            add(bet, dbet)
+                    col += o.C
         # ---- weight (and bias) gradients
         taps = k[0] * k[1] * k[2]
         pl = e["pad_lo"]
@@ -689,7 +712,8 @@ def trunk_forward_backward(base_net, clips, d_feat_fn, loss_scale=1024.0):
     d_feat_fn(feat_act) -> fp32 tensor [N,T',H',W',832] (channels-last) with the gradient of the loss w.r.t. the trunk
     output (e.g. the sum of the ROIAlign backward results of the refinement steps).
     Returns (feat Act, {parameter: fp32 gradient}): the conv weights, and the BatchNorms' gamma / beta where they require
-    grad (freeze_affine=False, networks.py:136-142; the statistics stay the running ones, networks.py:85-99)."""
+    grad (freeze_affine=False, networks.py:136-142).  A base_net built with freeze_stats=False and in training mode normalises
+    with batch statistics, and its forward updates the running statistics unless engine.running_stats_update(False) is on."""
     from . import engine as E
     dev = clips.device
     with torch.cuda.device(dev), torch.no_grad():
@@ -753,7 +777,8 @@ def step_frames(cfg, i):
 
 
 def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9, weight_decay=0.0, lambda_reg=5.0,
-               lambda_neighbor=1.0, loss_scale=1024.0, sgd_state=None, world_size=1, optimizer=None, scaler=None, dropout=False):
+               lambda_neighbor=1.0, loss_scale=1024.0, sgd_state=None, world_size=1, optimizer=None, scaler=None, dropout=False,
+               trunk_stats_updated=False):
     """One optimisation step of train.py:263-348 on the device, for already selected training samples
     (`train_select`, utils/utils.py:135-423, is step_b200.select_samples, which returns step_tubes and step_targets):
         conv_feat = base_net(clips); context_feat = context_net(conv_feat) unless cfg.no_context      train.py:266-269
@@ -784,8 +809,17 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     scripts/train_step.sh and train_cls.sh) draws its masks as the reference's training forward does, step by step, global
     then local, from the default CUDA generator of clips' device, and leaves that generator where those F.dropout calls
     leave it (head_forward_backward); nothing else here draws from it.  With one GPU this is the reference's draw sequence
-    exactly.  Not in a CUDA graph: the draws move the generator's offset on the host."""
+    exactly.  Not in a CUDA graph: the draws move the generator's offset on the host.
+    BatchNorm statistics: nets built with cfg.freeze_stats=False and in training mode (their train()) normalise with batch
+    statistics in the trunk, ContextNet and heads, and the backward goes through them (step_bn_*).  Each head's running
+    statistics are updated once by its forward.  trunk_stats_updated=True: the caller's own training-mode forward of
+    base_net and context_net has already updated theirs (train.py:266-269); the step then normalises with the same batch
+    statistics (the kernels are deterministic) and leaves their running statistics alone.  Without it the step updates
+    them once.  Batch statistics with world_size > 1 raise NotImplementedError, and a BatchNorm with momentum=None or
+    track_running_stats=False ValueError, before anything runs."""
+    from . import engine as E
     from .engine import Act
+    from .i3d import Unit3Dpy
     if optimizer is not None and lr is not None:
         raise ValueError("train_step: give either lr (sgd_step) or optimizer, not both")
     if scaler is not None:
@@ -794,6 +828,14 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
         loss_scale = scaler.scale
     base, roi_net = nets["base_net"], nets["roi_net"]
     check_bn_affine(nets)
+    stats_units = [m for mod in nets.values() if mod is not None for m in mod.modules()
+                   if isinstance(m, Unit3Dpy) and m.batch_stats()]
+    if stats_units and world_size > 1:
+        raise NotImplementedError("train_step: BatchNorm batch statistics (freeze_stats=False) with world_size > 1: the "
+                                  "reference's DataParallel statistics (per replica in the trunk, the whole batch in the "
+                                  "heads) are not implemented")
+    for m in stats_units:
+        E.check_batch_stats_bn(m.batch3d)
     pool_mode = roi_net.pool_mode
     if pool_mode not in ("align", "pool"):
         raise RuntimeError("train_step: ROINet pool_mode %r is neither 'align' nor 'pool'" % pool_mode)
@@ -837,8 +879,9 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
                                                       T_all * ctx.shape[2], L.ptr(ctx_mean), L.F32, L.stream()))
                 row_map = torch.div(flat[:, 0, 0], float(t_len), rounding_mode="floor").to(torch.int32)
                 context = (ctx_mean, row_map, ctx, t_start)
-            r = head_forward_backward(head, None, flat, step_targets[i].to(dev), context_feat=context, lambda_reg=lambda_reg,
-                                      lambda_neighbor=lambda_neighbor, loss_scale=loss_scale, cat=cat, dropout=dropout)
+            with E.running_stats_update(True):         # the heads' statistics: one update per step
+                r = head_forward_backward(head, None, flat, step_targets[i].to(dev), context_feat=context, lambda_reg=lambda_reg,
+                                          lambda_neighbor=lambda_neighbor, loss_scale=loss_scale, cat=cat, dropout=dropout)
             results.append(r)
             all_grads.update(r["grads"])
             if use_ctx and r["ctx_dropout"] is not None:
@@ -857,7 +900,9 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
             total.add_(gfeat.reshape(B * T_all, feat.H, feat.W, feat.C).float())             # scaled by loss_scale too
         return total.mul_(1.0 / loss_scale).view(B, T_all, feat.H, feat.W, feat.C)
 
-    feat, tg = trunk_forward_backward(base, clips, d_feat, loss_scale)
+    # the trunk's and ContextNet's forwards (d_feat runs ContextNet) update their running statistics unless the caller's did
+    with E.running_stats_update(not trunk_stats_updated):
+        feat, tg = trunk_forward_backward(base, clips, d_feat, loss_scale)
     all_grads.update(tg)
     loss = sum(r["loss"] for r in results)
     skipped = False

@@ -23,7 +23,7 @@ import torch.nn as nn
 from . import _lib as L
 from . import engine as E
 from .engine import Act
-from .i3d import I3D_head
+from .i3d import I3D_head, set_bn_eval, set_freeze_stats
 from .networks import to_act, weights_init
 
 __all__ = ['ContextNet', 'TwoBranchNet']
@@ -137,6 +137,7 @@ class ContextNet(nn.Module):
         self.freeze_affine = cfg.freeze_affine
         self.fp16 = cfg.fp16
         self.i3d_conv_context = build_conv(cfg.base_net, cfg.kinetics_pretrain, 'context', self.freeze_affine)
+        set_freeze_stats(self.i3d_conv_context, self.freeze_stats)
         self.avg_pool = nn.AvgPool3d((1, 13, 13), (1, 1, 1))  # kept for repr / state parity; not called
         self._init_net()
 
@@ -165,7 +166,10 @@ class ContextNet(nn.Module):
         self.device = device
 
     def train(self, mode=True):
+        """two_branch.py:146-161: with cfg.freeze_stats the BatchNorms go back to eval mode (running statistics)."""
         nn.Module.train(self, mode)
+        if mode and self.freeze_stats:
+            set_bn_eval(self.i3d_conv_context)
         return self
 
 
@@ -187,6 +191,7 @@ class TwoBranchNet(nn.Module):
         self.cls_only = cls_only
 
         self.i3d_conv = build_conv(cfg.base_net, cfg.kinetics_pretrain, 'global', self.freeze_affine)
+        set_freeze_stats(self.i3d_conv, self.freeze_stats)
         self.downsample = nn.Conv3d(1024, self.fc_dim, kernel_size=1, stride=1, bias=True)
         self.dropout = nn.Dropout(self.dropout_prob)
         self.global_cls = nn.Conv3d(self.fc_dim * self.pool_size ** 2 + (1024 if not self.no_context else 0),
@@ -402,5 +407,8 @@ class TwoBranchNet(nn.Module):
         self.device = device
 
     def train(self, mode=True):
+        """two_branch.py:358-373: with cfg.freeze_stats the BatchNorms go back to eval mode (running statistics)."""
         nn.Module.train(self, mode)
+        if mode and self.freeze_stats:
+            set_bn_eval(self.i3d_conv)
         return self
