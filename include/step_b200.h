@@ -472,6 +472,41 @@ int step_bn_bwd_f16(const void* dy, int dy_ld, const void* y, int y_ld, const vo
 int step_bn_bwd_f32(const float* dy, int dy_ld, const float* y, int y_ld, const float* z, int z_ld, long long M, int C,
                     const float* mean, const float* rstd, const float* gamma, int relu, float gscale, float* dz, int dz_ld,
                     float* dgamma, float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream);
+/* The same statistics and backward split around a cross-rank exchange (synchronised BatchNorm: several ranks, each holding
+ * some rows of one batch, normalise with the statistics of all of them).  Each rank runs the local entry on its own z, the
+ * caller gathers every rank's output into one [ranks, ...] array in rank order, and each rank runs the merge on that array.
+ * The merges combine the ranks in a fixed order, so every rank computes identical statistics and coefficients from the same
+ * gathered array; with ranks = 1 local + merge give the fused entries' outputs bit for bit.  A rank may hold M = 1 pixel;
+ * the merges refuse a total M < 2, as torch does.
+ * step_bn_stats_local: this rank's (count, mean, M2) of every channel of z [M, C] -> stats [3, stats_ld] fp32 (columns
+ *   [0, C)); workspace step_bn_stats_workspace_bytes(M, C).
+ * step_bn_stats_merge: stats [ranks, 3, stats_ld] (every rank's step_bn_stats_local, columns [0, C)) merged by Chan's formula
+ *   -> mean, rstd, scale, shift and the running-statistic update of step_bn_stats, with M the total count over the ranks.
+ * step_bn_bwd_sums: this rank's sums (sum g, sum g xhat) -> sums [2, sums_ld] fp32 (columns [0, C)), and its own
+ *   dbeta = gscale * sum g, dgamma = gscale * sum g xhat (either may be NULL); workspace step_bn_bwd_sums_workspace_bytes.
+ * step_bn_bwd_merge_dz: sums [ranks, 2, sums_ld] added in rank order, then dz of this rank's M rows as step_bn_bwd forms it,
+ *   with the total count M_total over the ranks; workspace step_bn_bwd_merge_dz_workspace_bytes(C). */
+int step_bn_stats_local_f16(const void* z, int z_ld, long long M, int C, float* stats, int stats_ld, void* workspace, size_t ws_bytes,
+                            step_stream_t stream);
+int step_bn_stats_local_f32(const float* z, int z_ld, long long M, int C, float* stats, int stats_ld, void* workspace, size_t ws_bytes,
+                            step_stream_t stream);
+int step_bn_stats_merge(const float* stats, int ranks, int stats_ld, long long M, int C, const float* gamma, const float* beta, float eps,
+                        float momentum, float* running_mean, float* running_var, float* mean, float* rstd, float* scale, float* shift,
+                        step_stream_t stream);
+size_t step_bn_bwd_sums_workspace_bytes(long long M, int C);
+int step_bn_bwd_sums_f16(const void* dy, int dy_ld, const void* y, int y_ld, const void* z, int z_ld, long long M, int C,
+                         const float* mean, const float* rstd, int relu, float gscale, float* sums, int sums_ld, float* dgamma,
+                         float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream);
+int step_bn_bwd_sums_f32(const float* dy, int dy_ld, const float* y, int y_ld, const float* z, int z_ld, long long M, int C,
+                         const float* mean, const float* rstd, int relu, float gscale, float* sums, int sums_ld, float* dgamma,
+                         float* dbeta, void* workspace, size_t ws_bytes, step_stream_t stream);
+size_t step_bn_bwd_merge_dz_workspace_bytes(int C);
+int step_bn_bwd_merge_dz_f16(const float* sums, int ranks, int sums_ld, long long M_total, const void* dy, int dy_ld, const void* y,
+                             int y_ld, const void* z, int z_ld, long long M, int C, const float* mean, const float* rstd,
+                             const float* gamma, int relu, void* dz, int dz_ld, void* workspace, size_t ws_bytes, step_stream_t stream);
+int step_bn_bwd_merge_dz_f32(const float* sums, int ranks, int sums_ld, long long M_total, const float* dy, int dy_ld, const float* y,
+                             int y_ld, const float* z, int z_ld, long long M, int C, const float* mean, const float* rstd,
+                             const float* gamma, int relu, float* dz, int dz_ld, void* workspace, size_t ws_bytes, step_stream_t stream);
 
 /* ------------------------------------------------------------------ the heads' dropout ---- */
 /* One draw of torch.nn.functional.dropout(x, p, training=True) on a CUDA fp32 tensor of n elements (n % 4 == 0, n < 2^31,

@@ -227,6 +227,31 @@ def running_stats_update(on):
         UPDATE_RUNNING_STATS = saved
 
 
+# Synchronised batch statistics: None, or (process group, rows of the batch over every rank of the group).  training.train_step
+# sets it around the heads of a step with world_size > 1, where the reference runs each head over the whole batch
+# (train.py:313-323): every BatchNorm then normalises with the statistics of all ranks' rows.
+SYNC_STATS = None
+
+
+@contextlib.contextmanager
+def batch_stats_sync(group, rows_total):
+    global SYNC_STATS
+    saved = SYNC_STATS
+    SYNC_STATS = (group, int(rows_total))
+    try:
+        yield
+    finally:
+        SYNC_STATS = saved
+
+
+def all_gather_rows(t, group):
+    """[W, *t.shape] of every rank's t in rank order: one all_gather into views of one buffer."""
+    import torch.distributed as dist
+    out = torch.empty((dist.get_world_size(group),) + tuple(t.shape), dtype=t.dtype, device=t.device)
+    dist.all_gather(list(out.unbind(0)), t, group=group)
+    return out
+
+
 def check_batch_stats_bn(bn):
     """The BatchNorm settings the batch-statistics kernels implement: an exponential running average (momentum) that is
     tracked, as the reference's BatchNorm3d defaults are."""
@@ -240,7 +265,10 @@ def _conv_batch_stats(x, w_packed, shift, outs, bns, k, stride, pad_lo, relu, a_
     """conv() for Unit3Dpy outputs whose BatchNorms normalise with batch statistics (bns: one BatchNorm3d per output of outs):
     the convolution writes z [M, sum C] with the identity epilogue (+ the conv bias `shift`), step_bn_stats forms each
     BatchNorm's statistics over z's column range (and, when UPDATE_RUNNING_STATS, updates its running statistics once), and
-    one step_bn_apply writes y = relu(scale z + shift) to every output.  The tape entry also keeps z, mean, rstd and bns."""
+    one step_bn_apply writes y = relu(scale z + shift) to every output.  The tape entry also keeps z, mean, rstd and bns.
+    Under batch_stats_sync the statistics are those of every rank's rows: step_bn_stats_local for each output, one
+    all-gather of the entry's [3, sum C] triples, and step_bn_stats_merge for each output over the gathered array (the same
+    on every rank); the tape entry then records the group and the total pixel count for the backward's exchange."""
     code, dev = x.code, x.device
     o0 = outs[0]
     n_total = sum(o.C for o in outs)
@@ -252,16 +280,38 @@ def _conv_batch_stats(x, w_packed, shift, outs, bns, k, stride, pad_lo, relu, a_
     stats = torch.empty((4, n_total), dtype=torch.float32, device=dev)          # mean, rstd, scale, shift
     nbytes = L.lib().step_bn_stats_workspace_bytes(M, max(o.C for o in outs))
     ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=dev)
-    bn_stats = L.lib().step_bn_stats_f16 if code == L.F16 else L.lib().step_bn_stats_f32
+    f16 = code == L.F16
     esz = z.buf.element_size()
+    at = lambda r, col: L.c_void_p(stats[r].data_ptr() + 4 * col)
+    for bn in bns:
+        check_batch_stats_bn(bn)
+    upd = UPDATE_RUNNING_STATS
+    sync = None
+    if SYNC_STATS is not None:
+        # each rank's (count, mean, M2) of every output, one exchange for the entry, then the same merge on every rank
+        group, rows_total = SYNC_STATS
+        M_total = M // o0.N * rows_total
+        local = torch.empty((3, n_total), dtype=torch.float32, device=dev)
+        stats_local = L.lib().step_bn_stats_local_f16 if f16 else L.lib().step_bn_stats_local_f32
+        col = 0
+        for o in outs:
+            L.check(stats_local(L.c_void_p(z.buf.data_ptr() + esz * col), n_total, M, o.C, L.c_void_p(local.data_ptr() + 4 * col),
+                                n_total, L.ptr(ws), nbytes, L.stream()))
+            col += o.C
+        gathered = all_gather_rows(local, group)
+        sync = dict(group=group, M_total=M_total)
+    bn_stats = L.lib().step_bn_stats_f16 if f16 else L.lib().step_bn_stats_f32
     col = 0
     for o, bn in zip(outs, bns):
-        check_batch_stats_bn(bn)
-        upd = UPDATE_RUNNING_STATS
-        at = lambda r, col=col: L.c_void_p(stats[r].data_ptr() + 4 * col)
-        L.check(bn_stats(L.c_void_p(z.buf.data_ptr() + esz * col), n_total, M, o.C, L.ptr(bn.weight.detach()),
-                         L.ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum), L.ptr(bn.running_mean) if upd else None,
-                         L.ptr(bn.running_var) if upd else None, at(0), at(1), at(2), at(3), L.ptr(ws), nbytes, L.stream()))
+        run = (L.ptr(bn.running_mean) if upd else None, L.ptr(bn.running_var) if upd else None, at(0, col), at(1, col),
+               at(2, col), at(3, col))
+        if sync is None:
+            L.check(bn_stats(L.c_void_p(z.buf.data_ptr() + esz * col), n_total, M, o.C, L.ptr(bn.weight.detach()),
+                             L.ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum), *run, L.ptr(ws), nbytes, L.stream()))
+        else:
+            L.check(L.lib().step_bn_stats_merge(L.c_void_p(gathered.data_ptr() + 4 * col), gathered.shape[0], n_total, M_total, o.C,
+                                                L.ptr(bn.weight.detach()), L.ptr(bn.bias.detach()), float(bn.eps),
+                                                float(bn.momentum), *run, L.stream()))
         if upd:
             # written in place by the kernel: the version bump re-keys the folded weights of a later eval-mode forward
             torch.autograd.graph.increment_version(bn.running_mean)
@@ -278,7 +328,7 @@ def _conv_batch_stats(x, w_packed, shift, outs, bns, k, stride, pad_lo, relu, a_
     if TAPE is not None:
         TAPE.append(dict(kind="conv", x=x, w=w_packed, scale=None, out=o0, extra_outs=list(outs[1:]), k=tuple(k),
                          stride=tuple(stride), pad_lo=tuple(pad_lo), relu=bool(relu), residual=None, tag=tag, z=z,
-                         mean=stats[0], rstd=stats[1], bn=list(bns)))
+                         mean=stats[0], rstd=stats[1], bn=list(bns), sync=sync))
     return o0
 
 

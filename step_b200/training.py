@@ -348,7 +348,41 @@ def tape_backward(tape, grads, loss_scale=1.0, need_input_grad=None):
         out_tags = [e["tag"][1]] if s2d else list(e["tag"]) if isinstance(e["tag"], (list, tuple)) else [e["tag"]]
         out_tags += [None] * (len(outs) - len(out_tags))        # every output gets its activation backward
         col = 0
-        if e.get("bn") is not None:   # batch statistics (engine._conv_batch_stats): dz through mean and variance
+        if e.get("bn") is not None and e.get("sync") is not None:
+            # batch statistics of every rank's rows (engine.batch_stats_sync): this rank's sums of every output, one
+            # exchange for the entry, then dz from the sums of all ranks (added in rank order: the same on every rank)
+            with _phase("bn_bwd"):
+                z = e["z"]
+                sums_fn = lib.step_bn_bwd_sums_f16 if f16 else lib.step_bn_bwd_sums_f32
+                merge_dz = lib.step_bn_bwd_merge_dz_f16 if f16 else lib.step_bn_bwd_merge_dz_f32
+                nbytes = max(lib.step_bn_bwd_sums_workspace_bytes(M, max(o.C for o in outs)),
+                             lib.step_bn_bwd_merge_dz_workspace_bytes(max(o.C for o in outs)))
+                ws = torch.empty((max(nbytes, 4) // 4,), dtype=torch.float32, device=x.device)
+                sums = torch.empty((2, n_total), dtype=torch.float32, device=x.device)
+                at = lambda t, c, es=4: L.c_void_p(t.data_ptr() + es * c)
+                for o, bn in zip(outs, e["bn"]):
+                    gy = grads.of(o)
+                    gam, bet = bn.weight, bn.bias
+                    dgam = torch.empty((o.C,), dtype=torch.float32, device=x.device) if gam.requires_grad else None
+                    dbet = torch.empty((o.C,), dtype=torch.float32, device=x.device) if bet.requires_grad else None
+                    L.check(sums_fn(L.c_void_p(gy.data_ptr()), gy.ld, L.c_void_p(o.data_ptr()), o.ld, at(z.buf, col, esz), n_total, M,
+                                    o.C, at(e["mean"], col), at(e["rstd"], col), 1 if e["relu"] else 0, inv, at(sums, col), n_total,
+                                    L.ptr(dgam), L.ptr(dbet), L.ptr(ws), nbytes, L.stream()))
+                    if dgam is not None:
+                        add(gam, dgam)
+                    if dbet is not None:
+                        add(bet, dbet)
+                    col += o.C
+                gathered = E.all_gather_rows(sums, e["sync"]["group"])
+                col = 0
+                for o, bn in zip(outs, e["bn"]):
+                    gy = grads.of(o)
+                    L.check(merge_dz(at(gathered, col), gathered.shape[0], n_total, e["sync"]["M_total"], L.c_void_p(gy.data_ptr()),
+                                     gy.ld, L.c_void_p(o.data_ptr()), o.ld, at(z.buf, col, esz), n_total, M, o.C, at(e["mean"], col),
+                                     at(e["rstd"], col), L.ptr(bn.weight.detach()), 1 if e["relu"] else 0, at(dz, col, esz), n_total,
+                                     L.ptr(ws), nbytes, L.stream()))
+                    col += o.C
+        elif e.get("bn") is not None:   # batch statistics (engine._conv_batch_stats): dz through mean and variance
             with _phase("bn_bwd"):
                 bn_bwd = lib.step_bn_bwd_f16 if f16 else lib.step_bn_bwd_f32
                 nbytes = lib.step_bn_bwd_workspace_bytes(M, max(o.C for o in outs))
@@ -770,6 +804,56 @@ def sgd_step(params_and_grads, lr, momentum=0.9, weight_decay=0.0, state=None, w
     return state
 
 
+def _sync_plan(cfg, nets, step_tubes, loss_scale, dev):
+    """The refusals of a train_step whose heads synchronise their batch statistics, decided from one all-gather of every
+    rank's number of steps, loss scale and per-step row counts, so that every rank raises the same error before anything
+    changes.  Returns the rows of each step over all ranks."""
+    import torch.distributed as dist
+    from . import engine as E
+    cap = int(cfg.max_iter)
+    n_steps = len(step_tubes)
+    mine = torch.zeros((2 + cap,), dtype=torch.float64)
+    mine[0], mine[1] = n_steps, float(loss_scale)
+    for i, t in enumerate(step_tubes[:cap]):
+        mine[2 + i] = t.shape[0]
+    plan = E.all_gather_rows(mine.to(dev), dist.group.WORLD).cpu()
+    steps, scales, rows = plan[:, 0], plan[:, 1], plan[:, 2:]
+    if bool((steps != steps[0]).any()) or bool((scales != scales[0]).any()):
+        raise ValueError("train_step: the ranks disagree on the number of steps %s or the loss scale %s"
+                         % (steps.long().tolist(), scales.tolist()))
+    if n_steps > cap:
+        raise ValueError("train_step: %d steps but cfg.max_iter = %d" % (n_steps, cap))
+    rows = rows[:, :n_steps].long()
+    if bool((rows == 0).any()):
+        raise ValueError("train_step: a rank has no rows in some step (rows per rank and step: %s); synchronised batch "
+                         "statistics need every rank to hold rows of every step" % rows.tolist())
+    rows_total = rows.sum(0).tolist()
+    for i in range(n_steps):
+        head = nets["det_net%d" % i]
+        values = rows_total[i] * step_frames(cfg, i + 1)[1] * head.pool_size ** 2
+        if values < 2:
+            raise ValueError("train_step: step %d's head BatchNorms would see %d value(s) per channel over all ranks: "
+                             "Expected more than 1 value per channel when training" % (i + 1, values))
+    return rows_total
+
+
+def _broadcast_running_stats(bns):
+    """Rank 0's running_mean, running_var and num_batches_tracked of every BatchNorm in bns to every rank: one broadcast of
+    one flat byte buffer."""
+    import torch.distributed as dist
+    ts = [t for bn in bns for t in (bn.running_mean, bn.running_var, bn.num_batches_tracked)]
+    if not ts:
+        return
+    flat = torch.cat([t.detach().reshape(-1).view(torch.uint8) for t in ts])
+    dist.broadcast(flat, src=0)
+    off = 0
+    with torch.no_grad():
+        for t in ts:
+            n = t.numel() * t.element_size()
+            t.copy_(flat[off:off + n].view(t.dtype).view_as(t))
+            off += n
+
+
 def step_frames(cfg, i):
     """(T_start, T_length) of refinement step i (1-based) -- train.py:294-298."""
     chunks = cfg.NUM_CHUNKS[i]
@@ -815,8 +899,17 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     statistics are updated once by its forward.  trunk_stats_updated=True: the caller's own training-mode forward of
     base_net and context_net has already updated theirs (train.py:266-269); the step then normalises with the same batch
     statistics (the kernels are deterministic) and leaves their running statistics alone.  Without it the step updates
-    them once.  Batch statistics with world_size > 1 raise NotImplementedError, and a BatchNorm with momentum=None or
-    track_running_stats=False ValueError, before anything runs."""
+    them once.  A BatchNorm with momentum=None or track_running_stats=False raises ValueError before anything runs.
+    Batch statistics with world_size > 1 (one process per GPU in the default process group of world_size ranks, rank r
+    holding DataParallel's chunk r of the batch, clips [r * ceil(B / W), ...), and the rows its clips select) follow the
+    reference's nn.DataParallel (train.py:141-148): the trunk and ContextNet normalise with each rank's own statistics and
+    every rank ends with rank 0's running statistics (one broadcast); each head normalises with the statistics of every
+    rank's rows of its step (engine.batch_stats_sync: an all-gather per convolution, forward and backward, and the same
+    merge on every rank, so the heads' running statistics are identical on every rank).  The averaged gradients are those
+    of (1 / W) sum_r L_r, the reference's whole-batch objective when every rank has the same rows in each step.  Without
+    an initialised default process group this raises NotImplementedError; with one of another size, ranks that disagree on
+    the number of steps or the loss scale, a rank with no rows in a step, or a head BatchNorm with fewer than 2 values per
+    channel over all ranks, ValueError on every rank before anything changes (one all-gather up front)."""
     from . import engine as E
     from .engine import Act
     from .i3d import Unit3Dpy
@@ -830,10 +923,16 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     check_bn_affine(nets)
     stats_units = [m for mod in nets.values() if mod is not None for m in mod.modules()
                    if isinstance(m, Unit3Dpy) and m.batch_stats()]
-    if stats_units and world_size > 1:
-        raise NotImplementedError("train_step: BatchNorm batch statistics (freeze_stats=False) with world_size > 1: the "
-                                  "reference's DataParallel statistics (per replica in the trunk, the whole batch in the "
-                                  "heads) are not implemented")
+    sync = bool(stats_units) and world_size > 1
+    if sync:
+        import torch.distributed as dist
+        if not (dist.is_available() and dist.is_initialized()):
+            raise NotImplementedError("train_step: BatchNorm batch statistics (freeze_stats=False) with world_size > 1 need the "
+                                      "default process group of the world_size ranks (torch.distributed.init_process_group): "
+                                      "the heads' statistics are exchanged between the ranks")
+        if dist.get_world_size() != world_size:
+            raise ValueError("train_step: world_size=%d but the default process group has %d ranks"
+                             % (world_size, dist.get_world_size()))
     for m in stats_units:
         E.check_batch_stats_bn(m.batch3d)
     pool_mode = roi_net.pool_mode
@@ -844,6 +943,7 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
         raise RuntimeError("train_step: cfg.no_context is False but nets has no 'context_net'")
     dev = clips.device
     n_steps = len(step_tubes)
+    rows_total = _sync_plan(cfg, nets, step_tubes, loss_scale, dev) if sync else None
     results = []
     all_grads = {}
 
@@ -879,7 +979,9 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
                                                       T_all * ctx.shape[2], L.ptr(ctx_mean), L.F32, L.stream()))
                 row_map = torch.div(flat[:, 0, 0], float(t_len), rounding_mode="floor").to(torch.int32)
                 context = (ctx_mean, row_map, ctx, t_start)
-            with E.running_stats_update(True):         # the heads' statistics: one update per step
+            # the heads' statistics: one update per step; with several ranks, those of every rank's rows of the step
+            sync_heads = E.batch_stats_sync(dist.group.WORLD, rows_total[i]) if sync else contextlib.nullcontext()
+            with E.running_stats_update(True), sync_heads:
                 r = head_forward_backward(head, None, flat, step_targets[i].to(dev), context_feat=context, lambda_reg=lambda_reg,
                                           lambda_neighbor=lambda_neighbor, loss_scale=loss_scale, cat=cat, dropout=dropout)
             results.append(r)
@@ -904,6 +1006,9 @@ def train_step(cfg, nets, clips, step_tubes, step_targets, lr=None, momentum=0.9
     with E.running_stats_update(not trunk_stats_updated):
         feat, tg = trunk_forward_backward(base, clips, d_feat, loss_scale)
     all_grads.update(tg)
+    if sync:   # DataParallel keeps device 0's replica's update of the trunk's and ContextNet's running statistics
+        _broadcast_running_stats([m.batch3d for k in ("base_net", "context_net") if nets.get(k) is not None
+                                  for m in nets[k].modules() if isinstance(m, Unit3Dpy) and m.batch_stats()])
     loss = sum(r["loss"] for r in results)
     skipped = False
     if optimizer is not None:
