@@ -91,6 +91,19 @@ int step_detect_scores_f32(const float* prob, int prob_ld, const float* box, int
 int step_detect_scores_check(const float* prob, int prob_ld, const float* box, int box_ld, const int* clip_offsets,
                              int n_clips, int n_rows, int max_per_clip, int ncls, int cap, const float* det,
                              const int* det_count);
+/* Cross-class merge of demo.py:176-198 on step_detect_f32's rows, read in place: det [n_clips, cap, 8], det_count
+ * [n_clips].  Per clip, over rows 0..det_count-1 in order, a row not yet taken leads a group and takes every later row
+ * not yet taken whose compute_box_iou with it (utils/tube_utils.py, float32, no "+1") is > thresh.  Each group's box is
+ * np.mean of its members' boxes (sequential float32 sum in row order, over float32(count)).  Groups whose means are equal
+ * bit for bit share one key of the reference's dict, which keeps the first group's position and the last group's members.
+ *   mbox   [n_clips, cap, 4]  the keys' mean boxes in dict order;
+ *   pairs  [n_clips, cap, 2]  int32 (det row, key index) in the order results.txt writes them (demo.py:209-217);
+ *   mcount [n_clips, 2]       int32 (keys, pairs).
+ * cap <= step_detect_merge_max_rows().  No atomics (bit-identical from run to run), no host synchronisation. */
+size_t step_detect_merge_workspace_bytes(int n_clips, int cap);
+int step_detect_merge_max_rows(void);
+int step_detect_merge_f32(const float* det, const int* det_count, int n_clips, int cap, float thresh, float* mbox,
+                          int* pairs, int* mcount, void* workspace, size_t ws_bytes, step_stream_t stream);
 
 /* ------------------------------------------------------------------ ROI ops -------------- */
 /* Reference layout (NCHW fp32 in, [R,C,ph,pw] fp32 out), arithmetic order of the reference. */

@@ -58,62 +58,127 @@ __global__ void __launch_bounds__(256) nms_rank_kernel(const float* __restrict__
   }
 }
 
-// ---- 2. upper-triangular 64x64 bitmask tiles on the sorted boxes
+// The pairwise predicates of the two greedy passes of this file.  prep(b) is the per-box value the predicate reuses (an
+// area); p(a, prep(a), b, prep(b)) says whether the earlier box a takes the later box b.
+struct NmsPred {   // nms_cpu.cpp:74-85: suppress when IoU >= thr (ge) or > thr, legacy "+1" areas
+  float thr;
+  int ge;
+  __device__ __forceinline__ float prep(float4 b) const { return box_area(b); }
+  __device__ __forceinline__ bool operator()(float4 a, float aa, float4 b, float ab) const {
+    return suppresses(a, aa, b, ab, thr, ge);
+  }
+};
+
+struct MergePred {  // demo.py:190  compute_box_iou(box, box2) > global_thresh  (utils/tube_utils.py:292-306, float32)
+  float thr;
+  __device__ __forceinline__ float prep(float4 b) const { return __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y)); }
+  __device__ __forceinline__ bool operator()(float4 a, float aa, float4 b, float ab) const {
+    const float iw = fmaxf(__fsub_rn(fminf(a.z, b.z), fmaxf(a.x, b.x)), 0.0f);
+    const float ih = fmaxf(__fsub_rn(fminf(a.w, b.w), fmaxf(a.y, b.y)), 0.0f);
+    const float inter = (iw > 0.0f && ih > 0.0f) ? __fmul_rn(iw, ih) : 0.0f;
+    // a zero union gives NaN (two identical zero-area boxes), which never merges
+    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(aa, ab), inter)) > thr;
+  }
+};
+
+// Where the greedy passes read their rows: count(z) rows of problem z (blockIdx.z of the mask pass, blockIdx.x of the
+// resolve), box(z, i) the i-th in greedy order.
+struct SortedRows {   // step_nms_f32: one problem, boxes already in score order
+  const float4* sb;
+  int n;
+  __device__ __forceinline__ int count(int) const { return n; }
+  __device__ __forceinline__ float4 box(int, int i) const { return sb[i]; }
+};
+
+struct DetRows {      // step_detect_merge_f32: clip z's rows det[z][0, det_count[z]) in step_detect_f32's order
+  const float* det;
+  const int* det_count;
+  int cap;
+  __device__ __forceinline__ int count(int z) const { return min(max(det_count[z], 0), cap); }
+  __device__ __forceinline__ float4 box(int z, int i) const {
+    return *reinterpret_cast<const float4*>(det + ((size_t)z * cap + i) * 8);
+  }
+};
+
+// ---- 2. upper-triangular 64x64 bitmask tiles: bit j of mask[r][col_blk] = pred(row r, row col_blk*64 + j), j > r.
+//         Problem z's mask starts at mask + z * mask_stride, col_blocks words per row.
 constexpr int kTile = 64;
-__global__ void __launch_bounds__(kTile) nms_mask_kernel(const float4* __restrict__ sb, int n, float thr,
-                                                         int ge, int col_blocks,
-                                                         unsigned long long* __restrict__ mask) {
+template <class Rows, class Pred>
+__global__ void __launch_bounds__(kTile) mask_tiles_kernel(Rows rows, Pred pred, int col_blocks, size_t mask_stride,
+                                                           unsigned long long* __restrict__ mask) {
+  const int z = blockIdx.z, n = rows.count(z);
   const int row_blk = blockIdx.y, col_blk = blockIdx.x;
-  if (col_blk < row_blk) return;  // never read by the resolve
+  if (col_blk < row_blk || col_blk * kTile >= n) return;  // never read by the resolve
+  mask += (size_t)z * mask_stride;
   __shared__ float4 cb[kTile];
   __shared__ float ca[kTile];
   const int col_size = min(n - col_blk * kTile, kTile);
   if (threadIdx.x < col_size) {
-    float4 b = sb[col_blk * kTile + threadIdx.x];
+    float4 b = rows.box(z, col_blk * kTile + threadIdx.x);
     cb[threadIdx.x] = b;
-    ca[threadIdx.x] = box_area(b);
+    ca[threadIdx.x] = pred.prep(b);
   }
   __syncthreads();
   const int r = row_blk * kTile + threadIdx.x;
   if (r < n) {
-    float4 a = sb[r];
-    float aa = box_area(a);
+    float4 a = rows.box(z, r);
+    float aa = pred.prep(a);
     unsigned long long bits = 0;
     int start = (row_blk == col_blk) ? threadIdx.x + 1 : 0;
     for (int j = start; j < col_size; ++j)
-      if (suppresses(a, aa, cb[j], ca[j], thr, ge)) bits |= 1ULL << j;
+      if (pred(a, aa, cb[j], ca[j])) bits |= 1ULL << j;
     mask[(size_t)r * col_blocks + col_blk] = bits;
   }
 }
 
-// ---- 3. greedy resolve on device: one CTA walks the 64-box blocks in score order.
-__global__ void __launch_bounds__(1024) nms_resolve_kernel(const unsigned long long* __restrict__ mask,
-                                                           const int* __restrict__ order, int n,
-                                                           int col_blocks, uint8_t* __restrict__ keep_flag) {
-  extern __shared__ unsigned long long remv[];  // [col_blocks]
+// ---- 3. greedy resolve on device: one CTA per problem walks its 64-row blocks in order.  A row is kept (a leader) unless
+//         an earlier kept row took it.  keep(z, i, k) stores row i's flag; claim(z, leader, col_blk, bits) is told which
+//         rows of column block col_blk the kept row `leader` is the first to take (leaders are visited in ascending order).
+struct KeepByOrder {  // step_nms_f32: flag at the row's original index
+  const int* order;
+  uint8_t* keep_flag;
+  __device__ __forceinline__ void operator()(int, int i, unsigned k) const { keep_flag[order[i]] = (uint8_t)k; }
+};
+
+struct NoClaim {
+  __device__ __forceinline__ void operator()(int, int, int, unsigned long long) const {}
+};
+
+template <class Rows, class Keep, class Claim>
+__global__ void __launch_bounds__(1024) resolve_kernel(const unsigned long long* __restrict__ mask, Rows rows,
+                                                       int col_ld, size_t mask_stride, Keep keep, Claim claim) {
+  extern __shared__ unsigned long long remv[];  // [col_ld]
   __shared__ unsigned long long diag[kTile];
   __shared__ unsigned long long kept_s;
+  const int z = blockIdx.x, n = rows.count(z), col_blocks = (n + kTile - 1) / kTile;
+  mask += (size_t)z * mask_stride;
   for (int j = threadIdx.x; j < col_blocks; j += blockDim.x) remv[j] = 0;
   __syncthreads();
   for (int blk = 0; blk < col_blocks; ++blk) {
     const int cnt = min(kTile, n - blk * kTile);
-    if (threadIdx.x < cnt) diag[threadIdx.x] = mask[(size_t)(blk * kTile + threadIdx.x) * col_blocks + blk];
+    if (threadIdx.x < cnt) diag[threadIdx.x] = mask[(size_t)(blk * kTile + threadIdx.x) * col_ld + blk];
     __syncthreads();
     if (threadIdx.x == 0) {
       unsigned long long r = remv[blk], kept = 0;
       for (int b = 0; b < cnt; ++b)
-        if (!((r >> b) & 1ULL)) { kept |= 1ULL << b; r |= diag[b]; }
+        if (!((r >> b) & 1ULL)) {
+          kept |= 1ULL << b;
+          claim(z, blk * kTile + b, blk, diag[b] & ~r);
+          r |= diag[b];
+        }
       kept_s = kept;
     }
     __syncthreads();
     const unsigned long long kept = kept_s;
-    if (threadIdx.x < cnt) keep_flag[order[blk * kTile + threadIdx.x]] = (uint8_t)((kept >> threadIdx.x) & 1ULL);
+    if (threadIdx.x < cnt) keep(z, blk * kTile + threadIdx.x, (unsigned)((kept >> threadIdx.x) & 1ULL));
     for (int j = blk + 1 + threadIdx.x; j < col_blocks; j += blockDim.x) {
       unsigned long long acc = remv[j], k = kept;
       while (k) {
         int b = __ffsll((long long)k) - 1;
         k &= k - 1;
-        acc |= mask[(size_t)(blk * kTile + b) * col_blocks + j];
+        const unsigned long long m = mask[(size_t)(blk * kTile + b) * col_ld + j];
+        claim(z, blk * kTile + b, j, m & ~acc);
+        acc |= m;
       }
       remv[j] = acc;
     }
@@ -356,6 +421,161 @@ __global__ void __launch_bounds__(256) detect_scores_kernel(const float* __restr
   if (threadIdx.x == 0) det_count[clip] = m < cap ? m : cap;
 }
 
+// ---- cross-class merge of demo.py:176-198 on step_detect_f32's rows --------------------------------------------------
+// Per clip, over the rows in order: a row not yet taken leads a group and takes every later untaken row whose
+// compute_box_iou with it is > thresh (float32).  That is greedy NMS with MergePred, so mask_tiles_kernel and
+// resolve_kernel find the leaders; their claim hook records which leader took each row (GroupClaim).  Then
+// merge_groups_kernel forms the reference's dict: the mean box of each group (np.mean: a sequential float32 sum over the
+// members in row order, over float32(count)), one key per distinct mean (bit-equal means are one key: it keeps its first
+// group's position and its last group's members) and the rows that results.txt writes, in order.
+// Rows of one clip: resolve_kernel keeps a ceil(cap/64)-word row of the bitmask in (default, 48 KB) shared memory.
+constexpr int kMergeMaxRows = 48 * 1024 / 8 * kTile;
+
+struct GroupKeep {    // a leader is its own group
+  int* group;
+  int ld;
+  __device__ __forceinline__ void operator()(int z, int i, unsigned k) const {
+    if (k) group[(size_t)z * ld + i] = i;
+  }
+};
+
+struct GroupClaim {
+  int* group;
+  int ld;
+  __device__ __forceinline__ void operator()(int z, int leader, int col_blk, unsigned long long bits) const {
+    int* g = group + (size_t)z * ld + col_blk * kTile;
+    while (bits) {
+      const int b = __ffsll((long long)bits) - 1;
+      bits &= bits - 1;
+      g[b] = leader;
+    }
+  }
+};
+
+// Exclusive prefix sum in index order over the whole CTA of kWarps warps: calls emit(i, sum of val(t) for t < i) for every
+// i in [0, n), and returns the total.
+template <int kWarps, class Val, class Emit>
+__device__ __forceinline__ int block_scan(int n, Val val, Emit emit) {
+  __shared__ int warp_tot[kWarps];
+  __shared__ int base_s;
+  if (threadIdx.x == 0) base_s = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (int start = 0; start < n; start += blockDim.x) {
+    const int i = start + threadIdx.x;
+    const int v = (i < n) ? val(i) : 0;
+    int incl = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += t;
+    }
+    if (lane == 31) warp_tot[wid] = incl;
+    __syncthreads();
+    int off = base_s;
+    for (int w = 0; w < wid; ++w) off += warp_tot[w];
+    if (i < n) emit(i, off + incl - v);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int t = 0;
+      for (int w = 0; w < kWarps; ++w) t += warp_tot[w];
+      base_s += t;
+    }
+    __syncthreads();
+  }
+  return base_s;
+}
+
+// Per-clip scratch of merge_groups_kernel, cap entries per clip (ws + clip * cap).
+struct MergeScratch {
+  int* group;    // [cap] leader of each row (resolve_kernel)
+  int* lead;     // [cap] the g-th leader's row
+  int* members;  // [cap] members of group g
+  int* first;    // [cap] first group with group g's mean
+  int* last;     // [cap] last group with group g's mean
+  int* key;      // [cap] key index of group g (g its key's first group)
+  int* offset;   // [cap] first write-order row of group g's key (g its key's first group)
+  float4* mean;  // [cap] mean box of group g
+};
+
+__global__ void __launch_bounds__(1024) merge_groups_kernel(const float* __restrict__ det, const int* __restrict__ det_count,
+                                                            int cap, MergeScratch ws, float* __restrict__ mbox,
+                                                            int* __restrict__ pairs, int* __restrict__ mcount) {
+  const int z = blockIdx.x;
+  const int n = min(max(det_count[z], 0), cap);
+  const size_t o = (size_t)z * cap;
+  const int* group = ws.group + o;
+  int *lead = ws.lead + o, *members = ws.members + o, *first = ws.first + o, *last = ws.last + o, *key = ws.key + o;
+  int* offset = ws.offset + o;
+  float* mean = reinterpret_cast<float*>(ws.mean + o);
+  const float* rows = det + o * 8;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  // 1. the leaders in row order: group g
+  const int G = ballot_compact<32>(n, [&](int i) { return (int)(group[i] == i); }, [&](int i, int slot) { lead[slot] = i; });
+  // 2. one warp per group: lane c < 4 sums coordinate c over the members in row order, ((b0 + b1) + b2) + ..., in float32
+  for (int g = wid; g < G; g += nwarps) {
+    const int L = lead[g];
+    float s = lane < 4 ? rows[(size_t)L * 8 + lane] : 0.0f;
+    int count = 1;
+    for (int base = L + 1; base < n; base += 32) {
+      const int i = base + lane;
+      unsigned bal = __ballot_sync(0xffffffffu, i < n && group[i] == L);
+      count += __popc(bal);
+      if (lane < 4)
+        while (bal) {
+          const int b = __ffs(bal) - 1;
+          bal &= bal - 1;
+          s = __fadd_rn(s, rows[(size_t)(base + b) * 8 + lane]);
+        }
+      __syncwarp();
+    }
+    if (lane < 4) mean[(size_t)g * 4 + lane] = __fdiv_rn(s, (float)count);
+    if (lane == 0) members[g] = count;
+  }
+  __syncthreads();
+  // 3. dict keys: groups with bit-equal means share one (str of a float32 round-trips)
+  const uint4* mbits = reinterpret_cast<const uint4*>(mean);
+  auto same = [](uint4 a, uint4 b) { return a.x == b.x && a.y == b.y && a.z == b.z && a.w == b.w; };
+  for (int g = threadIdx.x; g < G; g += blockDim.x) {
+    const uint4 m = mbits[g];
+    int f = g, l = g;
+    for (int h = 0; h < g; ++h)
+      if (same(mbits[h], m)) { f = h; break; }
+    for (int h = G - 1; h > g; --h)
+      if (same(mbits[h], m)) { l = h; break; }
+    first[g] = f;
+    last[g] = l;
+  }
+  __syncthreads();
+  // 4. keys in dict order (the first group of each), with their mean box
+  const int K = ballot_compact<32>(G, [&](int g) { return (int)(first[g] == g); }, [&](int g, int k) {
+    key[g] = k;
+    reinterpret_cast<float4*>(mbox)[o + k] = reinterpret_cast<const float4*>(mean)[g];
+  });
+  // 5. write order: each key's rows are its last group's members
+  const int P = block_scan<32>(G, [&](int g) { return first[g] == g ? members[last[g]] : 0; },
+                               [&](int g, int off) { offset[g] = off; });
+  for (int g = wid; g < G; g += nwarps) {
+    if (last[g] != g) continue;   // warp-uniform
+    const int L = lead[g], k = key[first[g]];
+    int* out = pairs + (o + offset[first[g]]) * 2;
+    if (lane == 0) { out[0] = L; out[1] = k; }
+    int r = 1;
+    for (int base = L + 1; base < n; base += 32) {
+      const int i = base + lane;
+      const bool mine = i < n && group[i] == L;
+      const unsigned bal = __ballot_sync(0xffffffffu, mine);
+      if (mine) {
+        const int at = r + __popc(bal & ((1u << lane) - 1));
+        out[at * 2] = i;
+        out[at * 2 + 1] = k;
+      }
+      r += __popc(bal);
+    }
+  }
+  if (threadIdx.x == 0) { mcount[z * 2] = K; mcount[z * 2 + 1] = P; }
+}
+
 static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 }  // namespace step
@@ -392,15 +612,17 @@ extern "C" int step_nms_f32(const float* boxes, const float* scores, int n, floa
 
   nms_rank_kernel<<<ceil_div(n, 256), 256, 0, s>>>(boxes, scores, n, sorted, order);
   STEP_LAUNCH_CHECK("nms_rank_kernel");
-  nms_mask_kernel<<<dim3(cb, cb), kTile, 0, s>>>(sorted, n, thr, ge, cb, mask);
-  STEP_LAUNCH_CHECK("nms_mask_kernel");
+  const SortedRows rows{sorted, n};
+  mask_tiles_kernel<<<dim3(cb, cb), kTile, 0, s>>>(rows, NmsPred{thr, ge}, cb, 0, mask);
+  STEP_LAUNCH_CHECK("mask_tiles_kernel");
   size_t smem = (size_t)cb * sizeof(unsigned long long);
+  auto resolve = resolve_kernel<SortedRows, KeepByOrder, NoClaim>;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(nms_resolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(resolve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return fail((int)e, "step_nms_f32: smem attr: %s", cudaGetErrorString(e));
   }
-  nms_resolve_kernel<<<1, 1024, smem, s>>>(mask, order, n, cb, flag);
-  STEP_LAUNCH_CHECK("nms_resolve_kernel");
+  resolve<<<1, 1024, smem, s>>>(mask, rows, cb, 0, KeepByOrder{order, flag}, NoClaim{});
+  STEP_LAUNCH_CHECK("resolve_kernel");
   nms_compact_kernel<<<1, 1024, 0, s>>>(flag, n, keep_out, n_keep);
   STEP_LAUNCH_CHECK("nms_compact_kernel");
   return 0;
@@ -464,5 +686,48 @@ extern "C" int step_detect_scores_f32(const float* prob, int prob_ld, const floa
   detect_scores_kernel<<<n_clips, 256, 0, cu(stream)>>>(prob, prob_ld, box, box_ld, clip_offsets, ncls, conf_thresh, norm_w,
                                                         norm_h, cap, det, det_count);
   STEP_LAUNCH_CHECK("detect_scores_kernel");
+  return 0;
+}
+
+// Workspace of step_detect_merge_f32, per clip: the bitmask (cap rows of ceil(cap/64) words), then MergeScratch.
+static size_t merge_mask_bytes(int cap) { return align256((size_t)cap * ceil_div(cap, kTile) * sizeof(unsigned long long)); }
+static size_t merge_ints_bytes(int n_clips, int cap) { return align256((size_t)n_clips * cap * sizeof(int)); }
+
+extern "C" size_t step_detect_merge_workspace_bytes(int n_clips, int cap) {
+  if (n_clips <= 0 || cap <= 0) return 256;
+  return (size_t)n_clips * merge_mask_bytes(cap) + 7 * merge_ints_bytes(n_clips, cap) +
+         align256((size_t)n_clips * cap * sizeof(float4)) + 256;
+}
+
+extern "C" int step_detect_merge_max_rows(void) { return kMergeMaxRows; }
+
+extern "C" int step_detect_merge_f32(const float* det, const int* det_count, int n_clips, int cap, float thresh, float* mbox,
+                                     int* pairs, int* mcount, void* workspace, size_t ws_bytes, step_stream_t stream) {
+  STEP_CHECK_ARG(n_clips >= 0 && n_clips <= 65535, "step_detect_merge_f32: n_clips %d (0..65535)", n_clips);
+  STEP_CHECK_ARG(cap > 0 && cap <= kMergeMaxRows, "step_detect_merge_f32: cap %d (1..%d)", cap, kMergeMaxRows);
+  if (n_clips == 0) return 0;
+  STEP_CHECK_ARG(det && det_count && mbox && pairs && mcount && workspace, "step_detect_merge_f32: null pointer");
+  STEP_CHECK_ARG(((uintptr_t)det & 15) == 0 && ((uintptr_t)mbox & 15) == 0 && ((uintptr_t)workspace & 255) == 0,
+                 "step_detect_merge_f32: det / mbox must be 16-byte and the workspace 256-byte aligned");
+  const size_t need = step_detect_merge_workspace_bytes(n_clips, cap);
+  STEP_CHECK_ARG(ws_bytes >= need, "step_detect_merge_f32: workspace %zu < %zu bytes", ws_bytes, need);
+  char* w = (char*)workspace;
+  unsigned long long* mask = (unsigned long long*)w;
+  w += (size_t)n_clips * merge_mask_bytes(cap);
+  MergeScratch ms;
+  int** ints[7] = {&ms.group, &ms.lead, &ms.members, &ms.first, &ms.last, &ms.key, &ms.offset};
+  for (int k = 0; k < 7; ++k) { *ints[k] = (int*)w; w += merge_ints_bytes(n_clips, cap); }
+  ms.mean = (float4*)w;
+  const int cb = ceil_div(cap, kTile);
+  const size_t stride = merge_mask_bytes(cap) / sizeof(unsigned long long);
+  const DetRows rows{det, det_count, cap};
+  cudaStream_t s = cu(stream);
+  mask_tiles_kernel<<<dim3(cb, cb, n_clips), kTile, 0, s>>>(rows, MergePred{thresh}, cb, stride, mask);
+  STEP_LAUNCH_CHECK("mask_tiles_kernel");
+  resolve_kernel<<<n_clips, 1024, (size_t)cb * sizeof(unsigned long long), s>>>(mask, rows, cb, stride, GroupKeep{ms.group, cap},
+                                                                               GroupClaim{ms.group, cap});
+  STEP_LAUNCH_CHECK("resolve_kernel");
+  merge_groups_kernel<<<n_clips, 1024, 0, s>>>(det, det_count, cap, ms, mbox, pairs, mcount);
+  STEP_LAUNCH_CHECK("merge_groups_kernel");
   return 0;
 }

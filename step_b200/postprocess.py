@@ -1,11 +1,15 @@
 """Detection post-processing on the device: the per-clip x per-class loop of the reference drivers
-(test.py:156-218, demo.py:121-198 -- B*60*max_iter tiny CPU NMS calls per batch) as TWO launches of libstep_b200
+(test.py:156-218, demo.py:140-174 -- B*60*max_iter tiny CPU NMS calls per batch) as TWO launches of libstep_b200
 (`step_detect_f32`), with no torch arithmetic, no gather tensors and no synchronisation: CUDA-graph capturable.
 
 For every (clip, class): keep tubes whose centre-frame score > conf_thresh, clamp their centre-frame box
 with valid_tubes (the drivers call it with its 400x400 defaults, test.py:191), run greedy NMS
 (cpu/nms_cpu.cpp semantics, bit-exact), normalise by (width, height), then per clip either every survivor in
 file order or the top-k scores in the order of the reference's tuple sort (test.py:205-208).
+
+demo.py then merges the overlapping detections across classes (demo.py:176-198): `Merger` does that on the device in
+three more launches (`step_detect_merge_f32`), and `merged_results` / `result_lines` turn one read-back of its result
+into the reference's `merged_result` dicts and results.txt lines (demo.py:200-217).
 """
 import numpy as np
 import torch
@@ -130,3 +134,71 @@ def to_lists(det, n_clips=None):
     for b in range(len(det["tubes_nums"]) if n_clips is None else n_clips):
         out.append([(rows[b, k, :4].copy(), int(rows[b, k, 5]), float(rows[b, k, 4])) for k in range(int(cnt[b]))])
     return out
+
+
+class Merger:
+    """The cross-class merge of demo.py:176-198 on a Detector's rows, with pre-allocated outputs, so `run` only launches
+    (what StepRunner captures).  Per clip, a row not yet taken leads a group and takes every later row not yet taken whose
+    compute_box_iou with it is > global_thresh (float32); each group's box is its members' np.mean.  run(det) returns
+      mbox [B, cap, 4]   the merged boxes in the order of the reference's dict;
+      pairs [B, cap, 2]  int32 (det row, key index) in the order results.txt lists them;
+      count [B, 2]       int32 (keys, pairs) of each clip."""
+
+    def __init__(self, detector, global_thresh):
+        self.detector = detector
+        self.B, self.cap, self.thr = detector.B, detector.cap, float(global_thresh)
+        if self.cap > L.lib().step_detect_merge_max_rows():
+            raise RuntimeError("merge: %d rows per clip exceed the %d-row merge" % (self.cap, L.lib().step_detect_merge_max_rows()))
+        dev, nb = detector.det.device, max(self.B, 1)
+        self.mbox = torch.zeros((nb, self.cap, 4), dtype=torch.float32, device=dev)
+        self.pairs = torch.zeros((nb, self.cap, 2), dtype=torch.int32, device=dev)
+        self.count = torch.zeros((nb, 2), dtype=torch.int32, device=dev)
+        self.ws = torch.empty((L.lib().step_detect_merge_workspace_bytes(self.B, self.cap),), dtype=torch.uint8, device=dev)
+        # host mirrors of the outputs and of the detector's rows: the materialisers read them back with one synchronisation
+        self.host = [torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
+                     for t in (self.mbox, self.pairs, self.count, detector.det)]
+
+    def run(self, det):
+        """det: the dict Detector.run returned (its det / count are read in place)."""
+        d, c = det["det"], det["count"]
+        if d.data_ptr() != self.detector.det.data_ptr() or c.data_ptr() != self.detector.count.data_ptr():
+            raise RuntimeError("merge: det is not the result of this Merger's Detector")
+        if self.B:
+            with torch.cuda.device(d.device):
+                L.check(L.lib().step_detect_merge_f32(L.ptr(d), L.ptr(c), self.B, self.cap, self.thr, L.ptr(self.mbox),
+                                                      L.ptr(self.pairs), L.ptr(self.count), L.ptr(self.ws), self.ws.numel(),
+                                                      L.stream(d.device)))
+        return {"mbox": self.mbox, "pairs": self.pairs, "count": self.count, "host": self.host, "tubes_nums": det["tubes_nums"]}
+
+
+def merged_results(merged, det, label_dict):
+    """Per clip, demo.py:177-198's `merged_result`: {mean box string: [(label, score), ...]} with the reference's keys,
+    lists and dict order (np.float32 scores), as overlay_image takes it.  One read-back of the merge and the detector's
+    rows (one synchronisation).  merged: Merger.run's result; det: the Detector.run result it was run on."""
+    host = merged["host"]
+    for h, t in zip(host, (merged["mbox"], merged["pairs"], merged["count"], det["det"])):
+        h.copy_(t, non_blocking=True)
+    torch.cuda.current_stream(merged["mbox"].device).synchronize()
+    mbox, pairs, count, rows = (h.numpy() for h in host)
+    out = []
+    for b in range(len(merged["tubes_nums"])):
+        n_keys, n_pairs = int(count[b, 0]), int(count[b, 1])
+        keys = [",".join(mbox[b, k].astype(str).tolist()) for k in range(n_keys)]     # demo.py:197
+        result = {k: [] for k in keys}
+        for r, k in pairs[b, :n_pairs].tolist():
+            result[keys[k]].append((label_dict[int(rows[b, r, 5])], rows[b, r, 4]))
+        out.append(result)
+    return out
+
+
+def result_lines(results, infos):
+    """demo.py:209-217: the results.txt lines (newline included) of the clips of one batch, from merged_results' dicts
+    and the loader's infos (video_name, fid)."""
+    lines = []
+    for result, info in zip(results, infos):
+        for key in result:
+            box = np.asarray(key.split(","), dtype=np.float32)
+            for l, s in result[key]:
+                lines.append("{0},{1:04},{2:.4},{3:.4},{4:.4},{5:.4},{6},{7:.4}\n".format(
+                    info["video_name"], info["fid"], box[0], box[1], box[2], box[3], l, s))
+    return lines

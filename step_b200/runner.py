@@ -16,7 +16,7 @@ import torch
 from . import _lib as L
 from . import engine as E
 from .inference import inference_device, stage_tubes
-from .postprocess import Detector
+from .postprocess import Detector, Merger
 from .transforms import frame_entry, frame_table
 
 
@@ -46,10 +46,14 @@ class StepRunner:
         self.history = None
         self.detections = None
         self.detectors = {}
+        self.merged = None
+        self.mergers = {}
         if detect is not None:
             for i in detect.get("steps", [cfg.max_iter - 1]):
                 self.detectors[i] = Detector(self.tubes_nums, cfg.num_classes, self.device, detect["conf_thresh"],
                                              detect["nms_thresh"], W, H, topk=detect.get("topk", 0))
+                if detect.get("merge") is not None:
+                    self.mergers[i] = Merger(self.detectors[i], detect["merge"])
         if not use_graph:
             return
         side = torch.cuda.Stream(device=self.device)
@@ -74,6 +78,8 @@ class StepRunner:
                                        self.clip_of_tube, self.tubes_nums)
             if self.detectors:
                 self.detections = {i: d.run(hist[i]["pred_prob"], hist[i]["pred_loc"]) for i, d in self.detectors.items()}
+            if self.mergers:
+                self.merged = {i: m.run(self.detections[i]) for i, m in self.mergers.items()}
         return hist
 
     def __call__(self, clips=None):
