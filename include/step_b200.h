@@ -343,6 +343,20 @@ int step_head_losses_f32(const float* logits, const float* local_loc, const floa
  * loss_cls and dlogits are zeros (the reference returns a [1] zero loss). */
 int step_cls_loss_f32(const float* logits, const float* targets, int N, int cls, float* loss_cls, int* flags, float* dlogits,
                       step_stream_t stream);
+/* The autograd of TwoBranchNet's tail (models/two_branch.py:272-342) from upstream gradients of its seven outputs
+ * (prob, local_loc, first_loc, last_loc, loss_cls, loss_loc, loss_nb) back to the pre-sigmoid logits, local_reg's output
+ * (dloc [N,T_len,4]) and the outputs of neighbor_reg1 / neighbor_reg2 (dfirst / dlast [N,Tc,4], the whole gradient of
+ * first_loc / last_loc, which dloc's slices receive too).  Operands as step_head_losses_f32's.  Every upstream gradient
+ * is nullable (NULL = zero): g_prob [N,cls], g_local_loc [N,T_len,4], g_first / g_last [N,Tc,4], g_loss_cls [N*cls],
+ * g_loss_loc / g_loss_nb [1].  A loss whose mask sums to zero was a constant in the forward: its upstream gradient is
+ * not read (decided on the device, no host synchronisation).  cls_only != 0: class-only heads; only logits, targets,
+ * g_prob, g_loss_cls and dlogits are used (the other pointers may be NULL, T_len / T / Tc are ignored).
+ * Deterministic, no atomics. */
+int step_head_outputs_bwd_f32(const float* logits, const float* local_loc, const float* first_loc, const float* last_loc,
+                              const float* tubes, const float* targets, int N, int cls, int T_len, int T, int Tc, int cls_only,
+                              const float* g_prob, const float* g_local_loc, const float* g_first, const float* g_last,
+                              const float* g_loss_cls, const float* g_loss_loc, const float* g_loss_nb, float* dlogits,
+                              float* dloc, float* dfirst, float* dlast, step_stream_t stream);
 /* Channels-last ROIAlign backward without atomics (replaces _C.roi_align_backward, vision.cpp:33 /
  * cuda/ROIAlign_cuda.cu:201-278, whose atomicAdd scatter is not repeatable): grad_out [R,ph,pw,C] (channel stride
  * out_ld, STEP_F32 / STEP_F16) -> grad_in [K,H,W,C] fp32 (channel stride in_ld), written completely by the call. */

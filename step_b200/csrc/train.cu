@@ -5,6 +5,8 @@
 //   * cls_loss_kernel          the loss of class-only heads (TwoBranchNet(cls_only=True), the first training stage of
 //                              train_cls.py) and d mean(loss_cls) / d logits, with the classification arithmetic of
 //                              head_losses_kernel (one shared device function);
+//   * head_outputs_bwd_kernel  the autograd of the head's tail (two_branch.py:272-342) from upstream gradients of its
+//                              seven outputs, with the loss arithmetic of head_losses_kernel (shared device functions);
 //   * roi_align_bwd_nhwc       channels-last ROIAlign backward WITHOUT float atomics: every feature pixel gathers its
 //                              contributions in a fixed order (ROI index, bin, sample), so the result is bit-for-bit
 //                              repeatable -- the reference's RoIAlignBackwardFeature (cuda/ROIAlign_cuda.cu:201-278) scatters
@@ -49,6 +51,8 @@ __device__ __forceinline__ float cls_mask_sum(const float* __restrict__ targets,
   return mc;
 }
 
+__device__ __forceinline__ float sigmoid_f32(float x) { return 1.0f / (1.0f + expf(-x)); }
+
 // Classification loss of the centre chunk (two_branch.py:291-297) over the [N, cls] logits, block-strided: BCE with logits
 // against the labels masked by the centre row's classification flag, and d mean(loss_cls) / d logit.  Without any
 // classification sample (has_cls false) both are zero.  Shared by head_losses_kernel and cls_loss_kernel so that the two
@@ -66,7 +70,7 @@ __device__ __forceinline__ void cls_loss_pass(const float* __restrict__ logits, 
       // ATen: (1 - t) * x - log_sigmoid(x),  log_sigmoid(x) = min(x, 0) - log1p(exp(-|x|))
       const float ls = __fsub_rn(fminf(x, 0.0f), log1pf(expf(-fabsf(x))));
       l = __fsub_rn(__fmul_rn(__fsub_rn(1.0f, t), x), ls);
-      const float sg = 1.0f / (1.0f + expf(-x));
+      const float sg = sigmoid_f32(x);
       gx = __fmul_rn(__fsub_rn(sg, t), inv_ncls);              // d mean(loss_cls) / d logit
     }
     loss_cls[i] = l;
@@ -82,6 +86,44 @@ struct LossGeom {
   float w_loc, w_nb;         // lambda_reg, lambda_neighbor (train.py:335-336)
 };
 
+// The three mask sums in tube order (two_branch.py:291-293, 307-309, 325-328): s[0] classification (centre rows), s[1]
+// the centre rows' regression mask repeated over the 4 coordinates, s[2] the first rows' then the last rows' likewise.
+// One thread.
+__device__ __forceinline__ void loss_mask_sums(const float* __restrict__ targets, int N, int tgt_ld, float* s) {
+  auto tgt = [&](int n, int j) { return targets + ((size_t)n * 3 + j) * tgt_ld; };
+  const float mc = cls_mask_sum(targets, N, tgt_ld);
+  float ml = 0.0f, mn = 0.0f;
+  for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) ml = __fadd_rn(ml, tgt(n, 1)[5]);
+  for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) mn = __fadd_rn(mn, tgt(n, 0)[5]);
+  for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) mn = __fadd_rn(mn, tgt(n, 2)[5]);
+  s[0] = mc; s[1] = ml; s[2] = mn;
+}
+
+// Regression term r of tube n (two_branch.py:299-333): r = 0 the centre prediction local_loc[n, centre], r = 1 / 2 the
+// neighbour predictions first_loc / last_loc[n, half_T], against encode_coef of the box of target row 1 / 0 / 2 on the
+// tube's box at frame centre / first_idx / last_idx.  `pred` points at the prediction's 4 coordinates
+// (reg_pred, at reg_offset of its tensor).
+// Writes the residuals pred - target and returns the row's regression mask (column 5).
+__device__ __forceinline__ size_t reg_offset(const LossGeom& g, int r, int n) {
+  return r == 0 ? ((size_t)n * g.T_len + g.centre) * 4 : ((size_t)n * g.Tc + g.half_T) * 4;
+}
+
+__device__ __forceinline__ const float* reg_pred(const LossGeom& g, int r, int n, const float* local_loc, const float* first_loc,
+                                                 const float* last_loc) {
+  return (r == 0 ? local_loc : (r == 1 ? first_loc : last_loc)) + reg_offset(g, r, n);
+}
+
+__device__ __forceinline__ float reg_residual(const LossGeom& g, int r, int n, const float* pred, const float* __restrict__ tubes,
+                                              const float* __restrict__ targets, float* d) {
+  const int row = r == 0 ? 1 : (r == 1 ? 0 : 2);
+  const int frame = r == 0 ? g.centre : (r == 1 ? g.first_idx : g.last_idx);
+  const float* tg = targets + ((size_t)n * 3 + row) * g.tgt_ld;
+  float enc[4];
+  st4(enc, encode_one(ld4(tg), ld4(tubes + ((size_t)n * g.T_len + frame) * 5 + 1)));
+  for (int k = 0; k < 4; ++k) d[k] = __fsub_rn(pred[k], enc[k]);
+  return tg[5];
+}
+
 // One CTA.  Sums are taken in tube order by one thread after a block-wide staging pass: N is a few hundred at most and
 // this keeps the reductions bit-for-bit repeatable.
 __global__ void __launch_bounds__(256) head_losses_kernel(LossGeom g, const float* __restrict__ logits,
@@ -95,16 +137,9 @@ __global__ void __launch_bounds__(256) head_losses_kernel(LossGeom g, const floa
   __shared__ float s_sum[3];   // sum of cls mask, loc mask x4, neighbour mask x4
   __shared__ float s_loss[2];
   const int N = g.N;
-  // targets[n][j] with j = 0 first, 1 centre, 2 last (two_branch.py:283-285: [:, 0], [:, 1], [:, -1])
-  auto tgt = [&](int n, int j) { return targets + ((size_t)n * 3 + j) * g.tgt_ld; };
   if (threadIdx.x == 0) {
-    const float mc = cls_mask_sum(targets, N, g.tgt_ld);
-    float ml = 0.0f, mn = 0.0f;
-    for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) ml = __fadd_rn(ml, tgt(n, 1)[5]);
-    for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) mn = __fadd_rn(mn, tgt(n, 0)[5]);
-    for (int n = 0; n < N; ++n) for (int k = 0; k < 4; ++k) mn = __fadd_rn(mn, tgt(n, 2)[5]);
-    s_sum[0] = mc; s_sum[1] = ml; s_sum[2] = mn;
-    flags[0] = mc != 0.0f; flags[1] = ml != 0.0f; flags[2] = mn != 0.0f;
+    loss_mask_sums(targets, N, g.tgt_ld, s_sum);
+    flags[0] = s_sum[0] != 0.0f; flags[1] = s_sum[1] != 0.0f; flags[2] = s_sum[2] != 0.0f;
   }
   __syncthreads();
   const bool has_cls = s_sum[0] != 0.0f, has_loc = s_sum[1] != 0.0f, has_nb = s_sum[2] != 0.0f;
@@ -115,29 +150,17 @@ __global__ void __launch_bounds__(256) head_losses_kernel(LossGeom g, const floa
   if (dfirst) for (int i = threadIdx.x; i < N * g.Tc * 4; i += blockDim.x) { dfirst[i] = 0.0f; dlast[i] = 0.0f; }
   __syncthreads();
   for (int n = threadIdx.x; n < N; n += blockDim.x) {
-    const float* tb = tubes + (size_t)n * g.T_len * 5;
-    float enc[4], gr;
-    // centre (two_branch.py:301-311)
-    st4(enc, encode_one(ld4(tgt(n, 1)), ld4(tb + (size_t)g.centre * 5 + 1)));
-    const float mloc = tgt(n, 1)[5];
-    for (int k = 0; k < 4; ++k) {
-      const float d = __fsub_rn(local_loc[((size_t)n * g.T_len + g.centre) * 4 + k], enc[k]);
-      const float l = smooth_l1(d, &gr);
-      scratch[((size_t)n * 3 + 0) * 4 + k] = __fmul_rn(l, mloc);
-      if (dloc && has_loc) dloc[((size_t)n * g.T_len + g.centre) * 4 + k] = __fdiv_rn(__fmul_rn(__fmul_rn(gr, mloc), g.w_loc), s_sum[1]);
-    }
-    // neighbours (two_branch.py:315-333): first then last
-    for (int j = 0; j < 2; ++j) {
-      const int tj = j == 0 ? 0 : 2, idx = j == 0 ? g.first_idx : g.last_idx;
-      const float* pred = (j == 0 ? first_loc : last_loc) + ((size_t)n * g.Tc + g.half_T) * 4;
-      float* dpred = (j == 0 ? dfirst : dlast);
-      st4(enc, encode_one(ld4(tgt(n, tj)), ld4(tb + (size_t)idx * 5 + 1)));
-      const float m = tgt(n, tj)[5];
+    // centre (two_branch.py:301-311), then the neighbours (two_branch.py:315-333): first then last
+    for (int r = 0; r < 3; ++r) {
+      float d[4], gr;
+      const float m = reg_residual(g, r, n, reg_pred(g, r, n, local_loc, first_loc, last_loc), tubes, targets, d);
+      float* dpred = r == 0 ? dloc : (r == 1 ? dfirst : dlast);
+      const bool has = r == 0 ? has_loc : has_nb;
+      const float w = r == 0 ? g.w_loc : g.w_nb, msum = s_sum[r == 0 ? 1 : 2];
       for (int k = 0; k < 4; ++k) {
-        const float d = __fsub_rn(pred[k], enc[k]);
-        const float l = smooth_l1(d, &gr);
-        scratch[((size_t)n * 3 + 1 + j) * 4 + k] = __fmul_rn(l, m);
-        if (dpred && has_nb) dpred[((size_t)n * g.Tc + g.half_T) * 4 + k] = __fdiv_rn(__fmul_rn(__fmul_rn(gr, m), g.w_nb), s_sum[2]);
+        const float l = smooth_l1(d[k], &gr);
+        scratch[((size_t)n * 3 + r) * 4 + k] = __fmul_rn(l, m);
+        if (dpred && has) dpred[reg_offset(g, r, n) + k] = __fdiv_rn(__fmul_rn(__fmul_rn(gr, m), w), msum);
       }
     }
   }
@@ -179,6 +202,83 @@ __global__ void __launch_bounds__(256) cls_loss_kernel(int N, int cls, const flo
   }
   __syncthreads();
   cls_loss_pass(logits, targets, N, cls, 6 + cls, s_mc != 0.0f, loss_cls, dlogits);
+}
+
+// Upstream gradients of the head's seven outputs (TwoBranchNet.forward with targets); nullptr stands for zero.
+struct HeadOutGrads {
+  const float* prob;       // [N, cls]
+  const float* local_loc;  // [N, T_len, 4]
+  const float* first;      // [N, Tc, 4]
+  const float* last;       // [N, Tc, 4]
+  const float* loss_cls;   // [N * cls]; ignored when the forward returned the [1] zero (no classification mask)
+  const float* loss_loc;   // [1]; ignored when the centre regression mask sums to zero
+  const float* loss_nb;    // [1]; ignored when the neighbour regression mask sums to zero
+};
+
+// The autograd of two_branch.py:272-342 from the head's outputs back to the class scores, local_reg's output and the two
+// neighbour regressors' outputs, for any upstream gradients.  One CTA, no atomics: every output element is written by one
+// thread in a fixed order.  The operand order of each product follows torch's backward formulas: sigmoid
+// g * (1 - p) * p, BCE-with-logits (sigmoid(x) - target) * g, the masked means' (g / sum(mask)) * mask, smooth-L1's x * g
+// or sign(x) * g.  first_loc / last_loc are clones of local_loc's slices [s0, s0 + Tc) / [e0, e0 + Tc) plus the neighbour
+// regressors (two_branch.py:265-270): their whole gradient is dfirst / dlast and is added into dloc's slices as well.
+__global__ void __launch_bounds__(256) head_outputs_bwd_kernel(LossGeom g, int cls_only, const float* __restrict__ logits,
+                                                               const float* __restrict__ local_loc, const float* __restrict__ first_loc,
+                                                               const float* __restrict__ last_loc, const float* __restrict__ tubes,
+                                                               const float* __restrict__ targets, HeadOutGrads up,
+                                                               float* __restrict__ dlogits, float* __restrict__ dloc,
+                                                               float* __restrict__ dfirst, float* __restrict__ dlast) {
+  __shared__ float s_sum[3];
+  const int N = g.N;
+  if (threadIdx.x == 0) loss_mask_sums(targets, N, g.tgt_ld, s_sum);
+  __syncthreads();
+  // the reference's host-side `if mask.sum():` branches (two_branch.py:293, 309, 330), as device flags
+  const bool use_cls = s_sum[0] != 0.0f && up.loss_cls != nullptr;
+  const bool use_loc = !cls_only && s_sum[1] != 0.0f && up.loss_loc != nullptr;
+  const bool use_nb = !cls_only && s_sum[2] != 0.0f && up.loss_nb != nullptr;
+  for (int i = threadIdx.x; i < N * g.cls; i += blockDim.x) {
+    const int n = i / g.cls, c = i - n * g.cls;
+    const float p = sigmoid_f32(logits[i]);
+    float gx = 0.0f;
+    if (up.prob) gx = __fmul_rn(__fmul_rn(up.prob[i], __fsub_rn(1.0f, p)), p);
+    if (use_cls) {
+      const float* tc = targets + ((size_t)n * 3 + 1) * g.tgt_ld;
+      const float t = __fmul_rn(tc[6 + c], tc[4]);
+      gx = __fadd_rn(gx, __fmul_rn(__fsub_rn(p, t), up.loss_cls[i]));
+    }
+    dlogits[i] = gx;
+  }
+  if (cls_only) return;
+  for (int i = threadIdx.x; i < N * g.T_len * 4; i += blockDim.x) dloc[i] = up.local_loc ? up.local_loc[i] : 0.0f;
+  for (int i = threadIdx.x; i < N * g.Tc * 4; i += blockDim.x) {
+    dfirst[i] = up.first ? up.first[i] : 0.0f;
+    dlast[i] = up.last ? up.last[i] : 0.0f;
+  }
+  __syncthreads();
+  const float c_loc = use_loc ? __fdiv_rn(up.loss_loc[0], s_sum[1]) : 0.0f;
+  const float c_nb = use_nb ? __fdiv_rn(up.loss_nb[0], s_sum[2]) : 0.0f;
+  for (int n = threadIdx.x; n < N; n += blockDim.x) {
+    for (int r = 0; r < 3; ++r) {
+      if (!(r == 0 ? use_loc : use_nb)) continue;
+      float d[4], gr;
+      const float m = reg_residual(g, r, n, reg_pred(g, r, n, local_loc, first_loc, last_loc), tubes, targets, d);
+      const float b = __fmul_rn(r == 0 ? c_loc : c_nb, m);
+      float* dpred = (r == 0 ? dloc : (r == 1 ? dfirst : dlast)) + reg_offset(g, r, n);
+      for (int k = 0; k < 4; ++k) {
+        smooth_l1(d[k], &gr);
+        dpred[k] = __fadd_rn(dpred[k], __fmul_rn(gr, b));
+      }
+    }
+  }
+  __syncthreads();
+  // the slices: element (n, r) of dfirst / dlast belongs to this thread alone, and the ranges [s0, s0 + Tc) and
+  // [e0, e0 + Tc) of dloc are identical (one chunk) or disjoint, so the updates never race and their order is fixed
+  for (int i = threadIdx.x; i < N * g.Tc * 4; i += blockDim.x) {
+    const int n = i / (g.Tc * 4), r = i - n * g.Tc * 4;
+    float* a = dloc + ((size_t)n * g.T_len + g.s0) * 4 + r;
+    *a = __fadd_rn(*a, dfirst[i]);
+    float* b = dloc + ((size_t)n * g.T_len + g.e0) * 4 + r;
+    *b = __fadd_rn(*b, dlast[i]);
+  }
 }
 
 // ---- ROIAlign backward, channels-last, deterministic ----------------------------------------------------------------
@@ -959,24 +1059,57 @@ inline WfPlan wgrad_f32_plan(long long M, int Cout, long long cols) {
 
 using namespace step;
 
+// The head's chunk geometry (two_branch.py:226-228, 265-266) for N tubes of T_len frames in chunks of T, Tc = frames of
+// first_loc / last_loc (python slice clipping); STEP_E_ARG naming `who` when it does not fit.
+static int loss_geom(const char* who, int N, int cls, int T_len, int T, int Tc, float w_loc, float w_nb, LossGeom* out) {
+  STEP_CHECK_ARG(N > 0 && cls > 0 && T > 0 && T_len >= T && T_len % T == 0, "%s: bad shape N=%d cls=%d T'=%d T=%d", who, N, cls,
+                 T_len, T);
+  LossGeom g;
+  const int chunks = T_len / T;
+  g.N = N; g.cls = cls; g.T_len = T_len; g.Tc = Tc; g.half_T = T / 2;
+  g.first_idx = T / 2; g.last_idx = (chunks - 1) * T + T / 2; g.centre = (chunks / 2) * T + T / 2;
+  g.s0 = g.first_idx - g.half_T; g.e0 = g.last_idx - g.half_T;
+  g.tgt_ld = 6 + cls; g.w_loc = w_loc; g.w_nb = w_nb;
+  STEP_CHECK_ARG(Tc > g.half_T && g.s0 >= 0 && g.s0 + Tc <= T_len && g.e0 + Tc <= T_len, "%s: chunk slices out of range", who);
+  *out = g;
+  return 0;
+}
+
 extern "C" int step_head_losses_f32(const float* logits, const float* local_loc, const float* first_loc, const float* last_loc,
                                     const float* tubes, const float* targets, int N, int cls, int T_len, int T, int Tc, float w_loc,
                                     float w_nb, float* loss_cls, float* loss_loc, float* loss_nb, int* flags, float* dlogits,
                                     float* dloc, float* dfirst, float* dlast, float* scratch, step_stream_t stream) {
-  STEP_CHECK_ARG(N > 0 && cls > 0 && T > 0 && T_len >= T && T_len % T == 0, "head_losses: bad shape N=%d cls=%d T'=%d T=%d", N, cls, T_len, T);
+  LossGeom g;
+  if (int rc = loss_geom("head_losses", N, cls, T_len, T, Tc, w_loc, w_nb, &g)) return rc;
   STEP_CHECK_ARG(logits && local_loc && first_loc && last_loc && tubes && targets && loss_cls && loss_loc && loss_nb && flags && scratch,
                  "head_losses: null pointer");
   STEP_CHECK_ARG((dfirst == nullptr) == (dlast == nullptr), "head_losses: dfirst / dlast go together");
-  LossGeom g;
-  const int chunks = T_len / T;
-  g.N = N; g.cls = cls; g.T_len = T_len; g.Tc = Tc; g.half_T = T / 2;   // Tc = frames of first_loc / last_loc (python slice clipping)
-  g.first_idx = T / 2; g.last_idx = (chunks - 1) * T + T / 2; g.centre = (chunks / 2) * T + T / 2;   // two_branch.py:226-228
-  g.s0 = g.first_idx - g.half_T; g.e0 = g.last_idx - g.half_T;
-  g.tgt_ld = 6 + cls; g.w_loc = w_loc; g.w_nb = w_nb;
-  STEP_CHECK_ARG(Tc > g.half_T && g.s0 >= 0 && g.s0 + Tc <= T_len && g.e0 + Tc <= T_len, "head_losses: chunk slices out of range");
   head_losses_kernel<<<1, 256, 0, cu(stream)>>>(g, logits, local_loc, first_loc, last_loc, tubes, targets, loss_cls, loss_loc, loss_nb,
                                                 flags, dlogits, dloc, dfirst, dlast, scratch);
   STEP_LAUNCH_CHECK("head_losses_kernel");
+  return 0;
+}
+
+extern "C" int step_head_outputs_bwd_f32(const float* logits, const float* local_loc, const float* first_loc,
+                                         const float* last_loc, const float* tubes, const float* targets, int N, int cls, int T_len,
+                                         int T, int Tc, int cls_only, const float* g_prob, const float* g_local_loc,
+                                         const float* g_first, const float* g_last, const float* g_loss_cls, const float* g_loss_loc,
+                                         const float* g_loss_nb, float* dlogits, float* dloc, float* dfirst, float* dlast,
+                                         step_stream_t stream) {
+  LossGeom g{};
+  if (cls_only) {
+    STEP_CHECK_ARG(N > 0 && cls > 0, "head_outputs_bwd: bad shape N=%d cls=%d", N, cls);
+    g.N = N; g.cls = cls; g.tgt_ld = 6 + cls;
+  } else {
+    if (int rc = loss_geom("head_outputs_bwd", N, cls, T_len, T, Tc, 0.0f, 0.0f, &g)) return rc;
+    STEP_CHECK_ARG(local_loc && first_loc && last_loc && tubes && dloc && dfirst && dlast,
+                   "head_outputs_bwd: null pointer (regression operands of a full head)");
+  }
+  STEP_CHECK_ARG(logits && targets && dlogits, "head_outputs_bwd: null pointer");
+  HeadOutGrads up{g_prob, g_local_loc, g_first, g_last, g_loss_cls, g_loss_loc, g_loss_nb};
+  head_outputs_bwd_kernel<<<1, 256, 0, cu(stream)>>>(g, cls_only ? 1 : 0, logits, local_loc, first_loc, last_loc, tubes, targets, up,
+                                                     dlogits, dloc, dfirst, dlast);
+  STEP_LAUNCH_CHECK("head_outputs_bwd_kernel");
   return 0;
 }
 

@@ -136,9 +136,17 @@ class BaseNet(nn.Module):
         set_freeze_stats(self.base_model, self.freeze_stats)
 
     def forward(self, x):
-        """x [N,T,C,H,W] fp32 CUDA -> conv_feat [N,T/4,832,H/16,W/16] (logical view)."""
+        """x [N,T,C,H,W] fp32 CUDA -> conv_feat [N,T/4,832,H/16,W/16] (logical view).  With grad mode on and a trainable
+        parameter, conv_feat carries a grad_fn (step_b200.autograd.BaseNetFunction); the clip itself has no gradient."""
+        from . import autograd
         L.need_cuda(x)
+        if torch.is_grad_enabled() and x.requires_grad:
+            raise RuntimeError("BaseNet: the clip requires grad, but the trunk has no input gradient (its stride-2 stem "
+                               "forms only its weight gradient); pass the clip detached")
+        params = autograd.trainable(self)
         with torch.cuda.device(x.device):   # nn.DataParallel replicas (test.py:83) run on their own device + stream
+            if autograd.wanted(params):
+                return autograd.BaseNetFunction.apply(self, x, *params)
             return self.forward_act(x).logical()
 
     def forward_act(self, x):

@@ -8,8 +8,11 @@ tensor-core weight gradient of the convolutions, max-pool backward, the backward
 columns of `global_cls` (`head_forward_backward`), of ContextNet (`context_forward` / `context_backward`) and of the I3D
 trunk (`trunk_forward_backward`), the SGD update with the gradient all-reduce (`sgd_step`) and the whole step in spatial
 and temporal mode with or without the context branch (`train_step`), which can also update through the optimizers of
-`optim` with dynamic loss scaling.  `BaseNet` / `ContextNet` / `TwoBranchNet` still run
-without autograd (their outputs carry no grad_fn): the backward walks the tape their forward records.
+`optim` with dynamic loss scaling.  The backward walks the tape the modules' forward records; the trunk's, ContextNet's
+and the head's are split into forward and backward halves (trunk_forward / trunk_backward, context_forward /
+context_backward, head_forward / head_backward, with head_outputs_backward for any upstream gradients of the head's
+outputs), which train_step calls in order and the modules' torch.autograd Functions (step_b200/autograd.py) call from
+autograd's backward.
 Every piece runs on both precision paths of the modules (cfg.fp16): fp16 activations and activation gradients with the
 tensor-core weight gradient, or fp32 storage throughout (the reference's default precision) with the fp32 SIMT kernels and
 `conv_wgrad_f32`.  Weight gradients are fp32 on both.
@@ -557,11 +560,34 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
     the second (None without context).  With dropout the second form's ctx_grad is the gradient of each tube's dropped
     context mean, and ctx_dropout holds what `context_grad_reduce` needs to take it through the draw."""
     from . import engine as E
+    with torch.cuda.device(cat.device if cat is not None else global_feat.device), torch.no_grad():
+        fwd, state = head_forward(net, global_feat, tubes, targets, context_feat=context_feat, cat=cat, dropout=dropout)
+        prob, loc, first, last, logits = fwd["prob"], fwd["loc"], fwd["first"], fwd["last"], fwd["logits"]
+        dev = state["dev"]
+        if net.cls_only:
+            # class-only heads: the regression losses are the reference's zeros (two_branch.py:252,276-280)
+            lc, dlogits = cls_loss(logits, targets, want_grads=True)
+            ll, ln = torch.zeros((1,), dtype=torch.float32, device=dev), torch.zeros((1,), dtype=torch.float32, device=dev)
+            g = {"logits": dlogits}
+        else:
+            lc, ll, ln, g = head_losses(logits, loc, first, last, tubes, targets, net.T, lambda_reg, lambda_neighbor, want_grads=True)
+        if objective_scale != 1.0:
+            for k_ in g:
+                g[k_].mul_(objective_scale)
+        r = head_backward(state, g, loss_scale)
+    loss = lc.mean() + lambda_reg * ll.mean() + lambda_neighbor * ln.mean()
+    return dict(prob=prob, loc=loc, first=first, last=last, losses=(lc, ll, ln), loss=loss, **r)
+
+
+def head_forward(net, global_feat, tubes, targets, context_feat=None, cat=None, dropout=False):
+    """The forward half of head_forward_backward (same arguments): the head's forward with the tape on, and with
+    dropout=True the reference's draws when the head's nn.Dropout trains.  Returns (dict(prob, loc, first, last, logits),
+    state for head_backward).  The state holds none of the returned tensors."""
+    from . import engine as E
     from .engine import Act
     from .networks import to_act
     code = E.dtype_code(net.fp16)
     fc, ps = net.fc_dim, net.pool_size
-    D = fc * ps * ps
     if cat is None:
         dev = L.same_device(global_feat, tubes, targets)
         N, Tl, C, Wd, Hd = global_feat.shape
@@ -611,16 +637,24 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
         tape, keep = [], {}
         with E.recording(tape):
             prob, loc, first, last, logits = net.forward_act(cat, ctx_mean, row_map, want_logits=True, keep=keep, dropout=drop)
-        if net.cls_only:
-            # class-only heads: the regression losses are the reference's zeros (two_branch.py:252,276-280)
-            lc, dlogits = cls_loss(logits, targets, want_grads=True)
-            ll, ln = torch.zeros((1,), dtype=torch.float32, device=dev), torch.zeros((1,), dtype=torch.float32, device=dev)
-            g = {"logits": dlogits}
-        else:
-            lc, ll, ln, g = head_losses(logits, loc, first, last, tubes, targets, net.T, lambda_reg, lambda_neighbor, want_grads=True)
-        if objective_scale != 1.0:
-            for k_ in g:
-                g[k_].mul_(objective_scale)
+    state = dict(net=net, hw=hw, dev=dev, code=code, N=N, Tl=Tl, C=C, cat=cat, tape=tape, keep=keep, drop=drop, ctx_mean=ctx_mean,
+                 row_map=row_map, ctx_module_form=ctx_module_form, feat_grad=global_feat is not None)
+    return dict(prob=prob, loc=loc, first=first, last=last, logits=logits), state
+
+
+def head_backward(state, g, loss_scale=1024.0):
+    """The backward half of head_forward_backward from the gradients g of the head's tail outputs: fp32 g["logits"]
+    [N,cls] (pre-sigmoid), and for full heads g["local_loc"] [N,T',4] (local_reg's output, with what flows back through
+    the first / last slices already added) and g["first_loc"] / g["last_loc"] [N,Tc,4] (neighbor_reg1 / 2's outputs), each
+    d(loss)/d(output) unscaled: the activation gradients are scaled by loss_scale and the results unscaled again.
+    Returns dict(grads, feat_grad, roi_grad, ctx_grad, ctx_dropout) as head_forward_backward describes them."""
+    from .engine import Act
+    net, hw, dev, code = state["net"], state["hw"], state["dev"], state["code"]
+    N, Tl, C, cat, keep, drop = state["N"], state["Tl"], state["C"], state["cat"], state["keep"], state["drop"]
+    ctx_mean, row_map, ctx_module_form = state["ctx_mean"], state["row_map"], state["ctx_module_form"]
+    fc, ps = net.fc_dim, net.pool_size
+    D = fc * ps * ps
+    with torch.cuda.device(dev), torch.no_grad():
         grads = GradStore()
         out = {}
         unperm = lambda w: w.view(-1, ps * ps, fc).permute(0, 2, 1).reshape(w.shape[0], -1)   # (p*fc + c) -> (c*49 + p)
@@ -675,13 +709,51 @@ def head_forward_backward(net, global_feat, tubes, targets, context_feat=None, l
                 f32_accum = L.lib().step_f32_accum_f16 if code == L.F16 else L.lib().step_f32_accum_f32
                 L.check(f32_accum(L.ptr(dlf2), N * Tl * ps * ps, fc, float(loss_scale), L.c_void_p(glf2.data_ptr()), glf2.ld, L.stream()))
         # ---- every convolution and pool of the head, in reverse
-        out.update(tape_backward(tape, grads, loss_scale))
+        out.update(tape_backward(state["tape"], grads, loss_scale))
         gcat = grads.of(cat)
-        fg = gcat.buf[..., :C].float().mul_(1.0 / loss_scale).permute(0, 1, 4, 2, 3).contiguous() if global_feat is not None else None
-    loss = lc.mean() + lambda_reg * ll.mean() + lambda_neighbor * ln.mean()
+        fg = gcat.buf[..., :C].float().mul_(1.0 / loss_scale).permute(0, 1, 4, 2, 3).contiguous() if state["feat_grad"] else None
     ctx_dropout = (drop[0], ps * ps, fc) if drop is not None and ctx_mean is not None and not ctx_module_form else None
-    return dict(prob=prob, loc=loc, first=first, last=last, losses=(lc, ll, ln), loss=loss, grads=out, feat_grad=fg,
-                roi_grad=Act(gcat.buf, C, 0), ctx_grad=ctx_grad, ctx_dropout=ctx_dropout)
+    return dict(grads=out, feat_grad=fg, roi_grad=Act(gcat.buf, C, 0), ctx_grad=ctx_grad, ctx_dropout=ctx_dropout)
+
+
+def head_outputs_backward(logits, loc, first, last, tubes, targets, T, cls_only, g_prob=None, g_loc=None, g_first=None,
+                          g_last=None, g_loss_cls=None, g_loss_loc=None, g_loss_nb=None):
+    """The gradients of the head's tail (two_branch.py:272-342) from upstream gradients of its seven outputs
+    (step_head_outputs_bwd_f32; None = zero): returns head_backward's g, {"logits"} and for full heads also {"local_loc",
+    "first_loc", "last_loc"}.  logits [N,cls] (pre-sigmoid) and loc / first / last are the forward's; a loss whose mask
+    sums to zero was a constant there and its upstream gradient is not read (decided on the device)."""
+    dev = L.same_device(logits, targets)
+    f32 = lambda t: None if t is None else t.detach().to(device=dev, dtype=torch.float32).contiguous()
+    logits, targets = f32(logits), f32(targets)
+    N, cls = logits.shape
+    if targets.shape != (N, 3, 6 + cls):
+        raise RuntimeError("head_outputs_backward: targets %s do not match N=%d, classes=%d" % (tuple(targets.shape), N, cls))
+    ups = [f32(t) for t in (g_prob, g_loc, g_first, g_last, g_loss_cls, g_loss_loc, g_loss_nb)]
+    with torch.cuda.device(dev):
+        g = {"logits": torch.empty_like(logits)}
+        if cls_only:
+            loc = first = last = tubes = None
+            T_len = Tc = 0
+        else:
+            loc, first, last, tubes = f32(loc), f32(first), f32(last), f32(tubes)
+            T_len, Tc = loc.shape[1], first.shape[1]
+            if tubes.shape != (N, T_len, 5) or loc.shape != (N, T_len, 4) or first.shape != last.shape or first.shape != (N, Tc, 4):
+                raise RuntimeError("head_outputs_backward: local_loc %s / first %s / last %s / tubes %s do not match N=%d"
+                                   % (tuple(loc.shape), tuple(first.shape), tuple(last.shape), tuple(tubes.shape), N))
+            g.update(local_loc=torch.empty_like(loc), first_loc=torch.empty_like(first), last_loc=torch.empty_like(last))
+        expect = [(N, cls), (N, T_len, 4), (N, Tc, 4), (N, Tc, 4), (N * cls,), (1,), (1,)]
+        for i, (u, shape) in enumerate(zip(ups, expect)):
+            if u is None or (cls_only and i in (1, 2, 3, 5, 6)):
+                ups[i] = None
+            elif i == 4 and u.numel() != N * cls:
+                ups[i] = None       # the forward's [1] zero: no classification mask, the kernel reads nothing
+            elif tuple(u.shape) != shape and u.numel() != int(torch.Size(shape).numel()):
+                raise RuntimeError("head_outputs_backward: upstream gradient %d has shape %s, expected %s" % (i, tuple(u.shape), shape))
+        L.check(L.lib().step_head_outputs_bwd_f32(L.ptr(logits), L.ptr(loc), L.ptr(first), L.ptr(last), L.ptr(tubes), L.ptr(targets),
+                                                  N, cls, T_len, int(T), Tc, 1 if cls_only else 0, *[L.ptr(u) for u in ups],
+                                                  L.ptr(g["logits"]), L.ptr(g.get("local_loc")), L.ptr(g.get("first_loc")),
+                                                  L.ptr(g.get("last_loc")), L.stream()))
+    return g
 
 
 def context_forward(context_net, feat):
@@ -748,21 +820,36 @@ def trunk_forward_backward(base_net, clips, d_feat_fn, loss_scale=1024.0):
     Returns (feat Act, {parameter: fp32 gradient}): the conv weights, and the BatchNorms' gamma / beta where they require
     grad (freeze_affine=False, networks.py:136-142).  A base_net built with freeze_stats=False and in training mode normalises
     with batch statistics, and its forward updates the running statistics unless engine.running_stats_update(False) is on."""
+    with torch.cuda.device(clips.device), torch.no_grad():
+        feat, state = trunk_forward(base_net, clips)
+        out = trunk_backward(state, d_feat_fn(feat), loss_scale)
+    return feat, out
+
+
+def trunk_forward(base_net, clips):
+    """The forward half of trunk_forward_backward: base_net.forward_act(clips) with the tape on.  Returns (feat Act
+    [N,T',H',W',832], state for trunk_backward)."""
     from . import engine as E
-    dev = clips.device
-    with torch.cuda.device(dev), torch.no_grad():
+    with torch.cuda.device(clips.device), torch.no_grad():
         tape = []
         with E.recording(tape):
             feat = base_net.forward_act(clips)
+    return feat, dict(tape=tape, feat=feat)
+
+
+def trunk_backward(state, d_feat, loss_scale=1024.0):
+    """The backward half of trunk_forward_backward from d_feat = d(loss)/d(conv_feat), [N,T',H',W',832] channels-last (any
+    strides, any float dtype; made fp32 contiguous here).  Returns {parameter: fp32 gradient}."""
+    feat, tape = state["feat"], state["tape"]
+    with torch.cuda.device(feat.device), torch.no_grad():
         grads = GradStore()
         gfeat = grads.of(feat)
-        d = d_feat_fn(feat).to(torch.float32).contiguous()
+        d = d_feat.to(torch.float32).contiguous()
         M = feat.N * feat.T * feat.H * feat.W
         f32_accum = L.lib().step_f32_accum_f16 if feat.code == L.F16 else L.lib().step_f32_accum_f32
         L.check(f32_accum(L.ptr(d), M, feat.C, float(loss_scale), L.c_void_p(gfeat.data_ptr()), gfeat.ld, L.stream()))
         stem = tape[0]                                # the clip needs no gradient
-        out = tape_backward(tape, grads, loss_scale, need_input_grad=lambda e: e is not stem)
-    return feat, out
+        return tape_backward(tape, grads, loss_scale, need_input_grad=lambda e: e is not stem)
 
 
 def _average_gradients(params_and_grads, world_size):

@@ -4,10 +4,12 @@ state_dict keys (models/two_branch.py:113-373), running on libstep_b200.so.
 TwoBranchNet.forward(global_feat[R,T',832,7,7], context_feat=None|[R,1024,T',1,1], tubes, targets)
   -> (global_prob[R,cls], local_loc[R,T',4], first_loc[R,T,4], last_loc[R,T,4], loss x3)
 With targets=None the three losses are returned as zeros exactly as the reference does
-(two_branch.py:278-280, 338-340); with targets they are computed on the device (step_b200/training.py::head_losses,
-eval-mode dropout; heads built with cls_only=True compute the classification loss alone, training.cls_loss).  The outputs
-carry no grad_fn: the backward of the head (with or without the context columns) and of ContextNet runs explicitly on the
-forward's tape (step_b200/training.py: head_forward_backward, context_backward, train_step).
+(two_branch.py:278-280, 338-340); with targets they are computed on the device (step_b200/training.py::head_losses;
+heads built with cls_only=True compute the classification loss alone, training.cls_loss).
+With grad mode on and a trainable parameter or an input requiring grad, the outputs carry a grad_fn
+(step_b200.autograd: TwoBranchNetFunction, ContextNetFunction) whose backward is the explicit one of
+step_b200/training.py (head_backward, context_backward), and a head in training mode draws the reference's dropout
+masks.  Otherwise (torch.no_grad(), or nothing requires grad) the forward is the inference one, with eval-mode dropout.
 
 Layout tricks (none changes results beyond fp rounding):
   * ROI features and the 1x1x1 `downsample` output share one [R*T',7,7,1088] buffer, so the concat
@@ -142,9 +144,16 @@ class ContextNet(nn.Module):
         self._init_net()
 
     def forward(self, conv_feat):
+        """With grad mode on and a trainable parameter or conv_feat requiring grad, the output carries a grad_fn
+        (step_b200.autograd.ContextNetFunction) that also gives conv_feat its gradient."""
+        from . import autograd
         L.need_cuda(conv_feat)
+        params = autograd.trainable(self)
         with torch.cuda.device(conv_feat.device):
-            ctx = self.forward_act(to_act(conv_feat, E.dtype_code(self.fp16)))  # [N, T', 1024] fp32
+            a = to_act(conv_feat, E.dtype_code(self.fp16))
+            if autograd.wanted(params, conv_feat):
+                return autograd.ContextNetFunction.apply(self, a, conv_feat, *params)
+            ctx = self.forward_act(a)  # [N, T', 1024] fp32
         return ctx.permute(0, 2, 1).unsqueeze(-1).unsqueeze(-1)
 
     def forward_act(self, a, keep=None):
@@ -242,6 +251,15 @@ class TwoBranchNet(nn.Module):
             if context_feat is not None:
                 context_feat = context_feat.to(dev)
         L.same_device(global_feat, context_feat)
+        from . import autograd
+        params = autograd.trainable(self)
+        if autograd.wanted(params, global_feat, context_feat):
+            if targets is not None and tubes is None:
+                raise RuntimeError("TwoBranchNet.forward: targets need tubes")
+            with torch.cuda.device(global_feat.device):
+                tb = None if tubes is None else tubes.detach().to(global_feat.device)
+                tg = None if targets is None else targets.detach().to(global_feat.device)
+                return autograd.TwoBranchNetFunction.apply(self, global_feat, context_feat, tb, tg, *params)
         code = E.dtype_code(self.fp16)
         N, T, C, W, H = global_feat.shape
         with torch.cuda.device(global_feat.device):   # kernels run on the device (and its stream) that owns the tensors
@@ -261,8 +279,8 @@ class TwoBranchNet(nn.Module):
         z = torch.tensor(0., device=prob.device)
         if targets is None:
             return prob, loc, first, last, z.view(-1), z.view(-1), z.view(-1)
-        # training-time outputs (two_branch.py:276-341), eval-mode dropout; the losses are computed on the device.
-        # NOTE: the outputs carry no grad_fn -- the backward runs explicitly (step_b200/training.py::head_forward_backward).
+        # training-time outputs (two_branch.py:276-341) without autograd, eval-mode dropout; the losses are computed on the
+        # device.
         from . import training
         if tubes is None:
             raise RuntimeError("TwoBranchNet.forward: targets need tubes")
