@@ -35,8 +35,8 @@ def demo_merge(dets, label_dict, global_thresh):
             if not taken[j] and box_iou(boxes[i], boxes[j]) > thr:
                 taken[j] = True
                 members.append(j)
-        total = boxes[members[0]].copy()             # np.mean(axis=0) of a (n, 4) array: b0 + b1 + ... in row order
-        for j in members[1:]:
+        total = (F32(0) + boxes[members[0]]).astype(F32)   # np.mean(axis=0) of a (n, 4) array: 0 + b0 + b1 + ... in
+        for j in members[1:]:                                # row order (the identity +0.0 first: -0.0 sums to +0.0)
             total = (total + boxes[j]).astype(F32)
         mean = (total / F32(len(members))).astype(F32)
         key = ",".join(str(F32(v)) for v in mean)    # shortest round-trip repr: equal strings <=> equal floats

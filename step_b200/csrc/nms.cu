@@ -18,12 +18,17 @@ __device__ __forceinline__ float box_area(float4 b) {
   return __fmul_rn(__fadd_rn(__fsub_rn(b.z, b.x), 1.0f), __fadd_rn(__fsub_rn(b.w, b.y), 1.0f));
 }
 
+// std::max(p, q) is (p < q) ? q : p and std::min(p, q) is (q < p) ? q : p: a NaN p is returned, a NaN q is dropped, and
+// p is returned when the two are equal (+0.0 against -0.0).  Python's builtin max / min follow the same rule.
+__device__ __forceinline__ float std_max(float p, float q) { return (p < q) ? q : p; }
+__device__ __forceinline__ float std_min(float p, float q) { return (q < p) ? q : p; }
+
 __device__ __forceinline__ bool suppresses(float4 a, float area_a, float4 b, float area_b, float thr, int ge) {
-  // nms_cpu.cpp:74-85
-  float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
-  float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-  float w = fmaxf(0.0f, __fadd_rn(__fsub_rn(xx2, xx1), 1.0f));
-  float h = fmaxf(0.0f, __fadd_rn(__fsub_rn(yy2, yy1), 1.0f));
+  // nms_cpu.cpp:74-85, a the earlier row (ix1...), b the later one (x1[j]...)
+  float xx1 = std_max(a.x, b.x), yy1 = std_max(a.y, b.y);
+  float xx2 = std_min(a.z, b.z), yy2 = std_min(a.w, b.w);
+  float w = std_max(0.0f, __fadd_rn(__fsub_rn(xx2, xx1), 1.0f));
+  float h = std_max(0.0f, __fadd_rn(__fsub_rn(yy2, yy1), 1.0f));
   float inter = __fmul_rn(w, h);
   float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
   return ge ? (ovr >= thr) : (ovr > thr);
@@ -31,18 +36,27 @@ __device__ __forceinline__ bool suppresses(float4 a, float area_a, float4 b, flo
 
 // ---- 1. ordering: rank sort (score desc, index asc).  O(n^2) compares, embarrassingly parallel;
 //         10k boxes = 1e8 compares ~ 10 us.  Deterministic and stable by construction, unlike the
-//         reference's torch.sort (unstable for n > 16).
+//         reference's torch.sort (unstable on ties).  NaN scores rank above every number, as
+//         scores.sort(0, descending=True) (nms_cpu.cpp:48) puts them first, and -0.0 ties with +0.0.  The compares run on
+//         order_key(score), an int with the same order, so every row gets a distinct rank: a float compare is false for
+//         every NaN, which would give all NaN rows and the best row rank 0 and leave slots of `order` unwritten.
+__device__ __forceinline__ int order_key(float s) {
+  if (s != s) return 0x7fffffff;                     // NaN: above +inf (0x7f800000)
+  const int b = __float_as_int(s == 0.0f ? 0.0f : s);  // -0.0 -> +0.0
+  return b >= 0 ? b : b ^ 0x7fffffff;                // negatives: larger magnitude -> smaller key
+}
+
 __global__ void __launch_bounds__(256) nms_rank_kernel(const float* __restrict__ boxes,
                                                        const float* __restrict__ scores, int n,
                                                        float4* __restrict__ sorted_boxes,
                                                        int* __restrict__ order) {
-  __shared__ float tile[1024];
+  __shared__ int tile[1024];
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  float si = i < n ? scores[i] : 0.0f;
+  int si = i < n ? order_key(scores[i]) : 0;
   int rank = 0;
   for (int base = 0; base < n; base += 1024) {
     int cnt = min(1024, n - base);
-    for (int t = threadIdx.x; t < cnt; t += blockDim.x) tile[t] = scores[base + t];
+    for (int t = threadIdx.x; t < cnt; t += blockDim.x) tile[t] = order_key(scores[base + t]);
     __syncthreads();
     if (i < n) {
       // elements before i in index order win ties; split the loop so the compare is branch-free
@@ -73,8 +87,9 @@ struct MergePred {  // demo.py:190  compute_box_iou(box, box2) > global_thresh  
   float thr;
   __device__ __forceinline__ float prep(float4 b) const { return __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y)); }
   __device__ __forceinline__ bool operator()(float4 a, float aa, float4 b, float ab) const {
-    const float iw = fmaxf(__fsub_rn(fminf(a.z, b.z), fmaxf(a.x, b.x)), 0.0f);
-    const float ih = fmaxf(__fsub_rn(fminf(a.w, b.w), fmaxf(a.y, b.y)), 0.0f);
+    // Python's max / min on the coordinates (tube_utils.py:292-295), np.maximum(v, 0.) on the sides (NaN kept)
+    const float iw = clamp_lo(__fsub_rn(std_min(a.z, b.z), std_max(a.x, b.x)), 0.0f);
+    const float ih = clamp_lo(__fsub_rn(std_min(a.w, b.w), std_max(a.y, b.y)), 0.0f);
     const float inter = (iw > 0.0f && ih > 0.0f) ? __fmul_rn(iw, ih) : 0.0f;
     // a zero union gives NaN (two identical zero-area boxes), which never merges
     return __fdiv_rn(inter, __fsub_rn(__fadd_rn(aa, ab), inter)) > thr;
@@ -226,7 +241,8 @@ __global__ void __launch_bounds__(1024) nms_compact_kernel(const uint8_t* __rest
 
 // ---- greedy NMS of one small problem in shared memory (nms_cpu.cpp:57-88), one CTA.  Rows i in [0, n) whose score
 //      passes the threshold are ranked (score descending, index ascending), then suppressed in rank order; the other rows
-//      are dropped.  The caller says how rows are read and where their keep flags go:
+//      are dropped.  Both callers' thresholds are ordered compares, so a NaN score never passes: it is dropped, as
+//      scores.gt(conf_thresh) drops it in test.py:180.  The caller says how rows are read and where their keep flags go:
 //        score(i)    row i's score;
 //        pass(s)     whether a row of score s takes part;
 //        box(i, s)   row i's box, asked once for every row before its threshold test;
@@ -288,7 +304,7 @@ __global__ void __launch_bounds__(256) nms_segmented_kernel(const float* __restr
   const int beg = seg_offsets[blockIdx.x], n = seg_offsets[blockIdx.x + 1] - beg;
   greedy_nms_smem(
       n, thr, ge, [&](int i) { return scores[beg + i]; },
-      [&](float s) { return s >= min_score; },   // the confidence threshold of test.py:183
+      [&](float s) { return s >= min_score; },   // the confidence threshold of test.py:180 (false for NaN)
       [&](int i, float) { return reinterpret_cast<const float4*>(boxes)[beg + i]; },
       [&](int i, uint8_t k) { keep_mask[beg + i] = k; });
 }
@@ -315,7 +331,7 @@ __global__ void __launch_bounds__(128) detect_nms_kernel(const float* __restrict
   const size_t cand0 = (size_t)beg * ncls + (size_t)c * n;
   greedy_nms_smem(
       n, thr, ge, [&](int i) { return prob[(size_t)(beg + i) * prob_ld + c]; },
-      [&](float s) { return s > conf; },   // test.py:183 scores.gt(conf)
+      [&](float s) { return s > conf; },   // test.py:180 scores.gt(conf): false for NaN
       [&](int i, float s) {
         const float4 b = valid_one(ld4(loc + (size_t)(beg + i) * loc_ld), vw, vh);   // test.py:191
         score_out[cand0 + i] = s;
@@ -512,10 +528,11 @@ __global__ void __launch_bounds__(1024) merge_groups_kernel(const float* __restr
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   // 1. the leaders in row order: group g
   const int G = ballot_compact<32>(n, [&](int i) { return (int)(group[i] == i); }, [&](int i, int slot) { lead[slot] = i; });
-  // 2. one warp per group: lane c < 4 sums coordinate c over the members in row order, ((b0 + b1) + b2) + ..., in float32
+  // 2. one warp per group: lane c < 4 sums coordinate c over the members in row order, ((0 + b0) + b1) + ..., in float32
+  //    (np.add.reduce starts from its identity +0.0, so a sum of -0.0 is +0.0)
   for (int g = wid; g < G; g += nwarps) {
     const int L = lead[g];
-    float s = lane < 4 ? rows[(size_t)L * 8 + lane] : 0.0f;
+    float s = lane < 4 ? __fadd_rn(0.0f, rows[(size_t)L * 8 + lane]) : 0.0f;
     int count = 1;
     for (int base = L + 1; base < n; base += 32) {
       const int i = base + lane;

@@ -5,10 +5,16 @@
 
 namespace step {
 
+// max(v, lo) and min(v, hi) with numpy's / torch's NaN rule: a NaN v is returned, and so is a v equal to the bound
+// (-0.0 stays -0.0 against a bound of 0).
+__device__ __forceinline__ float clamp_lo(float v, float lo) { return v < lo ? lo : v; }
+__device__ __forceinline__ float clamp_hi(float v, float hi) { return v > hi ? hi : v; }
+
 __device__ __forceinline__ float4 valid_one(float4 b, float width, float height) {
-  // tube_utils.py:72-88: clamp, then degenerate boxes become the whole image
-  b.x = fmaxf(0.0f, b.x); b.y = fmaxf(0.0f, b.y);
-  b.z = fminf(width, b.z); b.w = fminf(height, b.w);
+  // tube_utils.py:72-88: clamp, then degenerate boxes become the whole image.  np.maximum / np.minimum and torch.clamp
+  // keep a NaN coordinate (which then fails the test below) and keep -0.0; fmaxf / fminf would drop the NaN.
+  b.x = clamp_lo(b.x, 0.0f); b.y = clamp_lo(b.y, 0.0f);
+  b.z = clamp_hi(b.z, width); b.w = clamp_hi(b.w, height);
   if (!(b.x < __fsub_rn(b.z, 2.0f) && b.y < __fsub_rn(b.w, 2.0f))) { b.x = 0.0f; b.y = 0.0f; b.z = width; b.w = height; }
   return b;
 }
@@ -64,11 +70,11 @@ __device__ __forceinline__ void extrapolate_one(const float* __restrict__ in /*[
     int lo = T - i - 1;
     out[lo * 4 + comp] = __fsub_rn(__fmul_rn(a, out[(lo + 1) * 4 + comp]), __fmul_rn(b, out[(lo + T) * 4 + comp]));
   }
-  for (int t = 0; t < Lo; ++t) {  // tube_utils.py:22-25
+  for (int t = 0; t < Lo; ++t) {  // tube_utils.py:22-25, np.maximum / np.minimum: NaN kept
     float v = out[t * 4 + comp];
-    if (comp == 0 || comp == 1) v = fmaxf(0.0f, v);
-    else if (comp == 2) v = fminf(__fsub_rn(width, 1.0f), v);
-    else v = fminf(__fsub_rn(height, 1.0f), v);
+    if (comp == 0 || comp == 1) v = clamp_lo(v, 0.0f);
+    else if (comp == 2) v = clamp_hi(v, __fsub_rn(width, 1.0f));
+    else v = clamp_hi(v, __fsub_rn(height, 1.0f));
     out[t * 4 + comp] = v;
   }
 }

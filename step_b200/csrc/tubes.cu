@@ -46,10 +46,11 @@ __global__ void tube_extend_kernel(const float* __restrict__ tubes, int n, float
   float w = __fmul_rn(c.w, ratio), h = __fmul_rn(c.h, ratio);  // tube_utils.py:259-260
   float* o = out + 5 * (size_t)i;
   o[0] = r[0];
-  o[1] = fmaxf(__fsub_rn(c.x, __fmul_rn(0.5f, w)), 0.0f);
-  o[2] = fmaxf(__fsub_rn(c.y, __fmul_rn(0.5f, h)), 0.0f);
-  o[3] = fminf(__fsub_rn(__fadd_rn(c.x, __fmul_rn(0.5f, w)), 1.0f), __fsub_rn(width, 1.0f));
-  o[4] = fminf(__fsub_rn(__fadd_rn(c.y, __fmul_rn(0.5f, h)), 1.0f), __fsub_rn(height, 1.0f));
+  // tube_utils.py:261-264: torch.max / torch.min keep a NaN operand
+  o[1] = clamp_lo(__fsub_rn(c.x, __fmul_rn(0.5f, w)), 0.0f);
+  o[2] = clamp_lo(__fsub_rn(c.y, __fmul_rn(0.5f, h)), 0.0f);
+  o[3] = clamp_hi(__fsub_rn(__fadd_rn(c.x, __fmul_rn(0.5f, w)), 1.0f), __fsub_rn(width, 1.0f));
+  o[4] = clamp_hi(__fsub_rn(__fadd_rn(c.y, __fmul_rn(0.5f, h)), 1.0f), __fsub_rn(height, 1.0f));
 }
 
 // One CTA per tube (blockDim = 64 >= frames handled): decode -> extend -> validate -> re-flatten.

@@ -51,7 +51,8 @@ def nms(dets, scores, threshold):
     CPU tensors: every reference driver calls nms with CPU tensors (test.py:192); there is no CPU
     kernel here, so the rows are moved to the current CUDA device, resolved there with the CPU
     op's exact semantics (suppress when IoU >= thr, cpu/nms_cpu.cpp:84) and the indices are returned
-    on the CPU.  Ties between equal scores are visited in ascending index order.
+    on the CPU.  Ties between equal scores are visited in ascending index order; NaN scores rank above every number,
+    where scores.sort(descending=True) (nms_cpu.cpp:48) puts them, and -0.0 ties with +0.0.
     """
     if dets.dtype not in (torch.float32, torch.float64):
         raise RuntimeError('"nms" not implemented for \'%s\'' % str(dets.dtype).replace("torch.", ""))
@@ -88,7 +89,8 @@ _CUDA_GE = 1
 def nms_segmented(boxes, scores, seg_offsets, threshold, min_score=float("-inf"), ge=True, max_seg_rows=None):
     """Batched form of the per-clip x per-class loop of test.py:178-201: rows
     [seg_offsets[s], seg_offsets[s+1]) are independent NMS problems (<= 1024 rows each: pass the longest segment as
-    `max_seg_rows` when the host knows it, otherwise it is read back once).
+    `max_seg_rows` when the host knows it, otherwise it is read back once).  Only rows with score >= min_score take
+    part: a NaN score never does, as scores.gt(conf_thresh) drops it in test.py:180 (unlike `nms`, which ranks it first).
     Returns a uint8 keep mask over all rows; stays on device."""
     L.same_device(boxes, scores, seg_offsets)
     if max_seg_rows is None:   # the host knows the segment lengths in every caller of ours; a stray caller pays one sync

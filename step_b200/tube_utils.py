@@ -67,7 +67,9 @@ def valid_tubes(tubes, width=400, height=400):
 
 
 def extrapolate_tubes(tubes, T=6, height=400, width=400):
-    """tube_utils.py:10-27: [n,L,4] -> [n,L+2T,4]."""
+    """tube_utils.py:10-27: [n,L,4] -> [n,L+2T,4].  T = 1 raises ZeroDivisionError, as the reference's T/(T-1) does."""
+    if T == 1:
+        raise ZeroDivisionError("extrapolate_tubes: T/(T-1) with T = 1")
     is_np = isinstance(tubes, np.ndarray)
     t = _to_dev(tubes)
     n, Lf, _ = t.shape
