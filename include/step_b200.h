@@ -106,7 +106,10 @@ int step_detect_merge_f32(const float* det, const int* det_count, int n_clips, i
                           int* pairs, int* mcount, void* workspace, size_t ws_bytes, step_stream_t stream);
 
 /* ------------------------------------------------------------------ ROI ops -------------- */
-/* Reference layout (NCHW fp32 in, [R,C,ph,pw] fp32 out), arithmetic order of the reference. */
+/* Reference layout (NCHW fp32 in, [R,C,ph,pw] fp32 out), arithmetic order of the reference.  The backwards have no
+ * atomics: every element of grad_in sums its contributions in the order of the channels-last entries below, so the
+ * result repeats bit for bit and equals step_roi_align_bwd_nhwc / step_roi_pool_bwd_slice_nhwc (whole map) transposed.
+ * Rows whose frame index is outside [0, K) contribute nothing; any H x W. */
 int step_roi_align_fwd_nchw_f32(const float* feat, int K, int C, int H, int W, const float* rois, int R,
                                 float scale, int ph, int pw, int sampling_ratio, float* out,
                                 step_stream_t stream);
@@ -359,14 +362,16 @@ int step_head_outputs_bwd_f32(const float* logits, const float* local_loc, const
                               float* dloc, float* dfirst, float* dlast, step_stream_t stream);
 /* Channels-last ROIAlign backward without atomics (replaces _C.roi_align_backward, vision.cpp:33 /
  * cuda/ROIAlign_cuda.cu:201-278, whose atomicAdd scatter is not repeatable): grad_out [R,ph,pw,C] (channel stride
- * out_ld, STEP_F32 / STEP_F16) -> grad_in [K,H,W,C] fp32 (channel stride in_ld), written completely by the call. */
+ * out_ld, STEP_F32 / STEP_F16) -> grad_in [K,H,W,C] fp32 (channel stride in_ld), written completely by the call.
+ * Per element: rows of its frame in ascending order; per row, its samples in (bin, iy, ix) order in slices of 49 * 16,
+ * each slice's terms fl(fl(g w) / count) (taps in order) summed from +0.0f and the slice's sum added to the element's. */
 int step_roi_align_bwd_nhwc(const void* grad_out, int dtype, int out_ld, const float* rois, int R, float scale, int ph,
                             int pw, int K, int H, int W, int C, int sampling_ratio, float* grad_in, int in_ld,
                             step_stream_t stream);
 /* step_roi_align_bwd_nhwc for ROIs whose frame index f is relative to the slice conv_feat[:, t_start:t_start+roi_T] of a
  * [K = clips * feat_T, H, W, C] map (the frame map of step_roi_align_fwd_nhwc).  The contribution of each ROI frame is formed
- * completely, in the same order as step_roi_align_bwd_nhwc, in a workspace of
- * step_roi_align_bwd_slice_workspace_bytes(K, H, W, C, roi_T, feat_T) bytes and then ADDED to grad_in frame
+ * completely, in the same order as step_roi_align_bwd_nhwc (workspace: none is needed any more;
+ * step_roi_align_bwd_slice_workspace_bytes returns 0 and workspace may be NULL) and then ADDED to grad_in frame
  * (f / roi_T) * feat_T + t_start + f % roi_T; frames outside the slice are untouched.  Deterministic, no atomics: with
  * t_start = 0 and roi_T = feat_T, calls on a zeroed grad_in give bit for bit the sum of the step_roi_align_bwd_nhwc results. */
 size_t step_roi_align_bwd_slice_workspace_bytes(int K, int H, int W, int C, int roi_T, int feat_T);

@@ -12,9 +12,11 @@ multiplied by, and the parameter gradients come back with it (as torch.amp's Gra
 The path is taken only when grad mode is on and a trainable parameter or a tensor input requires grad (`wanted`);
 otherwise the modules run their forward exactly as before.  The saved tape is released by the first backward: a second
 backward through the same forward (retain_graph=True) raises.  Double backward is not supported.
-What the driver computes around the modules (the conv_feat slices' .contiguous(), the per-tube context copies, the NCHW
-ROIAlign / ROIPool backward with float atomics, autograd's sums of several gradients of one tensor) is torch's, so this
-path is not bit-reproducible from run to run; training.train_step remains the deterministic one."""
+What the driver computes around the modules (the conv_feat slices' .contiguous(), the per-tube context copies, autograd's
+sums of several gradients of one tensor) is torch's; the ROI pooling of those slices is roi_layers.py's, whose NCHW
+backward has no atomics.  The path repeats bit for bit: two train.py / train_cls.py iterations from the same nets, clips
+and generator state give identical gradients and identical parameters after step_b200.optim.Adam (fp32 ROIAlign and
+ROIPool, fp16 with a loss scale of 1024, the class-only stage; tests/test_gpu_roi_bwd_det.py)."""
 import torch
 from torch.autograd import Function
 from torch.autograd.function import once_differentiable

@@ -1,9 +1,9 @@
 """Run the reference's own drivers (test.py / demo.py, and train.py / train_cls.py on one GPU without apex) of
 NVlabs/STEP on step_b200 without editing them.  The training drivers then run their fp32 path (the reference forces
 args.fp16 = False without apex) and back-propagate with `loss.backward()` through the modules' torch.autograd Functions
-(step_b200/autograd.py), whose backward is train_step's.  What differs from step_b200.training.train_step: the driver's
-NCHW ROI backward uses float atomics, so its gradients are not bit-reproducible from run to run, and the optimizer is
-torch's unless the driver builds it from step_b200.optim (INTEGRATION.md).  nn.DataParallel over several GPUs and apex O1
+(step_b200/autograd.py), whose backward is train_step's; their gradients repeat bit for bit from run to run (the NCHW
+ROI backward has no atomics).  What differs from step_b200.training.train_step: the optimizer is torch's unless the
+driver builds it from step_b200.optim (INTEGRATION.md).  nn.DataParallel over several GPUs and apex O1
 are not covered.
 
     import step_b200.compat as compat

@@ -1,5 +1,5 @@
-// roi_math.cuh -- the ROIAlign sampling of cpu/ROIAlign_cpu.cpp shared by the forward kernels (roi.cu) and the backward
-// kernels (train.cu): both must sample the same points for the backward to be the adjoint of the forward.  Every fp32
+// roi_math.cuh -- the ROIAlign sampling of cpu/ROIAlign_cpu.cpp shared by the forward and the backward kernels (roi.cu):
+// both must sample the same points for the backward to be the adjoint of the forward.  Every fp32
 // operation is explicitly rounded in the reference's operand order; the including files are built with -fmad=false.
 #pragma once
 #include "common.cuh"
@@ -11,24 +11,39 @@ struct Tap {
   float w1, w2, w3, w4;
 };
 
+// One axis of the bilinear tap: the pixels lo, hi (of n along the axis) a sample at coordinate v reads and their weights
+// wlo = 1 - l, whi = l.  lo < 0: v is outside [-1, n] and the sample contributes nothing (ROIAlign_cpu.cpp:72-131).
+struct AxisTap {
+  int lo, hi;
+  float wlo, whi;
+};
+
+__device__ __forceinline__ AxisTap axis_tap(int n, float v) {
+  AxisTap a;
+  if (v < -1.0f || v > (float)n) {
+    a.lo = a.hi = -1;
+    a.wlo = a.whi = 0.0f;
+    return a;
+  }
+  if (v <= 0.0f) v = 0.0f;
+  a.lo = (int)v;
+  if (a.lo >= n - 1) { a.hi = a.lo = n - 1; v = (float)a.lo; } else { a.hi = a.lo + 1; }
+  a.whi = __fsub_rn(v, (float)a.lo);
+  a.wlo = __fsub_rn(1.0f, a.whi);
+  return a;
+}
+
 __device__ __forceinline__ Tap make_tap(int H, int W, float y, float x) {
   Tap t;
-  // ROIAlign_cpu.cpp:72-131
-  if (y < -1.0f || y > (float)H || x < -1.0f || x > (float)W) {
+  const AxisTap ay = axis_tap(H, y), ax = axis_tap(W, x);
+  if (ay.lo < 0 || ax.lo < 0) {
     t.p1 = t.p2 = t.p3 = t.p4 = -1;
     t.w1 = t.w2 = t.w3 = t.w4 = 0.0f;
     return t;
   }
-  if (y <= 0.0f) y = 0.0f;
-  if (x <= 0.0f) x = 0.0f;
-  int y_low = (int)y, x_low = (int)x, y_high, x_high;
-  if (y_low >= H - 1) { y_high = y_low = H - 1; y = (float)y_low; } else { y_high = y_low + 1; }
-  if (x_low >= W - 1) { x_high = x_low = W - 1; x = (float)x_low; } else { x_high = x_low + 1; }
-  float ly = __fsub_rn(y, (float)y_low), lx = __fsub_rn(x, (float)x_low);
-  float hy = __fsub_rn(1.0f, ly), hx = __fsub_rn(1.0f, lx);
-  t.w1 = __fmul_rn(hy, hx); t.w2 = __fmul_rn(hy, lx); t.w3 = __fmul_rn(ly, hx); t.w4 = __fmul_rn(ly, lx);
-  t.p1 = y_low * W + x_low;  t.p2 = y_low * W + x_high;
-  t.p3 = y_high * W + x_low; t.p4 = y_high * W + x_high;
+  t.w1 = __fmul_rn(ay.wlo, ax.wlo); t.w2 = __fmul_rn(ay.wlo, ax.whi); t.w3 = __fmul_rn(ay.whi, ax.wlo); t.w4 = __fmul_rn(ay.whi, ax.whi);
+  t.p1 = ay.lo * W + ax.lo; t.p2 = ay.lo * W + ax.hi;
+  t.p3 = ay.hi * W + ax.lo; t.p4 = ay.hi * W + ax.hi;
   return t;
 }
 
@@ -67,8 +82,8 @@ __device__ __forceinline__ float tap_dot(const Tap& t, float v1, float v2, float
                    __fmul_rn(t.w4, v4));
 }
 
-// Entries of the per-ROI shared-memory tap tables: 7x7 bins x sampling grids up to 4x4.  Larger grids are recomputed
-// (forward) or processed in slices of this size (backward).
+// Entries of the per-ROI shared-memory tap table of the forward: 7x7 bins x sampling grids up to 4x4; larger grids are
+// recomputed.  The backward forms a row's partial sums per kMaxTaps samples (roi.cu).
 constexpr int kMaxTaps = 49 * 16;
 
 }  // namespace step

@@ -7,12 +7,6 @@
 //                              head_losses_kernel (one shared device function);
 //   * head_outputs_bwd_kernel  the autograd of the head's tail (two_branch.py:272-342) from upstream gradients of its
 //                              seven outputs, with the loss arithmetic of head_losses_kernel (shared device functions);
-//   * roi_align_bwd_nhwc       channels-last ROIAlign backward WITHOUT float atomics: every feature pixel gathers its
-//                              contributions in a fixed order (ROI index, bin, sample), so the result is bit-for-bit
-//                              repeatable -- the reference's RoIAlignBackwardFeature (cuda/ROIAlign_cuda.cu:201-278) scatters
-//                              with atomicAdd and is not;
-//   * roi_align_bwd_slice_nhwc the same backward for ROIs pooled from a temporal slice of conv_feat (temporal mode of
-//                              train.py:294-309), accumulated into the gradient of the whole feature map;
 //   * ctx_grad_reduce          the gradient of ContextNet's output from the per-tube context inputs of the classifier
 //                              (train.py:317-321), summed per clip in tube order and spread over the step's frames;
 //   * linear_bwd_*             backward of the small-N linears of the head (global_cls, local_reg, neighbor_reg*):
@@ -30,7 +24,6 @@
 
 #include "common.cuh"
 #include "dropout.cuh"
-#include "roi_math.cuh"
 #include "tube_math.cuh"
 
 namespace step {
@@ -278,200 +271,6 @@ __global__ void __launch_bounds__(256) head_outputs_bwd_kernel(LossGeom g, int c
     *a = __fadd_rn(*a, dfirst[i]);
     float* b = dloc + ((size_t)n * g.T_len + g.e0) * 4 + r;
     *b = __fadd_rn(*b, dlast[i]);
-  }
-}
-
-// ---- ROIAlign backward, channels-last, deterministic ----------------------------------------------------------------
-// grad_in[k][h][w][c] = sum over ROIs r on frame k (ascending r), bins (ph, pw) and samples (iy, ix) in loop order of
-//   w_tap(r, bin, sample, this pixel) * grad_out[r][bin][c] / count(r)        (ROIAlign_cuda.cu:201-278)
-// One CTA per (frame, pixel row); the per-ROI sample table (each sample's Tap and bin, sampled exactly as the forward in
-// roi.cu) is built in shared memory by the CTA and scanned by every (pixel, channel vector) thread.  No atomics: a thread
-// owns its output element.
-struct RoiBwdSample { Tap tap; int bin; };
-
-// Adds the contributions of every ROI r with roi[0] == roi_frame to dst, this frame's [H*W, C] gradient (channel stride
-// dst_ld), which the caller has initialised: per ROI and element the samples are summed in a fixed order and the sum is
-// added to dst.  Called by the whole CTA; `tab` is the CTA's shared sample table.
-template <typename T>
-__device__ __forceinline__ void roi_align_bwd_frame(const T* __restrict__ grad_out, int out_ld, const float* __restrict__ rois,
-                                                    int R, float scale, int H, int W, int C, int ph, int pw, int sampling_ratio,
-                                                    int roi_frame, float* __restrict__ dst, int dst_ld, RoiBwdSample* tab) {
-  constexpr int VN = 4;
-  const int nvec = C / VN, npix = H * W;
-  for (int r = 0; r < R; ++r) {
-    const float* roi = rois + 5 * (size_t)r;
-    if ((int)roi[0] != roi_frame) continue;                   // uniform across the CTA
-    const RoiGeom g = roi_geometry(roi, scale, ph, pw, sampling_ratio);
-    const int per_bin = g.gh * g.gw, total = ph * pw * per_bin;
-    for (int base = 0; base < total; base += kMaxTaps) {
-      const int cnt = min(kMaxTaps, total - base);
-      __syncthreads();                                        // the previous table has been consumed
-      for (int s = threadIdx.x; s < cnt; s += blockDim.x) {
-        const int gidx = base + s;
-        const int bin = gidx / per_bin, rem = gidx - bin * per_bin;
-        const int iy = rem / g.gw, ix = rem - iy * g.gw;
-        const int p = bin / pw, q = bin - p * pw;
-        const float y = sample_coord(g.start_h, p, g.bin_h, iy, g.gh), x = sample_coord(g.start_w, q, g.bin_w, ix, g.gw);
-        tab[s] = RoiBwdSample{make_tap(H, W, y, x), bin};
-      }
-      __syncthreads();
-      const T* go = grad_out + (size_t)r * ph * pw * out_ld;
-      for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x) {
-        const int p = i / nvec, cv = i - p * nvec;
-        float acc[VN] = {0.f, 0.f, 0.f, 0.f};
-        bool hit = false;
-        for (int s = 0; s < cnt; ++s) {
-          const RoiBwdSample& e = tab[s];
-          // the four taps in order; ROIAlign_cuda.cu:263-271: g = top_diff * w / count
-          auto add_tap = [&](int pix, float w) {
-            if (pix != p) return;
-            float gv[VN];
-            if constexpr (sizeof(T) == 4) {
-              const float4 v = *reinterpret_cast<const float4*>(go + (size_t)e.bin * out_ld + cv * VN);
-              gv[0] = v.x; gv[1] = v.y; gv[2] = v.z; gv[3] = v.w;
-            } else {
-              const uint2 raw = *reinterpret_cast<const uint2*>(go + (size_t)e.bin * out_ld + cv * VN);
-              const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&raw.x));
-              const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&raw.y));
-              gv[0] = a.x; gv[1] = a.y; gv[2] = b.x; gv[3] = b.y;
-            }
-#pragma unroll
-            for (int c = 0; c < VN; ++c) acc[c] = __fadd_rn(acc[c], __fdiv_rn(__fmul_rn(gv[c], w), g.count));
-            hit = true;
-          };
-          add_tap(e.tap.p1, e.tap.w1);
-          add_tap(e.tap.p2, e.tap.w2);
-          add_tap(e.tap.p3, e.tap.w3);
-          add_tap(e.tap.p4, e.tap.w4);
-        }
-        if (hit) {
-          float4* d = reinterpret_cast<float4*>(dst + (size_t)p * dst_ld + cv * VN);
-          float4 cur = *d;
-          cur.x = __fadd_rn(cur.x, acc[0]); cur.y = __fadd_rn(cur.y, acc[1]); cur.z = __fadd_rn(cur.z, acc[2]); cur.w = __fadd_rn(cur.w, acc[3]);
-          *d = cur;
-        }
-      }
-    }
-  }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) roi_align_bwd_nhwc_kernel(const T* __restrict__ grad_out, int out_ld,
-                                                                 const float* __restrict__ rois, int R, float scale, int H,
-                                                                 int W, int C, int ph, int pw, int sampling_ratio,
-                                                                 float* __restrict__ grad_in, int in_ld) {
-  __shared__ RoiBwdSample tab[kMaxTaps];
-  const int frame = blockIdx.x;
-  const int nvec = C / 4, npix = H * W;
-  float* dst = grad_in + (size_t)frame * npix * in_ld;
-  // this CTA owns grad_in[frame]: zero it, then accumulate ROI by ROI (ascending index: fixed order)
-  for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x) {
-    const int p = i / nvec, cv = i - p * nvec;
-    *reinterpret_cast<float4*>(dst + (size_t)p * in_ld + cv * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  roi_align_bwd_frame<T>(grad_out, out_ld, rois, R, scale, H, W, C, ph, pw, sampling_ratio, frame, dst, in_ld, tab);
-}
-
-// The same backward for ROIs whose frame index f is relative to the slice conv_feat[:, t_start:t_start+roi_T]
-// (ROINet.pool_into's frame map): one CTA per ROI frame f forms the frame's whole contribution in its [H*W, C] workspace
-// frame exactly as roi_align_bwd_nhwc_kernel does, then adds it to grad_in frame (f / roi_T) * feat_T + t_start + f % roi_T.
-// Frames outside the slice are not touched, so successive refinement steps accumulate into one [B*feat_T, H, W, C] buffer.
-template <typename T>
-__global__ void __launch_bounds__(256) roi_align_bwd_slice_nhwc_kernel(const T* __restrict__ grad_out, int out_ld,
-                                                                       const float* __restrict__ rois, int R, float scale, int H,
-                                                                       int W, int C, int ph, int pw, int sampling_ratio, int roi_T,
-                                                                       int feat_T, int t_start, float* __restrict__ ws,
-                                                                       float* __restrict__ grad_in, int in_ld) {
-  __shared__ RoiBwdSample tab[kMaxTaps];
-  const int f = blockIdx.x;
-  const int nvec = C / 4, npix = H * W;
-  float* part = ws + (size_t)f * npix * C;
-  for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x)
-    *reinterpret_cast<float4*>(part + (size_t)i * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-  roi_align_bwd_frame<T>(grad_out, out_ld, rois, R, scale, H, W, C, ph, pw, sampling_ratio, f, part, C, tab);
-  __syncthreads();
-  float* dst = grad_in + ((size_t)(f / roi_T) * feat_T + t_start + f % roi_T) * npix * in_ld;
-  for (int i = threadIdx.x; i < npix * nvec; i += blockDim.x) {
-    const int p = i / nvec, cv = i - p * nvec;
-    const float4 a = *reinterpret_cast<const float4*>(part + (size_t)i * 4);
-    float4* d = reinterpret_cast<float4*>(dst + (size_t)p * in_ld + cv * 4);
-    float4 cur = *d;
-    cur.x = __fadd_rn(cur.x, a.x); cur.y = __fadd_rn(cur.y, a.y); cur.z = __fadd_rn(cur.z, a.z); cur.w = __fadd_rn(cur.w, a.w);
-    *d = cur;
-  }
-}
-
-// ---- ROIPool backward on a frame slice (the reference's ROIPool_cuda.cu:103-132 scatters with atomicAdd) -----------------
-// One CTA per (ROI frame f, chunk of `blockDim.x` channels) holds the frame's [H*W, chunk] fp32 accumulator in shared
-// memory; thread t owns channel c0 + t (and, at 32 channels or more, shared-memory bank t % 32).  The CTA streams the ROI rows in ascending order,
-// compacts those of frame f (in order, blockDim.x rows at a time: no cap on R, no workspace), and every thread adds
-// grad_out[row, bin, c] into acc[argmax[row, bin, c], c] bin by bin.  So each element sums its contributions in ascending
-// (row, ph, pw) order -- the loop order of torchvision's CPU roi_pool backward -- with no atomics and no bank conflicts.
-// The tile is then added into grad_in frame (f / roi_T) * feat_T + t_start + f % roi_T with 16-byte accesses; frames
-// without a ROI are not touched.
-constexpr int kPoolBwdMaxChunk = 64;           // the smallest chunk and the shared-memory budget: common.cuh
-constexpr int kPoolBwdBins = 16;               // bins whose (argmax, gradient) loads are in flight together
-
-template <typename T>
-__global__ void __launch_bounds__(kPoolBwdMaxChunk) roi_pool_bwd_slice_nhwc_kernel(const T* __restrict__ grad_out, int out_ld,
-                                                                                   const int32_t* __restrict__ argmax,
-                                                                                   const float* __restrict__ rois, int R, int nbins,
-                                                                                   int npix, int C, int roi_T, int feat_T, int t_start,
-                                                                                   float* __restrict__ grad_in, int in_ld) {
-  extern __shared__ float acc[];                // [npix][chunk]
-  __shared__ int rows[kPoolBwdMaxChunk];
-  __shared__ int warp_rows[kPoolBwdMaxChunk / 32];
-  const int chunk = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = (chunk + 31) >> 5;
-  const unsigned mask = chunk >= 32 ? 0xffffffffu : (1u << chunk) - 1u;
-  const int f = blockIdx.x, c0 = blockIdx.y * chunk, c = c0 + tid;
-  for (int i = tid; i < npix * chunk; i += chunk) acc[i] = 0.0f;
-  int seen = 0;                                 // rows of frame f so far (uniform across the CTA)
-  for (int base = 0; base < R; base += chunk) {
-    const int r = base + tid;
-    const bool keep = r < R && (int)rois[5 * (size_t)r] == f;
-    const unsigned bal = __ballot_sync(mask, keep);
-    __syncthreads();                            // the previous batch's rows have been consumed
-    if (lane == 0) warp_rows[warp] = __popc(bal);
-    __syncthreads();
-    int off = 0, n = 0;
-    for (int w = 0; w < nwarps; ++w) { off += w < warp ? warp_rows[w] : 0; n += warp_rows[w]; }
-    if (keep) rows[off + __popc(bal & ((1u << lane) - 1u))] = r;
-    __syncthreads();
-    seen += n;
-    if (c >= C) continue;
-    for (int j = 0; j < n; ++j) {
-      const int row = rows[j];
-      const T* g = grad_out + (size_t)row * nbins * out_ld + c;
-      const int32_t* a = argmax + (size_t)row * nbins * C + c;
-      for (int b0 = 0; b0 < nbins; b0 += kPoolBwdBins) {
-        int av[kPoolBwdBins];
-        float gv[kPoolBwdBins];
-#pragma unroll
-        for (int k = 0; k < kPoolBwdBins; ++k) {
-          const bool in = b0 + k < nbins;
-          av[k] = in ? a[(size_t)(b0 + k) * C] : -1;
-          gv[k] = in ? to_f32<T>(g[(size_t)(b0 + k) * out_ld]) : 0.0f;
-        }
-#pragma unroll
-        for (int k = 0; k < kPoolBwdBins; ++k)
-          if ((unsigned)av[k] < (unsigned)npix) {   // -1: empty bin, no contribution
-            float* s = acc + av[k] * chunk + tid;
-            *s = __fadd_rn(*s, gv[k]);
-          }
-      }
-    }
-  }
-  if (seen == 0) return;
-  __syncthreads();
-  float* dst = grad_in + ((size_t)(f / roi_T) * feat_T + t_start + f % roi_T) * npix * in_ld + c0;
-  const int nv = min(chunk, C - c0) / 4;
-  for (int i = tid; i < npix * nv; i += chunk) {
-    const int p = i / nv, v = i - p * nv;
-    const float4 s = *reinterpret_cast<const float4*>(acc + p * chunk + v * 4);
-    float4* d = reinterpret_cast<float4*>(dst + (size_t)p * in_ld + v * 4);
-    float4 cur = *d;
-    cur.x = __fadd_rn(cur.x, s.x); cur.y = __fadd_rn(cur.y, s.y); cur.z = __fadd_rn(cur.z, s.z); cur.w = __fadd_rn(cur.w, s.w);
-    *d = cur;
   }
 }
 
@@ -1119,91 +918,6 @@ extern "C" int step_cls_loss_f32(const float* logits, const float* targets, int 
   STEP_CHECK_ARG(logits && targets && loss_cls && flags, "cls_loss: null pointer");
   cls_loss_kernel<<<1, 256, 0, cu(stream)>>>(N, cls, logits, targets, loss_cls, flags, dlogits);
   STEP_LAUNCH_CHECK("cls_loss_kernel");
-  return 0;
-}
-
-extern "C" int step_roi_align_bwd_nhwc(const void* grad_out, int dtype, int out_ld, const float* rois, int R, float scale, int ph,
-                                       int pw, int K, int H, int W, int C, int sampling_ratio, float* grad_in, int in_ld,
-                                       step_stream_t stream) {
-  STEP_CHECK_ARG(K > 0 && H > 0 && W > 0 && C > 0 && R >= 0 && ph > 0 && pw > 0, "roi_align_bwd_nhwc: bad shape");
-  STEP_CHECK_ARG(dtype == STEP_F32 || dtype == STEP_F16, "roi_align_bwd_nhwc: bad dtype");
-  STEP_CHECK_ARG(C % 4 == 0 && in_ld % 4 == 0 && out_ld % 4 == 0 && in_ld >= C && out_ld >= C, "roi_align_bwd_nhwc: C / ld must be multiples of 4");
-  STEP_CHECK_ARG(grad_in && (R == 0 || (grad_out && rois)), "roi_align_bwd_nhwc: null pointer");
-  STEP_CHECK_ARG((((uintptr_t)grad_in | (uintptr_t)grad_out) & 15) == 0, "roi_align_bwd_nhwc: pointers must be 16-byte aligned");
-  if (dtype == STEP_F32)
-    roi_align_bwd_nhwc_kernel<float><<<K, 256, 0, cu(stream)>>>((const float*)grad_out, out_ld, rois, R, scale, H, W, C, ph, pw,
-                                                                 sampling_ratio, grad_in, in_ld);
-  else
-    roi_align_bwd_nhwc_kernel<__half><<<K, 256, 0, cu(stream)>>>((const __half*)grad_out, out_ld, rois, R, scale, H, W, C, ph, pw,
-                                                                  sampling_ratio, grad_in, in_ld);
-  STEP_LAUNCH_CHECK("roi_align_bwd_nhwc_kernel");
-  return 0;
-}
-
-extern "C" size_t step_roi_align_bwd_slice_workspace_bytes(int K, int H, int W, int C, int roi_T, int feat_T) {
-  if (K <= 0 || H <= 0 || W <= 0 || C <= 0 || roi_T <= 0 || feat_T <= 0) return 0;
-  return (size_t)(K / feat_T) * roi_T * H * W * C * sizeof(float);
-}
-
-extern "C" int step_roi_align_bwd_slice_nhwc(const void* grad_out, int dtype, int out_ld, const float* rois, int R, float scale, int ph,
-                                             int pw, int K, int H, int W, int C, int sampling_ratio, int roi_T, int feat_T, int t_start,
-                                             float* grad_in, int in_ld, void* workspace, size_t ws_bytes, step_stream_t stream) {
-  STEP_CHECK_ARG(K > 0 && H > 0 && W > 0 && C > 0 && R >= 0 && ph > 0 && pw > 0, "roi_align_bwd_slice_nhwc: bad shape");
-  STEP_CHECK_ARG(dtype == STEP_F32 || dtype == STEP_F16, "roi_align_bwd_slice_nhwc: bad dtype");
-  STEP_CHECK_ARG(C % 4 == 0 && in_ld % 4 == 0 && out_ld % 4 == 0 && in_ld >= C && out_ld >= C,
-                 "roi_align_bwd_slice_nhwc: C / ld must be multiples of 4");
-  STEP_CHECK_ARG(feat_T > 0 && K % feat_T == 0 && roi_T > 0 && t_start >= 0 && t_start + roi_T <= feat_T,
-                 "roi_align_bwd_slice_nhwc: bad frame map roi_T=%d feat_T=%d t_start=%d K=%d", roi_T, feat_T, t_start, K);
-  STEP_CHECK_ARG(grad_in && workspace && (R == 0 || (grad_out && rois)), "roi_align_bwd_slice_nhwc: null pointer");
-  STEP_CHECK_ARG((((uintptr_t)grad_in | (uintptr_t)grad_out | (uintptr_t)workspace) & 15) == 0,
-                 "roi_align_bwd_slice_nhwc: pointers must be 16-byte aligned");
-  const size_t need = step_roi_align_bwd_slice_workspace_bytes(K, H, W, C, roi_T, feat_T);
-  if (ws_bytes < need) return fail(STEP_E_WORKSPACE, "roi_align_bwd_slice_nhwc: workspace %zu < %zu", ws_bytes, need);
-  const int frames = (K / feat_T) * roi_T;
-  if (dtype == STEP_F32)
-    roi_align_bwd_slice_nhwc_kernel<float><<<frames, 256, 0, cu(stream)>>>((const float*)grad_out, out_ld, rois, R, scale, H, W, C, ph, pw,
-                                                                            sampling_ratio, roi_T, feat_T, t_start, (float*)workspace,
-                                                                            grad_in, in_ld);
-  else
-    roi_align_bwd_slice_nhwc_kernel<__half><<<frames, 256, 0, cu(stream)>>>((const __half*)grad_out, out_ld, rois, R, scale, H, W, C, ph,
-                                                                             pw, sampling_ratio, roi_T, feat_T, t_start, (float*)workspace,
-                                                                             grad_in, in_ld);
-  STEP_LAUNCH_CHECK("roi_align_bwd_slice_nhwc_kernel");
-  return 0;
-}
-
-extern "C" int step_roi_pool_bwd_slice_nhwc(const void* grad_out, int dtype, int out_ld, const int32_t* argmax, const float* rois, int R,
-                                            int ph, int pw, int K, int H, int W, int C, int roi_T, int feat_T, int t_start,
-                                            float* grad_in, int in_ld, step_stream_t stream) {
-  STEP_CHECK_ARG(K > 0 && H > 0 && W > 0 && C > 0 && R >= 0 && ph > 0 && pw > 0, "roi_pool_bwd_slice_nhwc: bad shape");
-  STEP_CHECK_ARG(dtype == STEP_F32 || dtype == STEP_F16, "roi_pool_bwd_slice_nhwc: bad dtype");
-  STEP_CHECK_ARG(C % 4 == 0 && in_ld % 4 == 0 && in_ld >= C && out_ld >= C,
-                 "roi_pool_bwd_slice_nhwc: C=%d in_ld=%d must be multiples of 4, out_ld=%d >= C", C, in_ld, out_ld);
-  STEP_CHECK_ARG(feat_T > 0 && K % feat_T == 0 && roi_T > 0 && t_start >= 0 && t_start + roi_T <= feat_T,
-                 "roi_pool_bwd_slice_nhwc: bad frame map roi_T=%d feat_T=%d t_start=%d K=%d", roi_T, feat_T, t_start, K);
-  STEP_CHECK_ARG(grad_in && (R == 0 || (grad_out && argmax && rois)), "roi_pool_bwd_slice_nhwc: null pointer");
-  STEP_CHECK_ARG(((uintptr_t)grad_in & 15) == 0, "roi_pool_bwd_slice_nhwc: grad_in must be 16-byte aligned");
-  const long long npix = (long long)H * W;
-  STEP_CHECK_ARG(npix <= kPoolBwdMaxPixels,
-                 "roi_pool_bwd_slice_nhwc: H*W=%lld exceeds the %d-pixel limit of the shared-memory accumulator (inputs up to ~1280x1280)",
-                 npix, kPoolBwdMaxPixels);
-  if (R == 0) return 0;
-  // the widest channel chunk whose accumulator fits, no wider than C needs
-  int chunk = kPoolBwdMaxChunk;
-  while (chunk > kPoolBwdMinChunk && (npix * chunk * (long long)sizeof(float) > kPoolBwdSmem || chunk >= 2 * C)) chunk /= 2;
-  const size_t smem = (size_t)npix * chunk * sizeof(float);
-  const dim3 grid((K / feat_T) * roi_T, ceil_div(C, chunk));
-  static std::atomic<unsigned long long> seen32{0}, seen16{0};
-  if (dtype == STEP_F32) {
-    if (int rc = allow_dynamic_smem(roi_pool_bwd_slice_nhwc_kernel<float>, seen32, kPoolBwdSmem, "roi_pool_bwd_slice_nhwc")) return rc;
-    roi_pool_bwd_slice_nhwc_kernel<float><<<grid, chunk, smem, cu(stream)>>>((const float*)grad_out, out_ld, argmax, rois, R, ph * pw,
-                                                                             (int)npix, C, roi_T, feat_T, t_start, grad_in, in_ld);
-  } else {
-    if (int rc = allow_dynamic_smem(roi_pool_bwd_slice_nhwc_kernel<__half>, seen16, kPoolBwdSmem, "roi_pool_bwd_slice_nhwc")) return rc;
-    roi_pool_bwd_slice_nhwc_kernel<__half><<<grid, chunk, smem, cu(stream)>>>((const __half*)grad_out, out_ld, argmax, rois, R, ph * pw,
-                                                                              (int)npix, C, roi_T, feat_T, t_start, grad_in, in_ld);
-  }
-  STEP_LAUNCH_CHECK("roi_pool_bwd_slice_nhwc_kernel");
   return 0;
 }
 

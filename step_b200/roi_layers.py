@@ -4,6 +4,10 @@ names, argument order, return types and error behaviour, implemented by libstep_
 
 Reference call sites: models/networks.py:28-31,44 (ROIAlign/ROIPool), test.py:192 / demo.py:158 /
 train.py:547 (nms).
+
+The ROIAlign / ROIPool backwards have no atomics (the reference's scatter with atomicAdd): their gradients repeat bit for
+bit from run to run and on any stream, and equal the channels-last backward of training.train_step transposed
+(tests/test_gpu_roi_bwd_det.py).
 """
 import torch
 from torch import nn

@@ -9,9 +9,9 @@ over K rounds after one warm-up of each (wall time around a device synchronise):
     ops, loss_back.backward()), parameter gradients zeroed before each;
   * train_step(..., loss_scale=1.0, dropout=True).
 Neither runs an optimizer.  Peak memory is torch.cuda.max_memory_allocated over one step of each.  One more autograd
-step runs under torch.profiler, and the device time of the NCHW ROIAlign / ROIPool backward kernels (the atomic ones the
-driver's contiguous conv_feat slices reach) is summed from its trace, beside that of train_step's deterministic
-channels-last ROI backward in a profiled train_step.  Prints one JSON line per pool mode with the card's name, power
+step runs under torch.profiler, and the device time of the NCHW ROIAlign / ROIPool backward kernels (the ones the
+driver's contiguous conv_feat slices reach; the field keeps the name it had when they scattered with atomics) is summed
+from its trace, beside that of train_step's channels-last ROI backward in a profiled train_step.  Prints one JSON line per pool mode with the card's name, power
 limit and maximum SM clock, and writes them to FILE (default profiles/h100_<power limit>_autograd_bench.jsonl)."""
 import argparse
 import json
